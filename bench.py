@@ -5,7 +5,7 @@ Workload (config.workload = "c2_bm25_or10_top1000"): BM25 10-term OR query, top-
 over a 100M-doc / 32-split synthetic hdfs-logs-shaped index resident in HBM on each GPU
 (3.125M docs per split; body terms with doc-frequency fractions {20,10,5,5,2,2,1,1,0.5,0.1}%).
 A "step" = one batch of Q = 4 such queries with DISJOINT term sets (the same 32 splits, different
-posting lists), so one step touches Q x postings + the fieldnorm arrays > the 126 MB L2 and the
+posting lists), so one step touches Q x postings + the fieldnorm arrays > the 50 MB L2 and the
 next step's data has been evicted by then ("inputs larger than L2").
 
 Metric: docs scored per second = postings visited (sum of the query terms' doc frequencies over all
@@ -44,22 +44,24 @@ sys.path.insert(0, ROOT)
 FRACS = [0.20, 0.10, 0.05, 0.05, 0.02, 0.02, 0.01, 0.01, 0.005, 0.001]
 Q_SETS = 4
 K = 1000
-# DRAM traffic per launch (dram__bytes_read.sum + dram__bytes_write.sum) cannot be measured inside the
-# timed bench; it is read from profiles/r2_traffic.json, which tools/ncu_traffic.py writes from an
-# `ncu --set full` capture of this same command (the capture file is named there).
-def ncu_traffic(kernel: str):
-    try:
-        t = json.load(open(os.path.join(ROOT, "profiles", "r2_traffic.json")))
-        e = t["kernels"][kernel]
-        return float(e["dram_bytes_per_launch"]), f"{t['capture']} ({e['launches']} launches, workload {e['workload']})"
-    except Exception:
-        return None, None
+# HBM3 bandwidth of the H100 SXM data sheet: the roofline denominator unless MEASURED_PEAKS.json gives a
+# measured one
+DATASHEET_HBM_GBS = 3350.0
+# --dump-outputs writes at most this many bytes; larger outputs are written as a fixed, seeded row sample
+DUMP_MAX_BYTES = 64 << 20
+
+
+def positive_int(text: str) -> int:
+    v = int(text)
+    if v < 1:
+        raise argparse.ArgumentTypeError(f"must be at least 1, got {v}")
+    return v
 
 
 def parse_args():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=200)
+    ap.add_argument("--steps", type=positive_int, default=200, help="timed steps per region (at least 1)")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="qwgpu", choices=["qwgpu", "reference"])
     ap.add_argument("--splits", type=int, default=32, help="splits per GPU")
@@ -67,6 +69,8 @@ def parse_args():
     ap.add_argument("--cpu-sample-splits", type=int, default=0, help="splits in the cpu_baseline sample (0 = auto)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-configs", action="store_true", help="skip the per-config block (C1 / C3 / C4)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step of each region returned as DIR/<name>.npy (float64)")
     return ap.parse_args()
 
 
@@ -140,13 +144,30 @@ class RawSearch:
         out[: len(order), 2] = sc[order, 2] & 0xFFFFFFFF
         return out
 
+    def outputs(self, first_split: int):
+        """What the last run() returned to its caller: num_hits per split, and every returned hit as a row
+        (global split ordinal, doc id, f32 score), in the library's order."""
+        from quickwit_b200 import ffi
+        hit = np.dtype([("v1", "<u8"), ("v2", "<u8"), ("doc_id", "<u4"), ("flags", "<u4"), ("score", "<f4"), ("reserved", "<u4")])
+        assert hit.itemsize == C.sizeof(ffi.QwHit)
+        rows = []
+        for i in range(self.n):
+            m = self.res[i].num_partial_hits
+            if not m:
+                continue
+            h = np.frombuffer(C.string_at(self.res[i].hits, m * hit.itemsize), dtype=hit)
+            rows.append(np.stack([np.full(m, first_split + i, dtype=np.float64), h["doc_id"].astype(np.float64),
+                                  h["score"].astype(np.float64)], axis=1))
+        num_hits = np.array([self.res[i].num_hits for i in range(self.n)], dtype=np.float64)
+        return num_hits, (np.concatenate(rows) if rows else np.zeros((0, 3)))
+
     def free(self):
         for i in range(self.n):
             self.L.qwgpu_split_result_free(C.byref(self.res[i]))
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index: int):
         self.index = index
@@ -288,12 +309,11 @@ def other_configs(ctx, imgs, peak, reps: int = 20, lat_runs: int = 60):
         docs = sum(im.num_docs for im in imgs)
         units = r["postings"] if r["postings"] else docs * len(aggs or {})
         achieved = r["alg_bytes"] / main_us / 1e3 if main_us else 0.0
-        traffic, tsrc = ncu_traffic(name)
         out[name] = {"value": units / (gpu_us * 1e-6), "unit": "postings/s" if r["postings"] else "column values/s",
                      "num_hits": dec["num_hits"], "device_us": gpu_us, "main_kernel_us": main_us, "launches": r["launches"],
                      "exact_fallbacks": r["fallbacks"], "leaf_search_p50_ms": 1e3 * lat[len(lat) // 2],
                      "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                                  "algorithmic_bytes_per_launch": r["alg_bytes"], "traffic": traffic, "traffic_source": tsrc}}
+                                  "algorithmic_bytes_per_launch": r["alg_bytes"]}}
     return out
 
 
@@ -493,6 +513,30 @@ def config5_mixed(ctx, imgs, peak, world: int, concurrency: int = 64, queries_pe
             "api": "qwgpu_leaf_search from 64 host threads; responses checked against the sequential ones"}
 
 
+def dump_outputs(out_dir: str, seam_c, e2e):
+    """--dump-outputs: the last timed step of both regions as float64 .npy files, so that two builds can be
+    compared output for output on the same seeded corpus. seam_c[q] = RawSearch.outputs() of query q;
+    e2e[q] = the decoded LeafSearchResponse of query q. Rows are (global split ordinal, doc id, score)."""
+    arrays = {"seam_c_num_hits": np.stack([nh for nh, _ in seam_c]),
+              "e2e_num_hits": np.array([float(d["num_hits"]) for d in e2e])}
+    for q, (_, rows) in enumerate(seam_c):
+        arrays[f"seam_c_hits_q{q}"] = rows
+    for q, d in enumerate(e2e):
+        arrays[f"e2e_hits_q{q}"] = np.array([(float(int(h["split_id"].rsplit("-", 1)[1])), float(h["doc_id"]),
+                                              float(h["sort_value"][1])) for h in d["partial_hits"]], dtype=np.float64).reshape(-1, 3)
+    total = sum(v.nbytes for v in arrays.values())
+    if total > DUMP_MAX_BYTES:  # keep the same seeded fraction of the rows of every hit list
+        rng = np.random.default_rng(0)
+        keep = DUMP_MAX_BYTES / total
+        for name, v in arrays.items():
+            if name.endswith("num_hits"):
+                continue
+            arrays[name] = v[np.sort(rng.choice(len(v), int(len(v) * keep), replace=False))]
+    os.makedirs(out_dir, exist_ok=True)
+    for name, v in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), v.astype(np.float64))
+
+
 def main():
     a = parse_args()
     rank = int(os.environ.get("RANK", "0"))
@@ -591,7 +635,8 @@ def main():
         gath_host = torch.zeros(world * Q_SETS * part_bytes, dtype=torch.uint8).pin_memory()
         by_query = torch.zeros(Q_SETS * world * part_bytes, dtype=torch.uint8)  # [query][rank][partial]
 
-    def step():
+    def step(keep: bool = False):
+        """keep: leave the results allocated so that they can be read after the timed region."""
         acc = dict(gpu_us=0.0, main_us=0.0, launches=0, postings=0, alg_bytes=0, d2h=0, h2d=0, fallbacks=0)
         for s in searches:
             r = s.run()
@@ -600,7 +645,8 @@ def main():
             for k in ("launches", "postings", "alg_bytes", "d2h", "fallbacks"):
                 acc[k] += r[k]
             acc["h2d"] += s.plan_bytes
-            s.free()
+            if not keep:
+                s.free()
         return acc
 
     last = {}
@@ -681,9 +727,14 @@ def main():
         sampler.start()
     sync()
     t0 = time.perf_counter()
-    accs = [step() for _ in range(a.steps)]
+    accs = [step(keep=bool(a.dump_outputs) and i == a.steps - 1) for i in range(a.steps)]
     sync()
     wall_c = time.perf_counter() - t0
+    seam_c_out = None
+    if a.dump_outputs:
+        seam_c_out = [s.outputs(rank * a.splits) for s in searches]
+        for s in searches:
+            s.free()
     for _ in range(max(a.warmup, 3)):
         step_e2e()
     sync()
@@ -711,6 +762,8 @@ def main():
         cold_ms = 1e3 * (time.perf_counter() - t)
     hits0 = proto.dec_leaf_search_response(last[0])
     assert len(hits0["partial_hits"]) == K and hits0["num_hits"] > 0
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, seam_c_out, [proto.dec_leaf_search_response(last[q]) for q in range(Q_SETS)])
 
     gpu_s = sum(x["gpu_us"] for x in accs) * 1e-6
     main_s = sum(x["main_us"] for x in accs) * 1e-6
@@ -734,9 +787,9 @@ def main():
     # figures are the slowest rank's
     c5 = None
     if not a.no_configs:
-        peak5 = 6650.0
+        peak5 = DATASHEET_HBM_GBS
         try:
-            peak5 = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))).get("hbm_gbs", 6650.0))
+            peak5 = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))).get("hbm_gbs", DATASHEET_HBM_GBS))
         except Exception:
             pass
         if world > 1:
@@ -777,7 +830,7 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", DATASHEET_HBM_GBS))
     achieved = (alg_bytes / n_main) / (main_s / n_main) / 1e9 if main_s > 0 else 0.0  # rank-0 kernel
     out = {
         "metric": "docs_scored_per_sec", "value": postings / gpu_s, "unit": "postings/s", "n_gpus": world,
@@ -797,10 +850,8 @@ def main():
         "gpu_launches": launches,
         "exact_fallbacks": sum(x["fallbacks"] for x in accs),
         "roofline": {"bound": "hbm", "kernel": "k_union<COLLECT>", "achieved": achieved, "peak": peak,
-                     "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peaks else "fallback 6650 GB/s",
+                     "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peaks else f"H100 SXM data sheet {DATASHEET_HBM_GBS:.0f} GB/s",
                      "unit": "GB/s", "frac": achieved / peak,
-                     "traffic": ncu_traffic("k_union<COLLECT>")[0] if (a.splits, a.docs_per_split) == (32, 3_125_000) else None,
-                     "traffic_source": ncu_traffic("k_union<COLLECT>")[1],
                      "algorithmic_bytes_per_launch": alg_bytes / n_main, "avg_launch_us": 1e6 * main_s / n_main},
         "clocks": clocks,
     }

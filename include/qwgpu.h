@@ -1,8 +1,8 @@
 /*
- * qwgpu.h — C ABI of libqwgpu.so: the B200-native drop-in for Quickwit's per-split leaf search.
+ * qwgpu.h — C ABI of libqwgpu.so: the H100-native drop-in for Quickwit's per-split leaf search.
  *
  * What each entry point replaces in the reference (paths relative to
- * /root/reference/quickwit/):
+ * the quickwit-oss/quickwit repository @ 544b50f):
  *
  *   qwgpu_leaf_search          SearchService::leaf_search(LeafSearchRequest) -> LeafSearchResponse
  *                              quickwit-search/src/service.rs:81,177-203 (seam A, SURVEY.md §3.4)

@@ -12,7 +12,7 @@
  * The image follows the SHAPES of a tantivy segment (SURVEY.md Appendix A: 128-doc bit-packed
  * posting blocks with 4-lane interleave + skip entries, 1-byte fieldnorm ids, bit-packed columns
  * with min/gcd header, dictionary-encoded string columns), but it is OUR format: tantivy's byte
- * layout is not pinned by anything in /root/reference (SURVEY.md §8c "NOT pinned").
+ * layout is not pinned by anything in the reference repository (SURVEY.md §8c "NOT pinned").
  */
 #ifndef QWGPU_FORMAT_H
 #define QWGPU_FORMAT_H

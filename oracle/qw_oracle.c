@@ -6,7 +6,7 @@
  *
  * PARITY STATUS: "semantics pinned, byte format unpinned". The arithmetic of this path lives in
  * tantivy 0.26.0 @ edfb02b (+ tantivy-columnar 0.7.0, tantivy-bitpacker 0.10.0, bitpacking 0.9.3),
- * an un-vendored git dependency absent from /root/reference (quickwit/Cargo.toml:385-391), and no
+ * an un-vendored git dependency absent from the reference repository (quickwit/Cargo.toml:385-391), and no
  * Rust toolchain exists here, so oracle/_ref cannot be built. This file restates the published
  * algorithms (SURVEY.md Appendix A) doc-at-a-time, the way tantivy drives a SegmentCollector, and
  * is pinned against every golden vector the reference's own tests hold for this path
@@ -14,7 +14,7 @@
  * (include/qwgpu_format.h), decoded here by an independent scalar reader.
  *
  * Each function cites the reference file:line whose behaviour it follows (paths relative to
- * /root/reference/quickwit/).
+ * the quickwit-oss/quickwit repository @ 544b50f).
  */
 #include <math.h>
 #include <stdint.h>

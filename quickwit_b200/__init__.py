@@ -1,7 +1,7 @@
-"""quickwit_b200 — B200-native drop-in for Quickwit's per-split leaf search hot path.
+"""quickwit_b200 — H100-native drop-in for Quickwit's per-split leaf search hot path.
 
 Layout (only what the path needs, see DESIGN.md):
-  csrc/        CUDA kernels (sm_100a) + C++ host side + the C ABI (include/qwgpu.h) -> libqwgpu.so
+  csrc/        CUDA kernels (sm_90a) + C++ host side + the C ABI (include/qwgpu.h) -> libqwgpu.so
   ffi.py       ctypes binding of the C ABI (no logic)
   service.py   host-side mirror of the reference interface: SearchService.leaf_search,
                LambdaLeafSearchInvoker.invoke_leaf_search, root-side merge

@@ -8,7 +8,7 @@ void set_last_error(const std::string& msg) { g_last_error = msg; }
 
 extern "C" {
 const char* qwgpu_last_error(void) { return qw::g_last_error.c_str(); }
-const char* qwgpu_version(void) { return "qwgpu 0.1.0 (sm_100a)"; }
+const char* qwgpu_version(void) { return "qwgpu 0.1.0 (sm_90a)"; }
 void qwgpu_buf_free(void* buf) { free(buf); }
 float qwgpu_bm25_weight(uint64_t doc_freq, uint64_t num_docs, float boost) {
   float w = qw::bm25_idf(doc_freq, num_docs) * (1.0f + qw::BM25_K1);

@@ -978,13 +978,14 @@ void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std:
     low[i].P.num_windows = low[i].empty ? 0 : (low[i].P.num_docs + W - 1) / W;
     max_windows = std::max(max_windows, low[i].P.num_windows);
   }
-  // sampling stride of the threshold-estimation pass: 1/16 of the windows (24 or 32 save ~15 us in the
-  // histogram pass but the looser threshold costs about as much in the collect pass)
+  // sampling stride of the threshold-estimation pass: 1/16 of the windows (a coarser sample shortens the histogram
+  // pass, but the looser threshold lets more candidates through the collect pass)
   static const uint32_t stride_cap = getenv("QWGPU_STRIDE_CAP") ? (uint32_t)atoi(getenv("QWGPU_STRIDE_CAP")) : 16u;
   uint32_t stride = std::min(std::max(stride_cap, 1u), std::max(1u, max_windows / 8));
   // BM25-union batches can sample the threshold over finer windows (W / QWGPU_HDIV: the same fraction of the docs in
-  // more work items). Measured on the bench workload: 1 and 2 are equal (1.22 ms per 4-query step), 4 and 8 are slower
-  // (1.28 / 1.48 ms: the per-window clause chain does not shrink with the window), so the default stays 1.
+  // more work items). Measured on the bench workload, one H100 80GB HBM3 (400 W power limit): 1 gives 1.175-1.183 ms per
+  // 4-query step, 2 gives 1.194-1.203 ms and 4 gives 1.216-1.231 ms (the per-window clause chain does not shrink with
+  // the window), so the default stays 1.
   static const uint32_t hdiv = getenv("QWGPU_HDIV") ? std::max(1u, (uint32_t)atoi(getenv("QWGPU_HDIV"))) : 1u;
   const uint32_t W_h = use_union ? std::max(1024u, (W / hdiv) & ~1023u) : W;
   if (use_union) {
@@ -996,9 +997,9 @@ void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std:
     }
     stride = std::min(std::max(stride_cap, 1u), std::max(1u, mw / 8));
     // Large requests: at most ONE sampled window per resident block (the sampled pass is latency bound — a block
-    // that gets two windows doubles its duration), up to a stride of 32. Bench workload (6528 windows, 296 blocks):
-    // stride 23 instead of 16, 1.146 against 1.186 ms per 4-query step (32: 1.169 — the looser threshold then costs
-    // more candidates in the collect pass than the sampled pass saves).
+    // that gets two windows doubles its duration), up to a stride of 32. Bench workload on one H100 80GB HBM3 (400 W
+    // power limit; 6528 windows, 132 SMs x 2 = 264 blocks): stride 25 instead of 16, 1.175-1.183 against 1.209-1.211 ms
+    // per 4-query step (a fixed stride of 32: 1.174-1.181 ms, no better).
     if (!getenv("QWGPU_STRIDE_CAP")) {
       const uint32_t per_block = (tw + (uint32_t)(sm_count * QU_MINB) - 1) / (uint32_t)(sm_count * QU_MINB);
       stride = std::max(stride, std::min({per_block, 32u, std::max(1u, mw / 8)}));
@@ -1073,9 +1074,10 @@ void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std:
   size_t out_bytes = do_merge ? (do_gather ? al(o_final + 16 + (size_t)merge->k * sizeof(qwk::DMergedHit)) : al(o_merged + rec_bytes)) : out_off[n];
 
   // Admission: at most QWGPU_MAX_IN_FLIGHT (default 16) searches drive the device at once; further callers wait here
-  // on a condition variable (no CUDA calls, no spinning). Measured on the mixed config-5 query set: 16 host threads
-  // sustain 1860 queries/s, 64 unthrottled threads 920 — beyond a dozen or so submitters the driver's per-context
-  // lock and 64 interleaved streams cost more than the extra overlap brings.
+  // on a condition variable (no CUDA calls, no spinning). Measured on the mixed config-5 query set from 64 host threads,
+  // one H100 80GB HBM3 (400 W power limit): with the limit at 16, 1643 queries/s (p99 66-72 ms) in both of two runs;
+  // with it at 64, 894 and 1517 queries/s (p99 341 and 174 ms) — the driver's per-context lock and 64 interleaved
+  // streams cost more than the extra overlap brings.
   static const int max_in_flight = getenv("QWGPU_MAX_IN_FLIGHT") ? std::max(1, atoi(getenv("QWGPU_MAX_IN_FLIGHT"))) : 16;
   CallSlot* slot = nullptr;
   {
@@ -1241,10 +1243,10 @@ void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std:
       u.first_work = q.first_work; u.n_splits = n; u.total_work = q.total_work; u.stride = q.stride; u.W = sampled ? W_h : W;
       u.sm = mode == qwk::MODE_HIST ? ulay_h : ulay_c;
       // QWGPU_DYNAMIC_WORK=1: windows handed out one at a time from a counter instead of a static chunk per block.
-      // Measured on the bench workload (uniform splits): 207 us against 194 us per launch — consecutive windows of a
-      // block then belong to different splits, and the per-window plan switch sits on the producer's critical path —
-      // with no gain for concurrent calls, so static chunks stay the default; the counter road is kept for skewed
-      // corpora (validated: the full GPU suite passes in both modes).
+      // Measured on the bench workload (uniform splits), one H100 80GB HBM3 (400 W power limit): 216-218 us against
+      // 201-202 us per launch — consecutive windows of a block then belong to different splits, and the per-window
+      // plan switch sits on the producer's critical path — so static chunks stay the default; the counter road is kept
+      // for skewed corpora and returns the same hits.
       static const bool dynamic_work = getenv("QWGPU_DYNAMIC_WORK") != nullptr;
       if (dynamic_work && n_ctr < 64) u.work_ctr = (uint32_t*)(slot->d_scratch + s_ctr) + n_ctr++;
 #ifdef QU_PROFILE

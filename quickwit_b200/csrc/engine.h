@@ -93,7 +93,7 @@ struct Engine {
   std::condition_variable loaded_cv;
   struct Loader { std::thread t; std::shared_ptr<SplitDev> sp; };
   std::vector<Loader> loaders;
-  int sm_count = 148;
+  int sm_count = 0;  // set from cudaDeviceProp in Engine::Engine
   int max_smem_optin = 0;
 
   explicit Engine(int dev);

@@ -1,4 +1,4 @@
-// kernels.cuh — sm_100a kernels of the per-split leaf search hot path.
+// kernels.cuh — sm_90a kernels of the per-split leaf search hot path.
 //
 // Execution model ("window engine"): a 512-thread block owns one doc-id WINDOW (16384 docs when shared
 // memory allows; 32768 for unscored plans) of one split and evaluates the whole boolean query over it
@@ -20,8 +20,7 @@
 //      survivors go to a candidate list that k_select reduces with the reference's total order.
 // This replaces tantivy's doc-at-a-time Scorer/Collector loop (SURVEY.md §3.3 step 10c, §8a rows
 // a3-a12). No tensor cores: the work is integer decode / compare plus one f32 multiply-add per
-// posting; the binding resource measured on B200 is instruction issue, well before HBM bandwidth
-// (DESIGN.md §5, profiles/r1_summary.md).
+// posting.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -1024,11 +1023,11 @@ __global__ void __launch_bounds__(QW_THREADS, QW_MIN_BLOCKS_PER_SM) k_window(con
             // clause order, but there is no block-wide barrier per clause and no warp idles while a
             // short clause finishes. Blocks of one clause touch distinct docs, so they commute.
             const uint32_t G = s_misc[0];
-            // (measured and rejected: a spare warp prefetching the next window's bytes into L2 made the
-            // kernel 4-5 % slower — the staging phases are not DRAM-latency bound enough to pay for it)
+            // (tried and rejected: a spare warp prefetching the next window's bytes into L2 — the staging
+            // phases are not DRAM-latency bound enough to pay for it)
             volatile uint32_t* ticket = (volatile uint32_t*)&s_misc[5];
             float* score = sm.f32(LV.ssum);
-            // (static round-robin assignment; handing blocks out from a shared counter measured slower)
+            // (static round-robin assignment; handing blocks out from a shared counter was tried and rejected)
             for (uint32_t g = warp; g < G; g += QW_WARPS) {
               const BlkRec r = s_blk[g];
               const DInstr& ti = s_instr[s_tinstr[r.slot]];

@@ -1,5 +1,5 @@
 // union_kernel.cuh — the BM25 top-K shape (pure OR of positive-weight scored terms ranked by _score)
-// as a warp-specialised TMA + mbarrier pipeline for sm_100a.
+// as a warp-specialised TMA + mbarrier pipeline for sm_90a (Hopper).
 //
 // Replaces tantivy's BufferedUnionScorer + Bm25Weight + TopDocs loop behind `searcher.search`
 // (quickwit-search/src/leaf.rs:637; SURVEY.md §8a rows a3-a5, a10-a11) for the headline query shape.
@@ -36,9 +36,10 @@
 namespace qwk {
 
 #ifndef QU_THREADS
-/* 13 consumer warps + the producer, two blocks per SM: 72 registers per thread. Measured against 512 threads (64
- * registers: 232 B of spills and re-materialised shared-window addresses in the block loop): 186.8 vs 196.0 us per launch
- * (384 threads / 80 registers: 188.4 us). */
+/* 13 consumer warps + the producer, two blocks per SM: 72 registers per thread (sm_90a: 252 B of spill stores in the
+ * COLLECT instantiation). Measured on one H100 80GB HBM3 (400 W power limit), k_union<COLLECT> per launch on the bench
+ * workload: 201-202 us; 384 threads / 80 registers (56 B of spills): 204-205 us; 512 threads / 64 registers (292 B of
+ * spills): 211-213 us. */
 #define QU_THREADS 448
 #endif
 #define QU_NCW (QU_THREADS / 32 - 1)   /* consumer warps; warp QU_NCW is the producer */
@@ -57,8 +58,9 @@ namespace qwk {
 #endif
 #ifndef QU_DEFER_SWEEP
 /* 1 = COLLECT sweeps a finished window only after the warp's first decode of the next window (overlaps the wait for the
- * window's last clauses with work). Measured: 369 us against 195 us per launch — the decoded pair has to stay live
- * across the sweep loop, and under the 64-register cap that spills the inner loop (384 B of spill stores) — so it is off. */
+ * window's last clauses with work). Measured on one H100 80GB HBM3 (400 W power limit): 401 us against 202 us per launch —
+ * the decoded pair has to stay live across the sweep loop, and under the register cap that spills the inner loop (sm_90a:
+ * 440 B of spill stores) — so it is off. */
 #define QU_DEFER_SWEEP 0
 #endif
 

@@ -27,7 +27,8 @@ def test_every_declared_symbol_is_exported():
 
 
 def test_no_cpu_fallback():
-    if os.path.exists("/dev/nvidia0"):
+    import torch
+    if torch.cuda.device_count() > 0:  # (a container may expose its GPU under another /dev/nvidia<N>)
         pytest.skip("a GPU is present")
     with pytest.raises(ffi.QwGpuError) as e:
         service.SearcherContext(0)

@@ -1,7 +1,7 @@
 """SASS evidence for the TMA / mbarrier pipelines: per kernel the opcode histogram and every bulk-copy (UBLKCP),
 mbarrier (SYNCS.*), shared-memory atomic (ATOMS) and bulk-fence instruction with two lines of context.
 
-    python tools/sass_summary.py quickwit_b200/libqwgpu.so k_union k_aggscan > profiles/r2_sass_summary.txt
+    python tools/sass_summary.py quickwit_b200/libqwgpu.so k_union k_aggscan > sass_summary.txt
 
 Needs cuobjdump (CUDA toolkit); runs on the build box, no GPU."""
 import collections
