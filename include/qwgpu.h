@@ -122,7 +122,21 @@ typedef struct qwgpu_split_result {
   uint32_t exact_fallbacks;  /* 1 when the sampled top-K threshold failed verification */
   uint64_t postings_scored; /* Σ doc_freq of the plan's terms ("docs scored", SURVEY.md §8d) */
   uint64_t algorithmic_bytes; /* SURVEY.md §8d numerator for this split/plan */
+  /* The path the call took (DESIGN.md §4.6). Per call: every split of the batch reports the same values. */
+  uint32_t kernel_mask;      /* QWGPU_KERNEL_* bits of the search kernels launched */
+  uint32_t window_docs;      /* docs per work item: the window size W, the driving term's block size (128) for
+                                k_driver, the 8192-doc chunk for k_aggscan */
+  uint32_t sample_stride;    /* stride of the sampled top-K threshold pass; 0 when no sampled pass ran */
+  uint32_t radix_passes;     /* exact radix rounds (histogram pass + digit pick) of the top-K threshold */
+  uint32_t refined;          /* 1 when a failed sampled threshold was repaired by the candidates-only pass */
 } qwgpu_split_result;
+
+/* qwgpu_split_result.kernel_mask */
+#define QWGPU_KERNEL_UNION 1u   /* k_union: BM25 unions (TMA + mbarrier pipeline) */
+#define QWGPU_KERNEL_DRIVER 2u  /* k_driver: one driving posting list + column filters */
+#define QWGPU_KERNEL_AGGSCAN 4u /* k_aggscan: match_all + flat aggregations */
+#define QWGPU_KERNEL_WINDOW 8u  /* k_window: the generic window kernel */
+#define QWGPU_KERNEL_PHRASE 16u /* k_phrase: the phrase pre-pass */
 
 /* Runs `num_splits` plans (plan i against split_ids[i]) in ONE batched launch sequence.
  * results[i] is filled for every split; status[i] is 0 or a QWGPU_E* code for that split. */

@@ -127,6 +127,11 @@ int qwgpu_split_search(qwgpu_ctx* ctx, uint32_t num_splits, const char* const* s
     r.exact_fallbacks = st.exact_fallbacks;
     r.postings_scored = outs[i].postings_scored;
     r.algorithmic_bytes = outs[i].algorithmic_bytes;
+    r.kernel_mask = st.kernel_mask;
+    r.window_docs = st.window_docs;
+    r.sample_stride = st.sample_stride;
+    r.radix_passes = st.radix_passes;
+    r.refined = st.refined;
   }
   if (!first_err.empty()) qw::set_last_error(first_err);
   return 0;

@@ -1220,6 +1220,7 @@ void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std:
       if (mode == qwk::MODE_HIST) qwk::k_driver<qwk::MODE_HIST><<<dgrid, QD_WARPS * 32, 0, st>>>(d);
       else qwk::k_driver<qwk::MODE_COLLECT><<<dgrid, QD_WARPS * 32, 0, st>>>(d);
       stats.launches++;
+      stats.kernel_mask |= QWGPU_KERNEL_DRIVER;
       return;
     }
     if (q.total_work == 0) return;
@@ -1234,6 +1235,7 @@ void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std:
       const uint32_t agrid = std::min<uint32_t>(q.total_work, (uint32_t)(sm_count * std::max(aocc, 1)));
       qwk::k_aggscan<<<agrid, QA_THREADS, alay.total, st>>>(a);
       stats.launches++;
+      stats.kernel_mask |= QWGPU_KERNEL_AGGSCAN;
       return;
     }
     if (use_union && flags == 0 && (mode == qwk::MODE_COLLECT || (level == 0 && !use_prefix))) {
@@ -1271,6 +1273,7 @@ void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std:
       }
 #endif
       stats.launches++;
+      stats.kernel_mask |= QWGPU_KERNEL_UNION;
       return;
     }
     uint32_t grid = std::min<uint32_t>(q.total_work, (uint32_t)(sm_count * occ));
@@ -1279,6 +1282,7 @@ void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std:
     else if (all_union && old_union) qwk::k_window<qwk::MODE_COLLECT, true><<<grid, QW_THREADS, lay.total, st>>>(q);
     else qwk::k_window<qwk::MODE_COLLECT, false><<<grid, QW_THREADS, lay.total, st>>>(q);
     stats.launches++;
+    stats.kernel_mask |= QWGPU_KERNEL_WINDOW;
   };
   const uint32_t sel_smem = 3 * 8 * QW_CAND_CAP;  // [all first words | 3 x QW_SEL_MAX survivors] or 3 x all (degenerate ties)
   auto run_collect = [&](uint32_t flags) {
@@ -1326,12 +1330,15 @@ void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std:
     const size_t psm = (size_t)QP_WARPS * QP_SMEM_WORDS(max_terms) * 4;
     qwk::k_phrase<<<(phrase_blocks + QP_WARPS - 1) / QP_WARPS, QP_WARPS * 32, psm, st>>>((const DPhrase*)(slot->d_blob + o_phr), n_phrases, phrase_blocks, max_terms);
     stats.launches++;
+    stats.kernel_mask |= QWGPU_KERNEL_PHRASE;
   }
+  stats.window_docs = use_driver ? QW_BLOCK_LEN : W;
   bool ok = true;
   float main_ms = 0;
   auto add_main = [&]() { float ms = 0; cudaEventElapsedTime(&ms, slot->ev2, slot->ev3); main_ms += ms; };
   if (any_topk && stride > 1) {
     // fast path: threshold from a 1/stride sample of the windows, verified after the collect pass
+    stats.sample_stride = stride;
     launch_window(qwk::MODE_HIST, true, 0, 0, 0);
     qwk::k_pick<<<n, 256, 0, st>>>(kp.plans, kp.thresh, 0, edge_sample ? 2 : 1, stride, nullptr);
     stats.launches++;
@@ -1383,10 +1390,12 @@ void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std:
       launch_window(qwk::MODE_HIST, false, level, level > 0 ? 1 : 0, refine ? F_REFINE : 0);
       qwk::k_pick<<<n, 256, 0, st>>>(kp.plans, kp.thresh, level, 0, 1, d_state);
       stats.launches++;
+      stats.radix_passes++;
       CUDA_CHECK(cudaMemcpyAsync(th.data(), slot->d_scratch + s_thr, n * sizeof(DThresh), cudaMemcpyDeviceToHost, st));
       wait_stream();
       done = all_done();
     }
+    stats.refined = refine ? 1 : 0;
     run_collect(refine ? (F_REFINE | F_CANDS_ONLY) : 0);
     CUDA_CHECK(cudaEventRecord(slot->ev1, st));
     wait_stream();

@@ -72,6 +72,12 @@ struct BatchStats {
   uint32_t launches = 0;
   uint32_t exact_fallbacks = 0;
   uint64_t h2d_bytes = 0, d2h_bytes = 0;
+  // the path the call took (qwgpu_split_result)
+  uint32_t kernel_mask = 0;    // QWGPU_KERNEL_*
+  uint32_t window_docs = 0;
+  uint32_t sample_stride = 0;  // 0: no sampled threshold pass
+  uint32_t radix_passes = 0;   // exact histogram + k_pick rounds
+  uint32_t refined = 0;        // 1: candidates-only repair of a failed sampled threshold
 };
 
 struct Engine {

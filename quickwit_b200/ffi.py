@@ -26,6 +26,8 @@ SORT_NONE, SORT_DOCID, SORT_SCORE, SORT_COLUMN = range(4)
 ORDER_ASC, ORDER_DESC = 0, 1
 AGG_TERMS, AGG_HISTOGRAM, AGG_RANGE, AGG_STATS = 1, 2, 3, 4
 ABSENT = 0xFFFFFFFF
+# qwgpu_split_result.kernel_mask (qwgpu.h)
+KERNEL_UNION, KERNEL_DRIVER, KERNEL_AGGSCAN, KERNEL_WINDOW, KERNEL_PHRASE = 1, 2, 4, 8, 16
 PLAN_MAGIC = 0x4E4C5051
 MAX_AGG_RANGES = 16
 
@@ -116,7 +118,9 @@ class SplitResult(C.Structure):
                 ("agg_cells", C.POINTER(QwAggCell)), ("gpu_time_us", C.c_float),
                 ("main_kernel_us", C.c_float), ("num_kernel_launches", C.c_uint32),
                 ("exact_fallbacks", C.c_uint32), ("postings_scored", C.c_uint64),
-                ("algorithmic_bytes", C.c_uint64)]
+                ("algorithmic_bytes", C.c_uint64), ("kernel_mask", C.c_uint32),
+                ("window_docs", C.c_uint32), ("sample_stride", C.c_uint32),
+                ("radix_passes", C.c_uint32), ("refined", C.c_uint32)]
 
 
 class SynthSpec(C.Structure):

@@ -34,6 +34,12 @@ class SplitSearchResult:
         self.num_kernel_launches = int(r.num_kernel_launches)
         self.postings_scored = int(r.postings_scored)
         self.algorithmic_bytes = int(r.algorithmic_bytes)
+        # the path the call took (per call, the same for every split of the batch)
+        self.kernel_mask = int(r.kernel_mask)
+        self.window_docs = int(r.window_docs)
+        self.sample_stride = int(r.sample_stride)
+        self.radix_passes = int(r.radix_passes)
+        self.refined = int(r.refined)
 
 
 class SearcherContext:

@@ -58,6 +58,35 @@ def range_agg(img, column: str, ranges) -> P.Agg:
     return P.Agg(ffi.AGG_RANGE, column=c, num_buckets=len(ranges), ranges=ranges)
 
 
+def bm25_norm(lengths: np.ndarray) -> np.ndarray:
+    """Per-doc BM25 length norm restated in numpy float32 (tantivy Bm25Weight; formula verified against the reference
+    golden in SURVEY.md Appendix B.1): k1 * (1 - b + b * fieldnorm / avg_fieldnorm), with the fieldnorm QUANTISED through
+    the 256-entry id table and avg_fieldnorm = total tokens / number of docs."""
+    L = ffi.img_lib()
+    lengths = np.asarray(lengths, dtype=np.int64)
+    uniq, inv = np.unique(lengths, return_inverse=True)
+    quant = np.array([L.qwgpu_id_to_fieldnorm(L.qwgpu_fieldnorm_to_id(int(x))) for x in uniq], dtype=np.float32)[inv]
+    f32 = np.float32
+    avg = f32(lengths.sum()) / f32(len(lengths))
+    k1, b = f32(1.2), f32(0.75)
+    return k1 * (f32(1) - b + b * quant / avg)
+
+
+def bm25_weight(doc_freq: int, num_docs: int) -> np.float32:
+    """idf * (1 + k1) in float32, idf = ln(1 + (N - n + 0.5) / (n + 0.5))."""
+    f32 = np.float32
+    idf = np.log(f32(1) + (f32(num_docs - doc_freq) + f32(0.5)) / (f32(doc_freq) + f32(0.5)), dtype=np.float32)
+    return idf * (f32(1) + f32(1.2))
+
+
+def bm25_contributions(tf: np.ndarray, norm: np.ndarray, weight) -> np.ndarray:
+    """One term's per-doc score, weight * (tf / (tf + norm)), 0 where the term is absent (tf == 0). A union adds the
+    contributions of its clauses in clause order, in float32."""
+    tf = np.asarray(tf, dtype=np.float32)
+    with np.errstate(invalid="ignore"):
+        return np.where(tf > 0, np.float32(weight) * (tf / (tf + norm)), np.float32(0)).astype(np.float32)
+
+
 def assert_same(got, want, f64_sum_cells: Sequence[int] = (), ctx: str = ""):
     """got: service.SplitSearchResult, want: oracle.OracleResult. Bit-exact everywhere (doc ids,
     sort values, f32 score bits, counts); f64 sums of f64 columns within 1e-9 relative."""

@@ -12,6 +12,7 @@ import pytest
 from quickwit_b200 import ffi, plan as P, proto, service, splitgen as S
 from quickwit_b200.proto import ASC, DESC
 from oracle import oracle as O
+from helpers import bm25_contributions, bm25_norm, bm25_weight
 from pipeline import MATCH_ALL, bool_, full_text, search_request, term
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -667,25 +668,11 @@ def test_bm25_scores_against_a_numpy_restatement_at_corpus_scale():
     mapping = {"field_mappings": [{"name": "body", "type": "text", "record": "freq", "fieldnorms": True}]}
     img = S.build_split(docs, mapping, "bm25-scale")
     dm = json.dumps(mapping)
-    L = ffi.img_lib()
-    L.qwgpu_fieldnorm_to_id.restype = C.c_uint8
-    L.qwgpu_fieldnorm_to_id.argtypes = [C.c_uint32]
-    L.qwgpu_id_to_fieldnorm.restype = C.c_uint32
-    L.qwgpu_id_to_fieldnorm.argtypes = [C.c_uint8]
-    f32 = np.float32
-    lens = np.array([len(d["body"].split()) for d in docs], dtype=np.int64)
-    quant = np.array([L.qwgpu_id_to_fieldnorm(L.qwgpu_fieldnorm_to_id(int(x))) for x in lens], dtype=np.float32)
-    avg = f32(lens.sum()) / f32(len(docs))
-    k1, b = f32(1.2), f32(0.75)
-    norm = k1 * (f32(1) - b + b * quant / avg)
+    norm = bm25_norm(np.array([len(d["body"].split()) for d in docs], dtype=np.int64))
 
     def contributions(word):
         tf = np.array([d["body"].split().count(word) for d in docs], dtype=np.float32)
-        n = int((tf > 0).sum())
-        idf = np.log(f32(1) + (f32(len(docs) - n) + f32(0.5)) / (f32(n) + f32(0.5)), dtype=np.float32)
-        weight = idf * (f32(1) + k1)
-        with np.errstate(invalid="ignore"):
-            return np.where(tf > 0, weight * (tf / (tf + norm)), f32(0)).astype(np.float32)
+        return bm25_contributions(tf, norm, bm25_weight(int((tf > 0).sum()), len(docs)))
 
     def check(ast, expected):
         r = O.split_search(img, service.compile_plan(img, search_request(ast, max_hits=len(docs), sort_fields=[("_score", DESC)]), dm))

@@ -116,7 +116,9 @@ def test_many_contributions_per_doc(gpu_ctx, clustered):
     fold = ["m3", "m0", "rare", "m4", "m1", "m2", "burst"]          # 5 contributions on every 97th doc
     for k in (10, 2000):
         got, _ = run_both(gpu_ctx, img, P.make_plan(P.bool_([B(img, t, boost=1.0 + 0.37 * i) for i, t in enumerate(fold)]), k, SCORE_DESC), ctx=f"fold k={k}")
-        assert got.exact_fallbacks == 0
+        # 120 000 docs are too few windows to sample: the exact radix descent runs from the start (the sampled
+        # threshold on these shapes is covered by test_gpu_topk_threshold.py)
+        assert got.sample_stride == 0 and got.exact_fallbacks == 0 and got.radix_passes >= 1
     dense = ["c0", "ends", "c1", "c2"]                               # 3 contributions on 36 000 consecutive docs
     run_both(gpu_ctx, img, P.make_plan(P.bool_([B(img, t, boost=1.0 + 0.21 * i) for i, t in enumerate(dense)]), 100, SCORE_DESC), ctx="dense")
     mixed = ["c0", "m0", "c1", "m1", "s3", "m2"]                     # two planes + list + sparse clauses
