@@ -137,6 +137,9 @@ typedef struct qwgpu_split_result {
 #define QWGPU_KERNEL_AGGSCAN 4u /* k_aggscan: match_all + flat aggregations */
 #define QWGPU_KERNEL_WINDOW 8u  /* k_window: the generic window kernel */
 #define QWGPU_KERNEL_PHRASE 16u /* k_phrase: the phrase pre-pass */
+#define QWGPU_KERNEL_TRACE_SELECT 32u /* k_trace_select: find_trace_ids top N over the per-trace maxima */
+#define QWGPU_KERNEL_TRACE_REPLAY 64u /* k_trace_replay: the reference's sentinel replay on a split whose N-th and
+                                         (N+1)-th trace timestamps tie */
 
 /* Runs `num_splits` plans (plan i against split_ids[i]) in ONE batched launch sequence.
  * results[i] is filled for every split; status[i] is 0 or a QWGPU_E* code for that split. */

@@ -136,7 +136,10 @@ enum {
   QW_COL_F64 = 2,
   QW_COL_BOOL = 3,
   QW_COL_DATETIME = 4, /* i64 nanoseconds, truncated to fast_precision at build time */
-  QW_COL_STR = 5       /* term ordinals into a sorted dictionary */
+  QW_COL_STR = 5,      /* term ordinals into a sorted dictionary */
+  QW_COL_BYTES = 6     /* `type: bytes` fast field: ordinals into a sorted dictionary of raw byte strings, stored like
+                          QW_COL_STR (dict_off / dict_num_terms). Only the find_trace_ids collector reads it; queries,
+                          sorts and aggregations on it are refused. */
 };
 enum { QW_CARD_FULL = 0, QW_CARD_OPTIONAL = 1, QW_CARD_MULTI = 2 };
 
@@ -228,7 +231,14 @@ enum {
   QW_AGG_TERMS = 1,
   QW_AGG_HISTOGRAM = 2,      /* also date_histogram (interval/offset pre-scaled to column units) */
   QW_AGG_RANGE = 3,
-  QW_AGG_STATS = 4           /* stats / avg / sum / min / max / value_count share one collector */
+  QW_AGG_STATS = 4,          /* stats / avg / sum / min / max / value_count share one collector */
+  QW_AGG_TRACE_IDS = 5       /* FindTraceIdsCollector (quickwit-search/src/find_trace_ids_collector.rs): the only node
+                                of its plan. `column` = the trace-id QW_COL_BYTES column, `reserved` = the span timestamp
+                                column (0xFFFFFFFF when absent from the split: every timestamp reads 0),
+                                `num_buckets` = num_traces (N). Its N cells hold the split's result in no particular
+                                order: cell j is a span when `count` == 1, with `sum_bits` = the trace id's
+                                ordinal in the column dictionary and `max_mapped` = the span timestamp in the
+                                order-preserving i64 mapping. */
 };
 
 #define QW_MAX_AGG_RANGES 16

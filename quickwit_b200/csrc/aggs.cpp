@@ -16,6 +16,7 @@
 #include <memory>
 
 #include "compile.h"
+#include "device_types.h"
 
 namespace qw {
 
@@ -126,9 +127,28 @@ static void parse_agg_map(const Json& j, std::vector<AggReq>& out, int depth) {
   }
 }
 
+// QuickwitAggregations is a serde untagged enum (collector.rs:600-640): the FindTraceIdsCollector shape is tried
+// first — an object with `num_traces` (usize), `trace_id_field_name` and `span_timestamp_field_name` (strings),
+// other keys ignored — and anything else is read as a tantivy aggregation map
+static bool parse_trace_ids(const Json& j, AggReq& a) {
+  const Json *n = j.get("num_traces"), *t = j.get("trace_id_field_name"), *s = j.get("span_timestamp_field_name");
+  if (!n || !t || !s || !t->is_str() || !s->is_str()) return false;
+  if (n->type == Json::U64) a.num_traces = n->u;
+  else if (n->type == Json::I64 && n->i >= 0) a.num_traces = (uint64_t)n->i;
+  else return false;
+  a.kind = AggReq::TraceIds;
+  a.field = t->s;
+  a.ts_field = s->s;
+  a.size = (uint32_t)std::min<uint64_t>(a.num_traces, 0xFFFFFFFFu);
+  return true;
+}
+
 std::vector<AggReq> parse_agg_request(const std::string& json) {
   std::vector<AggReq> out;
-  parse_agg_map(parse_json(json, QWGPU_EINVALID_AGG), out, 0);
+  const Json j = parse_json(json, QWGPU_EINVALID_AGG);
+  AggReq tr;
+  if (parse_trace_ids(j, tr)) { out.push_back(std::move(tr)); return out; }
+  parse_agg_map(j, out, 0);
   return out;
 }
 
@@ -162,6 +182,17 @@ static QwAggNode lower_one(const AggReq& a, const ImageView& img, AggBinding& b)
   b.column = c;
   const QwImgColumn* col = c >= 0 ? &img.columns[c] : nullptr;
   if (col) { n.column = (uint32_t)c; b.col_type = col->type; }
+  if (a.kind == AggReq::TraceIds) {
+    // the engine fails the split when the trace-id column is absent or not a bytes column (for_segment's error)
+    // and when the timestamp column exists but is not a date column; an absent timestamp column reads 0
+    if (a.num_traces > QW_MAX_TOPK) fail(QWGPU_EUNSUPPORTED, "find_trace_ids with num_traces = %llu exceeds the GPU limit %d", (unsigned long long)a.num_traces, QW_MAX_TOPK);
+    n.kind = QW_AGG_TRACE_IDS;
+    n.num_buckets = (uint32_t)a.num_traces;
+    const int tc = img.find_column(a.ts_field);
+    n.reserved = tc >= 0 ? (uint32_t)tc : 0xFFFFFFFFu;
+    return n;
+  }
+  if (col && col->type == QW_COL_BYTES) fail(QWGPU_EUNSUPPORTED, "aggregations on bytes field `%s` are not supported on the GPU path", a.field.c_str());
   switch (a.kind) {
     case AggReq::Terms: {
       n.kind = QW_AGG_TERMS;
@@ -487,8 +518,106 @@ static IAgg build_node(const BuildCtx& c, uint32_t ni, uint64_t parent_cell) {
   return a;
 }
 
+// ---- find_trace_ids: spans, postcard bytes, merge_segment_fruits -----------------------------------------------
+bool span_less(const TraceSpan& a, const TraceSpan& b) {
+  if (a.ts != b.ts) return a.ts > b.ts;
+  return memcmp(a.id, b.id, 16) < 0;
+}
+
+static void put_varint(std::string& o, uint64_t v) {
+  while (v >= 0x80) { o.push_back((char)(uint8_t)(v | 0x80)); v >>= 7; }
+  o.push_back((char)(uint8_t)v);
+}
+static uint64_t get_varint(const std::string& s, size_t& p) {
+  uint64_t v = 0;
+  for (int sh = 0; sh < 70; sh += 7) {
+    if (p >= s.size()) fail(QWGPU_EINTERNAL, "failed to merge intermediate aggregation results: Postcard error: truncated varint");
+    const uint8_t b = (uint8_t)s[p++];
+    if (sh == 63 && b > 1) fail(QWGPU_EINTERNAL, "failed to merge intermediate aggregation results: Postcard error: varint overflow");
+    v |= (uint64_t)(b & 0x7F) << sh;
+    if (!(b & 0x80)) return v;
+  }
+  fail(QWGPU_EINTERNAL, "failed to merge intermediate aggregation results: Postcard error: varint too long");
+}
+
+std::string encode_spans(const std::vector<TraceSpan>& v) {
+  std::string o;
+  o.reserve(5 + v.size() * 26);
+  put_varint(o, v.size());
+  for (const TraceSpan& sp : v) {
+    o.append((const char*)sp.id, 16);
+    put_varint(o, ((uint64_t)sp.ts << 1) ^ (uint64_t)(sp.ts >> 63));  // zigzag
+  }
+  return o;
+}
+
+std::vector<TraceSpan> decode_spans(const std::string& s) {
+  size_t p = 0;
+  const uint64_t n = get_varint(s, p);
+  if (n > s.size()) fail(QWGPU_EINTERNAL, "failed to merge intermediate aggregation results: Postcard error: bad length");
+  std::vector<TraceSpan> v((size_t)n);
+  for (TraceSpan& sp : v) {
+    if (s.size() - p < 16) fail(QWGPU_EINTERNAL, "failed to merge intermediate aggregation results: Postcard error: truncated span");
+    memcpy(sp.id, s.data() + p, 16);
+    p += 16;
+    const uint64_t z = get_varint(s, p);
+    sp.ts = (int64_t)((z >> 1) ^ (~(z & 1) + 1));
+  }
+  if (p != s.size()) fail(QWGPU_EINTERNAL, "failed to merge intermediate aggregation results: Postcard error: trailing bytes");
+  return v;
+}
+
+std::vector<TraceSpan> merge_span_fruits(std::vector<std::vector<TraceSpan>> fruits, uint64_t num_traces) {
+  for (auto& f : fruits) std::sort(f.begin(), f.end(), span_less);
+  // k-merge: equal spans (same timestamp and id) are interchangeable, so a stable heap order is not needed
+  struct Head { size_t f, i; };
+  auto worse = [&](const Head& a, const Head& b) { return span_less(fruits[b.f][b.i], fruits[a.f][a.i]); };
+  std::vector<Head> heap;
+  for (size_t f = 0; f < fruits.size(); f++) if (!fruits[f].empty()) heap.push_back({f, 0});
+  std::make_heap(heap.begin(), heap.end(), worse);
+  std::vector<TraceSpan> out;
+  std::vector<std::string> seen;
+  while (!heap.empty() && out.size() < num_traces) {
+    std::pop_heap(heap.begin(), heap.end(), worse);
+    Head h = heap.back();
+    const TraceSpan& sp = fruits[h.f][h.i];
+    std::string id((const char*)sp.id, 16);
+    auto it = std::lower_bound(seen.begin(), seen.end(), id);
+    if (it == seen.end() || *it != id) { seen.insert(it, id); out.push_back(sp); }
+    if (++h.i < fruits[h.f].size()) { heap.back() = h; std::push_heap(heap.begin(), heap.end(), worse); }
+    else heap.pop_back();
+  }
+  return out;
+}
+
+// the split's spans from the N cells of its QW_AGG_TRACE_IDS node (QwAggNode doc), sorted
+static std::vector<TraceSpan> trace_spans_of(const CompiledPlan& cp, const ImageView& img, const QwAggCell* cells, size_t ncells) {
+  const QwAggNode* nodes = (const QwAggNode*)(cp.bytes.data() + sizeof(QwPlanHeader) + (size_t)cp.header.num_nodes * sizeof(QwPlanNode));
+  const QwAggNode& n = nodes[0];
+  if (ncells != n.num_buckets) fail(QWGPU_EINTERNAL, "aggregation cell count mismatch (%u vs %zu)", n.num_buckets, ncells);
+  std::vector<TraceSpan> v;
+  for (size_t j = 0; j < ncells; j++) {
+    if (cells[j].count != 1) continue;
+    if (n.column >= img.hdr->num_columns) fail(QWGPU_EINTERNAL, "find_trace_ids: trace id column missing");
+    const QwImgColumn& col = img.columns[n.column];
+    if (cells[j].sum_bits >= col.dict_num_terms) fail(QWGPU_EINTERNAL, "find_trace_ids: trace id ordinal out of range");
+    const uint8_t* p;
+    uint32_t len;
+    img.dict_term(col, (uint32_t)cells[j].sum_bits, &p, &len);
+    if (len != 16) fail(QWGPU_EINTERNAL, "find_trace_ids: trace id of %u bytes (16 expected)", len);
+    TraceSpan sp;
+    memcpy(sp.id, p, 16);
+    sp.ts = u64_to_i64(cells[j].max_mapped);
+    v.push_back(sp);
+  }
+  std::sort(v.begin(), v.end(), span_less);
+  return v;
+}
+
 static std::vector<IAgg> build_top(const CompiledPlan& cp, const ImageView& img, const QwAggCell* cells, size_t ncells);
 std::string build_intermediate_aggs(const CompiledPlan& cp, const ImageView& img, const QwAggCell* cells, size_t ncells) {
+  // (a single split's spans go out sorted: the reference leaves them in select_nth_unstable order)
+  if (is_trace_ids_request(cp.agg_request)) return encode_spans(trace_spans_of(cp, img, cells, ncells));
   return ser_top(build_top(cp, img, cells, ncells));
 }
 static std::vector<IAgg> build_top(const CompiledPlan& cp, const ImageView& img, const QwAggCell* cells, size_t ncells) {
@@ -552,6 +681,11 @@ static void merge_into(const AggReq& req, IAgg& acc, IAgg&& other) {
 // merge_intermediate_aggs(build_intermediate_aggs(split) ...) yields, without serialising every split's
 // result only to parse it again.
 std::string build_and_merge_intermediate_aggs(const std::vector<AggReq>& reqs, const std::vector<SplitAggCells>& splits) {
+  if (is_trace_ids_request(reqs)) {
+    std::vector<std::vector<TraceSpan>> fruits;
+    for (const SplitAggCells& sp : splits) fruits.push_back(trace_spans_of(*sp.plan, *sp.img, sp.cells, sp.ncells));
+    return encode_spans(merge_span_fruits(std::move(fruits), reqs[0].num_traces));
+  }
   std::vector<IAgg> acc;
   for (const SplitAggCells& sp : splits) {
     std::vector<IAgg> top = build_top(*sp.plan, *sp.img, sp.cells, sp.ncells);
@@ -567,6 +701,13 @@ std::string build_and_merge_intermediate_aggs(const std::vector<AggReq>& reqs, c
 }
 
 std::string merge_intermediate_aggs(const std::vector<AggReq>& reqs, const std::vector<std::string>& parts) {
+  if (is_trace_ids_request(reqs)) {
+    // merge_intermediate_aggregation_result / IncrementalCollector (collector.rs:640-704,871-886); staged merges of
+    // the incremental collector give the same spans, so every part is merged at once
+    std::vector<std::vector<TraceSpan>> fruits;
+    for (auto& p : parts) fruits.push_back(decode_spans(p));
+    return encode_spans(merge_span_fruits(std::move(fruits), reqs[0].num_traces));
+  }
   std::vector<IAgg> acc;
   static const bool trace = getenv("QWGPU_TRACE_AGG") != nullptr;
   if (!trace) {
@@ -768,6 +909,20 @@ static void fin_aggs(const std::vector<AggReq>& reqs, const std::vector<IAgg>* a
 }
 
 std::string finalize_aggs_json(const std::vector<AggReq>& reqs, const std::string& intermediate) {
+  if (is_trace_ids_request(reqs)) {
+    // the root passes the merged bytes through (root.rs:1111-1113); this is their human-readable serde form:
+    // [{"trace_id": <32 hex digits>, "span_timestamp": <i64 ns>}, ...]
+    static const char* hex = "0123456789abcdef";
+    std::string out = "[";
+    const std::vector<TraceSpan> v = intermediate.empty() ? std::vector<TraceSpan>() : decode_spans(intermediate);
+    for (size_t i = 0; i < v.size(); i++) {
+      if (i) out += ",";
+      out += "{\"trace_id\":\"";
+      for (int k = 0; k < 16; k++) { out += hex[v[i].id[k] >> 4]; out += hex[v[i].id[k] & 15]; }
+      out += "\",\"span_timestamp\":" + std::to_string(v[i].ts) + "}";
+    }
+    return out + "]";
+  }
   std::vector<IAgg> top;
   if (!intermediate.empty()) top = de_top(intermediate);
   if (!top.empty() && top.size() != reqs.size()) fail(QWGPU_EINTERNAL, "intermediate aggregation result does not match the request");

@@ -25,7 +25,11 @@ bool parse_datetime_str(const std::string& s, int64_t* nanos);
 // ---- aggregation request (tantivy::aggregation::agg_req::Aggregations, Elasticsearch-shaped JSON;
 // semantics per docs/reference/aggregation.md) --------------------------------------------------------
 struct AggReq {
-  enum Kind { Terms, Histogram, DateHistogram, Range, Stats, Avg, Sum, Min, Max, Count } kind = Terms;
+  // TraceIds: quickwit's FindTraceIdsCollector (find_trace_ids_collector.rs), which takes the place of the whole
+  // aggregation request (`size` = num_traces, `field` = trace_id_field_name, `ts_field` = span_timestamp_field_name)
+  enum Kind { Terms, Histogram, DateHistogram, Range, Stats, Avg, Sum, Min, Max, Count, TraceIds } kind = Terms;
+  std::string ts_field;
+  uint64_t num_traces = 0;
   std::string name, field;
   // terms
   uint32_t size = 10, segment_size = 100;
@@ -42,9 +46,22 @@ struct AggReq {
   struct R { bool has_from = false, has_to = false; double from = 0, to = 0; std::string key; };
   std::vector<R> ranges;
   std::vector<AggReq> children;
-  bool is_metric() const { return kind >= Stats; }
+  bool is_metric() const { return kind >= Stats && kind <= Count; }
 };
 std::vector<AggReq> parse_agg_request(const std::string& json);
+inline bool is_trace_ids_request(const std::vector<AggReq>& r) { return r.size() == 1 && r[0].kind == AggReq::TraceIds; }
+
+// find_trace_ids results: Vec<Span> in postcard (varint length; per span the 16 trace-id bytes and the zigzag varint
+// of the i64 timestamp in ns), the bytes the reference puts into intermediate_aggregation_result
+struct TraceSpan {
+  uint8_t id[16];
+  int64_t ts;
+};
+bool span_less(const TraceSpan& a, const TraceSpan& b);  // Span::cmp: timestamp desc, then trace id bytes asc
+std::string encode_spans(const std::vector<TraceSpan>& v);
+std::vector<TraceSpan> decode_spans(const std::string& bytes);
+// merge_segment_fruits: sort each fruit, k-merge, keep the first span of every trace id, stop at num_traces
+std::vector<TraceSpan> merge_span_fruits(std::vector<std::vector<TraceSpan>> fruits, uint64_t num_traces);
 
 // How one QwAggNode of a split maps dense bucket indices back to keys
 struct AggBinding {

@@ -142,6 +142,15 @@ struct DSplitPlan {
   uint64_t out_cells;      // device address of QwAggCell[n_cells]
   uint64_t out_hits;       // device address of QwHit[max_hits]
   uint64_t out_nhits;      // device address of uint32 (hits written by k_select)
+  // find_trace_ids (trace_kernel.cuh); tr_on == 0 when the plan has no QW_AGG_TRACE_IDS node
+  uint64_t tr_best;        // device address of uint64[tr_num_ords]: latest span per trace ordinal (0 = none)
+  uint64_t tr_match;       // device address of uint32[ceil(num_docs / 32)]: the matched docs (read by the replay)
+  uint64_t tr_state;       // device address of a DTraceState
+  uint64_t tr_tie;         // device address of a uint32 in the split's output header: 1 = the replay ran
+  uint32_t tr_on, tr_n;    // N = num_traces
+  uint32_t tr_num_ords;    // entries of tr_best (the column dictionary's size, at least 1)
+  uint32_t tr_ord_col, tr_ts_col;  // DCol indices of the trace-id and timestamp columns (ts: 0xFFFFFFFF = absent)
+  uint32_t tr_pad[3];
 };
 
 static_assert(offsetof(DSplitPlan, key) % 16 == 0 && sizeof(DSplitPlan) % 16 == 0, "DKeySpec is read as uint4");

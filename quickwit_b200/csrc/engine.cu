@@ -14,6 +14,7 @@
 #include "phrase_kernel.cuh"
 #include "driver_kernel.cuh"
 #include "agg_kernel.cuh"
+#include "trace_kernel.cuh"
 
 namespace qw {
 
@@ -80,6 +81,9 @@ struct CallSlot {
   }
 };
 
+// k_trace_replay: the <= 2N-entry map (ordinal + timestamp) and one tile of matched docs in shared memory
+static int trace_replay_smem(uint32_t n) { return (int)(12u * (2u * n + QT_TILE)); }
+
 Engine::Engine(int dev) : device(dev) {
   int n = 0;
   cudaError_t e = cudaGetDeviceCount(&n);
@@ -100,6 +104,7 @@ Engine::Engine(int dev) : device(dev) {
   CUDA_CHECK(cudaFuncSetAttribute(qwk::k_union<qwk::MODE_COLLECT>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem_optin));
   CUDA_CHECK(cudaFuncSetAttribute(qwk::k_aggscan, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem_optin));
   CUDA_CHECK(cudaFuncSetAttribute(qwk::k_select, cudaFuncAttributeMaxDynamicSharedMemorySize, 3 * 8 * QW_CAND_CAP));
+  CUDA_CHECK(cudaFuncSetAttribute(qwk::k_trace_replay, cudaFuncAttributeMaxDynamicSharedMemorySize, trace_replay_smem(QW_MAX_TOPK)));
 }
 
 Engine::~Engine() {
@@ -127,6 +132,16 @@ static std::shared_ptr<SplitDev> open_split(const char* id, const uint8_t* img, 
   sp->view.strings = sp->dir.data() + full.hdr->strings_off;
   sp->view.data = nullptr;
   sp->data_len = full.hdr->data_len;
+  // bytes columns whose every dictionary entry is a 16-byte trace id (find_trace_ids fails the split otherwise)
+  sp->ids16.assign(full.hdr->num_columns, 0);
+  for (uint32_t c = 0; c < full.hdr->num_columns; c++) {
+    const QwImgColumn& col = sp->view.columns[c];
+    if (col.type != QW_COL_BYTES) continue;
+    const uint32_t* offs = (const uint32_t*)(sp->view.strings + col.dict_off);
+    bool ok = true;
+    for (uint32_t k = 0; k < col.dict_num_terms && ok; k++) ok = offs[k + 1] - offs[k] == 16;
+    sp->ids16[c] = ok ? 1 : 0;
+  }
   *full_out = full;
   return sp;
 }
@@ -330,6 +345,7 @@ struct Lowered {
   bool empty = false;                   // a required clause of the root cannot match in this split: no work at all
   std::vector<DPhrase> phrases;         // phrase pre-pass descriptors (out / first_work filled per batch)
   std::vector<uint32_t> phrase_instr;   // instruction that consumes phrases[i]
+  uint32_t tr_img_col = 0;              // find_trace_ids: the trace-id column of the image
 };
 
 static uint32_t use_col(Lowered& L, const SplitDev& sp, uint32_t c) {
@@ -663,6 +679,25 @@ static void lower_plan(Lowered& L, const SplitDev& sp, const uint8_t* plan, size
     L.aggs.push_back(d);
   }
   P.n_aggs = ph->num_aggs;
+  for (uint32_t i = 0; i < ph->num_aggs; i++) {
+    const QwAggNode& a = aggs[i];
+    if (a.kind != QW_AGG_TRACE_IDS) continue;
+    // FindTraceIdsCollector::for_segment: a missing trace-id bytes column or a timestamp field that is not a date
+    // column is an error of the split; an absent timestamp column reads 0 ns for every doc
+    if (ph->num_aggs != 1 || ph->max_hits) fail(QWGPU_EINVALID_ARG, "a find_trace_ids node must be the only aggregation of a plan without hits");
+    if (a.num_buckets > QW_MAX_TOPK) fail(QWGPU_EUNSUPPORTED, "find_trace_ids with num_traces = %u exceeds the GPU limit %d", a.num_buckets, QW_MAX_TOPK);
+    if (a.column >= sp.view.hdr->num_columns || sp.view.columns[a.column].type != QW_COL_BYTES)
+      fail(QWGPU_EINTERNAL, "failed to find column for trace_id field");
+    if (!sp.ids16[a.column]) fail(QWGPU_EINTERNAL, "the term dictionary of the trace_id field holds a value that is not a 16-byte trace id");
+    if (a.reserved != 0xFFFFFFFFu && (a.reserved >= sp.view.hdr->num_columns || sp.view.columns[a.reserved].type != QW_COL_DATETIME))
+      fail(QWGPU_EINTERNAL, "the span timestamp field is not a date fast field");
+    P.tr_on = 1;
+    L.tr_img_col = a.column;
+    P.tr_n = a.num_buckets;
+    P.tr_num_ords = std::max(sp.view.columns[a.column].dict_num_terms, 1u);
+    P.tr_ord_col = L.aggs[i].col;
+    P.tr_ts_col = use_col(L, sp, a.reserved);
+  }
   P.n_cols = (uint32_t)L.cols.size();
   // fast aggregation path: flat (no nesting) TERMS / HISTOGRAM nodes over always-present single-valued
   // columns. Histogram buckets are located through a raw-space boundary table built here with the
@@ -1059,7 +1094,17 @@ void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std:
          s_cut = al(s_hits + (do_merge ? (size_t)n * kmax * sizeof(QwHit) : 0)),
          s_grecv = al(s_cut + (size_t)std::max<uint32_t>(n, 64) * 4 + 1024),
          s_vblk = al(s_grecv + (gather && gather->world > 1 && do_merge ? (size_t)gather->world * (64 + (size_t)merge->k * sizeof(qwk::DMergedHit)) : 0)),
-         scratch_bytes = al(s_vblk + (size_t)phrase_blocks * sizeof(VBlk));
+         s_trace = al(s_vblk + (size_t)phrase_blocks * sizeof(VBlk));
+  // find_trace_ids: per split a DTraceState (one region, set to 0xFF bytes), then best[] + match bitmap (zeroed)
+  std::vector<size_t> tr_off(n + 1, 0);
+  bool any_trace = false;
+  for (uint32_t i = 0; i < n; i++) {
+    const DSplitPlan& P = low[i].P;
+    tr_off[i + 1] = tr_off[i] + (P.tr_on ? al((size_t)P.tr_num_ords * 8) + al((size_t)((P.num_docs + 31) / 32) * 4) : 0);
+    any_trace |= P.tr_on != 0;
+  }
+  const size_t s_trace_state = s_trace, s_trace_data = al(s_trace + (any_trace ? (size_t)n * sizeof(qwk::DTraceState) : 0));
+  const size_t scratch_bytes = al(s_trace_data + tr_off[n]);
   // out: per split [hdr 32B][hits][cells]
   std::vector<size_t> out_off(n + 1);
   out_off[0] = 0;
@@ -1151,6 +1196,12 @@ void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std:
     P.out_cells = (uint64_t)(ob + 32 + (do_merge ? 0 : (size_t)P.max_hits * sizeof(QwHit)));
     P.out_hist = (uint64_t)(slot->d_scratch + s_hist + (size_t)i * QW_HIST_BINS * 4);
     P.out_cands = (uint64_t)(slot->d_scratch + s_cand + (size_t)i * QW_CAND_CAP * 24);
+    if (P.tr_on) {
+      P.tr_state = (uint64_t)(slot->d_scratch + s_trace_state + (size_t)i * sizeof(qwk::DTraceState));
+      P.tr_best = (uint64_t)(slot->d_scratch + s_trace_data + tr_off[i]);
+      P.tr_match = P.tr_best + al((size_t)P.tr_num_ords * 8);
+      P.tr_tie = (uint64_t)(ob + 24);
+    }
     for (size_t k = 0; k < low[i].phrases.size(); k++) {
       DPhrase& ph = low[i].phrases[k];
       DInstr& pin = low[i].instrs[low[i].phrase_instr[k]];
@@ -1285,11 +1336,24 @@ void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std:
     stats.kernel_mask |= QWGPU_KERNEL_WINDOW;
   };
   const uint32_t sel_smem = 3 * 8 * QW_CAND_CAP;  // [all first words | 3 x QW_SEL_MAX survivors] or 3 x all (degenerate ties)
+  uint32_t tie_max_n = 0;
+  for (auto& L : low) if (L.P.tr_on) tie_max_n = std::max(tie_max_n, L.P.tr_n);
   auto run_collect = [&](uint32_t flags) {
     if (!(flags & F_CANDS_ONLY)) CUDA_CHECK(cudaMemsetAsync(slot->d_out, 0, out_bytes, st));
+    if (any_trace && !(flags & F_CANDS_ONLY)) {
+      CUDA_CHECK(cudaMemsetAsync(slot->d_scratch + s_trace_state, 0xFF, (size_t)n * sizeof(qwk::DTraceState), st));
+      CUDA_CHECK(cudaMemsetAsync(slot->d_scratch + s_trace_data, 0, tr_off[n], st));
+    }
     CUDA_CHECK(cudaEventRecord(slot->ev2, st));
     launch_window(qwk::MODE_COLLECT, false, 0, 0, flags);
     CUDA_CHECK(cudaEventRecord(slot->ev3, st));
+    if (any_trace && !(flags & F_CANDS_ONLY)) {
+      // top N of the per-trace maxima; splits whose N-th and (N+1)-th maxima tie replay the reference's selection
+      qwk::k_trace_select<<<n, 1024, 0, st>>>(kp.plans);
+      qwk::k_trace_replay<<<n, QT_TILE, trace_replay_smem(tie_max_n), st>>>(kp.plans, kp.cols);
+      stats.launches += 2;
+      stats.kernel_mask |= QWGPU_KERNEL_TRACE_SELECT;
+    }
     if (any_topk) { qwk::k_select<<<n, 1024, sel_smem, st>>>(kp.plans, kp.cols); stats.launches++; }
     if (do_merge) {
       uint32_t* d_cut = (uint32_t*)(slot->d_scratch + s_cut);
@@ -1446,6 +1510,18 @@ void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std:
     const QwAggCell* c = (const QwAggCell*)(ob + 32 + (do_merge ? 0 : (size_t)P.max_hits * sizeof(QwHit)));
     o.cells.assign(c, c + P.n_cells);
     for (auto& cell : o.cells) cell.min_mapped = ~cell.min_mapped;  // device keeps max(~m); see agg_stats
+    if (P.tr_on) {
+      if (*(const uint32_t*)(ob + 24)) stats.kernel_mask |= QWGPU_KERNEL_TRACE_REPLAY;
+      // a matched doc without a trace id reads ordinal 0: with an empty dictionary the reference's ord_to_bytes fails
+      const QwImgColumn& tc = sp[idx[i]]->view.columns[low[i].tr_img_col];
+      for (const QwAggCell& cell : o.cells)
+        if (cell.count == 1 && cell.sum_bits >= tc.dict_num_terms) {
+          o.status = QWGPU_EINTERNAL;
+          o.error = "failed to look up a trace id in the column term dictionary";
+          o.cells.clear();
+          break;
+        }
+    }
     o.postings_scored = low[i].postings;
     // SURVEY.md §8d algorithmic bytes: postings (+ fieldnorms, added at lowering) + column probes
     uint64_t bytes = low[i].alg_bytes;

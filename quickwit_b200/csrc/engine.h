@@ -20,6 +20,7 @@ struct SplitDev {
   uint8_t* d_data = nullptr; // device copy of the data region
   float* d_tabs = nullptr;   // device float[num_fields][256] BM25 norm tables
   uint64_t data_len = 0;
+  std::vector<uint8_t> ids16;  // per column: 1 = a bytes column whose dictionary holds only 16-byte values
   // residency: recency for the LRU, state of an asynchronous upload (0 loading, 1 ready, 2 failed)
   uint64_t last_use = 0;
   int state = 1;

@@ -253,7 +253,7 @@ static void add_column(qwgpu_imgb* b, const char* name, uint32_t type, uint32_t 
     memcpy(c.index.data(), index, 4ull * (nd + 1));
     if (((const uint32_t*)c.index.data())[nd] != num_vals) fail(QWGPU_EINVALID_ARG, "MULTI column: start[num_docs] != num_vals");
   }
-  if (type == QW_COL_STR) {
+  if (type == QW_COL_STR || type == QW_COL_BYTES) {
     uint64_t blen = dict_n ? dict_offs[dict_n] : 0;
     c.dict.resize(4ull * (dict_n + 1) + blen);
     if (dict_n) memcpy(c.dict.data(), dict_offs, 4ull * (dict_n + 1));

@@ -648,11 +648,16 @@ __device__ __forceinline__ uint32_t agg_values(const DAgg& g, const DCol* cols, 
   missing = on && (a == b) && g.kind == QW_AGG_TERMS && g.has_missing;
   return on ? (missing ? 1u : (uint32_t)(b - a)) : 0u;
 }
+__device__ __forceinline__ void trace_collect(const DSplitPlan& P, const DCol* cols, const uint8_t* base, uint32_t doc, bool on, uint32_t lane);  // trace_kernel.cuh
 __device__ void agg_collect_doc(const KParams& p, const Sm& sm, const DSplitPlan& P, const DAgg* aggs, const DCol* cols,
                                 const uint8_t* base, QwAggCell* cells, uint32_t doc, bool on, uint32_t lane) {
   for (uint32_t gi = 0; gi < P.n_aggs; gi++) {
     const DAgg& g = aggs[gi];
     if (g.parent != 0xFFFFFFFFu) continue;
+    if (g.kind == QW_AGG_TRACE_IDS) {
+      trace_collect(P, cols, base, doc, on, lane);
+      continue;
+    }
     if (g.kind == QW_AGG_STATS) {
       if (g.col != 0xFFFFFFFFu) agg_stats(g, cols[g.col], base, cells, 0, doc, on, lane);
       continue;
@@ -1425,6 +1430,11 @@ __global__ void __launch_bounds__(QW_THREADS, QW_MIN_BLOCKS_PER_SM) k_window(con
         if (rec && my_top) atomicMax(&s_misc[4], my_top);
       }
       __syncthreads();
+      if (P.tr_on && !p.cands_only) {
+        // find_trace_ids: the window's matches, for a replay of the reference's sentinel (trace_kernel.cuh)
+        const uint32_t nwd = (P.num_docs + 31) >> 5;
+        for (uint32_t wd = tid; wd < NW && (ws >> 5) + wd < nwd; wd += QW_THREADS) ((uint32_t*)P.tr_match)[(ws >> 5) + wd] = res[wd];
+      }
       if (tid == 0 && !p.cands_only) {
         const uint32_t hits = s_misc[2];
         if (hits) atomicAdd((unsigned long long*)P.out_num_hits, (unsigned long long)hits);

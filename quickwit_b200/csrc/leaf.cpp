@@ -14,6 +14,7 @@
 #include <tuple>
 
 #include "compile.h"
+#include "device_types.h"
 #include "engine.h"
 #include "comm.h"
 
@@ -224,11 +225,23 @@ static void sort_orders(const pb::SearchRequest& r, int* o1, int* o2);
 // reach the top-K, so the response is the same; here all splits of a request run in one batch and that
 // feedback has nothing to act on.
 struct SplitFilter {
-  enum Kind { Uninformative, SplitIdHigher, SplitTimestampHigher, SplitTimestampLower } kind = Uninformative;
+  enum Kind { Uninformative, SplitIdHigher, SplitTimestampHigher, SplitTimestampLower, FindTraceIdsAggregation } kind = Uninformative;
 };
+static bool is_trace_ids_on(const pb::SearchRequest& r, const std::string& timestamp_field) {
+  if (r.max_hits != 0 || !r.aggregation_request || timestamp_field.empty()) return false;
+  try {
+    const std::vector<AggReq> a = parse_agg_request(*r.aggregation_request);
+    return is_trace_ids_request(a) && a[0].ts_field == timestamp_field;
+  } catch (const Error&) {
+    return false;  // (a malformed request fails later, in compile_plan)
+  }
+}
 static SplitFilter split_filter_from_request(const pb::SearchRequest& r, const std::string& timestamp_field) {
   SplitFilter f;
-  if (r.sort_fields.empty()) f.kind = SplitFilter::SplitIdHigher;
+  // find_trace_ids over the index's timestamp field: the splits with the latest spans first (leaf.rs:1082-1090); they
+  // are never skipped (leaf.rs:1420), which the aggregation request already guarantees below
+  if (is_trace_ids_on(r, timestamp_field)) f.kind = SplitFilter::FindTraceIdsAggregation;
+  else if (r.sort_fields.empty()) f.kind = SplitFilter::SplitIdHigher;
   else if (!timestamp_field.empty() && r.sort_fields[0].field_name == timestamp_field)
     f.kind = r.sort_fields[0].sort_order == 0 ? SplitFilter::SplitTimestampLower : SplitFilter::SplitTimestampHigher;
   return f;
@@ -262,7 +275,7 @@ static std::vector<SplitRequest> optimize_split_requests(const pb::SearchRequest
   std::vector<size_t> order(splits.size());
   for (size_t i = 0; i < order.size(); i++) order[i] = i;
   if (f.kind == SplitFilter::SplitIdHigher) std::stable_sort(order.begin(), order.end(), [&](size_t a, size_t b) { return splits[a].split_id > splits[b].split_id; });
-  else if (f.kind == SplitFilter::SplitTimestampHigher) std::stable_sort(order.begin(), order.end(), [&](size_t a, size_t b) { return ts_end(a) > ts_end(b); });
+  else if (f.kind == SplitFilter::SplitTimestampHigher || f.kind == SplitFilter::FindTraceIdsAggregation) std::stable_sort(order.begin(), order.end(), [&](size_t a, size_t b) { return ts_end(a) > ts_end(b); });
   else if (f.kind == SplitFilter::SplitTimestampLower) std::stable_sort(order.begin(), order.end(), [&](size_t a, size_t b) { return ts_start(a) < ts_start(b); });
   std::vector<SplitRequest> out;
   for (size_t i : order) out.push_back({i, false, false, false});
@@ -582,6 +595,7 @@ namespace {
 //   agg bytes (<= kAggCap) — last, so that the used part of a partial is a prefix of it (partial_used_bytes)
 const uint64_t kPartMagic = 0x5452415057515157ull;
 const size_t kHitBytes = 64, kAggCap = 1 << 20, kTailCap = 4096;
+static_assert(kAggCap >= (size_t)QW_MAX_TOPK * 26 + 5, "a partial holds the largest find_trace_ids result (N spans of <= 26 bytes + length)");
 uint64_t partial_bytes_for(const qw::pb::SearchRequest& r) {
   size_t k = (size_t)(r.max_hits + r.start_offset);
   bool aggs = r.aggregation_request && !r.aggregation_request->empty();

@@ -356,6 +356,8 @@ static TQ full_text(const Ctx& cx, const std::string& field, const std::string& 
   int f = cx.img.find_field(field);
   if (f < 0) {
     int c = cx.img.find_column(field);
+    if (c >= 0 && cx.img.columns[c].type == QW_COL_BYTES)
+      fail(QWGPU_EUNSUPPORTED, "queries on bytes field `%s` are not supported on the GPU path", field.c_str());
     if (c >= 0 && cx.img.columns[c].type != QW_COL_STR) {
       // numeric / bool / datetime field: TermQuery on the typed value == column equality
       Json lit; lit.type = Json::Str; lit.s = text;
@@ -423,6 +425,7 @@ static TQ range_query(const Ctx& cx, const std::string& field, const Json* lower
     return tq_none();  // fast field with no value in this split
   }
   const QwImgColumn& col = cx.img.columns[c];
+  if (col.type == QW_COL_BYTES) fail(QWGPU_EUNSUPPORTED, "range queries on bytes field `%s` are not supported on the GPU path", field.c_str());
   if (col.type == QW_COL_BOOL) fail(QWGPU_EINVALID_QUERY, "invalid query: range queries are not supported for field `%s` of type `bool`", field.c_str());
   uint64_t lo = 0, hi = ~0ull;
   const Json* v;
@@ -793,6 +796,7 @@ CompiledPlan compile_plan(const ImageView& img, const std::string& split_id, con
       if (c >= 0) {
         uint32_t t = img.columns[c].type;
         if (t == QW_COL_STR) fail(QWGPU_EINVALID_ARG, "Unsupported sort field type `Str`.");
+        if (t == QW_COL_BYTES) fail(QWGPU_EUNSUPPORTED, "sorting on bytes field `%s` is not supported on the GPU path", sf.field_name.c_str());
         h.sort[i].column = (uint32_t)c;
         sft[i] = t == QW_COL_U64 ? SFT_U64 : t == QW_COL_I64 ? SFT_I64 : t == QW_COL_F64 ? SFT_F64 : t == QW_COL_BOOL ? SFT_BOOL : SFT_DATETIME;
       }
@@ -831,6 +835,9 @@ CompiledPlan compile_plan(const ImageView& img, const std::string& split_id, con
   std::vector<QwAggNode> aggs;
   if (req.aggregation_request && !req.aggregation_request->empty()) {
     cp.agg_request = parse_agg_request(*req.aggregation_request);
+    // Jaeger's trace search sends the find_trace_ids collector with max_hits 0; the GPU path runs it alone
+    if (is_trace_ids_request(cp.agg_request) && h.max_hits > 0)
+      fail(QWGPU_EUNSUPPORTED, "find_trace_ids combined with max_hits > 0 is not implemented on the GPU path");
     aggs = lower_aggs(cp.agg_request, img, cp.agg_bindings);
   }
   h.num_aggs = (uint32_t)aggs.size();

@@ -18,16 +18,17 @@ EINTERNAL, EINVALID_QUERY, EINVALID_AGG, EINVALID_ARG, ENODEVICE, ENOTFOUND, EUN
 # qwgpu_format.h enums
 FIELD_HAS_FREQS, FIELD_HAS_FIELDNORMS, FIELD_HAS_POSITIONS = 1, 2, 4
 TOK_RAW, TOK_DEFAULT = 0, 1
-COL_U64, COL_I64, COL_F64, COL_BOOL, COL_DATETIME, COL_STR = range(6)
+COL_U64, COL_I64, COL_F64, COL_BOOL, COL_DATETIME, COL_STR, COL_BYTES = range(7)
 CARD_FULL, CARD_OPTIONAL, CARD_MULTI = range(3)
 NODE_TERM, NODE_RANGE, NODE_BOOL, NODE_ALL, NODE_NONE, NODE_EXISTS, NODE_PHRASE = 1, 2, 3, 4, 5, 6, 7
 OCCUR_MUST, OCCUR_SHOULD, OCCUR_MUST_NOT, OCCUR_FILTER = range(4)
 SORT_NONE, SORT_DOCID, SORT_SCORE, SORT_COLUMN = range(4)
 ORDER_ASC, ORDER_DESC = 0, 1
-AGG_TERMS, AGG_HISTOGRAM, AGG_RANGE, AGG_STATS = 1, 2, 3, 4
+AGG_TERMS, AGG_HISTOGRAM, AGG_RANGE, AGG_STATS, AGG_TRACE_IDS = 1, 2, 3, 4, 5
 ABSENT = 0xFFFFFFFF
 # qwgpu_split_result.kernel_mask (qwgpu.h)
 KERNEL_UNION, KERNEL_DRIVER, KERNEL_AGGSCAN, KERNEL_WINDOW, KERNEL_PHRASE = 1, 2, 4, 8, 16
+KERNEL_TRACE_SELECT, KERNEL_TRACE_REPLAY = 32, 64
 PLAN_MAGIC = 0x4E4C5051
 MAX_AGG_RANGES = 16
 

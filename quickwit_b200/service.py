@@ -215,6 +215,37 @@ def finalize_aggregation(aggregation_request_json: str, intermediate: bytes) -> 
         L.qwgpu_buf_free(out)
 
 
+def decode_spans(intermediate: bytes) -> List[Tuple[bytes, int]]:
+    """find_trace_ids result bytes (postcard `Vec<Span>`: varint length, then per span the 16 trace-id bytes and
+    the zigzag varint of the i64 timestamp in ns) -> [(trace_id, span_timestamp_ns), ...] in wire order."""
+    pos = 0
+
+    def varint() -> int:
+        nonlocal pos
+        v = sh = 0
+        while True:
+            if pos >= len(intermediate):
+                raise ValueError("truncated varint")
+            b = intermediate[pos]
+            pos += 1
+            v |= (b & 0x7F) << sh
+            if not b & 0x80:
+                return v
+            sh += 7
+
+    spans = []
+    for _ in range(varint()):
+        if len(intermediate) - pos < 16:
+            raise ValueError("truncated span")
+        tid = bytes(intermediate[pos:pos + 16])
+        pos += 16
+        z = varint()
+        spans.append((tid, (z >> 1) ^ -(z & 1)))
+    if pos != len(intermediate):
+        raise ValueError("trailing bytes")
+    return spans
+
+
 def build_leaf_response(img: SplitImage, search_request_pb: bytes, doc_mapper_json: str, num_hits: int,
                         hits: Sequence[Tuple[int, int, int, int, float]], cells: Sequence[Tuple[int, int, int, int]],
                         split_id: str = "") -> bytes:

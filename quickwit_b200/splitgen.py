@@ -7,13 +7,16 @@ C++ writer behind `qwgpu_imgb_*`; this module only tokenizes and groups.
 
 Doc-mapping dialect: the subset of Quickwit's doc mapper JSON this path needs
 (quickwit-doc-mapper/src/doc_mapper/field_mapping_entry.rs): `field_mappings[]` entries with
-`name`, `type` (text|u64|i64|f64|bool|datetime), `tokenizer` (default|raw), `record`
+`name`, `type` (text|u64|i64|f64|bool|datetime|bytes), `tokenizer` (default|raw), `record`
 (basic|freq|position; default basic, :447), `fieldnorms` (default false, :326), `fast`,
-`fast_precision` (seconds|milliseconds|microseconds|nanoseconds), plus `timestamp_field` and
-`mode: dynamic` (unknown JSON keys become fast raw-text / numeric columns and raw-indexed text).
+`fast_precision` (seconds|milliseconds|microseconds|nanoseconds), `input_format` (bytes: base64|hex,
+default base64), plus `timestamp_field` and `mode: dynamic` (unknown JSON keys become fast raw-text /
+numeric columns and raw-indexed text). A fast bytes field becomes a QW_COL_BYTES column: ordinals into
+the sorted dictionary of its raw values.
 """
 from __future__ import annotations
 
+import base64
 import ctypes as C
 import datetime as _dt
 import struct
@@ -153,6 +156,17 @@ def parse_datetime_nanos(v: Any) -> int:
 
 
 # ---- tokenizers ----------------------------------------------------------------------------------
+
+def decode_bytes_value(v: Any, input_format: str = "base64") -> bytes:
+    """A `type: bytes` field value as the doc mapper reads it: a base64 (default) or hex string; bytes pass as is."""
+    if isinstance(v, (bytes, bytearray)):
+        return bytes(v)
+    if input_format == "hex":
+        return bytes.fromhex(str(v))
+    if input_format == "base64":
+        return base64.b64decode(str(v), validate=True)
+    raise ValueError(f"unknown bytes input_format `{input_format}`")
+
 
 def tokenize_default(text: str) -> List[str]:
     """tantivy "default" tokenizer (SimpleTokenizer + RemoveLong(255) + LowerCaser), restricted to
@@ -347,6 +361,12 @@ def build_split(docs: Sequence[Dict[str, Any]], doc_mapping: Dict[str, Any], spl
                 ords = {t: i for i, t in enumerate(dictionary)}
                 per_doc = [[ords[str(v).encode()] for v in vs] for vs in values]
                 _column_from_values(b, name, ffi.COL_STR, per_doc, dictionary)
+        elif ftype == "bytes":
+            if m.get("fast", False):
+                raw = [[decode_bytes_value(v, m.get("input_format", "base64")) for v in vs] for vs in values]
+                dictionary = sorted({v for vs in raw for v in vs})
+                ords = {t: i for i, t in enumerate(dictionary)}
+                _column_from_values(b, name, ffi.COL_BYTES, [[ords[v] for v in vs] for vs in raw], dictionary)
         else:
             prec = _PRECISION_NS[m.get("fast_precision", "seconds")] if ftype == "datetime" else 1
             if m.get("fast", False) or m.get("_dynamic"):
