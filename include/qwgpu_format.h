@@ -171,6 +171,7 @@ typedef struct QwImgColumn {
 #define QW_PLAN_MAGIC 0x4E4C5051u /* "QPLN" */
 #define QW_MAX_PLAN_DEPTH 4
 #define QW_MAX_PHRASE_TERMS 8
+#define QW_MAX_PREFIX_EXPANSIONS 1024 /* expansion children of one PHRASE_PREFIX node */
 
 enum {
   QW_NODE_TERM = 1,   /* tantivy TermQuery */
@@ -179,12 +180,21 @@ enum {
   QW_NODE_ALL = 4,    /* AllQuery; score 1 */
   QW_NODE_NONE = 5,   /* EmptyQuery */
   QW_NODE_EXISTS = 6, /* ExistsQuery on a column; const score 1 */
-  QW_NODE_PHRASE = 7  /* tantivy PhraseQuery, slop 0: children = its TERM nodes in phrase order, all of one field
+  QW_NODE_PHRASE = 7, /* tantivy PhraseQuery, slop 0: children = its TERM nodes in phrase order, all of one field
                          with positions; child k's `lo` = position offset of the term inside the phrase. A doc
                          matches when some base position b has term k at b + lo_k for every k; phrase_count =
                          number of such b. Score = bm25_weight * tf-factor(phrase_count, fieldnorm) with
                          bm25_weight = (sum of the terms' idf, duplicates included) * (1 + K1) * boost
                          (Bm25Weight::for_terms). */
+  QW_NODE_PHRASE_PREFIX = 8 /* tantivy PhrasePrefixQuery with at least one exact term: children = the k exact TERM
+                               nodes in phrase order, then the E expansion TERM nodes of the last slot (the field's
+                               first max_expansions terms, in byte order, that start with the prefix); the node's
+                               `lo` = k; each child's `lo` = its position offset, so every expansion carries the last
+                               offset. All of one field with positions; 1 <= k < QW_MAX_PHRASE_TERMS,
+                               1 <= E <= QW_MAX_PREFIX_EXPANSIONS. A doc matches when some base position b has exact
+                               term i at b + lo_i for every i and some expansion at b + lo_last. Never scored: the
+                               node is only valid where its score is not read (filter / must_not, or any sort
+                               other than _score). */
 };
 enum { QW_OCCUR_MUST = 0, QW_OCCUR_SHOULD = 1, QW_OCCUR_MUST_NOT = 2, QW_OCCUR_FILTER = 3 };
 

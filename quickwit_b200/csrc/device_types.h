@@ -58,8 +58,10 @@ struct DPhrase {
   uint64_t tab;        // the field's BM25 tables (device address): float[256] norms, then tff[16][256]
   float weight;        // (sum of the terms' idf) * (1 + K1) * boost
   uint32_t n_terms, driver, scored;
-  uint32_t first_work, pad[3];  // prefix of driver blocks over the batch's phrases
-  DPhraseTerm t[QW_MAX_PHRASE_TERMS];
+  uint32_t first_work;  // prefix of driver blocks over the batch's phrases
+  uint32_t n_exp;       // phrase prefix: number of expansions of the last slot (0 = a plain phrase)
+  uint64_t exp;         // phrase prefix: DPhraseTerm[n_exp] (device address; while lowering, index into Lowered)
+  DPhraseTerm t[QW_MAX_PHRASE_TERMS];  // phrase prefix: the n_terms exact terms
 };
 
 struct DCol {  // 48 bytes

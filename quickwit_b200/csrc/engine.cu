@@ -345,6 +345,7 @@ struct Lowered {
   bool empty = false;                   // a required clause of the root cannot match in this split: no work at all
   std::vector<DPhrase> phrases;         // phrase pre-pass descriptors (out / first_work filled per batch)
   std::vector<uint32_t> phrase_instr;   // instruction that consumes phrases[i]
+  std::vector<DPhraseTerm> phrase_exp;  // expansions of the phrase prefixes (phrases[i].exp indexes it until staging)
   uint32_t tr_img_col = 0;              // find_trace_ids: the trace-id column of the image
 };
 
@@ -524,6 +525,57 @@ static void lower_node(Lowered& L, const SplitDev& sp, const QwPlanNode* nodes, 
       in.n = drv.num_blocks;
       in.f = n.bm25_weight;
       if (scored) L.score_max += n.bm25_weight > 0 ? n.bm25_weight : 0.f;
+      L.phrase_instr.push_back((uint32_t)L.instrs.size());
+      L.phrases.push_back(ph);
+      L.instrs.push_back(in);
+      break;
+    }
+    case QW_NODE_PHRASE_PREFIX: {
+      // the phrase pre-pass over the k exact terms (the rarest drives) plus its suffix stage over the E expansions
+      // (phrase_kernel.cuh 2b); consumed like a phrase (OP_PHRASE), never scored
+      const uint32_t k = (uint32_t)n.lo;
+      if (n.lo < 1 || n.lo >= QW_MAX_PHRASE_TERMS || n.num_children <= k || n.first_child + n.num_children > nn)
+        fail(QWGPU_EINVALID_ARG, "phrase prefix node with %llu exact terms and %u children", (unsigned long long)n.lo, n.num_children);
+      const uint32_t n_exp = n.num_children - k;
+      if (n_exp > QW_MAX_PREFIX_EXPANSIONS)
+        fail(QWGPU_EUNSUPPORTED, "phrase prefix with %u expansions (the GPU path takes at most %d)", n_exp, QW_MAX_PREFIX_EXPANSIONS);
+      if (scored)
+        fail(QWGPU_EUNSUPPORTED, "phrase prefix in a scoring clause of a query ranked by _score is not implemented on the GPU path");
+      DPhrase ph;
+      memset(&ph, 0, sizeof ph);
+      ph.data_base = (uint64_t)sp.d_data;
+      ph.n_terms = k;
+      ph.n_exp = n_exp;
+      ph.exp = L.phrase_exp.size();
+      ph.fn_off = ~0ull;
+      uint64_t best_df = ~0ull;
+      uint32_t field_id = 0;
+      for (uint32_t i = 0; i < n.num_children; i++) {
+        const QwPlanNode& c = nodes[n.first_child + i];
+        if (c.kind != QW_NODE_TERM || c.term_ord >= sp.view.hdr->num_terms) fail(QWGPU_EINVALID_ARG, "phrase prefix child %u is not a term of this split", i);
+        const QwImgTerm& t = sp.view.terms[c.term_ord];
+        if (!t.pidx_off) fail(QWGPU_EINVALID_ARG, "phrase prefix over a field without positions");
+        if (i && t.field_id != field_id) fail(QWGPU_EINVALID_ARG, "phrase prefix terms of different fields");
+        if (i > k && c.lo != nodes[n.first_child + k].lo) fail(QWGPU_EINVALID_ARG, "phrase prefix expansions at different offsets");
+        if (c.lo > 0xFFFFFFFFull) fail(QWGPU_EINVALID_ARG, "phrase prefix offset out of range");
+        field_id = t.field_id;
+        DPhraseTerm pt;
+        pt.data_off = t.data_off; pt.skip_off = t.skip_off; pt.pos_off = t.pos_off; pt.pidx_off = t.pidx_off;
+        pt.nblk = t.num_blocks; pt.offset = (uint32_t)c.lo;
+        if (i < k) {
+          ph.t[i] = pt;
+          if (t.doc_freq < best_df) { best_df = t.doc_freq; ph.driver = i; }
+        } else L.phrase_exp.push_back(pt);
+        L.alg_bytes += t.data_len - t.fn_len;
+      }
+      const QwImgTerm& drv = sp.view.terms[nodes[n.first_child + ph.driver].term_ord];
+      L.postings += drv.doc_freq;
+      L.alg_bytes += (uint64_t)drv.doc_freq * 4 * n.num_children;  // positions probed per candidate (lower bound)
+      if (occur == QW_OCCUR_MUST || occur == QW_OCCUR_FILTER) L.min_required_df = std::min<uint64_t>(L.min_required_df, drv.doc_freq);
+      in.op = OP_PHRASE;
+      in.c = drv.skip_off;
+      in.n = drv.num_blocks;
+      in.f = 0.f;
       L.phrase_instr.push_back((uint32_t)L.instrs.size());
       L.phrases.push_back(ph);
       L.instrs.push_back(in);
@@ -1075,13 +1127,17 @@ void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std:
   }
   // phrases: one uncompressed posting block per block of each phrase's driver term (phrase_kernel.cuh)
   uint32_t n_phrases = 0, phrase_blocks = 0;
-  for (auto& L : low)
+  size_t n_phrase_exp = 0;  // expansions of the batch's phrase prefixes
+  for (auto& L : low) {
     for (size_t k = 0; k < L.phrases.size(); k++) { n_phrases++; phrase_blocks += L.instrs[L.phrase_instr[k]].n; }
+    n_phrase_exp += L.phrase_exp.size();
+  }
   auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
   size_t o_plans = 0, o_instr = al(o_plans + n * sizeof(DSplitPlan)), o_cols = al(o_instr + tot_instr * sizeof(DInstr)),
          o_aggs = al(o_cols + std::max(tot_cols, 1u) * sizeof(DCol)), o_fwa = al(o_aggs + std::max(tot_aggs, 1u) * sizeof(DAgg)),
          o_fws = al(o_fwa + (n + 1) * 4), o_bounds = al(o_fws + (n + 1) * 4), o_rank = al(o_bounds + (size_t)tot_bounds * 8),
-         o_smp = al(o_rank + (size_t)n * 4), o_phr = al(o_smp + sample_win.size() * 4), o_fwd = al(o_phr + (size_t)n_phrases * sizeof(DPhrase)),
+         o_smp = al(o_rank + (size_t)n * 4), o_phr = al(o_smp + sample_win.size() * 4), o_pexp = al(o_phr + (size_t)n_phrases * sizeof(DPhrase)),
+         o_fwd = al(o_pexp + n_phrase_exp * sizeof(DPhraseTerm)),
          o_fwds = al(o_fwd + (use_driver ? (size_t)(n + 1) * 4 : 0)), blob_bytes = al(o_fwds + (use_driver ? (size_t)(n + 1) * 4 : 0));
   // device-side cross-split merge: the per-split hit lists stay in scratch, only the merged top-K comes back
   const bool do_merge = merge && merged && merge->k > 0 && any_topk && merge->rank.size() == n_in;
@@ -1184,6 +1240,7 @@ void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std:
   cudaStream_t st = slot->stream;
 
   uint32_t phr_done = 0, phr_blocks_done = 0;
+  size_t pexp_done = 0;
   for (uint32_t i = 0; i < n; i++) {
     DSplitPlan& P = low[i].P;
     // privatised counters + stats triples must fit the (dead at collect time) staging area
@@ -1207,9 +1264,15 @@ void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std:
       DInstr& pin = low[i].instrs[low[i].phrase_instr[k]];
       ph.first_work = phr_blocks_done;
       ph.out = (uint64_t)(slot->d_scratch + s_vblk + (size_t)phr_blocks_done * sizeof(VBlk));
+      DPhrase staged = ph;  // (ph.exp stays an index into phrase_exp)
+      if (ph.n_exp) {
+        memcpy(slot->h_blob + o_pexp + pexp_done * sizeof(DPhraseTerm), low[i].phrase_exp.data() + ph.exp, (size_t)ph.n_exp * sizeof(DPhraseTerm));
+        staged.exp = (uint64_t)(slot->d_blob + o_pexp + pexp_done * sizeof(DPhraseTerm));
+        pexp_done += ph.n_exp;
+      }
       pin.a = ph.out;
       phr_blocks_done += pin.n;
-      memcpy(slot->h_blob + o_phr + (size_t)phr_done++ * sizeof(DPhrase), &ph, sizeof ph);
+      memcpy(slot->h_blob + o_phr + (size_t)phr_done++ * sizeof(DPhrase), &staged, sizeof staged);
     }
     memcpy(slot->h_blob + o_plans + i * sizeof(DSplitPlan), &P, sizeof P);
     memcpy(slot->h_blob + o_instr + P.instr_base * sizeof(DInstr), low[i].instrs.data(), P.n_instr * sizeof(DInstr));
@@ -1392,7 +1455,11 @@ void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std:
     uint32_t max_terms = 1;
     for (auto& L : low) for (auto& ph : L.phrases) max_terms = std::max(max_terms, ph.n_terms);
     const size_t psm = (size_t)QP_WARPS * QP_SMEM_WORDS(max_terms) * 4;
-    qwk::k_phrase<<<(phrase_blocks + QP_WARPS - 1) / QP_WARPS, QP_WARPS * 32, psm, st>>>((const DPhrase*)(slot->d_blob + o_phr), n_phrases, phrase_blocks, max_terms);
+    const uint32_t pgrid = (phrase_blocks + QP_WARPS - 1) / QP_WARPS;
+    const DPhrase* d_phr = (const DPhrase*)(slot->d_blob + o_phr);
+    // the suffix stage of phrase prefixes lives in its own instantiation: plain phrases keep the lean kernel
+    if (n_phrase_exp) qwk::k_phrase<true><<<pgrid, QP_WARPS * 32, psm, st>>>(d_phr, n_phrases, phrase_blocks, max_terms);
+    else qwk::k_phrase<false><<<pgrid, QP_WARPS * 32, psm, st>>>(d_phr, n_phrases, phrase_blocks, max_terms);
     stats.launches++;
     stats.kernel_mask |= QWGPU_KERNEL_PHRASE;
   }

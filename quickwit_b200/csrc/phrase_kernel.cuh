@@ -16,6 +16,14 @@
 //      (contribution = weight * tf-factor(phrase_count, fieldnorm), the same table / divide as a term's BM25).
 // The window kernel then consumes the phrase like a term whose blocks are already decoded (OP_PHRASE,
 // kernels.cuh::fold_vblock), finding the blocks of a window through the driver term's skip list.
+//
+// A phrase prefix (tantivy PhrasePrefixQuery, QW_NODE_PHRASE_PREFIX) is the same pre-pass over its exact terms, the
+// rarest of them driving, whose last slot is a SET of terms (the prefix's expansions). Step 3 is replaced by a suffix
+// stage (2b): per expansion, in order, the candidates still alive and not yet matched are looked up in the
+// expansion's blocks like in step 2, and every position q >= offset_last of a present candidate tests the base
+// b = q - offset_last against every exact term's positions. The loop ends once every alive candidate of the warp has
+// matched. The output is unscored (val = 0). Only the k_phrase<true> instantiation carries the stage, so batches
+// without a phrase prefix run the plain kernel unchanged.
 #pragma once
 #include "kernels.cuh"
 
@@ -92,6 +100,9 @@ __device__ __forceinline__ uint32_t phrase_first_block(const QwSkip* sk, uint32_
 // shared memory per warp: 3 + 2 * max_terms arrays of 128 words (max_terms = the longest phrase of the batch), so that
 // short phrases — the usual case — leave room for three times as many warps per SM as a layout sized for 8 terms
 #define QP_SMEM_WORDS(max_terms) ((3u + 2u * (max_terms)) * QW_BLOCK_LEN)
+// kPrefix: the batch holds at least one phrase prefix (n_exp > 0); its plain phrases take the same path as in
+// k_phrase<false>
+template <bool kPrefix>
 __global__ void __launch_bounds__(QP_WARPS * 32) k_phrase(const DPhrase* phrases, uint32_t n_phrases, uint32_t total_blocks, uint32_t max_terms) {
   // per warp: the decoded block of the term being probed + every term's {first position index, tf} per candidate
   extern __shared__ __align__(16) uint8_t qp_smem[];
@@ -192,8 +203,96 @@ __global__ void __launch_bounds__(QP_WARPS * 32) k_phrase(const DPhrase* phrases
     }
   }
 
-  // ---- 3. positions: base positions at which every term lines up -----------------------------------------------
   VBlk* out = (VBlk*)ph.out + b;
+  if constexpr (kPrefix) {
+    if (ph.n_exp) {
+      // ---- 2b. phrase prefix: the expansions of the last slot ----------------------------------------------------
+      const DPhraseTerm* X = (const DPhraseTerm*)ph.exp;
+      const uint32_t doc_first = __shfl_sync(0xFFFFFFFFu, cdoc[0], 0);
+      const uint32_t doc_last = __ldg(&((const QwSkip*)(base + D.skip_off))[b].last_doc);
+      uint32_t matched = 0;  // bit j: candidate j holds the phrase with some expansion
+      for (uint32_t e = 0; e < ph.n_exp; e++) {
+        const uint32_t open = alive & ~matched;
+        if (!__ballot_sync(0xFFFFFFFFu, open != 0)) break;  // every alive candidate of the warp has matched
+        const DPhraseTerm& T = X[e];
+        const QwSkip* sk = (const QwSkip*)(base + T.skip_off);
+        const uint32_t* pidx = (const uint32_t*)(base + T.pidx_off);
+        const uint32_t r_lo = phrase_first_block(sk, T.nblk, doc_first, lane);
+        if (r_lo >= T.nblk) continue;  // every posting of the expansion lies before the driver block
+        const uint32_t r_hi = r_lo + phrase_first_block(sk + r_lo, T.nblk - r_lo, doc_last, lane);
+        uint32_t need[4];
+#pragma unroll
+        for (int j = 0; j < 4; j++) {
+          need[j] = QP_NONE;
+          if ((open >> j) & 1u) {
+            uint32_t lo = r_lo, hi = min(r_hi + 1, T.nblk);
+            while (lo < hi) {
+              const uint32_t mid = (lo + hi) >> 1;
+              if (__ldg(&sk[mid].last_doc) < cdoc[j]) lo = mid + 1; else hi = mid;
+            }
+            if (lo < T.nblk) need[j] = lo;
+          }
+        }
+        for (;;) {
+          uint32_t cur = min(min(need[0], need[1]), min(need[2], need[3]));
+#pragma unroll
+          for (int o = 16; o > 0; o >>= 1) cur = min(cur, __shfl_xor_sync(0xFFFFFFFFu, cur, o));
+          if (cur == QP_NONE) break;
+          uint32_t d[4], f[4], pre[4], cnt;
+          phrase_decode(base + T.data_off + __ldg(&sk[cur].byte_off), lane, d, f, cnt);
+          block_excl_prefix(f, lane, pre);
+          __syncwarp();
+#pragma unroll
+          for (int j = 0; j < 4; j++) {
+            bdoc[lane * 4 + j] = lane * 4 + j < cnt ? d[j] : QP_NONE;
+            bpre[lane * 4 + j] = pre[j];
+            btf[lane * 4 + j] = f[j];
+          }
+          __syncwarp();
+          const uint32_t first = __ldg(pidx + cur);
+#pragma unroll
+          for (int j = 0; j < 4; j++) {
+            if (need[j] != cur) continue;
+            need[j] = QP_NONE;
+            uint32_t lo = 0, hi = cnt;
+            while (lo < hi) {
+              const uint32_t mid = (lo + hi) >> 1;
+              if (bdoc[mid] < cdoc[j]) lo = mid + 1; else hi = mid;
+            }
+            if (lo >= cnt || bdoc[lo] != cdoc[j]) continue;
+            const uint32_t c = lane * 4 + j;
+            const uint32_t* pe = (const uint32_t*)(base + T.pos_off) + first + bpre[lo];
+            const uint32_t ne = btf[lo];
+            for (uint32_t i = 0; i < ne; i++) {
+              const uint32_t q = __ldg(pe + i);
+              if (q < T.offset) continue;  // the phrase would start before position 0
+              const uint32_t start = q - T.offset;
+              bool all = true;
+              for (uint32_t t = 0; t < ph.n_terms && all; t++) {
+                const uint32_t want = start + ph.t[t].offset;
+                const uint32_t* pt = (const uint32_t*)(base + ph.t[t].pos_off) + S_POS(t, c);
+                uint32_t plo = 0, phi = S_TF(t, c);
+                while (plo < phi) {
+                  const uint32_t mid = (plo + phi) >> 1;
+                  if (__ldg(pt + mid) < want) plo = mid + 1; else phi = mid;
+                }
+                all = plo < S_TF(t, c) && __ldg(pt + plo) == want;
+              }
+              if (all) { matched |= 1u << j; break; }
+            }
+          }
+        }
+      }
+      uint32_t odoc[4];
+#pragma unroll
+      for (int j = 0; j < 4; j++) odoc[j] = (matched >> j) & 1u ? cdoc[j] : QP_NONE;
+      *reinterpret_cast<uint4*>(&out->doc[lane * 4]) = make_uint4(odoc[0], odoc[1], odoc[2], odoc[3]);
+      *reinterpret_cast<float4*>(&out->val[lane * 4]) = make_float4(0.f, 0.f, 0.f, 0.f);
+      return;
+    }
+  }
+
+  // ---- 3. positions: base positions at which every term lines up -----------------------------------------------
   const uint32_t off_d = D.offset;
   uint32_t odoc[4];
   float oval[4];

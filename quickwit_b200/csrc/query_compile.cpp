@@ -127,8 +127,9 @@ static int64_t truncate_ns(int64_t ns, int64_t prec) {  // DateTime::truncate
 
 // ---- TantivyQueryAst mirror ------------------------------------------------------------------------
 struct TQ {
-  enum Kind { Bool, Term, Range, Exists, All, None, Phrase } kind = None;
-  std::vector<uint32_t> phrase_terms;  // Phrase: term ords in phrase order (offset k = position k)
+  enum Kind { Bool, Term, Range, Exists, All, None, Phrase, PhrasePrefix } kind = None;
+  std::vector<uint32_t> phrase_terms;  // Phrase / PhrasePrefix: (exact) term ords in phrase order (offset k = position k)
+  std::vector<uint32_t> prefix_terms;  // PhrasePrefix: the expansions of the last slot (offset = phrase_terms.size())
   bool opaque = false;  // wrapped in a BoostQuery leaf: not subject to bool flattening / const folding
   std::vector<TQ> must, must_not, should, filter;
   bool has_msm = false;
@@ -341,6 +342,78 @@ static TQ term_leaf(const Ctx& cx, uint32_t field, const std::string& token) {
   t.term_ord = ord < 0 ? 0xFFFFFFFFu : (uint32_t)ord;
   return t;
 }
+// ---- phrase prefix queries (quickwit-query/src/query_ast/phrase_prefix_query.rs, tantivy PhrasePrefixQuery) -----
+
+// Tokenizer named by a phrase_prefix / bool_prefix query (FullTextParams::text_analyzer): the image applies `raw` and
+// `default`; the other analyzers quickwit registers (tokenizers/mod.rs) are refused, any other name is an error.
+static uint32_t prefix_query_tokenizer(const std::string& name, uint32_t field_tokenizer) {
+  if (name.empty()) return field_tokenizer;
+  if (name == "raw") return QW_TOK_RAW;
+  if (name == "default") return QW_TOK_DEFAULT;
+  static const char* registered[] = {"raw_lowercase", "lowercase", "whitespace", "chinese_compatible", "source_code_default", "source_code_with_hex"};
+  for (const char* r : registered)
+    if (name == r) fail(QWGPU_EUNSUPPORTED, "tokenizer `%s` is not implemented on the GPU path", name.c_str());
+  fail(QWGPU_EINVALID_QUERY, "invalid query: no tokenizer named `%s` is registered", name.c_str());
+}
+
+// The prefix's expansions in one split: the field's first `max_expansions` terms, in byte order, that start with
+// `prefix` (the TermRange [prefix, prefix_end) with limit max_expansions of query_builder.rs)
+static std::vector<uint32_t> expand_prefix(const ImageView& img, uint32_t field, const std::string& prefix, uint64_t max_expansions) {
+  const QwImgField& F = img.fields[field];
+  auto less = [&](uint32_t t) {  // term t < prefix
+    const QwImgTerm& T = img.terms[t];
+    const uint32_t m = std::min<uint32_t>(T.bytes_len, (uint32_t)prefix.size());
+    const int c = memcmp(img.term_bytes + T.bytes_off, prefix.data(), m);
+    return c < 0 || (c == 0 && T.bytes_len < prefix.size());
+  };
+  uint32_t lo = F.first_term, hi = F.first_term + F.num_terms;
+  while (lo < hi) {
+    const uint32_t mid = lo + (hi - lo) / 2;
+    if (less(mid)) lo = mid + 1; else hi = mid;
+  }
+  std::vector<uint32_t> out;
+  for (uint32_t t = lo; t < F.first_term + F.num_terms && out.size() < max_expansions; t++) {
+    const QwImgTerm& T = img.terms[t];
+    if (T.bytes_len < prefix.size() || memcmp(img.term_bytes + T.bytes_off, prefix.data(), prefix.size()) != 0) break;
+    out.push_back(t);
+  }
+  return out;
+}
+
+// PhrasePrefixQuery::new_with_offset(tokens) with max_expansions, on a text field of the split. One token: a doc
+// matches when it holds any expansion (tantivy's range query with a limit) — an unscored set filter of TERM nodes,
+// the wildcard shape. More tokens: QW_NODE_PHRASE_PREFIX. Both are constant-score in tantivy's sense only as far as
+// the visible sources go, so neither is served in a scoring clause under _score ranking.
+static TQ phrase_prefix_leaf(const Ctx& cx, uint32_t f, const std::vector<std::string>& tokens, uint64_t max_expansions) {
+  if (tokens.size() > 1 && !(cx.img.fields[f].flags & QW_FIELD_HAS_POSITIONS))
+    fail(QWGPU_EINVALID_QUERY, "invalid query: trying to run a phrase prefix query on a field which does not have positions indexed");
+  if (tokens.size() > QW_MAX_PHRASE_TERMS)
+    fail(QWGPU_EUNSUPPORTED, "phrase prefixes of more than %d terms are not implemented on the GPU path", QW_MAX_PHRASE_TERMS);
+  refuse_const_score_under_ranking(cx, "phrase_prefix");
+  TQ ph;
+  ph.kind = TQ::PhrasePrefix;
+  for (size_t i = 0; i + 1 < tokens.size(); i++) {
+    const int ord = cx.img.find_term(f, (const uint8_t*)tokens[i].data(), (uint32_t)tokens[i].size());
+    if (ord < 0) return tq_none();  // a split without one of the exact terms matches nothing
+    ph.phrase_terms.push_back((uint32_t)ord);
+  }
+  ph.prefix_terms = expand_prefix(cx.img, f, tokens.back(), max_expansions);
+  if (ph.prefix_terms.empty()) return tq_none();
+  if (tokens.size() > 1) return ph;
+  TQ b;
+  b.kind = TQ::Bool;
+  for (uint32_t t : ph.prefix_terms) {
+    TQ leaf;
+    leaf.kind = TQ::Term;
+    leaf.term_ord = t;
+    b.should.push_back(std::move(leaf));
+  }
+  TQ outer;
+  outer.kind = TQ::Bool;
+  outer.filter.push_back(std::move(b));
+  return outer;
+}
+
 static TQ range_leaf(uint32_t column, uint64_t lo, uint64_t hi) {
   TQ t;
   t.kind = TQ::Range;
@@ -352,7 +425,8 @@ static TQ range_leaf(uint32_t column, uint64_t lo, uint64_t hi) {
 
 // full_text_query / FullTextParams::make_query (full_text_query.rs:103-160, utils.rs:73-200)
 static TQ full_text(const Ctx& cx, const std::string& field, const std::string& text, const std::string& tokenizer_override,
-                    const std::string& mode, bool op_and, int zero_terms_all, bool lenient, uint32_t slop = 0) {
+                    const std::string& mode, bool op_and, int zero_terms_all, bool lenient, uint32_t slop = 0,
+                    uint64_t max_expansions = 50) {
   int f = cx.img.find_field(field);
   if (f < 0) {
     int c = cx.img.find_column(field);
@@ -377,7 +451,8 @@ static TQ full_text(const Ctx& cx, const std::string& field, const std::string& 
     fail(QWGPU_EINVALID_QUERY, "invalid query: field does not exist: `%s`", field.c_str());
   }
   uint32_t tok = cx.img.fields[f].tokenizer;
-  if (!tokenizer_override.empty()) tok = tokenizer_override == "raw" ? QW_TOK_RAW : QW_TOK_DEFAULT;
+  if (mode == "bool_prefix") tok = prefix_query_tokenizer(tokenizer_override, tok);
+  else if (!tokenizer_override.empty()) tok = tokenizer_override == "raw" ? QW_TOK_RAW : QW_TOK_DEFAULT;
   std::vector<std::string> tokens = tokenize_text(text, tok);
   if (tokens.empty()) return zero_terms_all ? tq_all() : tq_none();
   if (tokens.size() == 1) return term_leaf(cx, (uint32_t)f, tokens[0]);
@@ -398,7 +473,16 @@ static TQ full_text(const Ctx& cx, const std::string& field, const std::string& 
     }
     return ph;
   }
-  if (mode == "bool_prefix") fail(QWGPU_EUNSUPPORTED, "bool_prefix queries are not implemented on the GPU path yet");
+  if (mode == "bool_prefix") {
+    // FullTextMode::BoolPrefix (full_text_query.rs:124-139): every token but the last is a term query, the last a
+    // one-token phrase prefix; clauses joined by the operator
+    TQ b;
+    b.kind = TQ::Bool;
+    std::vector<TQ>& clauses = op_and ? b.must : b.should;
+    for (size_t i = 0; i + 1 < tokens.size(); i++) clauses.push_back(term_leaf(cx, (uint32_t)f, tokens[i]));
+    clauses.push_back(phrase_prefix_leaf(cx, (uint32_t)f, {tokens.back()}, max_expansions));
+    return b;
+  }
   TQ b;
   b.kind = TQ::Bool;
   bool conj = mode == "phrase_fallback_to_intersection" ? true : op_and;
@@ -490,17 +574,47 @@ static TQ build(const Ctx& cx, const Json& q, int depth) {
     bool op_and = false;
     int zero_all = 0;
     uint32_t slop = 0;
+    uint64_t max_expansions = 50;
     if (params) {
       tok = params->str_or("tokenizer", "");
       if (const Json* m = params->get("mode")) {
         mode = m->str_or("type", "bool");
         if (const Json* sl = m->get("slop")) slop = (uint32_t)sl->as_f64();
+        if (const Json* me = m->get("max_expansions")) if (me->is_num()) max_expansions = (uint64_t)me->as_f64();
         std::string op = m->str_or("operator", "Or");
         op_and = op == "And" || op == "AND" || op == "and";
       }
       zero_all = params->str_or("zero_terms_query", "none") == "all";
     }
-    return full_text(cx, q.str_or("field", ""), q.str_or("text", ""), tok, mode, op_and, zero_all, q.bool_or("lenient", false), slop);
+    return full_text(cx, q.str_or("field", ""), q.str_or("text", ""), tok, mode, op_and, zero_all, q.bool_or("lenient", false), slop, max_expansions);
+  }
+  if (type == "phrase_prefix") {
+    // PhrasePrefixQuery::build_tantivy_ast_impl (phrase_prefix_query.rs): `lenient` covers a missing field only
+    const std::string field = q.str_or("field", ""), phrase = q.str_or("phrase", "");
+    uint64_t max_expansions = 50;
+    if (const Json* me = q.get("max_expansions")) if (me->is_num()) max_expansions = (uint64_t)me->as_f64();
+    const Json* params = q.get("params");
+    const std::string tok_name = params ? params->str_or("tokenizer", "") : "";
+    const bool zero_all = params && params->str_or("zero_terms_query", "none") == "all";
+    const int f = cx.img.find_field(field);
+    if (f < 0) {
+      const int c = cx.img.find_column(field);
+      bool known = false, text = true;
+      uint32_t field_tok = QW_TOK_DEFAULT;
+      for (auto& fd : cx.dm.fields)
+        if (fd.name == field) { known = true; text = fd.type == "text" || fd.type == "json"; field_tok = fd.tokenizer == "raw" ? QW_TOK_RAW : QW_TOK_DEFAULT; }
+      if ((c >= 0 && cx.img.columns[c].type != QW_COL_STR) || !text)
+        fail(QWGPU_EINVALID_QUERY, "invalid query: trying to run a PhrasePrefix query on a non-text field");
+      if (!known && !q.bool_or("lenient", false)) fail(QWGPU_EINVALID_QUERY, "invalid query: field does not exist: `%s`", field.c_str());
+      if (!known) return tq_none();
+      // declared in the doc mapping but without a single term in this split: no expansion can exist
+      const uint32_t tok = prefix_query_tokenizer(tok_name, field_tok);
+      return zero_all && tokenize_text(phrase, tok).empty() ? tq_all() : tq_none();
+    }
+    const uint32_t tok = prefix_query_tokenizer(tok_name, cx.img.fields[f].tokenizer);
+    std::vector<std::string> tokens = tokenize_text(phrase, tok);
+    if (tokens.empty()) return zero_all ? tq_all() : tq_none();
+    return phrase_prefix_leaf(cx, (uint32_t)f, tokens, max_expansions);
   }
   if (type == "range") return range_query(cx, q.str_or("field", ""), q.get("lower_bound"), q.get("upper_bound"));
   if (type == "field_presence") {
@@ -580,7 +694,7 @@ static TQ build(const Ctx& cx, const Json& q, int depth) {
   }
   if (type == "user_input")
     fail(QWGPU_EINVALID_QUERY, "invalid query: user_input queries must be parsed by the root before reaching a leaf");
-  if (type == "regex" || type == "phrase_prefix")
+  if (type == "regex")
     fail(QWGPU_EUNSUPPORTED, "`%s` queries are not implemented on the GPU path yet", type.c_str());
   fail(QWGPU_EINVALID_QUERY, "invalid query: unknown query type `%s`", type.c_str());
 }
@@ -630,6 +744,27 @@ static void emit(const TQ& t, uint32_t occur, const ImageView& img, std::vector<
         c.term_ord = t.phrase_terms[k]; c.field_id = field_id; c.column = 0xFFFFFFFFu;
         c.bm25_weight = bm25_idf(img.terms[c.term_ord].doc_freq, img.hdr->num_docs) * (1.0f + BM25_K1);
         c.lo = k;  // position offset inside the phrase
+      }
+      break;
+    }
+    case TQ::PhrasePrefix: {
+      // never scored (refused in scoring clauses under _score ranking): children = exact terms, then expansions
+      n.kind = QW_NODE_PHRASE_PREFIX;
+      const uint32_t field_id = img.terms[t.phrase_terms[0]].field_id;
+      const size_t k = t.phrase_terms.size(), e = t.prefix_terms.size();
+      n.field_id = field_id;
+      n.lo = k;
+      const size_t first = out.size();  // (`n` dangles after the resize below)
+      out[idx].first_child = (uint32_t)first;
+      out[idx].num_children = (uint32_t)(k + e);
+      out.resize(first + k + e);
+      for (size_t i = 0; i < k + e; i++) {
+        QwPlanNode& c = out[first + i];
+        memset(&c, 0, sizeof c);
+        c.kind = QW_NODE_TERM; c.occur = QW_OCCUR_MUST; c.boost = 1.0f; c.min_should_match = 0xFFFFFFFFu;
+        c.term_ord = i < k ? t.phrase_terms[i] : t.prefix_terms[i - k]; c.field_id = field_id; c.column = 0xFFFFFFFFu;
+        c.bm25_weight = bm25_idf(img.terms[c.term_ord].doc_freq, img.hdr->num_docs) * (1.0f + BM25_K1);
+        c.lo = i < k ? i : k;  // position offset inside the phrase; every expansion sits in the last slot
       }
       break;
     }

@@ -21,6 +21,8 @@ TOK_RAW, TOK_DEFAULT = 0, 1
 COL_U64, COL_I64, COL_F64, COL_BOOL, COL_DATETIME, COL_STR, COL_BYTES = range(7)
 CARD_FULL, CARD_OPTIONAL, CARD_MULTI = range(3)
 NODE_TERM, NODE_RANGE, NODE_BOOL, NODE_ALL, NODE_NONE, NODE_EXISTS, NODE_PHRASE = 1, 2, 3, 4, 5, 6, 7
+NODE_PHRASE_PREFIX = 8
+MAX_PHRASE_TERMS, MAX_PREFIX_EXPANSIONS = 8, 1024
 OCCUR_MUST, OCCUR_SHOULD, OCCUR_MUST_NOT, OCCUR_FILTER = range(4)
 SORT_NONE, SORT_DOCID, SORT_SCORE, SORT_COLUMN = range(4)
 ORDER_ASC, ORDER_DESC = 0, 1

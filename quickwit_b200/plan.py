@@ -50,6 +50,59 @@ def phrase(img: SplitImage, field: str, terms: Sequence[str], occur=ffi.OCCUR_MU
     return Node(ffi.NODE_PHRASE, occur, boost, children=kids, field_id=img.field_names().index(field), weight=w)
 
 
+def prefix_expansions(img: SplitImage, field: str, prefix: bytes | str, max_expansions: int) -> List[int]:
+    """Term ords of the field's first `max_expansions` terms, in byte order, that start with `prefix` (the
+    expansion of a phrase prefix in one split)."""
+    if isinstance(prefix, str):
+        prefix = prefix.encode()
+    names = img.field_names()
+    if field not in names:
+        return []
+    _h, _s, tbytes, fields, terms, _c = img._directory()
+    f = fields[names.index(field)]
+    out: List[int] = []
+    for t in range(f.first_term, f.first_term + f.num_terms):
+        if len(out) >= max_expansions:
+            break
+        b = tbytes[terms[t].bytes_off: terms[t].bytes_off + terms[t].bytes_len]
+        if b.startswith(prefix):
+            out.append(t)
+        elif b > prefix:
+            break
+    return out
+
+
+def phrase_prefix(img: SplitImage, field: str, tokens: Sequence[str], max_expansions: int = 50,
+                  occur=ffi.OCCUR_MUST, boost: float = 1.0) -> Node:
+    """tantivy PhrasePrefixQuery over `tokens` (the last one is the prefix), never scored. One token: the unscored
+    set filter of its expansions; more: a PHRASE_PREFIX node. An absent exact term or no expansion matches nothing."""
+    fid = img.field_names().index(field) if field in img.field_names() else 0
+    ords = [img.term_ord(field, t) for t in tokens[:-1]]
+    exps = prefix_expansions(img, field, tokens[-1], max_expansions)
+    if any(o < 0 for o in ords) or not exps:
+        return Node(ffi.NODE_NONE, occur)
+
+    def kid(o, lo, occ=ffi.OCCUR_MUST):
+        return Node(ffi.NODE_TERM, occ, 1.0, term_ord=o, field_id=fid, weight=bm25_weight(img.doc_freq(o), img.num_docs), lo=lo)
+
+    if not ords:
+        inner = Node(ffi.NODE_BOOL, ffi.OCCUR_FILTER, children=[kid(o, 0, ffi.OCCUR_SHOULD) for o in exps])
+        return Node(ffi.NODE_BOOL, occur, children=[inner])
+    k = len(ords)
+    kids = [kid(o, i) for i, o in enumerate(ords)] + [kid(o, k) for o in exps]
+    return Node(ffi.NODE_PHRASE_PREFIX, occur, boost, children=kids, field_id=fid, lo=k)
+
+
+def phrase_prefix_as_phrases(node: Node, occur: Optional[int] = None) -> Node:
+    """The same match set as a multi-token PHRASE_PREFIX node, as a bool that ORs one plain phrase per expansion
+    (scores aside: the phrases are scored where they sit in a scoring clause, the phrase prefix never is)."""
+    assert node.kind == ffi.NODE_PHRASE_PREFIX
+    k = node.lo
+    exact, exps = node.children[:k], node.children[k:]
+    phrases = [Node(ffi.NODE_PHRASE, ffi.OCCUR_SHOULD, 1.0, children=list(exact) + [e], field_id=node.field_id) for e in exps]
+    return Node(ffi.NODE_BOOL, node.occur if occur is None else occur, children=phrases)
+
+
 def range_(img: SplitImage, column: str, lo: int, hi: int, occur=ffi.OCCUR_FILTER, boost=1.0) -> Node:
     c = img.column_ord(column)
     return Node(ffi.NODE_RANGE, occur, boost, column=c if c >= 0 else ffi.ABSENT, lo=lo, hi=hi)
