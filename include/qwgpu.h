@@ -129,6 +129,10 @@ typedef struct qwgpu_split_result {
   uint32_t sample_stride;    /* stride of the sampled top-K threshold pass; 0 when no sampled pass ran */
   uint32_t radix_passes;     /* exact radix rounds (histogram pass + digit pick) of the top-K threshold */
   uint32_t refined;          /* 1 when a failed sampled threshold was repaired by the candidates-only pass */
+  /* Plans in the hashed aggregation layout (qw_agg_hashed, DESIGN.md §4.4) return entries instead of cells:
+   * num_agg_cells is 0 and agg_entries holds the entries that a matched doc reached, in no particular order. */
+  uint32_t num_agg_entries;
+  QwAggEntry* agg_entries;   /* malloc'ed; free with qwgpu_buf_free */
 } qwgpu_split_result;
 
 /* qwgpu_split_result.kernel_mask */
@@ -142,6 +146,16 @@ typedef struct qwgpu_split_result {
                                          (N+1)-th trace timestamps tie */
 #define QWGPU_KERNEL_FAST_AGGS 128u /* k_window aggregated with the fast path (privatised counters and stats cells,
                                       histogram buckets through the raw-space boundary table) for a split of the batch */
+#define QWGPU_KERNEL_HASHED_AGGS 256u /* k_window aggregated a split of the batch into hashed cells */
+#define QWGPU_KERNEL_HASHED_AGGS_RETRY 512u /* a hashed split outgrew its initial capacity (QWGPU_HASHED_INIT_CELLS)
+                                               and the batch ran again with every hashed table at its bound. The
+                                               other statistics of such a call (time, launches, radix passes,
+                                               fallbacks, bytes) add up both runs. */
+/* Initial capacity of a split's hashed cell table: min(this, the split's bound on distinct cells). */
+#define QWGPU_HASHED_INIT_CELLS 65536u
+/* Largest total of the hashed tables (cells, key records and slots, each at its split's bound) that one call may
+ * need; beyond it every hashed split of the call fails with QWGPU_EUNSUPPORTED before any launch. */
+#define QWGPU_HASHED_MAX_BYTES (8ull << 30)
 
 /* Runs `num_splits` plans (plan i against split_ids[i]) in ONE batched launch sequence.
  * results[i] is filled for every split; status[i] is 0 or a QWGPU_E* code for that split. */
@@ -157,6 +171,18 @@ int qwgpu_build_leaf_response(const uint8_t* img, uint64_t img_len, const char* 
                               const char* doc_mapper_json, uint64_t num_hits, const QwHit* hits,
                               uint32_t num_partial_hits, const QwAggCell* cells, uint32_t num_cells,
                               uint8_t** resp, size_t* resp_len);
+/* The same from a result in the hashed layout (qwgpu_split_result.agg_entries). Any plan's aggregation tree can be
+ * given as entries: the response is the one qwgpu_build_leaf_response gives for the equivalent dense cells. */
+int qwgpu_build_leaf_response_entries(const uint8_t* img, uint64_t img_len, const char* split_id,
+                                      const uint8_t* search_request_pb, size_t search_request_len,
+                                      const char* doc_mapper_json, uint64_t num_hits, const QwHit* hits,
+                                      uint32_t num_partial_hits, const QwAggEntry* entries, uint32_t num_entries,
+                                      uint8_t** resp, size_t* resp_len);
+/* The aggregation layout a plan takes on a split, host only: *hashed = qw_agg_hashed(); for hashed plans
+ * *bound_cells = the guaranteed upper bound on the split's distinct cells (0 for dense plans). Fails with
+ * QWGPU_EUNSUPPORTED when the table at that bound exceeds QWGPU_HASHED_MAX_BYTES, as a search would. */
+int qwgpu_agg_layout(const uint8_t* img, uint64_t img_len, const char* split_id, const uint8_t* plan, size_t plan_len,
+                     uint32_t* hashed, uint64_t* bound_cells);
 
 /* Pre-search pruning (SURVEY.md 8a row a16), host only: what qwgpu_leaf_search does to the request of every
  * split before it searches — CanSplitDoBetter::{from_request, optimize_split_order, optimize}

@@ -304,7 +304,7 @@ typedef struct QwHit {
   uint32_t reserved;
 } QwHit;
 
-/* Dense aggregation result. Every QwAggNode owns `cells(node)` = Π num_buckets over its ancestor
+/* Dense aggregation result (plans for which qw_agg_hashed() is 0). Every QwAggNode owns `cells(node)` = Π num_buckets over its ancestor
  * chain (itself included; metric nodes count 1) cells, laid out row-major (outermost ancestor
  * slowest). Bucket nodes use only `count` (doc_count). Metric nodes (QW_AGG_STATS) use all four:
  * `sum_bits`: where qw_stats_sum_exact() holds, the exact integer sum of the RAW offsets (value =
@@ -320,6 +320,50 @@ typedef struct QwAggCell {
   uint64_t min_mapped;
   uint64_t max_mapped;
 } QwAggCell;
+
+/* Hashed aggregation result (DESIGN.md §4.4, hashed cells): one entry per (node, parent entry, bucket key) that
+ * a matched doc of the split reached, instead of Π num_buckets dense cells per node. A split's plan takes this
+ * layout when its tree is deeper than bucket -> bucket -> metric, its dense cells add up to more than
+ * QW_AGG_DENSE_MAX_CELLS, or a TERMS node's dense space exceeds QW_AGG_DENSE_MAX_TERMS (qw_agg_hashed).
+ *   key: TERMS = the bit-packed raw value (0 with QW_AGG_ENTRY_MISSING: the `missing` bucket); HISTOGRAM = the
+ *        bucket index relative to base_pos (agg_bucket's f64 formula); RANGE = the range index; STATS = 0.
+ *   cell: as in the dense layout (bucket entries use `count` only). */
+#define QW_AGG_DENSE_MAX_CELLS (1ull << 26)
+#define QW_AGG_DENSE_MAX_TERMS (1ull << 24)
+#define QW_AGG_NO_PARENT 0xFFFFFFFFu
+enum { QW_AGG_ENTRY_MISSING = 1u };
+typedef struct QwAggEntry {
+  uint32_t node;
+  uint32_t parent; /* index of the parent bucket's entry; QW_AGG_NO_PARENT for top-level nodes */
+  uint64_t key;
+  uint32_t flags;  /* QW_AGG_ENTRY_* */
+  uint32_t reserved;
+  QwAggCell cell;
+} QwAggEntry; /* 56 bytes */
+
+/* 1 when the plan's aggregation tree takes the hashed layout: a node below two bucket ancestors that is not a
+ * metric (or any node below three), the dense cells of all nodes adding up to more than QW_AGG_DENSE_MAX_CELLS,
+ * or a TERMS node whose dense space (num_buckets without the `missing` slot) exceeds QW_AGG_DENSE_MAX_TERMS.
+ * Reads only the plan; the caller has checked every parent index. */
+static inline int qw_agg_hashed(const QwAggNode* nodes, uint32_t n) {
+  uint64_t total = 0;
+  for (uint32_t i = 0; i < n; i++) {
+    const QwAggNode* g = &nodes[i];
+    if (g->kind == QW_AGG_TERMS && (uint64_t)g->num_buckets - (g->has_missing ? 1u : 0u) > QW_AGG_DENSE_MAX_TERMS) return 1;
+    uint32_t depth = 0;
+    uint64_t cells = g->kind == QW_AGG_STATS ? 1 : g->num_buckets;
+    for (uint32_t p = g->parent; p != 0xFFFFFFFFu; p = nodes[p].parent) {
+      depth++;
+      if (depth > n) return 1; /* (a parent cycle: lowering refuses it) */
+      cells *= nodes[p].num_buckets;
+      if (cells > QW_AGG_DENSE_MAX_CELLS) cells = QW_AGG_DENSE_MAX_CELLS + 1;
+    }
+    if (depth > 2 || (depth == 2 && g->kind != QW_AGG_STATS)) return 1;
+    total += cells;
+    if (total > QW_AGG_DENSE_MAX_CELLS) return 1;
+  }
+  return 0;
+}
 
 static inline uint32_t qw_bit_length(uint64_t x) {
   uint32_t n = 0;

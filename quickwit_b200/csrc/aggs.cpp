@@ -13,6 +13,8 @@
 #include <chrono>
 #include <cmath>
 #include <map>
+#include <set>
+#include <tuple>
 #include <memory>
 
 #include "compile.h"
@@ -196,10 +198,11 @@ static QwAggNode lower_one(const AggReq& a, const ImageView& img, AggBinding& b)
   switch (a.kind) {
     case AggReq::Terms: {
       n.kind = QW_AGG_TERMS;
-      uint64_t nb = col ? (col->max_value - col->min_value) / col->gcd + 1 : 0;
-      if (col && col->num_vals == 0) nb = 0;
-      if (nb > (1u << 24)) fail(QWGPU_EUNSUPPORTED, "terms aggregation over %llu distinct dense slots is not supported on the GPU path", (unsigned long long)nb);
-      n.num_buckets = (uint32_t)nb + (a.has_missing ? 1 : 0);
+      // dense space beyond QW_AGG_DENSE_MAX_TERMS slots: the plan takes the hashed layout, where the bucket key is
+      // the raw value itself and num_buckets only has to exceed that limit (saturated at 0xFFFFFFFF)
+      uint64_t span = col ? (col->max_value - col->min_value) / col->gcd : 0;
+      uint64_t nb = col && col->num_vals ? std::min<uint64_t>(span, 0xFFFFFFFEull) + 1 : 0;
+      n.num_buckets = (uint32_t)std::min<uint64_t>(nb + (a.has_missing ? 1 : 0), 0xFFFFFFFFull);
       n.has_missing = a.has_missing;
       break;
     }
@@ -406,9 +409,9 @@ static std::vector<IAgg> build_children(const BuildCtx& c, uint32_t ni, uint64_t
   return out;
 }
 
-static IKey term_key(const BuildCtx& c, const AggBinding& b, const QwAggNode& n, uint32_t bucket) {
+static IKey term_key(const ImageView& img, const AggBinding& b, uint64_t raw, bool missing) {
   IKey k;
-  if (n.has_missing && bucket == n.num_buckets - 1) {
+  if (missing) {
     const Json& m = b.req->missing;
     if (m.type == Json::Str) { k.kind = IKey::Str; k.s = m.s; }
     else if (m.type == Json::U64) { k.kind = IKey::U64; k.u = m.u; }
@@ -416,10 +419,10 @@ static IKey term_key(const BuildCtx& c, const AggBinding& b, const QwAggNode& n,
     else { k.kind = IKey::F64; k.f = m.as_f64(); }
     return k;
   }
-  const QwImgColumn& col = c.img.columns[b.column];
-  uint64_t mapped = col.min_value + col.gcd * (uint64_t)bucket;
+  const QwImgColumn& col = img.columns[b.column];
+  uint64_t mapped = col.min_value + col.gcd * raw;
   switch (col.type) {
-    case QW_COL_STR: { const uint8_t* p; uint32_t len; c.img.dict_term(col, (uint32_t)mapped, &p, &len); k.kind = IKey::Str; k.s.assign((const char*)p, len); break; }
+    case QW_COL_STR: { const uint8_t* p; uint32_t len; img.dict_term(col, (uint32_t)mapped, &p, &len); k.kind = IKey::Str; k.s.assign((const char*)p, len); break; }
     case QW_COL_F64: k.kind = IKey::F64; k.f = u64_to_f64(mapped); break;
     case QW_COL_I64: case QW_COL_DATETIME: k.kind = IKey::I64; k.i = u64_to_i64(mapped); break;
     default: k.kind = IKey::U64; k.u = mapped; break;
@@ -465,49 +468,34 @@ static void sort_term_buckets(const AggReq& req, std::vector<IBucket>& bs) {
   });
 }
 
-static IAgg build_node(const BuildCtx& c, uint32_t ni, uint64_t parent_cell) {
-  const QwAggNode& n = c.nodes[ni];
-  const AggBinding& b = c.cp.agg_bindings[ni];
-  const AggReq& req = *b.req;
-  const QwAggCell* base = c.cells + c.bases[ni];
+// metric node ni from its cell (a cell with count 0 where no value reached it)
+static IAgg metric_from_cell(const CompiledPlan& cp, const ImageView& img, const QwAggNode* nodes, uint32_t ni, const QwAggCell& cell) {
+  const AggBinding& b = cp.agg_bindings[ni];
   IAgg a;
-  a.kind = (uint8_t)req.kind;
-  if (req.is_metric()) {
-    const QwAggCell& cell = base[parent_cell];
-    a.m_count = cell.count;
-    if (cell.count && b.column >= 0) {
-      uint32_t t = b.col_type;
-      const QwImgColumn& col = c.img.columns[b.column];
-      if (!qw_stats_sum_exact(c.img.columns, c.nodes, ni)) memcpy(&a.m_sum, &cell.sum_bits, 8);
-      else {
-        // exact: sum of the typed values = count * min + gcd * (sum of raw offsets); the mapped u64 of an
-        // i64 / datetime is value + 2^63
-        __int128 sum = (__int128)(unsigned __int128)col.min_value * (__int128)cell.count + (__int128)((unsigned __int128)col.gcd * cell.sum_bits);
-        if (!(t == QW_COL_U64 || t == QW_COL_BOOL)) sum -= ((__int128)1 << 63) * (__int128)cell.count;
-        a.m_sum = (double)sum;
-      }
-      a.m_min = mapped_to_f64(t, cell.min_mapped);
-      a.m_max = mapped_to_f64(t, cell.max_mapped);
+  a.kind = (uint8_t)b.req->kind;
+  a.m_count = cell.count;
+  if (cell.count && b.column >= 0) {
+    uint32_t t = b.col_type;
+    const QwImgColumn& col = img.columns[b.column];
+    if (!qw_stats_sum_exact(img.columns, nodes, ni)) memcpy(&a.m_sum, &cell.sum_bits, 8);
+    else {
+      // exact: sum of the typed values = count * min + gcd * (sum of raw offsets); the mapped u64 of an
+      // i64 / datetime is value + 2^63
+      __int128 sum = (__int128)(unsigned __int128)col.min_value * (__int128)cell.count + (__int128)((unsigned __int128)col.gcd * cell.sum_bits);
+      if (!(t == QW_COL_U64 || t == QW_COL_BOOL)) sum -= ((__int128)1 << 63) * (__int128)cell.count;
+      a.m_sum = (double)sum;
     }
-    return a;
+    a.m_min = mapped_to_f64(t, cell.min_mapped);
+    a.m_max = mapped_to_f64(t, cell.max_mapped);
   }
-  a.is_date = req.kind == AggReq::DateHistogram;
-  for (uint32_t k = 0; k < n.num_buckets; k++) {
-    uint64_t cell = parent_cell * n.num_buckets + k;
-    uint64_t cnt = base[cell].count;
-    if (cnt == 0 && req.kind != AggReq::Range) continue;
-    IBucket bk;
-    bk.count = cnt;
-    if (req.kind == AggReq::Terms) bk.key = term_key(c, b, n, k);
-    else if (req.kind == AggReq::Range) bk.hkey = (double)k;
-    else bk.hkey = (double)(n.base_pos + (int64_t)k) * n.interval + n.offset;
-    bk.subs = build_children(c, ni, cell);
-    a.buckets.push_back(std::move(bk));
-  }
+  return a;
+}
+
+// per-split cut of a terms node to segment_size (cut_off_buckets): error bound = doc count of the first dropped
+// bucket, sum_other = sum of dropped doc counts
+static void cut_terms(const AggReq& req, IAgg& a) {
   if (req.kind == AggReq::Terms && req.order_target.find('.') == std::string::npos &&
       (req.order_target == "_count" || req.order_target == "_key")) {
-    // per-split cut to segment_size (cut_off_buckets): error bound = doc count of the first dropped
-    // bucket, sum_other = sum of dropped doc counts
     sort_term_buckets(req, a.buckets);
     if (a.buckets.size() > req.segment_size) {
       if (req.order_target == "_count" && req.order_desc) a.error_bound = a.buckets[req.segment_size].count;
@@ -515,7 +503,139 @@ static IAgg build_node(const BuildCtx& c, uint32_t ni, uint64_t parent_cell) {
       a.buckets.resize(req.segment_size);
     }
   }
+}
+
+static IAgg build_node(const BuildCtx& c, uint32_t ni, uint64_t parent_cell) {
+  const QwAggNode& n = c.nodes[ni];
+  const AggBinding& b = c.cp.agg_bindings[ni];
+  const AggReq& req = *b.req;
+  const QwAggCell* base = c.cells + c.bases[ni];
+  if (req.is_metric()) return metric_from_cell(c.cp, c.img, c.nodes, ni, base[parent_cell]);
+  IAgg a;
+  a.kind = (uint8_t)req.kind;
+  a.is_date = req.kind == AggReq::DateHistogram;
+  for (uint32_t k = 0; k < n.num_buckets; k++) {
+    uint64_t cell = parent_cell * n.num_buckets + k;
+    uint64_t cnt = base[cell].count;
+    if (cnt == 0 && req.kind != AggReq::Range) continue;
+    IBucket bk;
+    bk.count = cnt;
+    if (req.kind == AggReq::Terms) bk.key = term_key(c.img, b, k, n.has_missing && k == n.num_buckets - 1);
+    else if (req.kind == AggReq::Range) bk.hkey = (double)k;
+    else bk.hkey = (double)(n.base_pos + (int64_t)k) * n.interval + n.offset;
+    bk.subs = build_children(c, ni, cell);
+    a.buckets.push_back(std::move(bk));
+  }
+  cut_terms(req, a);
   return a;
+}
+
+// ---- build from hashed entries (QwAggEntry) --------------------------------------------------------------------
+// The same IAgg tree as build_node gives for the equivalent dense cells: buckets in dense order (terms by raw key
+// with `missing` last, histograms by position, every range in request order, empty ones included).
+struct EntryCtx {
+  const CompiledPlan& cp;
+  const ImageView& img;
+  const QwAggNode* nodes;
+  const QwAggEntry* entries;
+  std::map<std::pair<uint32_t, uint32_t>, std::vector<uint32_t>> kids;  // (parent entry, node) -> entries
+};
+static const uint32_t kNoEntry = 0xFFFFFFFEu;  // the parent of an empty range bucket: has no entries below it
+
+static IAgg build_node_e(const EntryCtx& c, uint32_t ni, uint32_t parent) {
+  const QwAggNode& n = c.nodes[ni];
+  const AggBinding& b = c.cp.agg_bindings[ni];
+  const AggReq& req = *b.req;
+  static const std::vector<uint32_t> none;
+  auto it = c.kids.find({parent, ni});
+  const std::vector<uint32_t>& es = it == c.kids.end() ? none : it->second;
+  if (req.is_metric()) {
+    QwAggCell empty = {0, 0, ~0ull, 0};
+    return metric_from_cell(c.cp, c.img, c.nodes, ni, es.empty() ? empty : c.entries[es[0]].cell);
+  }
+  auto subs = [&](uint32_t e) {
+    std::vector<IAgg> out;
+    for (uint32_t k = 0; k < n.num_children; k++) out.push_back(build_node_e(c, n.first_child + k, e));
+    return out;
+  };
+  IAgg a;
+  a.kind = (uint8_t)req.kind;
+  a.is_date = req.kind == AggReq::DateHistogram;
+  if (req.kind == AggReq::Range) {
+    for (uint32_t k = 0; k < n.num_ranges; k++) {
+      uint32_t e = kNoEntry;
+      for (uint32_t x : es) if (c.entries[x].key == k) e = x;
+      IBucket bk;
+      bk.count = e == kNoEntry ? 0 : c.entries[e].cell.count;
+      bk.hkey = (double)k;
+      bk.subs = subs(e);
+      a.buckets.push_back(std::move(bk));
+    }
+    return a;
+  }
+  std::vector<uint32_t> order(es);
+  std::sort(order.begin(), order.end(), [&](uint32_t x, uint32_t y) {
+    const QwAggEntry &p = c.entries[x], &q = c.entries[y];
+    const bool pm = p.flags & QW_AGG_ENTRY_MISSING, qm = q.flags & QW_AGG_ENTRY_MISSING;
+    return pm != qm ? qm : p.key < q.key;
+  });
+  for (uint32_t e : order) {
+    const QwAggEntry& x = c.entries[e];
+    if (x.cell.count == 0) continue;
+    IBucket bk;
+    bk.count = x.cell.count;
+    if (req.kind == AggReq::Terms) bk.key = term_key(c.img, b, x.key, (x.flags & QW_AGG_ENTRY_MISSING) != 0);
+    else bk.hkey = (double)(n.base_pos + (int64_t)x.key) * n.interval + n.offset;
+    bk.subs = subs(e);
+    a.buckets.push_back(std::move(bk));
+  }
+  cut_terms(req, a);
+  return a;
+}
+
+static std::vector<IAgg> build_top_entries(const CompiledPlan& cp, const ImageView& img, const QwAggEntry* entries, size_t nentries) {
+  const QwPlanHeader& h = cp.header;
+  const QwAggNode* nodes = (const QwAggNode*)(cp.bytes.data() + sizeof(QwPlanHeader) + (size_t)h.num_nodes * sizeof(QwPlanNode));
+  EntryCtx c{cp, img, nodes, entries, {}};
+  // entries come from the caller: every one must name a bucket of its node's key space, once, under its parent
+  std::set<std::tuple<uint32_t, uint32_t, uint64_t, uint32_t>> seen;
+  for (size_t e = 0; e < nentries; e++) {
+    const QwAggEntry& x = entries[e];
+    if (x.node >= h.num_aggs || (x.parent != QW_AGG_NO_PARENT && (x.parent >= nentries || entries[x.parent].node != nodes[x.node].parent)) ||
+        (x.parent == QW_AGG_NO_PARENT && nodes[x.node].parent != 0xFFFFFFFFu))
+      fail(QWGPU_EINVALID_ARG, "aggregation entry %zu does not match the plan's tree", e);
+    const QwAggNode& n = nodes[x.node];
+    const AggBinding& b = cp.agg_bindings[x.node];
+    bool ok = x.flags == 0 || (n.kind == QW_AGG_TERMS && x.flags == QW_AGG_ENTRY_MISSING);
+    if (ok && (x.flags & QW_AGG_ENTRY_MISSING)) ok = n.has_missing && x.key == 0;
+    else if (ok) {
+      switch (n.kind) {
+        case QW_AGG_STATS: ok = x.key == 0; break;
+        case QW_AGG_HISTOGRAM: ok = x.key < n.num_buckets; break;
+        case QW_AGG_RANGE: ok = x.key < n.num_ranges; break;
+        case QW_AGG_TERMS: {
+          ok = b.column >= 0 && img.columns[b.column].num_vals > 0 && img.columns[b.column].gcd &&
+               x.key <= (img.columns[b.column].max_value - img.columns[b.column].min_value) / img.columns[b.column].gcd;
+          const QwImgColumn& col = img.columns[b.column >= 0 ? b.column : 0];
+          if (ok && col.type == QW_COL_STR) ok = col.min_value + col.gcd * x.key < col.dict_num_terms;
+          break;
+        }
+        default: ok = false;
+      }
+    }
+    if (!ok) fail(QWGPU_EINVALID_ARG, "aggregation entry %zu: key %llu (flags %u) is not a bucket of node %u", e, (unsigned long long)x.key, x.flags, x.node);
+    if (!seen.insert(std::make_tuple(x.parent, x.node, x.key, x.flags)).second)
+      fail(QWGPU_EINVALID_ARG, "aggregation entry %zu repeats a bucket of node %u under the same parent", e, x.node);
+    c.kids[{x.parent, x.node}].push_back((uint32_t)e);
+  }
+  std::vector<IAgg> top;
+  for (uint32_t i = 0; i < h.num_aggs; i++) if (nodes[i].parent == 0xFFFFFFFFu) top.push_back(build_node_e(c, i, QW_AGG_NO_PARENT));
+  return top;
+}
+
+std::string build_intermediate_aggs_entries(const CompiledPlan& cp, const ImageView& img, const QwAggEntry* entries, size_t nentries) {
+  if (is_trace_ids_request(cp.agg_request)) fail(QWGPU_EINVALID_ARG, "find_trace_ids results are not given as entries");
+  return ser_top(build_top_entries(cp, img, entries, nentries));
 }
 
 // ---- find_trace_ids: spans, postcard bytes, merge_segment_fruits -----------------------------------------------
@@ -688,7 +808,7 @@ std::string build_and_merge_intermediate_aggs(const std::vector<AggReq>& reqs, c
   }
   std::vector<IAgg> acc;
   for (const SplitAggCells& sp : splits) {
-    std::vector<IAgg> top = build_top(*sp.plan, *sp.img, sp.cells, sp.ncells);
+    std::vector<IAgg> top = sp.hashed ? build_top_entries(*sp.plan, *sp.img, sp.entries, sp.nentries) : build_top(*sp.plan, *sp.img, sp.cells, sp.ncells);
     if (acc.empty() && !top.empty()) {
       // same normalisation as a serialise / parse round trip would apply: none needed — the first
       // split's tree becomes the accumulator

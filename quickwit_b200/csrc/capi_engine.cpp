@@ -121,6 +121,11 @@ int qwgpu_split_search(qwgpu_ctx* ctx, uint32_t num_splits, const char* const* s
       r.agg_cells = (QwAggCell*)malloc(outs[i].cells.size() * sizeof(QwAggCell));
       memcpy(r.agg_cells, outs[i].cells.data(), outs[i].cells.size() * sizeof(QwAggCell));
     }
+    r.num_agg_entries = (uint32_t)outs[i].entries.size();
+    if (!outs[i].entries.empty()) {
+      r.agg_entries = (QwAggEntry*)malloc(outs[i].entries.size() * sizeof(QwAggEntry));
+      memcpy(r.agg_entries, outs[i].entries.data(), outs[i].entries.size() * sizeof(QwAggEntry));
+    }
     r.gpu_time_us = st.gpu_time_us;
     r.main_kernel_us = st.main_kernel_us;
     r.num_kernel_launches = st.launches;
@@ -142,8 +147,10 @@ void qwgpu_split_result_free(qwgpu_split_result* r) {
   if (!r) return;
   free(r->hits);
   free(r->agg_cells);
+  free(r->agg_entries);
   r->hits = nullptr;
   r->agg_cells = nullptr;
+  r->agg_entries = nullptr;
 }
 
 }  // extern "C"

@@ -89,12 +89,17 @@ CompiledPlan compile_plan(const ImageView& img, const std::string& split_id, con
 // postcard-style byte layout — the reference layout is a tantivy-internal struct, SURVEY.md §7 hard
 // part iv) -----------------------------------------------------------------------------------------------
 std::string build_intermediate_aggs(const CompiledPlan& cp, const ImageView& img, const QwAggCell* cells, size_t ncells);
+// the same from the entries of the hashed layout (QwAggEntry; any plan's tree can be given this way)
+std::string build_intermediate_aggs_entries(const CompiledPlan& cp, const ImageView& img, const QwAggEntry* entries, size_t nentries);
 std::string merge_intermediate_aggs(const std::vector<AggReq>& reqs, const std::vector<std::string>& parts);
 struct SplitAggCells {
   const CompiledPlan* plan;
   const ImageView* img;
   const QwAggCell* cells;
   size_t ncells;
+  bool hashed = false;  // the split's result is `entries` (hashed layout), not `cells`
+  const QwAggEntry* entries = nullptr;
+  size_t nentries = 0;
 };
 std::string build_and_merge_intermediate_aggs(const std::vector<AggReq>& reqs, const std::vector<SplitAggCells>& splits);
 std::string finalize_aggs_json(const std::vector<AggReq>& reqs, const std::string& intermediate);
@@ -103,7 +108,8 @@ std::string finalize_aggs_json(const std::vector<AggReq>& reqs, const std::strin
 // SegmentPartialHit::into_partial_hit (collector.rs:493-521): QwHit -> PartialHit with typed sort values
 pb::LeafSearchResponse build_split_response(const CompiledPlan& cp, const ImageView& img, const std::string& split_id,
                                             uint64_t num_hits, const QwHit* hits, size_t nhits,
-                                            const QwAggCell* cells, size_t ncells);
+                                            const QwAggCell* cells, size_t ncells,
+                                            const QwAggEntry* entries = nullptr, size_t nentries = 0, bool hashed = false);
 // merge_leaf_responses + merge_fruits truncation (collector.rs:832-974)
 pb::LeafSearchResponse merge_responses(const pb::SearchRequest& req, std::vector<pb::LeafSearchResponse> parts);
 

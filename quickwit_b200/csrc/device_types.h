@@ -154,8 +154,24 @@ struct DSplitPlan {
   uint32_t tr_on, tr_n;    // N = num_traces
   uint32_t tr_num_ords;    // entries of tr_best (the column dictionary's size, at least 1)
   uint32_t tr_ord_col, tr_ts_col;  // DCol indices of the trace-id and timestamp columns (ts: 0xFFFFFFFF = absent)
-  uint32_t tr_pad[3];
+  // hashed aggregation cells (qw_agg_hashed; kernels.cuh agg_collect_hashed); hashed == 0 for dense plans
+  uint32_t hashed;
+  uint32_t h_cap;          // cell capacity of this run
+  uint32_t h_mask;         // table slots - 1 (slots: a power of two >= h_cap)
+  uint64_t h_table;        // device address of uint32[slots]: cell id, QW_HSLOT_EMPTY / _BUSY / _FULL
+  uint64_t h_keys;         // device address of DHKey[h_cap]
+  uint64_t h_cells;        // device address of QwAggCell[h_cap]
+  uint64_t h_ctr;          // device address of a uint32 in the split's output header: cells claimed | overflow << 31
 };
+// key record of a hashed cell (the rest of its QwAggEntry)
+struct DHKey {
+  uint64_t key;
+  uint32_t node_flags;  // node | QwAggEntry.flags << 8
+  uint32_t parent;
+};
+#define QW_HSLOT_EMPTY 0xFFFFFFFFu
+#define QW_HSLOT_BUSY 0xFFFFFFFEu
+#define QW_HSLOT_FULL 0xFFFFFFFDu
 
 static_assert(offsetof(DSplitPlan, key) % 16 == 0 && sizeof(DSplitPlan) % 16 == 0, "DKeySpec is read as uint4");
 

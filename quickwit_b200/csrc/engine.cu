@@ -55,7 +55,7 @@ struct CallSlot {
     }
     if (scratch > scratch_cap) {
       if (d_scratch) cudaFree(d_scratch);
-      scratch_cap = scratch * 2;
+      scratch_cap = scratch <= ((size_t)1 << 30) ? scratch * 2 : scratch;  // (no headroom for the rare huge call)
       CUDA_CHECK(cudaMalloc(&d_scratch, scratch_cap));
     }
     if (out > out_cap) {
@@ -98,6 +98,7 @@ Engine::Engine(int dev) : device(dev) {
   max_smem_optin = (int)prop.sharedMemPerBlockOptin;
   CUDA_CHECK(cudaFuncSetAttribute(qwk::k_window<qwk::MODE_HIST, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem_optin));
   CUDA_CHECK(cudaFuncSetAttribute(qwk::k_window<qwk::MODE_COLLECT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem_optin));
+  CUDA_CHECK(cudaFuncSetAttribute(qwk::k_window<qwk::MODE_COLLECT, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem_optin));
   CUDA_CHECK(cudaFuncSetAttribute(qwk::k_window<qwk::MODE_COLLECT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem_optin));
   CUDA_CHECK(cudaFuncSetAttribute(qwk::k_window<qwk::MODE_HIST, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem_optin));
   CUDA_CHECK(cudaFuncSetAttribute(qwk::k_union<qwk::MODE_HIST>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem_optin));
@@ -313,9 +314,55 @@ uint64_t agg_cell_layout(const QwAggNode* aggs, uint32_t n, std::vector<uint32_t
     while (p != 0xFFFFFFFFu) { cells *= aggs[p].num_buckets; p = aggs[p].parent; }
     if (bases) (*bases)[i] = (uint32_t)total;
     total += cells;
-    if (total > (1ull << 26)) fail(QWGPU_EINVALID_AGG, "aggregation bucket space too large (%llu cells)", (unsigned long long)total);
+    if (total > QW_AGG_DENSE_MAX_CELLS) fail(QWGPU_EINVALID_AGG, "aggregation bucket space too large (%llu cells)", (unsigned long long)total);
   }
   return total;
+}
+
+// Hashed layout: a cell exists per (node, parent cell, key) that some (doc, value path) reaches, so a node has at
+// most min(its dense cells, the (doc, value path) tuples of its bucket chain) cells. A chain of single-valued
+// columns gives at most one path per doc; a multi-valued level multiplies by that column's value count (Σ_d Π v_l(d)
+// <= Π Σ_d v_l(d)), a `missing` bucket adds one value per doc, a range node every range.
+static uint64_t sat_mul(uint64_t a, uint64_t b) {
+  const uint64_t lim = 1ull << 62;
+  return (b && a > lim / b) ? lim : std::min(a * b, lim);
+}
+uint64_t agg_hashed_bound(const QwAggNode* aggs, uint32_t n, const ImageView& img) {
+  const uint64_t num_docs = img.hdr->num_docs;
+  uint64_t total = 0;
+  for (uint32_t i = 0; i < n; i++) {
+    uint64_t dense = 1, reps = 1, multi = 1;
+    bool any_multi = false;
+    uint32_t depth = 0;
+    for (uint32_t b = aggs[i].kind == QW_AGG_STATS ? aggs[i].parent : i; b != 0xFFFFFFFFu && depth <= n; b = aggs[b].parent, depth++) {
+      const QwAggNode& g = aggs[b];
+      dense = sat_mul(dense, g.num_buckets);
+      if (g.kind == QW_AGG_RANGE) reps = sat_mul(reps, g.num_ranges);
+      if (g.column < img.hdr->num_columns && img.columns[g.column].cardinality == QW_CARD_MULTI) {
+        any_multi = true;
+        multi = sat_mul(multi, img.columns[g.column].num_vals + (g.kind == QW_AGG_TERMS && g.has_missing ? num_docs : 0));
+      }
+    }
+    total = std::min<uint64_t>(total + std::min(dense, sat_mul(any_multi ? multi : num_docs, reps)), 1ull << 62);
+  }
+  return total;
+}
+uint32_t agg_hashed_slots(uint64_t cap) {
+  uint64_t slots = 2;
+  while (slots < 2 * cap) slots <<= 1;  // load factor <= 1/2: short probe sequences
+  return (uint32_t)std::min<uint64_t>(slots, 1ull << 31);
+}
+uint64_t agg_hashed_table_bytes(uint64_t cap) {
+  const uint64_t slots = agg_hashed_slots(cap);
+  return slots * 4 + cap * (sizeof(DHKey) + sizeof(QwAggCell));
+}
+uint64_t agg_hashed_layout(const QwAggNode* aggs, uint32_t n, const ImageView& img, const char* split_id) {
+  const uint64_t bound = std::max<uint64_t>(agg_hashed_bound(aggs, n, img), 1);
+  const uint64_t bytes = bound >= (1ull << 30) ? ~0ull : agg_hashed_table_bytes(bound);
+  if (bytes > QWGPU_HASHED_MAX_BYTES)
+    fail(QWGPU_EUNSUPPORTED, "split `%s`: the aggregation may create up to %llu buckets, whose hashed table exceeds the GPU limit of %llu bytes per call",
+         split_id, (unsigned long long)bound, (unsigned long long)QWGPU_HASHED_MAX_BYTES);
+  return bound;
 }
 
 // ---- lowering: QwPlan tree -> window-engine program ----------------------------------------------
@@ -347,6 +394,7 @@ struct Lowered {
   std::vector<uint32_t> phrase_instr;   // instruction that consumes phrases[i]
   std::vector<DPhraseTerm> phrase_exp;  // expansions of the phrase prefixes (phrases[i].exp indexes it until staging)
   uint32_t tr_img_col = 0;              // find_trace_ids: the trace-id column of the image
+  uint64_t h_bound = 0;                 // hashed aggregation layout: upper bound on the split's distinct cells
 };
 
 static uint32_t use_col(Lowered& L, const SplitDev& sp, uint32_t c) {
@@ -706,9 +754,15 @@ static void lower_plan(Lowered& L, const SplitDev& sp, const uint8_t* plan, size
   else ks.top_mode = QW_TOP_FULL;
   // aggregations
   if (ph->num_aggs > QW_MAX_DAGGS) fail(QWGPU_EUNSUPPORTED, "more than %d aggregation nodes", QW_MAX_DAGGS);
-  std::vector<uint32_t> bases;
-  uint64_t ncells = agg_cell_layout(aggs, ph->num_aggs, &bases);
-  P.n_cells = (uint32_t)ncells;
+  for (uint32_t i = 0; i < ph->num_aggs; i++) {
+    uint32_t depth = 0;
+    for (uint32_t p = aggs[i].parent; p != 0xFFFFFFFFu; p = aggs[p].parent)
+      if (p >= ph->num_aggs || ++depth > ph->num_aggs) fail(QWGPU_EINVALID_ARG, "aggregation parent out of range");
+  }
+  std::vector<uint32_t> bases(ph->num_aggs, 0);
+  P.hashed = qw_agg_hashed(aggs, ph->num_aggs) ? 1u : 0u;
+  if (P.hashed) L.h_bound = agg_hashed_layout(aggs, ph->num_aggs, sp.view, sp.id.c_str());
+  else P.n_cells = (uint32_t)agg_cell_layout(aggs, ph->num_aggs, &bases);
   for (uint32_t i = 0; i < ph->num_aggs; i++) {
     const QwAggNode& a = aggs[i];
     DAgg d;
@@ -720,13 +774,7 @@ static void lower_plan(Lowered& L, const SplitDev& sp, const uint8_t* plan, size
     d.base_pos = a.base_pos;
     memcpy(d.range_from, a.range_from, sizeof d.range_from);
     memcpy(d.range_to, a.range_to, sizeof d.range_to);
-    if (a.parent != 0xFFFFFFFFu) {
-      if (a.parent >= ph->num_aggs) fail(QWGPU_EINVALID_ARG, "aggregation parent out of range");
-      uint32_t depth = 1, p = a.parent;
-      while (aggs[p].parent != 0xFFFFFFFFu) { depth++; p = aggs[p].parent; }
-      if (depth > 2 || (depth == 2 && a.kind != QW_AGG_STATS)) fail(QWGPU_EUNSUPPORTED, "aggregation nesting deeper than bucket -> bucket -> metric");
-      if (aggs[a.parent].kind == QW_AGG_STATS) fail(QWGPU_EINVALID_AGG, "metric aggregations cannot have sub-aggregations");
-    }
+    if (a.parent != 0xFFFFFFFFu && aggs[a.parent].kind == QW_AGG_STATS) fail(QWGPU_EINVALID_AGG, "metric aggregations cannot have sub-aggregations");
     if (a.kind == QW_AGG_RANGE && a.num_ranges > QW_MAX_AGG_RANGES) fail(QWGPU_EUNSUPPORTED, "more than %d ranges", QW_MAX_AGG_RANGES);
     L.aggs.push_back(d);
   }
@@ -758,7 +806,7 @@ static void lower_plan(Lowered& L, const SplitDev& sp, const uint8_t* plan, size
   // columns. Histogram buckets are located through a raw-space boundary table built here with the
   // reference formula (agg_bucket in kernels.cuh == tantivy's ((val - offset) / interval).floor()),
   // which is monotone in the raw value.
-  bool fast = ph->num_aggs > 0;
+  bool fast = ph->num_aggs > 0 && !P.hashed;
   P.n_stat_cells = 0;
   for (DAgg& d : L.aggs) {
     const bool full_col = d.col != 0xFFFFFFFFu && L.cols[d.col].card == QW_CARD_FULL;
@@ -883,9 +931,10 @@ static qwk::USmem make_union_layout(uint32_t W, bool hist, uint32_t budget) {
   return L;
 }
 
-void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std::vector<const uint8_t*>& plans,
-                    const std::vector<size_t>& plan_lens, std::vector<SplitOutput>& outs, BatchStats& stats,
-                    const MergeSpec* merge, std::vector<MergedHit>* merged, const GatherSpec* gather, std::vector<RankHeader>* rank_headers) {
+bool Engine::search_once(const std::vector<std::shared_ptr<SplitDev>>& sp, const std::vector<const uint8_t*>& plans,
+                         const std::vector<size_t>& plan_lens, std::vector<SplitOutput>& outs, BatchStats& stats,
+                         const MergeSpec* merge, std::vector<MergedHit>* merged, const GatherSpec* gather,
+                         std::vector<RankHeader>* rank_headers, bool at_bound) {
   const uint32_t n_in = (uint32_t)sp.size();
   outs.assign(n_in, SplitOutput());
   static const bool trace = getenv("QWGPU_TRACE") != nullptr;  // host phase timings on stderr
@@ -906,6 +955,30 @@ void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std:
     } catch (const Error& e) {
       outs[i].status = e.code;
       outs[i].error = e.what();
+    }
+  }
+  {
+    // a re-run after an overflow sizes every hashed table of the call at its bound: the call's tables together must
+    // fit QWGPU_HASHED_MAX_BYTES, else every hashed split of the call fails here, before any launch
+    uint64_t total = 0;
+    uint32_t n_hashed = 0;
+    for (const Lowered& L : low)
+      if (L.P.hashed) { total += agg_hashed_table_bytes(L.h_bound); n_hashed++; }
+    if (total > QWGPU_HASHED_MAX_BYTES) {
+      std::vector<Lowered> keep;
+      std::vector<uint32_t> keep_idx;
+      for (size_t k = 0; k < low.size(); k++) {
+        if (!low[k].P.hashed) { keep.push_back(std::move(low[k])); keep_idx.push_back(idx[k]); continue; }
+        char msg[512];
+        snprintf(msg, sizeof msg, "split `%s`: the aggregation may create up to %llu buckets; the hashed tables of the call's %u "
+                 "hashed splits need %llu bytes at their bounds, more than the GPU limit of %llu bytes per call",
+                 sp[idx[k]]->id.c_str(), (unsigned long long)low[k].h_bound, n_hashed, (unsigned long long)total,
+                 (unsigned long long)QWGPU_HASHED_MAX_BYTES);
+        outs[idx[k]].status = QWGPU_EUNSUPPORTED;
+        outs[idx[k]].error = msg;
+      }
+      low.swap(keep);
+      idx.swap(keep_idx);
     }
   }
   const uint32_t n = (uint32_t)low.size();
@@ -942,7 +1015,7 @@ void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std:
       cudaStreamDestroy(st0);
       cudaFree(d);
     }
-    return;
+    return true;
   }
   const auto t_lowered = tclock::now();
 
@@ -1163,7 +1236,21 @@ void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std:
     any_trace |= P.tr_on != 0;
   }
   const size_t s_trace_state = s_trace, s_trace_data = al(s_trace + (any_trace ? (size_t)n * sizeof(qwk::DTraceState) : 0));
-  const size_t scratch_bytes = al(s_trace_data + tr_off[n]);
+  // hashed aggregation cells: per split [slot table][key records][cells], at min(bound, QWGPU_HASHED_INIT_CELLS)
+  // cells, or at the bound when the batch runs again after an overflow
+  const size_t s_hash = al(s_trace_data + tr_off[n]);
+  std::vector<size_t> h_off(n + 1, 0);
+  bool any_hashed = false;
+  for (uint32_t i = 0; i < n; i++) {
+    DSplitPlan& P = low[i].P;
+    if (P.hashed) {
+      any_hashed = true;
+      P.h_cap = (uint32_t)(at_bound ? low[i].h_bound : std::min<uint64_t>(low[i].h_bound, QWGPU_HASHED_INIT_CELLS));
+      P.h_mask = agg_hashed_slots(P.h_cap) - 1;
+    }
+    h_off[i + 1] = h_off[i] + (P.hashed ? al((size_t)(P.h_mask + 1) * 4) + al((size_t)P.h_cap * sizeof(DHKey)) + al((size_t)P.h_cap * sizeof(QwAggCell)) : 0);
+  }
+  const size_t scratch_bytes = al(s_hash + h_off[n]);
   // out: per split [hdr 32B][hits][cells]
   std::vector<size_t> out_off(n + 1);
   out_off[0] = 0;
@@ -1263,6 +1350,12 @@ void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std:
       P.tr_best = (uint64_t)(slot->d_scratch + s_trace_data + tr_off[i]);
       P.tr_match = P.tr_best + al((size_t)P.tr_num_ords * 8);
       P.tr_tie = (uint64_t)(ob + 24);
+    }
+    if (P.hashed) {
+      P.h_table = (uint64_t)(slot->d_scratch + s_hash + h_off[i]);
+      P.h_keys = P.h_table + al((size_t)(P.h_mask + 1) * 4);
+      P.h_cells = P.h_keys + al((size_t)P.h_cap * sizeof(DHKey));
+      P.h_ctr = (uint64_t)(ob + 28);
     }
     for (size_t k = 0; k < low[i].phrases.size(); k++) {
       DPhrase& ph = low[i].phrases[k];
@@ -1399,11 +1492,13 @@ void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std:
     if (mode == qwk::MODE_HIST && all_union && old_union && level == 0 && !use_prefix) qwk::k_window<qwk::MODE_HIST, true><<<grid, QW_THREADS, lay.total, st>>>(q);
     else if (mode == qwk::MODE_HIST) qwk::k_window<qwk::MODE_HIST, false><<<grid, QW_THREADS, lay.total, st>>>(q);
     else if (all_union && old_union) qwk::k_window<qwk::MODE_COLLECT, true><<<grid, QW_THREADS, lay.total, st>>>(q);
+    else if (any_hashed) qwk::k_window<qwk::MODE_COLLECT, false, true><<<grid, QW_THREADS, lay.total, st>>>(q);
     else qwk::k_window<qwk::MODE_COLLECT, false><<<grid, QW_THREADS, lay.total, st>>>(q);
     stats.launches++;
     stats.kernel_mask |= QWGPU_KERNEL_WINDOW;
     // (k_window aggregates on the fast path where the plan's and the launch's flags both allow it)
     if (mode == qwk::MODE_COLLECT && !(flags & F_CANDS_ONLY) && any_fast_aggs && kp.smem_aggs) stats.kernel_mask |= QWGPU_KERNEL_FAST_AGGS;
+    if (mode == qwk::MODE_COLLECT && !(flags & F_CANDS_ONLY) && any_hashed) stats.kernel_mask |= QWGPU_KERNEL_HASHED_AGGS;
   };
   const uint32_t sel_smem = 3 * 8 * QW_CAND_CAP;  // [all first words | 3 x QW_SEL_MAX survivors] or 3 x all (degenerate ties)
   uint32_t tie_max_n = 0;
@@ -1414,6 +1509,13 @@ void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std:
       CUDA_CHECK(cudaMemsetAsync(slot->d_scratch + s_trace_state, 0xFF, (size_t)n * sizeof(qwk::DTraceState), st));
       CUDA_CHECK(cudaMemsetAsync(slot->d_scratch + s_trace_data, 0, tr_off[n], st));
     }
+    if (any_hashed && !(flags & F_CANDS_ONLY))
+      for (uint32_t i = 0; i < n; i++) {
+        const DSplitPlan& P = low[i].P;
+        if (!P.hashed) continue;
+        CUDA_CHECK(cudaMemsetAsync((void*)P.h_table, 0xFF, (size_t)(P.h_mask + 1) * 4, st));
+        CUDA_CHECK(cudaMemsetAsync((void*)P.h_cells, 0, (size_t)P.h_cap * sizeof(QwAggCell), st));
+      }
     CUDA_CHECK(cudaEventRecord(slot->ev2, st));
     launch_window(qwk::MODE_COLLECT, false, 0, 0, flags);
     CUDA_CHECK(cudaEventRecord(slot->ev3, st));
@@ -1539,6 +1641,35 @@ void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std:
     wait_stream();
     if (!verify()) fail(QWGPU_EINTERNAL, "top-K candidate selection failed verification");
   }
+  // hashed cells: a split that outgrew its capacity sends the batch round again at the bound (before any
+  // cross-rank collective, which must run once); otherwise only the used cells come back
+  std::vector<std::vector<DHKey>> h_keys(n);
+  std::vector<std::vector<QwAggCell>> h_cells(n);
+  if (any_hashed) {
+    bool overflow = false;
+    for (uint32_t i = 0; i < n; i++)
+      if (low[i].P.hashed && (*(const uint32_t*)(slot->h_out + out_off[i] + 28) >> 31)) overflow = true;
+    if (overflow) {
+      if (at_bound) fail(QWGPU_EINTERNAL, "hashed aggregation cells overflowed their bound");
+      float ms = 0;
+      cudaEventElapsedTime(&ms, slot->ev0, slot->ev1);
+      stats.gpu_time_us += ms * 1000.f;
+      add_main();
+      return false;
+    }
+    for (uint32_t i = 0; i < n; i++) {
+      const DSplitPlan& P = low[i].P;
+      if (!P.hashed) continue;
+      const uint32_t used = std::min(*(const uint32_t*)(slot->h_out + out_off[i] + 28), P.h_cap);
+      h_keys[i].resize(used);
+      h_cells[i].resize(used);
+      if (!used) continue;
+      CUDA_CHECK(cudaMemcpyAsync(h_keys[i].data(), (const void*)P.h_keys, (size_t)used * sizeof(DHKey), cudaMemcpyDeviceToHost, st));
+      CUDA_CHECK(cudaMemcpyAsync(h_cells[i].data(), (const void*)P.h_cells, (size_t)used * sizeof(QwAggCell), cudaMemcpyDeviceToHost, st));
+      stats.d2h_bytes += (size_t)used * (sizeof(DHKey) + sizeof(QwAggCell));
+    }
+    wait_stream();
+  }
   if (do_gather) {
     // Cross-rank phase, after this rank's result is final (a verification fallback above must not repeat a
     // collective the other ranks run once): the rank's record -> every rank (one NCCL all-gather on this
@@ -1584,6 +1715,20 @@ void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std:
     const QwAggCell* c = (const QwAggCell*)(ob + 32 + (do_merge ? 0 : (size_t)P.max_hits * sizeof(QwHit)));
     o.cells.assign(c, c + P.n_cells);
     for (auto& cell : o.cells) cell.min_mapped = ~cell.min_mapped;  // device keeps max(~m); see agg_stats
+    if (P.hashed) {
+      o.hashed = true;
+      o.entries.resize(h_keys[i].size());
+      for (size_t e = 0; e < o.entries.size(); e++) {
+        QwAggEntry& x = o.entries[e];
+        x.node = h_keys[i][e].node_flags & 0xFFu;
+        x.flags = h_keys[i][e].node_flags >> 8;
+        x.parent = h_keys[i][e].parent;
+        x.key = h_keys[i][e].key;
+        x.reserved = 0;
+        x.cell = h_cells[i][e];
+        x.cell.min_mapped = ~x.cell.min_mapped;
+      }
+    }
     if (P.tr_on) {
       if (*(const uint32_t*)(ob + 24)) stats.kernel_mask |= QWGPU_KERNEL_TRACE_REPLAY;
       // a matched doc without a trace id reads ordinal 0: with an empty dictionary the reference's ord_to_bytes fails
@@ -1644,6 +1789,17 @@ void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std:
     fprintf(stderr, "[qwgpu] search: lower %ld us, stage %ld us, launch+wait %ld us (device %.0f us), unpack %ld us\n", us(t_begin, t_lowered),
             us(t_lowered, t_staged), us(t_staged, t_searched), stats.gpu_time_us, us(t_searched, tclock::now()));
   }
+  return true;
+}
+
+void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std::vector<const uint8_t*>& plans,
+                    const std::vector<size_t>& plan_lens, std::vector<SplitOutput>& outs, BatchStats& stats,
+                    const MergeSpec* merge, std::vector<MergedHit>* merged, const GatherSpec* gather, std::vector<RankHeader>* rank_headers) {
+  if (search_once(sp, plans, plan_lens, outs, stats, merge, merged, gather, rank_headers, false)) return;
+  // a split's hashed aggregation cells outgrew QWGPU_HASHED_INIT_CELLS: the batch runs again with every hashed
+  // split's table at its bound, where it cannot overflow (the first run's device time stays in the stats)
+  stats.kernel_mask |= QWGPU_KERNEL_HASHED_AGGS_RETRY;
+  search_once(sp, plans, plan_lens, outs, stats, merge, merged, gather, rank_headers, true);
 }
 
 }  // namespace qw

@@ -34,6 +34,8 @@ struct SplitOutput {
   uint64_t num_hits = 0;
   std::vector<QwHit> hits;
   std::vector<QwAggCell> cells;
+  bool hashed = false;              // the plan took the hashed layout: `entries` holds its result, `cells` is empty
+  std::vector<QwAggEntry> entries;
   int status = 0;
   std::string error;
   uint64_t postings_scored = 0;
@@ -117,10 +119,21 @@ struct Engine {
               const std::vector<size_t>& plan_lens, std::vector<SplitOutput>& outs, BatchStats& stats,
               const MergeSpec* merge = nullptr, std::vector<MergedHit>* merged = nullptr,
               const GatherSpec* gather = nullptr, std::vector<RankHeader>* rank_headers = nullptr);
+  // one run of the batch; false (nothing returned yet) when a split's hashed aggregation cells overflowed their
+  // initial capacity. at_bound: every hashed split's table is sized at its bound.
+  bool search_once(const std::vector<std::shared_ptr<SplitDev>>& sp, const std::vector<const uint8_t*>& plans,
+                   const std::vector<size_t>& plan_lens, std::vector<SplitOutput>& outs, BatchStats& stats,
+                   const MergeSpec* merge, std::vector<MergedHit>* merged, const GatherSpec* gather,
+                   std::vector<RankHeader>* rank_headers, bool at_bound);
 };
 
 // plan validation helper shared with the compiler: total agg cells + per-node bases
 uint64_t agg_cell_layout(const QwAggNode* aggs, uint32_t n, std::vector<uint32_t>* bases);
+// hashed layout: guaranteed upper bound on a split's distinct cells, and the device bytes of a table of `cap`
+// cells; agg_hashed_layout fails with QWGPU_EUNSUPPORTED when the table at the bound exceeds QWGPU_HASHED_MAX_BYTES
+uint64_t agg_hashed_bound(const QwAggNode* aggs, uint32_t n, const ImageView& img);
+uint64_t agg_hashed_table_bytes(uint64_t cap);
+uint64_t agg_hashed_layout(const QwAggNode* aggs, uint32_t n, const ImageView& img, const char* split_id);
 
 }  // namespace qw
 

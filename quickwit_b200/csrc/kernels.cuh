@@ -707,6 +707,152 @@ __device__ void agg_collect_doc(const KParams& p, const Sm& sm, const DSplitPlan
   }
 }
 
+// ---- hashed aggregation cells (DSplitPlan::hashed, DESIGN.md §4.4) ------------------------------------------
+// One open-addressing table per split: slot -> cell id, ids handed out by the split's counter, key records and
+// QwAggCells indexed by id. A lane claims an empty slot with atomicCAS (EMPTY -> BUSY), takes an id, writes the
+// key record and publishes the id (fence, then release by atomicExch); readers load slots with ld.acquire before
+// they read a key record, and lanes meeting a BUSY slot wait for the id. Past the capacity the slot is marked FULL
+// (skipped by every probe) and the overflow bit is set: the engine runs the batch again at the bound, so from then on
+// the pass only has to finish — every lookup and every walk of the split returns at once. The table has at least
+// twice as many slots as ids, so a probe sequence stays short.
+__device__ __forceinline__ uint32_t ld_acquire_u32(const volatile uint32_t* p) {
+  uint32_t v;
+  asm volatile("ld.acquire.gpu.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ bool hcell_overflowed(const DSplitPlan& P) { return (*(const volatile uint32_t*)P.h_ctr) >> 31; }
+__device__ __forceinline__ uint32_t hcell_hash(uint32_t node_flags, uint32_t parent, uint64_t key) {
+  uint64_t h = key * 0x9E3779B97F4A7C15ull ^ ((uint64_t)parent << 32 | node_flags) * 0xC2B2AE3D27D4EB4Full;
+  h ^= h >> 29;
+  h *= 0xBF58476D1CE4E5B9ull;
+  return (uint32_t)(h ^ (h >> 32));
+}
+__device__ uint32_t hcell_find_or_insert(const DSplitPlan& P, uint32_t node_flags, uint32_t parent, uint64_t key) {
+  volatile uint32_t* tab = (volatile uint32_t*)P.h_table;
+  volatile DHKey* keys = (volatile DHKey*)P.h_keys;
+  if (hcell_overflowed(P)) return QW_HSLOT_EMPTY;
+  uint32_t s = hcell_hash(node_flags, parent, key) & P.h_mask;
+  for (uint32_t probe = 0; probe <= P.h_mask; probe++, s = (s + 1) & P.h_mask) {
+    uint32_t v = ld_acquire_u32(&tab[s]);
+    if (v == QW_HSLOT_EMPTY) {
+      if (hcell_overflowed(P)) return QW_HSLOT_EMPTY;
+      v = atomicCAS((uint32_t*)&tab[s], QW_HSLOT_EMPTY, QW_HSLOT_BUSY);
+      if (v != QW_HSLOT_EMPTY) v = ld_acquire_u32(&tab[s]);  // (a slot only moves EMPTY -> BUSY -> id / FULL)
+      else {
+        const uint32_t id = atomicAdd((uint32_t*)P.h_ctr, 1u) & 0x7FFFFFFFu;
+        if (id >= P.h_cap) {
+          atomicOr((uint32_t*)P.h_ctr, 0x80000000u);
+          atomicExch((uint32_t*)&tab[s], QW_HSLOT_FULL);
+          return QW_HSLOT_EMPTY;
+        }
+        keys[id].key = key;
+        keys[id].node_flags = node_flags;
+        keys[id].parent = parent;
+        __threadfence();
+        atomicExch((uint32_t*)&tab[s], id);
+        return id;
+      }
+    }
+    while (v == QW_HSLOT_BUSY) v = ld_acquire_u32(&tab[s]);
+    if (v == QW_HSLOT_FULL) continue;
+    if (keys[v].key == key && keys[v].node_flags == node_flags && keys[v].parent == parent) return v;
+  }
+  atomicOr((uint32_t*)P.h_ctr, 0x80000000u);
+  return QW_HSLOT_EMPTY;
+}
+// Warp-converged: lanes with the same (node, parent, key) find the cell once (their leader probes) and add their
+// doc count with one atomic. Returns the lane's cell id, QW_HSLOT_EMPTY when `on` is false or the table is full.
+__device__ __forceinline__ uint32_t hcell_count(const DSplitPlan& P, uint32_t node_flags, uint32_t parent, uint64_t key, bool on,
+                                                bool count, uint32_t lane) {
+  const uint32_t act = __ballot_sync(QW_FULL, on);
+  if (act == 0) return QW_HSLOT_EMPTY;
+  const uint32_t peers = __match_any_sync(QW_FULL, key) & __match_any_sync(QW_FULL, parent) & __match_any_sync(QW_FULL, node_flags) & act;
+  const uint32_t lead = on ? (uint32_t)__ffs(peers) - 1 : lane;
+  uint32_t id = QW_HSLOT_EMPTY;
+  if (on && lead == lane) {
+    id = hcell_find_or_insert(P, node_flags, parent, key);
+    if (count && id != QW_HSLOT_EMPTY) atomicAdd((unsigned long long*)&((QwAggCell*)P.h_cells)[id].count, (unsigned long long)__popc(peers));
+  }
+  __syncwarp();
+  id = __shfl_sync(QW_FULL, id, lead);
+  return on ? id : QW_HSLOT_EMPTY;
+}
+// Every matched doc walks the tree depth-first, visiting every value of a multi-valued column at every level (the
+// cartesian product, as agg_collect_doc). Loop bounds are warp-uniform; the per-level state lives in local memory
+// (the walk only runs for hashed plans).
+__device__ __forceinline__ void agg_collect_hashed(const DSplitPlan& P, const DAgg* aggs, const DCol* cols, const uint8_t* base,
+                                                uint32_t doc, bool on, uint32_t lane) {
+  // a split whose table overflowed runs again at its bound: the rest of this pass is wasted work
+  if (__shfl_sync(QW_FULL, lane == 0 && hcell_overflowed(P) ? 1u : 0u, 0)) return;
+  QwAggCell* cells = (QwAggCell*)P.h_cells;
+  // per level: node, value loop (k < maxv, r < nrep), next child; per lane: values [a, a + nv), parent cell, own cell
+  uint32_t node[QW_MAX_DAGGS], k[QW_MAX_DAGGS], r[QW_MAX_DAGGS], maxv[QW_MAX_DAGGS], child[QW_MAX_DAGGS];
+  uint64_t a[QW_MAX_DAGGS];
+  uint32_t nv[QW_MAX_DAGGS], parent[QW_MAX_DAGGS], cell[QW_MAX_DAGGS];
+  uint32_t flags = 0;  // per lane, bit d: the lane is live at level d; bit 8 + d: level d is the `missing` bucket
+  for (uint32_t top = 0; top < P.n_aggs; top++) {
+    if (aggs[top].parent != 0xFFFFFFFFu) continue;
+    int d = 0;
+    node[0] = top;
+    parent[0] = QW_AGG_NO_PARENT;
+    flags = on ? 1u : 0u;
+    bool fresh = true;
+    while (d >= 0) {
+      const DAgg& g = aggs[node[d]];
+      const bool live = (flags >> d) & 1u;
+      if (fresh) {
+        fresh = false;
+        if (g.kind == QW_AGG_STATS) {
+          if (g.col != 0xFFFFFFFFu) {
+            uint64_t va = 0, vb = 0;
+            if (live) col_range(base, cols[g.col], doc, va, vb);
+            const uint32_t id = hcell_count(P, node[d], parent[d], 0ull, live && vb > va, false, lane);
+            agg_stats(g, cols[g.col], base, cells, id, doc, id != QW_HSLOT_EMPTY, lane);
+          }
+          d--;
+          continue;
+        }
+        bool missing;
+        nv[d] = agg_values(g, cols, base, doc, live, a[d], missing);
+        flags = (flags & ~(0x100u << d)) | (missing ? 0x100u << d : 0u);
+        maxv[d] = __reduce_max_sync(QW_FULL, nv[d]);
+        k[d] = 0;
+        r[d] = 0;
+        child[d] = QW_HSLOT_EMPTY;  // no cell yet
+      }
+      if (child[d] == QW_HSLOT_EMPTY) {
+        // the cell of the next (value, range) of this level, or leave the level
+        if (k[d] >= maxv[d]) { d--; continue; }
+        const bool missing = (flags >> (8 + d)) & 1u;
+        bool ok = k[d] < nv[d];
+        uint64_t key = 0;
+        if (ok && !missing) {
+          if (g.kind == QW_AGG_TERMS) key = col_raw(base, cols[g.col], a[d] + k[d]);
+          else {
+            uint32_t bk = 0;
+            ok = agg_bucket(g, cols[g.col], base, a[d] + k[d], r[d], bk);
+            key = bk;
+          }
+        }
+        cell[d] = hcell_count(P, node[d] | (missing ? QW_AGG_ENTRY_MISSING << 8 : 0u), parent[d], key, ok, true, lane);
+        child[d] = 0;
+        if (++r[d] >= (g.kind == QW_AGG_RANGE ? g.num_ranges : 1u)) { r[d] = 0; k[d]++; }
+      }
+      if (child[d] < g.num_children) {
+        const uint32_t c = g.first_child + child[d]++;
+        const bool child_live = cell[d] != QW_HSLOT_EMPTY;
+        d++;
+        node[d] = c;
+        parent[d] = cell[d - 1];
+        flags = (flags & ~(1u << d)) | (child_live ? 1u << d : 0u);
+        fresh = true;
+        continue;
+      }
+      child[d] = QW_HSLOT_EMPTY;  // every child visited: next value
+    }
+  }
+}
+
 enum { MODE_HIST = 0, MODE_COLLECT = 1 };
 
 // ---- warp-private helpers (each warp owns the doc sub-range [lo, lo + S) of the window) ------------
@@ -845,7 +991,9 @@ struct BlkRec {  // one staged posting block of the window
 // see lower_plan): the program degenerates to "zero the accumulator, fold every term", matches and
 // the hit count come from the score array in the fused collect sweep, and none of the bitmap
 // machinery is compiled in. The host launches it only when the whole batch qualifies.
-template <int MODE, bool UNION>
+// HASHED = true compiles in the hashed aggregation walk (agg_collect_hashed); the host launches that collect
+// instantiation only for batches with a hashed plan, so the other instantiations keep their register allocation.
+template <int MODE, bool UNION, bool HASHED = false>
 __global__ void __launch_bounds__(QW_THREADS, QW_MIN_BLOCKS_PER_SM) k_window(const KParams p) {
   Sm sm{&p.sm};
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -1410,6 +1558,7 @@ __global__ void __launch_bounds__(QW_THREADS, QW_MIN_BLOCKS_PER_SM) k_window(con
           }
           if (n_aggs) {
             if (fast_aggs) agg_collect_fast(sm, P, s_aggs, s_cols, base, doc, on, lane);
+            else if (HASHED && P.hashed) agg_collect_hashed(P, s_aggs, s_cols, base, doc, on, lane);
             else agg_collect_doc(p, sm, P, s_aggs, s_cols, base, cells, doc, on, lane);
           }
         });

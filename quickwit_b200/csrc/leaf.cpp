@@ -88,7 +88,8 @@ static pb::SortValue typed_sort_value(uint32_t kind, int sft, uint64_t v) {
 
 pb::LeafSearchResponse build_split_response(const CompiledPlan& cp, const ImageView& img, const std::string& split_id,
                                             uint64_t num_hits, const QwHit* hits, size_t nhits,
-                                            const QwAggCell* cells, size_t ncells) {
+                                            const QwAggCell* cells, size_t ncells,
+                                            const QwAggEntry* entries, size_t nentries, bool hashed) {
   pb::LeafSearchResponse r;
   r.num_hits = num_hits;
   r.num_attempted_splits = 1;
@@ -102,7 +103,8 @@ pb::LeafSearchResponse build_split_response(const CompiledPlan& cp, const ImageV
     if (hits[i].flags & 2) { h.has_sv2 = true; h.sv2 = typed_sort_value(cp.header.sort[1].kind, cp.sort_field_type[1], hits[i].v2); }
     r.partial_hits.push_back(std::move(h));
   }
-  if (cp.header.num_aggs) r.intermediate_aggregation_result = build_intermediate_aggs(cp, img, cells, ncells);
+  if (cp.header.num_aggs)
+    r.intermediate_aggregation_result = hashed ? build_intermediate_aggs_entries(cp, img, entries, nentries) : build_intermediate_aggs(cp, img, cells, ncells);
   return r;
 }
 
@@ -454,7 +456,8 @@ static std::vector<pb::LambdaSingleSplitResult> run_leaf(Engine& eng, const pb::
     SplitOutput& o = run.outs[k];
     if (o.status) { results[i].is_error = true; results[i].error = o.error; continue; }
     pb::LeafSearchResponse r = build_split_response(run.jobs[i].plan, run.jobs[i].dev->view, run.jobs[i].meta.split_id, o.num_hits,
-                                                    o.hits.data(), o.hits.size(), o.cells.data(), o.cells.size());
+                                                    o.hits.data(), o.hits.size(), o.cells.data(), o.cells.size(),
+                                                    o.entries.data(), o.entries.size(), o.hashed);
     r.resource_stats = split_stats(run, k);
     results[i].response = std::move(r);
   }
@@ -520,7 +523,8 @@ static pb::LeafSearchResponse leaf_merge_fast(const pb::SearchRequest& sreq, Lea
     m.num_successful_splits += 1;
     if (!o.hits.empty()) heap.push_back(head_of(s, o.hits[0]));
     const SplitJob& j = run.jobs[run.which[s]];
-    if (j.plan.header.num_aggs) agg_parts.push_back({&j.plan, &j.dev->view, o.cells.data(), o.cells.size()});
+    if (j.plan.header.num_aggs)
+      agg_parts.push_back({&j.plan, &j.dev->view, o.cells.data(), o.cells.size(), o.hashed, o.entries.data(), o.entries.size()});
     add_leaf_stats(stats_acc, split_stats(run, s));
     any_stats = true;
   }
@@ -652,7 +656,8 @@ int qwgpu_leaf_search(qwgpu_ctx* ctx, const uint8_t* req, size_t req_len, uint8_
     for (size_t k = 0; k < run.which.size(); k++) {
       const qw::SplitJob& j = run.jobs[run.which[k]];
       qw::SplitOutput& o = run.outs[k];
-      qw::pb::LeafSearchResponse r = qw::build_split_response(j.plan, j.dev->view, j.meta.split_id, o.num_hits, o.hits.data(), o.hits.size(), o.cells.data(), o.cells.size());
+      qw::pb::LeafSearchResponse r = qw::build_split_response(j.plan, j.dev->view, j.meta.split_id, o.num_hits, o.hits.data(), o.hits.size(), o.cells.data(), o.cells.size(),
+                                                              o.entries.data(), o.entries.size(), o.hashed);
       r.resource_stats = qw::split_stats(run, k);
       parts.push_back(std::move(r));
     }
@@ -870,6 +875,43 @@ int qwgpu_build_leaf_response(const uint8_t* img, uint64_t img_len, const char* 
   qw::CompiledPlan cp = qw::compile_plan(v, split_id ? split_id : "", req, dm, nullptr);
   qw::pb::LeafSearchResponse r = qw::build_split_response(cp, v, split_id ? split_id : "", num_hits, hits, num_partial_hits, cells, num_cells);
   give(qw::pb::encode_leaf_search_response(r), resp, resp_len);
+  return 0;
+  QW_API_END
+}
+
+int qwgpu_build_leaf_response_entries(const uint8_t* img, uint64_t img_len, const char* split_id, const uint8_t* search_request_pb,
+                                      size_t search_request_len, const char* doc_mapper_json, uint64_t num_hits, const QwHit* hits,
+                                      uint32_t num_partial_hits, const QwAggEntry* entries, uint32_t num_entries, uint8_t** resp, size_t* resp_len) {
+  QW_API_BEGIN
+  qw::ImageView v;
+  v.open(img, img_len);
+  qw::pb::SearchRequest req = qw::pb::decode_search_request(qw::pb::Reader(search_request_pb, search_request_len));
+  qw::DocMapperInfo dm = qw::parse_doc_mapper(doc_mapper_json ? doc_mapper_json : "");
+  qw::CompiledPlan cp = qw::compile_plan(v, split_id ? split_id : "", req, dm, nullptr);
+  qw::pb::LeafSearchResponse r = qw::build_split_response(cp, v, split_id ? split_id : "", num_hits, hits, num_partial_hits, nullptr, 0,
+                                                          entries, num_entries, true);
+  give(qw::pb::encode_leaf_search_response(r), resp, resp_len);
+  return 0;
+  QW_API_END
+}
+
+int qwgpu_agg_layout(const uint8_t* img, uint64_t img_len, const char* split_id, const uint8_t* plan, size_t plan_len,
+                     uint32_t* hashed, uint64_t* bound_cells) {
+  QW_API_BEGIN
+  qw::ImageView v;
+  v.open(img, img_len);
+  if (plan_len < sizeof(QwPlanHeader)) qw::fail(QWGPU_EINVALID_ARG, "plan too short");
+  const QwPlanHeader* ph = (const QwPlanHeader*)plan;
+  if (plan_len < sizeof(QwPlanHeader) + (size_t)ph->num_nodes * sizeof(QwPlanNode) + (size_t)ph->num_aggs * sizeof(QwAggNode))
+    qw::fail(QWGPU_EINVALID_ARG, "plan truncated");
+  const QwAggNode* aggs = (const QwAggNode*)(plan + sizeof(QwPlanHeader) + (size_t)ph->num_nodes * sizeof(QwPlanNode));
+  for (uint32_t i = 0; i < ph->num_aggs; i++) {
+    uint32_t depth = 0;
+    for (uint32_t p = aggs[i].parent; p != 0xFFFFFFFFu; p = aggs[p].parent)
+      if (p >= ph->num_aggs || ++depth > ph->num_aggs) qw::fail(QWGPU_EINVALID_ARG, "aggregation parent out of range");
+  }
+  *hashed = qw_agg_hashed(aggs, ph->num_aggs) ? 1u : 0u;
+  *bound_cells = *hashed ? qw::agg_hashed_layout(aggs, ph->num_aggs, v, split_id ? split_id : "") : 0;
   return 0;
   QW_API_END
 }

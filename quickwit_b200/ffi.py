@@ -31,6 +31,12 @@ ABSENT = 0xFFFFFFFF
 # qwgpu_split_result.kernel_mask (qwgpu.h)
 KERNEL_UNION, KERNEL_DRIVER, KERNEL_AGGSCAN, KERNEL_WINDOW, KERNEL_PHRASE = 1, 2, 4, 8, 16
 KERNEL_TRACE_SELECT, KERNEL_TRACE_REPLAY, KERNEL_FAST_AGGS = 32, 64, 128
+KERNEL_HASHED_AGGS, KERNEL_HASHED_AGGS_RETRY = 256, 512
+# hashed aggregation cells (qwgpu_format.h qw_agg_hashed, qwgpu.h): dense-layout limits, the initial capacity of a
+# split's table, the largest table a split may need, the `missing` flag of an entry
+AGG_DENSE_MAX_CELLS, AGG_DENSE_MAX_TERMS = 1 << 26, 1 << 24
+HASHED_INIT_CELLS, HASHED_MAX_BYTES = 65536, 8 << 30
+AGG_NO_PARENT, AGG_ENTRY_MISSING = 0xFFFFFFFF, 1
 PLAN_MAGIC = 0x4E4C5051
 MAX_AGG_RANGES = 16
 
@@ -79,6 +85,11 @@ class QwAggCell(C.Structure):
                 ("min_mapped", C.c_uint64), ("max_mapped", C.c_uint64)]
 
 
+class QwAggEntry(C.Structure):
+    _fields_ = [("node", C.c_uint32), ("parent", C.c_uint32), ("key", C.c_uint64), ("flags", C.c_uint32),
+                ("reserved", C.c_uint32), ("cell", QwAggCell)]
+
+
 class QwPlanNode(C.Structure):
     _fields_ = [("kind", C.c_uint32), ("occur", C.c_uint32), ("boost", C.c_float),
                 ("first_child", C.c_uint32), ("num_children", C.c_uint32),
@@ -123,7 +134,8 @@ class SplitResult(C.Structure):
                 ("exact_fallbacks", C.c_uint32), ("postings_scored", C.c_uint64),
                 ("algorithmic_bytes", C.c_uint64), ("kernel_mask", C.c_uint32),
                 ("window_docs", C.c_uint32), ("sample_stride", C.c_uint32),
-                ("radix_passes", C.c_uint32), ("refined", C.c_uint32)]
+                ("radix_passes", C.c_uint32), ("refined", C.c_uint32),
+                ("num_agg_entries", C.c_uint32), ("agg_entries", C.POINTER(QwAggEntry))]
 
 
 class SynthSpec(C.Structure):
@@ -189,6 +201,8 @@ def lib() -> C.CDLL:
                                 C.POINTER(SplitResult), C.POINTER(C.c_int)])
     bind("qwgpu_split_result_free", [C.POINTER(SplitResult)], None)
     bind("qwgpu_build_leaf_response", [vp, u64, cp, vp, sz, cp, u64, vp, u32, vp, u32, C.POINTER(vp), C.POINTER(sz)])
+    bind("qwgpu_build_leaf_response_entries", [vp, u64, cp, vp, sz, cp, u64, vp, u32, vp, u32, C.POINTER(vp), C.POINTER(sz)])
+    bind("qwgpu_agg_layout", [vp, u64, cp, vp, sz, C.POINTER(u32), C.POINTER(u64)])
     bind("qwgpu_merge_leaf_responses", [vp, sz, u32, C.POINTER(vp), C.POINTER(sz),
                                         C.POINTER(vp), C.POINTER(sz)])
     bind("qwgpu_optimize_leaf_request", [vp, sz, C.POINTER(vp), C.POINTER(sz)])

@@ -28,6 +28,11 @@ class SplitSearchResult:
             (h.doc_id, h.flags, h.v1, h.v2, h.score) for h in (r.hits[i] for i in range(r.num_partial_hits))]
         self.cells = [(c.count, c.sum_bits, c.min_mapped, c.max_mapped)
                       for c in (r.agg_cells[i] for i in range(r.num_agg_cells))]
+        # hashed aggregation layout: the raw QwAggEntry array (copied: `r` is freed by the caller), turned into
+        # tuples only when `entries` is read — a split can return millions of entries
+        self.num_entries = int(r.num_agg_entries)
+        self._entries_raw = C.string_at(r.agg_entries, self.num_entries * C.sizeof(ffi.QwAggEntry)) if self.num_entries else b""
+        self._entries = None
         self.gpu_time_us = float(r.gpu_time_us)
         self.main_kernel_us = float(r.main_kernel_us)
         self.exact_fallbacks = int(r.exact_fallbacks)
@@ -40,6 +45,15 @@ class SplitSearchResult:
         self.sample_stride = int(r.sample_stride)
         self.radix_passes = int(r.radix_passes)
         self.refined = int(r.refined)
+
+    @property
+    def entries(self) -> List[tuple]:
+        """(node, parent entry, key, flags, (count, sum_bits, min_mapped, max_mapped)) per entry."""
+        if self._entries is None:
+            arr = (ffi.QwAggEntry * self.num_entries).from_buffer_copy(self._entries_raw) if self.num_entries else []
+            self._entries = [(e.node, e.parent, e.key, e.flags,
+                              (e.cell.count, e.cell.sum_bits, e.cell.min_mapped, e.cell.max_mapped)) for e in arr]
+        return self._entries
 
 
 class SearcherContext:
@@ -264,6 +278,38 @@ def build_leaf_response(img: SplitImage, search_request_pb: bytes, doc_mapper_js
                                           len(search_request_pb), doc_mapper_json.encode(), num_hits, harr, len(hits),
                                           carr, len(cells), C.byref(out), C.byref(n)))
     return ffi.take_bytes(out, n.value)
+
+
+def build_leaf_response_entries(img: SplitImage, search_request_pb: bytes, doc_mapper_json: str, num_hits: int,
+                                hits: Sequence[Tuple[int, int, int, int, float]], entries: Sequence[tuple],
+                                split_id: str = "") -> bytes:
+    """build_leaf_response for a result in the hashed aggregation layout: entries are
+    (node, parent entry, key, flags, (count, sum_bits, min_mapped, max_mapped)), as SplitSearchResult.entries."""
+    L = ffi.lib()
+    rb = C.create_string_buffer(search_request_pb, len(search_request_pb))
+    harr = (ffi.QwHit * max(len(hits), 1))()
+    for i, (doc, flags, v1, v2, score) in enumerate(hits):
+        harr[i].doc_id, harr[i].flags, harr[i].v1, harr[i].v2, harr[i].score = doc, flags, v1, v2, score
+    earr = (ffi.QwAggEntry * max(len(entries), 1))()
+    for i, (node, parent, key, flags, (cnt, s, mn, mx)) in enumerate(entries):
+        e = earr[i]
+        e.node, e.parent, e.key, e.flags = node, parent, key, flags
+        e.cell.count, e.cell.sum_bits, e.cell.min_mapped, e.cell.max_mapped = cnt, s, mn, mx
+    out, n = C.c_void_p(), C.c_size_t()
+    ffi.check(L.qwgpu_build_leaf_response_entries(img.ptr, img.nbytes, (split_id or img.split_id).encode(), C.addressof(rb),
+                                                  len(search_request_pb), doc_mapper_json.encode(), num_hits, harr,
+                                                  len(hits), earr, len(entries), C.byref(out), C.byref(n)))
+    return ffi.take_bytes(out, n.value)
+
+
+def agg_layout(img: SplitImage, plan: bytes, split_id: str = "") -> Tuple[bool, int]:
+    """(hashed, bound on the split's distinct cells) of a plan's aggregation tree on a split (qwgpu_agg_layout)."""
+    L = ffi.lib()
+    pb = C.create_string_buffer(plan, len(plan))
+    hashed, bound = C.c_uint32(), C.c_uint64()
+    ffi.check(L.qwgpu_agg_layout(img.ptr, img.nbytes, (split_id or img.split_id).encode(), C.addressof(pb), len(plan),
+                                 C.byref(hashed), C.byref(bound)))
+    return bool(hashed.value), int(bound.value)
 
 
 # ---- multi-GPU partial exchange (SURVEY.md §8e): one fixed-size all-gather stands in for the root merge
