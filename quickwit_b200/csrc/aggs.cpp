@@ -10,7 +10,6 @@
 //   * final: into_final_result (quickwit-search/src/root.rs:1105-1135): buckets cut to `size`,
 //     histogram gaps filled when min_doc_count == 0, extended_bounds, key_as_string.
 #include <algorithm>
-#include <chrono>
 #include <cmath>
 #include <map>
 #include <set>
@@ -829,27 +828,8 @@ std::string merge_intermediate_aggs(const std::vector<AggReq>& reqs, const std::
     return encode_spans(merge_span_fruits(std::move(fruits), reqs[0].num_traces));
   }
   std::vector<IAgg> acc;
-  static const bool trace = getenv("QWGPU_TRACE_AGG") != nullptr;
-  if (!trace) {
-    for (auto& p : parts) merge_lists(reqs, acc, de_top(p));
-    return ser_top(acc);
-  }
-  using clk = std::chrono::steady_clock;
-  long de = 0, mg = 0;
-  for (auto& p : parts) {
-    auto t0 = clk::now();
-    std::vector<IAgg> d = de_top(p);
-    auto t1 = clk::now();
-    merge_lists(reqs, acc, std::move(d));
-    auto t2 = clk::now();
-    de += std::chrono::duration_cast<std::chrono::nanoseconds>(t1 - t0).count();
-    mg += std::chrono::duration_cast<std::chrono::nanoseconds>(t2 - t1).count();
-  }
-  auto t0 = clk::now();
-  std::string out = ser_top(acc);
-  long se = std::chrono::duration_cast<std::chrono::nanoseconds>(clk::now() - t0).count();
-  fprintf(stderr, "[qwgpu] merge_intermediate_aggs: %zu parts, decode %ld us, merge %ld us, encode %ld us\n", parts.size(), de / 1000, mg / 1000, se / 1000);
-  return out;
+  for (auto& p : parts) merge_lists(reqs, acc, de_top(p));
+  return ser_top(acc);
 }
 
 // ---- finalize -----------------------------------------------------------------------------------------------

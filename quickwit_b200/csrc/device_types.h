@@ -5,12 +5,8 @@
 
 #include "../../include/qwgpu_format.h"
 
-#ifndef QW_THREADS
 #define QW_THREADS 512
-#endif
-#ifndef QW_MIN_BLOCKS_PER_SM
 #define QW_MIN_BLOCKS_PER_SM 2
-#endif
 #define QW_WARPS (QW_THREADS / 32)
 #define QW_MAX_INSTR 96
 #define QW_MAX_DCOLS 16

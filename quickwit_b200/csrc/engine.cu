@@ -96,11 +96,9 @@ Engine::Engine(int dev) : device(dev) {
   CUDA_CHECK(cudaGetDeviceProperties(&prop, dev));
   sm_count = prop.multiProcessorCount;
   max_smem_optin = (int)prop.sharedMemPerBlockOptin;
-  CUDA_CHECK(cudaFuncSetAttribute(qwk::k_window<qwk::MODE_HIST, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem_optin));
-  CUDA_CHECK(cudaFuncSetAttribute(qwk::k_window<qwk::MODE_COLLECT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem_optin));
-  CUDA_CHECK(cudaFuncSetAttribute(qwk::k_window<qwk::MODE_COLLECT, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem_optin));
+  CUDA_CHECK(cudaFuncSetAttribute(qwk::k_window<qwk::MODE_HIST>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem_optin));
+  CUDA_CHECK(cudaFuncSetAttribute(qwk::k_window<qwk::MODE_COLLECT>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem_optin));
   CUDA_CHECK(cudaFuncSetAttribute(qwk::k_window<qwk::MODE_COLLECT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem_optin));
-  CUDA_CHECK(cudaFuncSetAttribute(qwk::k_window<qwk::MODE_HIST, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem_optin));
   CUDA_CHECK(cudaFuncSetAttribute(qwk::k_union<qwk::MODE_HIST>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem_optin));
   CUDA_CHECK(cudaFuncSetAttribute(qwk::k_union<qwk::MODE_COLLECT>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem_optin));
   CUDA_CHECK(cudaFuncSetAttribute(qwk::k_aggscan, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem_optin));
@@ -657,7 +655,7 @@ static void lower_plan(Lowered& L, const SplitDev& sp, const uint8_t* plan, size
     lower_node(L, sp, nodes, ph->num_nodes, 0, 0, QW_OCCUR_MUST, scoring);
   } else if (nodes[0].kind == QW_NODE_TERM && scoring) {
     // a scored single-term query is the one-clause case of the BM25 union: lower it as
-    // bool{should: [term]} so that it takes the UNION kernels (same matches, same f32 score)
+    // bool{should: [term]} so that it takes k_union (same matches, same f32 score)
     QwPlanNode wrap[2];
     memset(wrap, 0, sizeof wrap);
     wrap[0].kind = QW_NODE_BOOL; wrap[0].occur = QW_OCCUR_MUST; wrap[0].boost = 1.0f;
@@ -867,7 +865,6 @@ static void lower_plan(Lowered& L, const SplitDev& sp, const uint8_t* plan, size
 
 // shared-memory arena for a batch (max over the batch's plans)
 static uint32_t stage_bytes_for(uint32_t W) {
-  if (const char* e = getenv("QWGPU_STAGE")) return (uint32_t)atoi(e) & ~15u;
   return std::min<uint32_t>(std::max<uint32_t>(W, 8192), 24576);
 }
 
@@ -918,8 +915,7 @@ static qwk::USmem make_union_layout(uint32_t W, bool hist, uint32_t budget) {
   if (hist) L.hist = take(QW_HIST_BINS * 4);
   L.cands = take(QU_NCW * QU_CANDS * 8 + QU_NCW * 4);
   const uint32_t fixed = QU_MAXBLK * 16 + QU_MAX_TERMS * 16 + 32 + QU_PAD;
-  uint32_t cap = budget > off + QU_SLOTS * (fixed + 2048) ? ((budget - off) / QU_SLOTS - fixed) & ~15u : 2048;
-  if (const char* e = getenv("QWGPU_UCAP")) cap = (uint32_t)atoi(e) & ~15u;
+  const uint32_t cap = budget > off + QU_SLOTS * (fixed + 2048) ? ((budget - off) / QU_SLOTS - fixed) & ~15u : 2048;
   L.cap = cap;
   L.payload = 0;
   L.recs = cap + QU_PAD;
@@ -1028,7 +1024,7 @@ bool Engine::search_once(const std::vector<std::shared_ptr<SplitDev>>& sp, const
   // level-0 histogram and every window's best digit, so that a failed sampled threshold is repaired
   // by a candidates-only pass over the few windows that can hold candidates
   bool rec_l0 = true, rangeq = false;
-  // every plan has the BM25 top-K shape => the specialised UNION instantiation of the collect kernel
+  // every plan has the BM25 top-K shape => the BM25-union pipeline (k_union)
   bool all_union = true, all_driver = true;
   for (auto& L : low) {
     if (!(L.P.fused_score_root && L.P.max_hits && !L.P.sa.present && !L.P.n_aggs && L.P.key.kind[0] == QW_SORT_SCORE &&
@@ -1070,19 +1066,14 @@ bool Engine::search_once(const std::vector<std::shared_ptr<SplitDev>>& sp, const
   // window size: as large as shared memory allows for the configured blocks/SM (per-window fixed
   // costs — staging, program interpretation, barriers — amortise over more postings)
   uint32_t W = 32768;
-  if (const char* e = getenv("QWGPU_W")) W = (uint32_t)atoi(e);
-  // BM25-union batches run the TMA + mbarrier pipeline (union_kernel.cuh): fixed 16384-doc windows,
-  // two blocks per SM; QWGPU_OLD_UNION=1 keeps the round-1 window kernel for A/B runs
-  static const bool old_union = getenv("QWGPU_OLD_UNION") != nullptr;
-  // (QWGPU_NO_DRIVER=1 keeps the window engine for these shapes: A/B runs)
-  static const bool driver_on = getenv("QWGPU_NO_DRIVER") == nullptr;
-  const bool use_driver = all_driver && driver_on;
+  // BM25-union batches run the TMA + mbarrier pipeline (union_kernel.cuh): fixed 15360-doc windows,
+  // two blocks per SM
+  const bool use_driver = all_driver;
   if (use_driver) rec_l0 = false;
-  const bool use_union = all_union && !old_union && !use_driver;
+  const bool use_union = all_union && !use_driver;
   const uint32_t u_budget = (uint32_t)(max_smem_optin + 1024) / QU_MINB - 1024 - 64;
   // match_all + flat terms / histogram aggregations, no hits: the streaming column kernel (agg_kernel.cuh)
-  static const bool old_aggs = getenv("QWGPU_OLD_AGGS") != nullptr;
-  bool use_aggscan = !old_aggs;
+  bool use_aggscan = true;
   qwk::ASmem alay;
   memset(&alay, 0, sizeof alay);
   {
@@ -1117,8 +1108,7 @@ bool Engine::search_once(const std::vector<std::shared_ptr<SplitDev>>& sp, const
   }
   if (use_aggscan) W = QA_CHUNK;  // the flat work list is the list of 8192-doc chunks
   qwk::USmem ulay_c, ulay_h;
-  if (use_union && !getenv("QWGPU_W"))
-    W = getenv("QWGPU_UW") ? (uint32_t)atoi(getenv("QWGPU_UW")) : 15360u * 2 / QU_MINB;
+  if (use_union) W = 15360u * 2 / QU_MINB;
   SmemLayout lay;
   for (;;) {
     lay = make_layout(W, n_levels, need_cnt, need_msum, need_ssum, max_instr, max_cols, max_aggs, n_fn, rec_l0, rangeq);
@@ -1143,14 +1133,13 @@ bool Engine::search_once(const std::vector<std::shared_ptr<SplitDev>>& sp, const
   }
   // sampling stride of the threshold-estimation pass: 1/16 of the windows (a coarser sample shortens the histogram
   // pass, but the looser threshold lets more candidates through the collect pass)
-  static const uint32_t stride_cap = getenv("QWGPU_STRIDE_CAP") ? (uint32_t)atoi(getenv("QWGPU_STRIDE_CAP")) : 16u;
-  uint32_t stride = std::min(std::max(stride_cap, 1u), std::max(1u, max_windows / 8));
-  // BM25-union batches can sample the threshold over finer windows (W / QWGPU_HDIV: the same fraction of the docs in
-  // more work items). Measured on the bench workload, one H100 80GB HBM3 (400 W power limit): 1 gives 1.175-1.183 ms per
-  // 4-query step, 2 gives 1.194-1.203 ms and 4 gives 1.216-1.231 ms (the per-window clause chain does not shrink with
-  // the window), so the default stays 1.
-  static const uint32_t hdiv = getenv("QWGPU_HDIV") ? std::max(1u, (uint32_t)atoi(getenv("QWGPU_HDIV"))) : 1u;
-  const uint32_t W_h = use_union ? std::max(1024u, (W / hdiv) & ~1023u) : W;
+  const uint32_t stride_cap = 16;
+  uint32_t stride = std::min(stride_cap, std::max(1u, max_windows / 8));
+  // BM25-union batches sample the threshold over the collect pass's window size rounded down to 1024 docs. Finer
+  // windows (the same fraction of the docs in more work items) were measured on the bench workload, one H100 80GB HBM3
+  // (400 W power limit): W gives 1.175-1.183 ms per 4-query step, W / 2 gives 1.194-1.203 ms and W / 4 gives
+  // 1.216-1.231 ms (the per-window clause chain does not shrink with the window).
+  const uint32_t W_h = use_union ? std::max(1024u, W & ~1023u) : W;
   if (use_union) {
     uint32_t mw = 0, tw = 0;
     for (uint32_t i = 0; i < n; i++) {
@@ -1158,15 +1147,13 @@ bool Engine::search_once(const std::vector<std::shared_ptr<SplitDev>>& sp, const
       mw = std::max(mw, nw);
       tw += nw;
     }
-    stride = std::min(std::max(stride_cap, 1u), std::max(1u, mw / 8));
+    stride = std::min(stride_cap, std::max(1u, mw / 8));
     // Large requests: at most ONE sampled window per resident block (the sampled pass is latency bound — a block
     // that gets two windows doubles its duration), up to a stride of 32. Bench workload on one H100 80GB HBM3 (400 W
     // power limit; 6528 windows, 132 SMs x 2 = 264 blocks): stride 25 instead of 16, 1.175-1.183 against 1.209-1.211 ms
     // per 4-query step (a fixed stride of 32: 1.174-1.181 ms, no better).
-    if (!getenv("QWGPU_STRIDE_CAP")) {
-      const uint32_t per_block = (tw + (uint32_t)(sm_count * QU_MINB) - 1) / (uint32_t)(sm_count * QU_MINB);
-      stride = std::max(stride, std::min({per_block, 32u, std::max(1u, mw / 8)}));
-    }
+    const uint32_t per_block = (tw + (uint32_t)(sm_count * QU_MINB) - 1) / (uint32_t)(sm_count * QU_MINB);
+    stride = std::max(stride, std::min({per_block, 32u, std::max(1u, mw / 8)}));
   }
   // posting-driven kernel: the work list is the driving term's posting blocks; the threshold sample takes every
   // stride-th BLOCK (128 postings, fine enough for keys that follow doc order: what lies between two sampled
@@ -1175,7 +1162,7 @@ bool Engine::search_once(const std::vector<std::shared_ptr<SplitDev>>& sp, const
   if (use_driver) {
     uint32_t max_blocks = 0;
     for (uint32_t i = 0; i < n; i++) max_blocks = std::max(max_blocks, low[i].empty ? 0u : low[i].instrs[1].n);
-    stride = std::min(std::max(stride_cap, 1u), std::max(1u, max_blocks / 64));
+    stride = std::min(stride_cap, std::max(1u, max_blocks / 64));
     for (uint32_t i = 0; i < n; i++) {
       const uint32_t nb = low[i].empty ? 0u : low[i].instrs[1].n, phase = stride > 1 ? i % stride : 0;
       fw_drv[i + 1] = fw_drv[i] + nb;
@@ -1221,7 +1208,7 @@ bool Engine::search_once(const std::vector<std::shared_ptr<SplitDev>>& sp, const
   for (auto& L : low) kmax = std::max(kmax, L.P.max_hits);
   // scratch: thresholds, histograms, candidates
   size_t s_thr = 0, s_hist = al(s_thr + n * sizeof(DThresh)), s_state = al(s_hist + (size_t)n * QW_HIST_BINS * 4),
-         s_ctr = al(s_state + (size_t)n * 4), s_wmax = al(s_ctr + 64 * 4), s_cand = al(s_wmax + (rec_l0 ? (size_t)fw_all[n] * 2 : 0)),
+         s_wmax = al(s_state + (size_t)n * 4), s_cand = al(s_wmax + (rec_l0 ? (size_t)fw_all[n] * 2 : 0)),
          s_hits = al(s_cand + (any_topk ? (size_t)n * QW_CAND_CAP * 24 : 0)),
          s_cut = al(s_hits + (do_merge ? (size_t)n * kmax * sizeof(QwHit) : 0)),
          s_grecv = al(s_cut + (size_t)std::max<uint32_t>(n, 64) * 4 + 1024),
@@ -1406,10 +1393,9 @@ bool Engine::search_once(const std::vector<std::shared_ptr<SplitDev>>& sp, const
   kp.wmax = (uint16_t*)(slot->d_scratch + s_wmax);
   kp.split_state = (const uint32_t*)(slot->d_scratch + s_state);
   int occ = 1;
-  CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, qwk::k_window<qwk::MODE_COLLECT, false>, QW_THREADS, lay.total));
+  CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, qwk::k_window<qwk::MODE_COLLECT>, QW_THREADS, lay.total));
   occ = std::max(occ, 1);
   enum { F_REC = 1, F_REFINE = 2, F_CANDS_ONLY = 4 };
-  uint32_t n_ctr = 0;  // work counters handed to k_union launches (zeroed with the scratch region)
   auto launch_window = [&](int mode, bool sampled, uint32_t level, uint32_t use_prefix, uint32_t flags) {
     KParams q = kp;
     q.first_work = (const uint32_t*)(slot->d_blob + (sampled ? o_fws : o_fwa));
@@ -1456,44 +1442,20 @@ bool Engine::search_once(const std::vector<std::shared_ptr<SplitDev>>& sp, const
       u.plans = kp.plans; u.instrs = kp.instrs; u.cols = kp.cols; u.thresh = kp.thresh;
       u.first_work = q.first_work; u.n_splits = n; u.total_work = q.total_work; u.stride = q.stride; u.W = sampled ? W_h : W;
       u.sm = mode == qwk::MODE_HIST ? ulay_h : ulay_c;
-      // QWGPU_DYNAMIC_WORK=1: windows handed out one at a time from a counter instead of a static chunk per block.
-      // Measured on the bench workload (uniform splits), one H100 80GB HBM3 (400 W power limit): 216-218 us against
-      // 201-202 us per launch — consecutive windows of a block then belong to different splits, and the per-window
-      // plan switch sits on the producer's critical path — so static chunks stay the default; the counter road is kept
-      // for skewed corpora and returns the same hits.
-      static const bool dynamic_work = getenv("QWGPU_DYNAMIC_WORK") != nullptr;
-      if (dynamic_work && n_ctr < 64) u.work_ctr = (uint32_t*)(slot->d_scratch + s_ctr) + n_ctr++;
-#ifdef QU_PROFILE
-      static unsigned long long* d_prof = nullptr;
-      if (!d_prof) CUDA_CHECK(cudaMalloc(&d_prof, 16 * 8));
-      if (mode == qwk::MODE_COLLECT) { CUDA_CHECK(cudaMemsetAsync(d_prof, 0, 16 * 8, st)); u.prof = d_prof; }
-#endif
       // cross-rank calls leave a few block slots free: the persistent grid would otherwise hold every SM's shared
       // memory, a concurrent call's NCCL kernel would take the place of one of its blocks, and that block — with its
       // static share of the windows — would only start when another one has finished (twice the kernel time)
       const uint32_t ugrid = std::min<uint32_t>(q.total_work, (uint32_t)(sm_count * QU_MINB) - (do_gather ? 4u : 0u));
       if (mode == qwk::MODE_HIST) qwk::k_union<qwk::MODE_HIST><<<ugrid, QU_THREADS, u.sm.total, st>>>(u);
       else qwk::k_union<qwk::MODE_COLLECT><<<ugrid, QU_THREADS, u.sm.total, st>>>(u);
-#ifdef QU_PROFILE
-      if (u.prof && getenv("QWGPU_UPROF")) {
-        unsigned long long h[16];
-        CUDA_CHECK(cudaMemcpyAsync(h, d_prof, sizeof h, cudaMemcpyDeviceToHost, st));
-        wait_stream();
-        const double np = (double)ugrid, nc = (double)h[15];
-        fprintf(stderr, "[uprof] producer/CTA: total %.0f cyc, empty-wait %.0f, phaseA %.0f, window(A+B) %.0f, windows %.1f, slots %.1f | consumer/warp: total %.0f, full-wait %.0f, chain-wait %.0f (end-of-window %.0f), sweep %.0f, block-loop %.0f, blocks %.1f\n",
-                h[0] / np, h[1] / np, h[2] / np, h[3] / np, h[4] / np, h[5] / np, h[8] / nc, h[9] / nc, h[10] / nc, h[11] / nc, h[12] / nc, h[13] / nc, h[14] / nc);
-      }
-#endif
       stats.launches++;
       stats.kernel_mask |= QWGPU_KERNEL_UNION;
       return;
     }
     uint32_t grid = std::min<uint32_t>(q.total_work, (uint32_t)(sm_count * occ));
-    if (mode == qwk::MODE_HIST && all_union && old_union && level == 0 && !use_prefix) qwk::k_window<qwk::MODE_HIST, true><<<grid, QW_THREADS, lay.total, st>>>(q);
-    else if (mode == qwk::MODE_HIST) qwk::k_window<qwk::MODE_HIST, false><<<grid, QW_THREADS, lay.total, st>>>(q);
-    else if (all_union && old_union) qwk::k_window<qwk::MODE_COLLECT, true><<<grid, QW_THREADS, lay.total, st>>>(q);
-    else if (any_hashed) qwk::k_window<qwk::MODE_COLLECT, false, true><<<grid, QW_THREADS, lay.total, st>>>(q);
-    else qwk::k_window<qwk::MODE_COLLECT, false><<<grid, QW_THREADS, lay.total, st>>>(q);
+    if (mode == qwk::MODE_HIST) qwk::k_window<qwk::MODE_HIST><<<grid, QW_THREADS, lay.total, st>>>(q);
+    else if (any_hashed) qwk::k_window<qwk::MODE_COLLECT, true><<<grid, QW_THREADS, lay.total, st>>>(q);
+    else qwk::k_window<qwk::MODE_COLLECT><<<grid, QW_THREADS, lay.total, st>>>(q);
     stats.launches++;
     stats.kernel_mask |= QWGPU_KERNEL_WINDOW;
     // (k_window aggregates on the fast path where the plan's and the launch's flags both allow it)

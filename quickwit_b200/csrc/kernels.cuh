@@ -11,10 +11,9 @@
 //      same load round turns the terms' skip-list entries into the window's block table;
 //   3. terms are decoded block-per-warp (4-lane-interleaved bit-unpack -> warp-shuffle prefix scan ->
 //      doc ids), BM25 is applied in f32 and accumulated into per-window score arrays in the
-//      reference's clause order (bit-reproducible sums) — with a barrier per clause in the generic
-//      program, with a ticket counter and no barrier in the BM25-union instantiation (UNION) — and
-//      match sets are shared-memory bitmaps combined with AND / OR / AND-NOT exactly like tantivy's
-//      BooleanWeight;
+//      reference's clause order (bit-reproducible sums, one barrier per clause; batches of the
+//      BM25-union shape run k_union in union_kernel.cuh instead) — and match sets are shared-memory
+//      bitmaps combined with AND / OR / AND-NOT exactly like tantivy's BooleanWeight;
 //   4. the matched docs of the window are counted, aggregated (bucket counts privatised in shared
 //      memory) and filtered against a per-split top-K threshold over compacted hits (full warps);
 //      survivors go to a candidate list that k_select reduces with the reference's total order.
@@ -293,75 +292,6 @@ __device__ __forceinline__ void fold_vblock(const VBlk* vb, uint32_t ws, uint32_
     if (sc) score[rel] = __fadd_rn(score[rel], val[j]);
     if (cn) cnt[rel] = (uint8_t)(cnt[rel] + 1);
     atomicOr(&bits[rel >> 5], 1u << (rel & 31));
-  }
-}
-
-// BM25-union pipeline, first half: decode a STAGED posting block and compute the score contribution
-// of each of the lane's 4 postings (weight * tf-factor) WITHOUT touching the accumulator, so that it
-// can run ahead of the clause order; `inmask` bit j = posting j exists and lies inside the window.
-__device__ __forceinline__ void union_decode(uint32_t blk_off, uint32_t ws, uint32_t wlen, const TermTarget& tg, uint32_t lane,
-                                             uint32_t (&rel)[4], float (&contrib)[4], uint32_t& inmask) {
-  const uint8_t* blk = qw_smem + blk_off;
-  const uint4 h = *reinterpret_cast<const uint4*>(blk);  // QwSkip: last_doc, prev_last_doc, byte_off, bits/count
-  const uint32_t last_doc = h.x, prev = h.y;
-  const uint32_t doc_bits = h.w & 0xFF, tf_bits = (h.w >> 8) & 0xFF, count = h.w >> 16;
-  inmask = 0;
-  if (last_doc < ws) return;
-  if (prev != QW_NO_PREV_DOC && prev + 1 >= ws + wlen) return;
-  const uint4* dp = reinterpret_cast<const uint4*>(blk + 16);
-  uint32_t v0 = 0, v1 = 0, v2 = 0, v3 = 0;
-  if (doc_bits) {
-    uint32_t bitpos = lane * doc_bits, wi = bitpos >> 5, sh = bitpos & 31;
-    uint4 A = dp[wi];
-    uint4 B = (sh + doc_bits > 32) ? dp[wi + 1] : make_uint4(0, 0, 0, 0);
-    uint32_t mask = 0xFFFFFFFFu >> (32 - doc_bits);
-    v0 = __funnelshift_r(A.x, B.x, sh) & mask;
-    v1 = __funnelshift_r(A.y, B.y, sh) & mask;
-    v2 = __funnelshift_r(A.z, B.z, sh) & mask;
-    v3 = __funnelshift_r(A.w, B.w, sh) & mask;
-  }
-  uint32_t d0 = v0 + 1, d1 = d0 + v1 + 1, d2 = d1 + v2 + 1, d3 = d2 + v3 + 1;
-  uint32_t incl = d3;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    uint32_t n = __shfl_up_sync(0xFFFFFFFFu, incl, o);
-    if ((int)lane >= o) incl += n;
-  }
-  const uint32_t basev = prev + (incl - d3) - ws;  // mod 2^32; window-relative
-  rel[0] = basev + d0; rel[1] = basev + d1; rel[2] = basev + d2; rel[3] = basev + d3;
-  const uint32_t nvalid = count > lane * 4 ? count - lane * 4 : 0;
-  uint32_t tf[4] = {1, 1, 1, 1};
-  if (tg.has_tf && tf_bits) {
-    const uint4* tp = dp + doc_bits;
-    uint32_t bitpos = lane * tf_bits, wi = bitpos >> 5, sh = bitpos & 31;
-    uint4 A = tp[wi];
-    uint4 B = (sh + tf_bits > 32) ? tp[wi + 1] : make_uint4(0, 0, 0, 0);
-    uint32_t mask = 0xFFFFFFFFu >> (32 - tf_bits);
-    tf[0] = __funnelshift_r(A.x, B.x, sh) & mask;
-    tf[1] = __funnelshift_r(A.y, B.y, sh) & mask;
-    tf[2] = __funnelshift_r(A.z, B.z, sh) & mask;
-    tf[3] = __funnelshift_r(A.w, B.w, sh) & mask;
-  }
-  const float* tab = tg.gtab;
-  const uint8_t* fn = qw_smem + tg.fn;
-  const bool has_fn = tg.fn != 0xFFFFFFFFu;
-  uint32_t f[4];
-#pragma unroll
-  for (int j = 0; j < 4; j++) {
-    const bool in = (uint32_t)j < nvalid && rel[j] < wlen;  // rel = doc - ws (unsigned wrap before the window)
-    inmask |= (in ? 1u : 0u) << j;
-    f[j] = (has_fn && in) ? fn[rel[j]] : 1u;
-  }
-#pragma unroll
-  for (int j = 0; j < 4; j++) {
-    // Bm25Weight::score: weight * (tf / (tf + cache[fieldnorm_id])), f32 round-to-nearest
-    const uint32_t t = tf[j];
-    float tfn = 0.0f;
-    if ((inmask >> j) & 1) {
-      if (t < QW_TFF_ROWS) tfn = __ldg(tab + 256 + t * 256 + f[j]);
-      else { float tff = (float)t; tfn = __fdiv_rn(tff, __fadd_rn(tff, __ldg(tab + f[j]))); }
-    }
-    contrib[j] = __fmul_rn(tg.weight, tfn);
   }
 }
 
@@ -986,14 +916,9 @@ struct BlkRec {  // one staged posting block of the window
 // The window engine (see the file header): phases 1-3 stage the window's bytes and build the block
 // table, then the boolean program runs block-wide, then the matches are collected.
 //
-// UNION = true is the specialised instantiation for the BM25 top-K shape (every plan of the batch is
-// a pure OR of positive-weight scored terms ranked by _score desc, no search_after, no aggregations;
-// see lower_plan): the program degenerates to "zero the accumulator, fold every term", matches and
-// the hit count come from the score array in the fused collect sweep, and none of the bitmap
-// machinery is compiled in. The host launches it only when the whole batch qualifies.
 // HASHED = true compiles in the hashed aggregation walk (agg_collect_hashed); the host launches that collect
 // instantiation only for batches with a hashed plan, so the other instantiations keep their register allocation.
-template <int MODE, bool UNION, bool HASHED = false>
+template <int MODE, bool HASHED = false>
 __global__ void __launch_bounds__(QW_THREADS, QW_MIN_BLOCKS_PER_SM) k_window(const KParams p) {
   Sm sm{&p.sm};
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -1013,7 +938,6 @@ __global__ void __launch_bounds__(QW_THREADS, QW_MIN_BLOCKS_PER_SM) k_window(con
   uint32_t* s_hist = sm.u32(p.sm.hist);
   uint8_t* s_stage = sm.u8(p.sm.stage);
   uint32_t loaded_split = 0xFFFFFFFFu;
-  bool ssum_clean = false;  // level-0 should-score array is all zero (left so by a fused collect)
 
   const uint32_t per = (p.total_work + gridDim.x - 1) / gridDim.x;
   const uint32_t w_begin = blockIdx.x * per;
@@ -1057,7 +981,6 @@ __global__ void __launch_bounds__(QW_THREADS, QW_MIN_BLOCKS_PER_SM) k_window(con
       src = (const uint4*)&P.key;
       if (tid < sizeof(DKeySpec) / 16) ((uint4*)sm.u8(p.sm.key))[tid] = __ldg(src + tid);
       loaded_split = split;
-      ssum_clean = false;
       __syncthreads();
       if (tid < P.n_instr && s_instr[tid].op == OP_TERM) s_tinstr[s_instr[tid].t] = (uint8_t)tid;  // term slot -> instruction (kept per split)
       __syncthreads();
@@ -1152,102 +1075,18 @@ __global__ void __launch_bounds__(QW_THREADS, QW_MIN_BLOCKS_PER_SM) k_window(con
     // memory (direct mode).
     uint32_t ip = 0;
     uint32_t req_init = 0;  // bit per level, uniform across the block
-    // fused BM25 shape (COLLECT pass only): matches / hit count come from the score array, which the
-    // collect loop also re-zeroes for the next window of the same split plan
-    constexpr bool fused = UNION;
     {
       while (ip < n_instr) {
         const DInstr& in = s_instr[ip];
         const uint32_t op = in.op, level = in.level, occur = in.occur;
         const SmemLevel& LV = p.sm.lvl[level];
         const bool scored = (in.flags & IF_SCORED) != 0;
-        if (UNION && op == OP_BOOL_BEGIN) {
-          if (!ssum_clean) zero_f4(sm.f32(LV.ssum), W, tid);
-          if (tid == 0) s_misc[5] = 0;  // ticket: posting blocks applied so far
-          __syncthreads();
-          ip++;
-          if (s_misc[6] == 0) {
-            // Every term of the window is staged: run the whole union as ONE pipelined pass over the
-            // flat block table (blocks are numbered in clause order). A warp decodes its next block
-            // right away and only the read-modify-write of the accumulator waits until every block of
-            // the EARLIER clauses has been applied (ticket counter) — the f32 sums keep the reference's
-            // clause order, but there is no block-wide barrier per clause and no warp idles while a
-            // short clause finishes. Blocks of one clause touch distinct docs, so they commute.
-            const uint32_t G = s_misc[0];
-            // (tried and rejected: a spare warp prefetching the next window's bytes into L2 — the staging
-            // phases are not DRAM-latency bound enough to pay for it)
-            volatile uint32_t* ticket = (volatile uint32_t*)&s_misc[5];
-            float* score = sm.f32(LV.ssum);
-            // (static round-robin assignment; handing blocks out from a shared counter was tried and rejected)
-            for (uint32_t g = warp; g < G; g += QW_WARPS) {
-              const BlkRec r = s_blk[g];
-              const DInstr& ti = s_instr[s_tinstr[r.slot]];
-              TermTarget tg;
-              tg.bits = 0xFFFFFFFFu;
-              tg.cnt = 0xFFFFFFFFu;
-              tg.score = LV.ssum;
-              tg.weight = ti.f;
-              tg.has_tf = (ti.flags & IF_HAS_TF) != 0;
-              tg.fn = (ti.flags & IF_HAS_FN) ? p.sm.fn[ti.r] : 0xFFFFFFFFu;
-              tg.gtab = (const float*)P.bm25_tab[ti.r];
-              uint32_t rel[4], inmask;
-              float contrib[4];
-              union_decode(p.sm.stage + r.soff, ws, wlen, tg, lane, rel, contrib, inmask);
-              const uint32_t need = s_tblk[2 * r.slot];  // first block of this clause = blocks of earlier clauses
-              if (need) {
-                if (lane == 0) {
-                  while (*ticket < need) __nanosleep(20);
-                  __threadfence_block();
-                }
-                __syncwarp();
-              }
-              float old[4];
-#pragma unroll
-              for (int j = 0; j < 4; j++) old[j] = ((inmask >> j) & 1) ? score[rel[j]] : 0.0f;
-#pragma unroll
-              for (int j = 0; j < 4; j++) if ((inmask >> j) & 1) score[rel[j]] = __fadd_rn(old[j], contrib[j]);
-              __syncwarp();
-              if (lane == 0) {
-                __threadfence_block();
-                atomicAdd(&s_misc[5], 1u);
-              }
-            }
-            __syncthreads();
-            ip = n_instr;  // the TERM / BOOL_END instructions are done
-          }
-        } else if (UNION && op == OP_BOOL_END) {
-          ip++;
-        } else if (UNION) {  // OP_TERM, should + scored, bitmap implied by the score
-          const uint32_t slot = in.t;
-          TermTarget tg;
-          tg.bits = 0xFFFFFFFFu;
-          tg.cnt = 0xFFFFFFFFu;
-          tg.score = LV.ssum;
-          tg.weight = in.f;
-          tg.has_tf = (in.flags & IF_HAS_TF) != 0;
-          tg.fn = (in.flags & IF_HAS_FN) ? p.sm.fn[in.r] : 0xFFFFFFFFu;
-          tg.gtab = (const float*)P.bm25_tab[in.r];
-          if (s_rng[4 * slot + 2] != 0xFFFFFFFFu) {
-            const uint32_t g0 = s_tblk[2 * slot], nb = s_tblk[2 * slot + 1];
-            for (uint32_t k = warp; k < nb; k += QW_WARPS) fold_block<true, false, true, false>(p.sm.stage + s_blk[g0 + k].soff, nullptr, ws, 0, wlen, tg, lane);
-          } else if (s_rng[4 * slot + 1]) {
-            const QwSkip* skips = (const QwSkip*)(base + in.c);
-            const uint32_t bfirst = first_block_ge(skips, in.n, ws, lane);
-            const uint8_t* tdata = base + in.a;
-            for (uint32_t bb = bfirst + warp; bb < in.n; bb += QW_WARPS) {
-              uint4 h = __ldg((const uint4*)&skips[bb]);
-              if (h.y != QW_NO_PREV_DOC && h.y + 1 >= we) break;
-              fold_block<true, false, false, false>(0, tdata + h.z, ws, 0, wlen, tg, lane);
-            }
-          }
-          __syncthreads();
-          ip++;
-        } else if (op == OP_BOOL_BEGIN) {
+        if (op == OP_BOOL_BEGIN) {
           zero_f4((float*)sm.u32(LV.shd), NW, tid);
           zero_f4((float*)sm.u32(LV.nt), NW, tid);
           if (LV.cnt != 0xFFFFFFFFu) zero_f4((float*)sm.u32(LV.cnt), W >> 2, tid);
           if (LV.msum != 0xFFFFFFFFu) zero_f4(sm.f32(LV.msum), W, tid);
-          if (LV.ssum != 0xFFFFFFFFu && !(fused && level == 0 && ssum_clean)) zero_f4(sm.f32(LV.ssum), W, tid);
+          if (LV.ssum != 0xFFFFFFFFu) zero_f4(sm.f32(LV.ssum), W, tid);
           req_init &= ~(1u << level);
           __syncthreads();
           ip++;
@@ -1383,7 +1222,7 @@ __global__ void __launch_bounds__(QW_THREADS, QW_MIN_BLOCKS_PER_SM) k_window(con
         // BooleanWeight combination: all required AND NOT any excluded AND >= r should clauses
         uint32_t* req = sm.u32(LV.req);
         const uint32_t need = in.r, n_req = in.n;
-        if ((in.flags & IF_BITS_FROM_SCORE) && !(fused && level == 0)) {
+        if (in.flags & IF_BITS_FROM_SCORE) {
           // every contribution of the flagged should-terms is > 0, so "matched some of them" == (ssum > 0)
           const float* ss = sm.f32(LV.ssum);
           uint32_t* shd = sm.u32(LV.shd);
@@ -1456,7 +1295,7 @@ __global__ void __launch_bounds__(QW_THREADS, QW_MIN_BLOCKS_PER_SM) k_window(con
     const uint32_t max_hits = P.max_hits, sa_present = P.sa.present;
     const uint32_t n_aggs = (MODE == MODE_COLLECT && p.cands_only) ? 0u : P.n_aggs;
     QwAggCell* cells = (QwAggCell*)P.out_cells;
-    const bool rec = MODE == MODE_COLLECT && p.rec_l0 && max_hits && !fused;
+    const bool rec = MODE == MODE_COLLECT && p.rec_l0 && max_hits;
     const bool fast_aggs = P.fast_aggs && p.smem_aggs;
     uint32_t* s_l0 = sm.u32(p.sm.l0hist);
     if (MODE == MODE_HIST || (p.smem_aggs && n_aggs) || rec) {
@@ -1475,7 +1314,7 @@ __global__ void __launch_bounds__(QW_THREADS, QW_MIN_BLOCKS_PER_SM) k_window(con
       const uint32_t thr_top = (uint32_t)(thr.w0 >> 53);
       uint32_t my_hits = 0, my_elig = 0, my_top = 0;
       // hit count: one popc per bitmap word
-      if (!fused && !p.cands_only) for (uint32_t wd = tid; wd < NW; wd += QW_THREADS) my_hits += __popc(res[wd]);
+      if (!p.cands_only) for (uint32_t wd = tid; wd < NW; wd += QW_THREADS) my_hits += __popc(res[wd]);
       auto emit = [&](const Key& k) {
         const uint32_t pos = atomicAdd((uint32_t*)P.out_cand_count, 1u);
         if (pos < QW_CAND_CAP) {
@@ -1490,25 +1329,7 @@ __global__ void __launch_bounds__(QW_THREADS, QW_MIN_BLOCKS_PER_SM) k_window(con
           if (key_ge(dk.key, thr)) emit(dk.key);
         }
       };
-      if (fused) {
-        // fused BM25 pass: one sweep over the score array counts the matches (score > 0), filters them
-        // against the float lower bound of the threshold bucket and clears the array for the next window
-        float s_lo = -1.0f;
-        if (thr_top >= 1024u) s_lo = __fmul_rn(__fdiv_rn((float)(thr_top & 1023u), ks.score_scale), 0.999999f);
-        float4* sc4 = reinterpret_cast<float4*>(sm.f32(p.sm.lvl[0].ssum));
-        my_hits = 0;
-        for (uint32_t q = tid; q < (W >> 2); q += QW_THREADS) {
-          const float4 v = sc4[q];
-          sc4[q] = make_float4(0.f, 0.f, 0.f, 0.f);
-          my_hits += (v.x > 0.0f) + (v.y > 0.0f) + (v.z > 0.0f) + (v.w > 0.0f);
-          if (v.x > 0.0f && v.x >= s_lo) slow_path(4 * q + 0, v.x);
-          if (v.y > 0.0f && v.y >= s_lo) slow_path(4 * q + 1, v.y);
-          if (v.z > 0.0f && v.z >= s_lo) slow_path(4 * q + 2, v.z);
-          if (v.w > 0.0f && v.w >= s_lo) slow_path(4 * q + 3, v.w);
-        }
-        if (p.cands_only) my_hits = 0;
-        ssum_clean = true;
-      } else if (max_hits && ks.kind[0] == QW_SORT_SCORE && ks.order[0] == QW_ORDER_DESC && !sa_present && rscore && !n_aggs && !rec) {
+      if (max_hits && ks.kind[0] == QW_SORT_SCORE && ks.order[0] == QW_ORDER_DESC && !sa_present && rscore && !n_aggs && !rec) {
         // fast path (BM25 top-K): a float lower bound of the threshold bucket filters 4 docs per lane
         // per step; only survivors build the composite key. s_lo is conservative (one part in 2^20).
         float s_lo = -1.0f;
@@ -1628,20 +1449,7 @@ __global__ void __launch_bounds__(QW_THREADS, QW_MIN_BLOCKS_PER_SM) k_window(con
         }
       }
     } else {
-      if (UNION) {
-        // level-0 histogram of a BM25 union straight from the score array (digit = [1 | lin:10]);
-        // the sweep also clears the array for the next window
-        float4* sc4 = reinterpret_cast<float4*>(sm.f32(p.sm.lvl[0].ssum));
-        for (uint32_t q = tid; q < (W >> 2); q += QW_THREADS) {
-          const float4 v = sc4[q];
-          sc4[q] = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (v.x > 0.0f) atomicAdd(&s_hist[1024u | score_lin(ks, v.x, true)], 1u);
-          if (v.y > 0.0f) atomicAdd(&s_hist[1024u | score_lin(ks, v.y, true)], 1u);
-          if (v.z > 0.0f) atomicAdd(&s_hist[1024u | score_lin(ks, v.z, true)], 1u);
-          if (v.w > 0.0f) atomicAdd(&s_hist[1024u | score_lin(ks, v.w, true)], 1u);
-        }
-        ssum_clean = true;
-      } else if (max_hits) {
+      if (max_hits) {
         warp_for_hits(res, NW, warp, lane, s_hitq, [&](uint32_t i, bool on) {
           const uint32_t doc = ws + i;
           const float sc = (on && rscore) ? rscore[i] : 0.0f;

@@ -333,22 +333,21 @@ static void run_leaf_raw(Engine& eng, const pb::LeafSearchRequest& lr, LeafRun& 
     std::vector<SplitRequest> opt = optimize_split_requests(sreq, ast, dm.timestamp_field, ref.split_offsets);
     std::vector<const SplitRequest*> by_pos(ref.split_offsets.size(), nullptr);
     for (const SplitRequest& q : opt) by_pos[q.input_pos] = &q;
-    static const bool no_prune = getenv("QWGPU_NO_PRUNING") != nullptr;
     pb::SearchRequest count_req;
     bool have_count_req = false;
     for (size_t si = 0; si < ref.split_offsets.size(); si++) {
       const pb::SplitIdAndFooterOffsets& so = ref.split_offsets[si];
       const SplitRequest& q = *by_pos[si];
-      if (q.skipped && !comm && !no_prune) continue;  // (PrunedBeforeWarmup: contributes nothing, not even to the split counters)
+      if (q.skipped && !comm) continue;  // (PrunedBeforeWarmup: contributes nothing, not even to the split counters)
       SplitJob j;
       j.meta = so;
-      if (q.metadata_count && !comm && !no_prune) {
+      if (q.metadata_count && !comm) {
         j.metadata_count = true;
         run.jobs.push_back(std::move(j));
         continue;
       }
       const pb::SearchRequest* req = &sreq;
-      if (q.hits_disabled && !no_prune) {
+      if (q.hits_disabled) {
         if (!have_count_req) { count_req = sreq; disable_search_request_hits(count_req); have_count_req = true; }
         req = &count_req;
       }
@@ -379,12 +378,11 @@ static void run_leaf_raw(Engine& eng, const pb::LeafSearchRequest& lr, LeafRun& 
   auto t0 = clock::now();
   if (getenv("QWGPU_TRACE"))
     fprintf(stderr, "[qwgpu] compile: %ld us for %zu splits\n", (long)std::chrono::duration_cast<std::chrono::microseconds>(t0 - t_compile).count(), run.jobs.size());
-  static const bool host_merge = getenv("QWGPU_HOST_MERGE") != nullptr;
   MergeSpec ms;
   GatherSpec gs;
   const bool gathering = comm && comm->world > 1 && sreq.max_hits + sreq.start_offset > 0;
   if (gathering && !same_sort_types(run.jobs, run.which)) fail(QWGPU_EUNSUPPORTED, "the splits of this rank disagree on the sort field types: cross-rank merge on the device is not possible");
-  if ((gathering || (want_merged && !host_merge && devs.size() > 1)) && sreq.max_hits + sreq.start_offset > 0 && same_sort_types(run.jobs, run.which)) {
+  if ((gathering || (want_merged && devs.size() > 1)) && sreq.max_hits + sreq.start_offset > 0 && same_sort_types(run.jobs, run.which)) {
     int o1, o2;
     sort_orders(sreq, &o1, &o2);
     ms.k = (uint32_t)(sreq.max_hits + sreq.start_offset);

@@ -6,7 +6,7 @@
 //
 // One 448-thread block = 13 consumer warps + 1 producer warp, two blocks per SM. The block owns one
 // 16384-doc window of one split at a time (f32 score accumulator of the window in shared memory);
-// windows are handed out dynamically from a global counter.
+// each block walks its own contiguous chunk of the flat (split, window) list.
 //
 //   producer warp   per window: (1) lane = term: one load of the term's window-index entry (QwWinIdx)
 //                   gives the ordinals of the posting blocks overlapping the window; (2) lane = block:
@@ -35,34 +35,21 @@
 
 namespace qwk {
 
-#ifndef QU_THREADS
-/* 13 consumer warps + the producer, two blocks per SM: 72 registers per thread (sm_90a: 252 B of spill stores in the
+/* 13 consumer warps + the producer, two blocks per SM: 72 registers per thread (sm_90a: 204 B of spill stores in the
  * COLLECT instantiation). Measured on one H100 80GB HBM3 (400 W power limit), k_union<COLLECT> per launch on the bench
  * workload: 201-202 us; 384 threads / 80 registers (56 B of spills): 204-205 us; 512 threads / 64 registers (292 B of
  * spills): 211-213 us. */
 #define QU_THREADS 448
-#endif
 #define QU_NCW (QU_THREADS / 32 - 1)   /* consumer warps; warp QU_NCW is the producer */
 #define QU_NCT (QU_NCW * 32)
 #define QU_SLOTS 2
 #define QU_MAXBLK 128           /* block records per slot */
 #define QU_CHAIN 128            /* mbarriers in the stage ring (a warp is never > 70 stages ahead) */
 #define QU_MAX_TERMS 32
-#ifndef QU_SUSPEND_NS
 #define QU_SUSPEND_NS 100000u   /* try_wait suspend-time hint: a waiting warp sleeps in hardware instead of polling */
-#endif
 #define QU_PAD 32               /* decode may read one 16-byte word past a block */
 #define QU_CANDS 16             /* per-warp buffer of docs that reached the score lower bound */
-#ifndef QU_MINB
 #define QU_MINB 2               /* blocks per SM */
-#endif
-#ifndef QU_DEFER_SWEEP
-/* 1 = COLLECT sweeps a finished window only after the warp's first decode of the next window (overlaps the wait for the
- * window's last clauses with work). Measured on one H100 80GB HBM3 (400 W power limit): 401 us against 202 us per launch —
- * the decoded pair has to stay live across the sweep loop, and under the register cap that spills the inner loop (sm_90a:
- * 440 B of spill stores) — so it is off. */
-#define QU_DEFER_SWEEP 0
-#endif
 
 enum { QU_F_FIRST = 1u, QU_F_LAST = 2u, QU_F_END = 4u };
 
@@ -84,17 +71,8 @@ struct UParams {
   const DThresh* thresh;
   const uint32_t* first_work;  // prefix over splits of (sampled) window counts; [n_splits + 1]
   uint32_t n_splits, total_work, stride, W;
-  unsigned long long* prof;    // QU_PROFILE builds: cycle counters (see k_union)
-  uint32_t* work_ctr;          // dynamic hand-out of the windows (zero at launch); null = static chunks per block
   USmem sm;
 };
-#ifdef QU_PROFILE
-#define QU_T(x) const long long x = clock64()
-#define QU_ACC(acc, t0) acc += clock64() - (t0)
-#else
-#define QU_T(x)
-#define QU_ACC(acc, t0)
-#endif
 
 struct UHdr {  // 32 bytes, written by the producer when it closes a slot
   uint32_t ws, wlen, split, flags;
@@ -180,7 +158,9 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
   }
   __syncthreads();
 
-  // this block's chunk of the flat (split, window) list
+  // this block's chunk of the flat (split, window) list (handing windows out one at a time from a global counter was
+  // slower: consecutive windows of a block then belong to different splits, and the plan switch sits on the
+  // producer's critical path)
   const uint32_t w_begin = (uint32_t)(((uint64_t)p.total_work * blockIdx.x) / gridDim.x);
   const uint32_t w_end = (uint32_t)(((uint64_t)p.total_work * (blockIdx.x + 1)) / gridDim.x);
 
@@ -188,10 +168,6 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
     // ================================ producer ======================================================
     uint32_t seq = 0;            // slots closed so far
     uint32_t cur_split = 0;
-#ifdef QU_PROFILE
-    long long pt_empty = 0, pt_a = 0, pt_b = 0, pt_win = 0;
-    const long long pt_start = clock64();
-#endif
     // lane = term slot of the current split's plan
     uint64_t t_data = 0, t_widx = 0, t_skip = 0, t_tab = 0;
     uint32_t t_nblk = 0, t_shift = 0, t_fl = 0, t_sub16 = 0;
@@ -207,9 +183,7 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
     auto slot_base = [&](uint32_t s) { return p.sm.slot0 + s * p.sm.slot_stride; };
     auto open_slot = [&]() {
       slot = seq % QU_SLOTS;
-      QU_T(pt_e0);
       mbar_wait(bar_empty(slot), ((seq / QU_SLOTS) & 1u) ^ 1u);
-      QU_ACC(pt_empty, pt_e0);
       open = true; off = 0; cnt = 0;
       if (lane == 0) *(uint32_t*)(qw_smem + slot_base(slot) + p.sm.hdr + 32) = 0;  // next block to hand out
       if (lane < n_terms) {
@@ -264,15 +238,6 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
     auto window_of = [&](uint32_t work, uint32_t split) {
       return (work - __ldg(p.first_work + split)) * p.stride + (p.stride > 1 ? split % p.stride : 0);
     };
-
-    // Work items (windows) come either from this block's static chunk of the flat list or, when the host passes a
-    // counter, one at a time from that counter: blocks that start late (their SM was busy with another call's
-    // kernel) or hit denser windows simply take fewer, so the kernel's duration does not hinge on full residency.
-    const bool dyn = p.work_ctr != nullptr;
-    const uint32_t w_limit = dyn ? p.total_work : w_end;
-    uint32_t grabbed = 0;
-    auto grab_issue = [&]() { if (dyn && lane == 0) grabbed = atomicAdd(p.work_ctr, 1u); };
-    auto grab_take = [&](uint32_t after) { return dyn ? __shfl_sync(QW_FULL, grabbed, 0) : after + 1; };
     // split of a work item: number of prefix entries <= work, minus one (lane-parallel; empty splits share their entry)
     auto split_of = [&](uint32_t work) {
       uint32_t cnt = 0;
@@ -284,15 +249,12 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
     };
     uint32_t split = 0;
     uint32_t work = w_begin, next_work = w_begin + 1;
-    if (dyn) { grab_issue(); work = grab_take(0); grab_issue(); next_work = grab_take(0); }
-    if (work < w_limit) {
+    if (work < w_end) {
       split = split_of(work);
       load_plan(split);
       load_widx(window_of(work, split));
     }
-    for (; work < w_limit; ) {
-      grab_issue();  // the item after next: its latency hides behind this window's packing
-      QU_T(pt_w0);
+    for (; work < w_end; ) {
       const uint32_t window = window_of(work, split);
       ws = window * W;
       const uint32_t we = min(ws + W, num_docs);
@@ -304,7 +266,6 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
       const uint32_t incl_nb = warp_incl_scan(nb);
       const uint32_t gbase = incl_nb - nb;
       const uint32_t G = __shfl_sync(QW_FULL, incl_nb, 31);
-      QU_ACC(pt_a, pt_w0);
       // ---- lane = block: skip + checkpoint entries -> record, runs of blocks -> bulk copies ----------
       auto round_loads = [&](uint32_t q0, uint32_t& t_out, uint4& r_out, uint4& c_out, uint64_t& dat_out, uint32_t& tfl_out) {
         const uint32_t q = q0 + lane;
@@ -332,10 +293,9 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
       if (G) round_loads(0, t, r, ck, dat, tfl);
       // the next window's index entries fly while this window is packed (same split: same term constants)
       uint32_t nx_split = split;
-      const bool have_next = next_work < w_limit;
+      const bool have_next = next_work < w_end;
       if (have_next) {
-        if (dyn) nx_split = split_of(next_work);
-        else while (__ldg(p.first_work + nx_split + 1) <= next_work) nx_split++;
+        while (__ldg(p.first_work + nx_split + 1) <= next_work) nx_split++;
         if (nx_split == split) load_widx(window_of(next_work, split));
       }
       for (uint32_t q0 = 0; q0 < G; q0 += 32) {
@@ -387,10 +347,6 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
         }
         t = t2; tfl = tfl2; r = r2; ck = ck2; dat = dat2;
       }
-#ifdef QU_PROFILE
-      pt_win++;
-      QU_ACC(pt_b, pt_w0);
-#endif
       if (open) close_slot(QU_F_LAST);
       if (have_next && nx_split != split) {
         split = nx_split;
@@ -398,22 +354,12 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
         load_widx(window_of(next_work, split));
       }
       work = next_work;
-      next_work = grab_take(next_work);
+      next_work = work + 1;
     }
     // terminal slot
     open_slot();
     cnt = 0;
     close_slot(QU_F_END);
-#ifdef QU_PROFILE
-    if (lane == 0 && p.prof) {
-      atomicAdd(p.prof + 0, (unsigned long long)(clock64() - pt_start));
-      atomicAdd(p.prof + 1, (unsigned long long)pt_empty);
-      atomicAdd(p.prof + 2, (unsigned long long)pt_a);
-      atomicAdd(p.prof + 3, (unsigned long long)pt_b);
-      atomicAdd(p.prof + 4, (unsigned long long)pt_win);
-      atomicAdd(p.prof + 5, (unsigned long long)seq);
-    }
-#endif
   } else {
     // ================================ consumers =====================================================
     float* score = (float*)(qw_smem + p.sm.score);
@@ -434,10 +380,6 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
     uint2* cands = (uint2*)(qw_smem + p.sm.cands) + warp * QU_CANDS;
     uint32_t* ncand = (uint32_t*)(qw_smem + p.sm.cands + QU_NCW * QU_CANDS * 8) + warp;
     if (lane == 0) *ncand = 0;
-#ifdef QU_PROFILE
-    long long ct_full = 0, ct_chain = 0, ct_sweep = 0, ct_blocks = 0, ct_endwait = 0, ct_nblk = 0;
-    const long long ct_start = clock64();
-#endif
     auto pass_to = [&](uint32_t st) {  // arrive at every stage below st
       if (my_stage < st) {
         __syncwarp();
@@ -448,9 +390,7 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
     };
     auto wait_below = [&](uint32_t st) {  // all stages below st complete
       if (waited < st) {
-        QU_T(t0);
         mbar_wait(bar_chain(st - 1), chain_parity(st - 1));
-        QU_ACC(ct_chain, t0);
         waited = st;
       }
     };
@@ -498,18 +438,8 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
       my_hits = 0;
     };
 
-    // QU_DEFER_SWEEP builds: the sweep of a finished window is deferred until this warp has decoded its first pair of
-    // blocks of the next window (decode needs no ordering), so that the wait for the window's last clauses overlaps
-    // with work. Off by default (see the macro).
-    constexpr bool DEFER = (MODE == MODE_COLLECT) && (QU_DEFER_SWEEP != 0);
-    bool pend = false;
-    uint32_t p_ws = 0, p_split = 0, p_end = 0;
-    float p_hdr = 0.f;
     auto collect_sweep = [&](const uint32_t ws, const uint32_t split, const float s_lo, const uint32_t end_stage) {
-      QU_T(te0);
       wait_below(end_stage);  // every contribution of the window is in
-      QU_ACC(ct_endwait, te0);
-      QU_T(ts0);
       float4* sc4 = reinterpret_cast<float4*>(score);
       const uint32_t s_lo_bits = s_lo > 0.0f ? __float_as_uint(s_lo) : 1u;  // no threshold yet: every match goes on
 #pragma unroll 4
@@ -535,28 +465,20 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
       if (lane == 0) mbar_arrive(bar_chain(end_stage));
       my_stage = end_stage + 1;
       if (*ncand >= QU_CANDS / 2) flush_cands();  // (after the arrival: nobody waits for the global atomics)
-      QU_ACC(ct_sweep, ts0);
     };
 
     for (uint32_t seq = 0;; seq++) {
       const uint32_t slot = seq % QU_SLOTS;
-      QU_T(tf0);
       mbar_wait(bar_full(slot), (seq / QU_SLOTS) & 1u);
-      QU_ACC(ct_full, tf0);
-      QU_T(tb0);
       const uint32_t sl = p.sm.slot0 + slot * p.sm.slot_stride;
       const uint4 h0 = *(const uint4*)(qw_smem + sl + p.sm.hdr);
       const uint4 h1 = *(const uint4*)(qw_smem + sl + p.sm.hdr + 16);
       const uint32_t ws = h0.x, wlen = h0.y, split = h0.z, flags = h0.w;
       const uint32_t G = h1.x, n_terms = h1.y, t_last = h1.z;
       const float hdr_f = __uint_as_float(h1.w);
-      if (flags & QU_F_END) {
-        if (pend) collect_sweep(p_ws, p_split, p_hdr, p_end);
-        break;
-      }
+      if (flags & QU_F_END) break;
       if (flags & QU_F_FIRST) wbase = next_base;
       if (split != cur_split) {
-        if (pend) { collect_sweep(p_ws, p_split, p_hdr, p_end); pend = false; }  // (its hits belong to the old split)
         flush_hits();
         cur_split = split;
       }
@@ -567,9 +489,6 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
       // 32 x 4 split, a 4-step scan, and eight independent postings per lane for the scheduler to overlap.
       const uint32_t half = lane >> 4, hl = lane & 15u;
       for (uint32_t g0 = 2u * warp; g0 < G; g0 += 2u * QU_NCW) {
-#ifdef QU_PROFILE
-        ct_nblk += (g0 + 1 < G) ? 2 : 1;
-#endif
         const bool on = g0 + half < G;
         const uint4 rec = *(const uint4*)(qw_smem + recs + 16u * (on ? g0 + half : g0));  // prev_last_doc, shared address, widths/count, clause | interior
         const uint32_t t = rec.w & 0xFFu;
@@ -578,8 +497,7 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
         const uint32_t st = wbase + t;
         const uint32_t st_lo = __shfl_sync(QW_FULL, st, 0);
         const uint32_t st_hi = __shfl_sync(QW_FULL, on ? st : 0u, 16);  // (0: the upper half has no block)
-        const bool deferred = DEFER && pend;  // (warp-uniform) the previous window's sweep comes after this decode
-        if (!deferred) pass_to(st_lo);
+        pass_to(st_lo);
         const uint4 tt = *(const uint4*)(qw_smem + ttab + 16u * t);
         const float weight = __uint_as_float(tt.x);
         const float* tab = (const float*)(((uint64_t)tt.w << 32) | tt.z);
@@ -710,11 +628,6 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
             for (int j = 0; j < 8; j++) if (in[j]) score[r[j]] = __fadd_rn(o[j], c[j]);
           }
         };
-        if (deferred) {
-          collect_sweep(p_ws, p_split, p_hdr, p_end);
-          pend = false;
-          pass_to(st_lo);
-        }
         wait_below(st_lo);
         if (st_hi == st_lo || st_hi == 0u) apply();  // (lanes of an absent upper block have nvalid == 0)
         else {
@@ -725,10 +638,6 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
           if (half == 1) apply();
         }
       }
-#ifdef QU_PROFILE
-      ct_blocks += clock64() - tb0;
-#endif
-      if (DEFER && pend) { collect_sweep(p_ws, p_split, p_hdr, p_end); pend = false; }  // (no block of this slot was this warp's)
       // this warp is done reading the slot
       __syncwarp();
       if (lane == 0) mbar_arrive(bar_empty(slot));
@@ -749,8 +658,7 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
       if (MODE == MODE_COLLECT) {
         // ---- sweep: count matches (score > 0), test against the threshold, clear ----------------------
         next_base = end_stage + 1;
-        if (DEFER) { pend = true; p_ws = ws; p_split = split; p_hdr = hdr_f; p_end = end_stage; }
-        else collect_sweep(ws, split, hdr_f, end_stage);
+        collect_sweep(ws, split, hdr_f, end_stage);
       } else {
         // level-0 digit histogram of the sampled windows: digit = [1 | lin:10] (score_lin)
         wait_below(end_stage);  // every contribution of the window is in
@@ -782,18 +690,6 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
       }
     }
     flush_hits();
-#ifdef QU_PROFILE
-    if (lane == 0 && p.prof) {
-      atomicAdd(p.prof + 8, (unsigned long long)(clock64() - ct_start));
-      atomicAdd(p.prof + 9, (unsigned long long)ct_full);
-      atomicAdd(p.prof + 10, (unsigned long long)ct_chain);   // includes the end-of-window wait
-      atomicAdd(p.prof + 11, (unsigned long long)ct_endwait);
-      atomicAdd(p.prof + 12, (unsigned long long)ct_sweep);
-      atomicAdd(p.prof + 13, (unsigned long long)ct_blocks);  // block loop incl. chain waits inside it
-      atomicAdd(p.prof + 14, (unsigned long long)ct_nblk);
-      atomicAdd(p.prof + 15, 1ull);
-    }
-#endif
   }
 }
 
