@@ -151,6 +151,8 @@ typedef struct qwgpu_split_result {
                                                and the batch ran again with every hashed table at its bound. The
                                                other statistics of such a call (time, launches, radix passes,
                                                fallbacks, bytes) add up both runs. */
+#define QWGPU_KERNEL_COMPOSITE_CUT 1024u /* k_composite_cut cut the composite aggregations of the batch's hashed
+                                            splits to their first `size` buckets before the copy-back */
 /* Initial capacity of a split's hashed cell table: min(this, the split's bound on distinct cells). */
 #define QWGPU_HASHED_INIT_CELLS 65536u
 /* Largest total of the hashed tables (cells, key records and slots, each at its split's bound) that one call may

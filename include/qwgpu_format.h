@@ -253,6 +253,35 @@ enum {
 
 #define QW_MAX_AGG_RANGES 16
 
+/* Composite aggregation (DESIGN.md §4.4, composite): a composite with sources s1..sn lowers to a chain of n
+ * QW_AGG_TERMS / QW_AGG_HISTOGRAM nodes, each the only child of the one before, with the composite's
+ * sub-aggregations below the last. Each source node carries the composite descriptor in fields its kind does not
+ * use:
+ *   reserved      = QW_AGG_COMP_* flags (0 on every node that is not a composite source);
+ *   range_to[0]   = the composite's `size`;
+ *   range_from[0] = the split's bound for the `after` value of this source, in the node's key space (TERMS: the
+ *                   bit-packed raw value, HISTOGRAM: the bucket index relative to base_pos): with ascending order
+ *                   the smallest key that is not before `after`, with descending order the largest; EXACT when
+ *                   that key equals `after`, AFTER_ALL when every key of the split comes before it.
+ * A `missing_bucket` source sets has_missing; on a HISTOGRAM node the missing bucket is the last of num_buckets
+ * and its entries carry QW_AGG_ENTRY_MISSING, as on TERMS. The walk keeps a key of a composite level only when its
+ * path is not before the `after` tuple; HAS_AFTER is cleared on every level when a split cannot place `after` in
+ * its key spaces (the host filters then, and AFTER_HOST is set). After the walk, k_composite_cut keeps each
+ * composite's first `size` leaves with their chains and sub-aggregation entries (composite_kernel.cuh). */
+enum {
+  QW_AGG_COMP_LEVEL = 1u,      /* the node is a source of a composite aggregation */
+  QW_AGG_COMP_LAST = 2u,       /* the last source of its composite */
+  QW_AGG_COMP_DESC = 4u,       /* `order: desc` (null last; ascending order puts null first) */
+  QW_AGG_COMP_MISSING = 8u,    /* `missing_bucket: true` */
+  QW_AGG_COMP_HAS_AFTER = 16u, /* filter this level against range_from[0] */
+  QW_AGG_COMP_AFTER_NULL = 32u,/* the `after` value of this source is null */
+  QW_AGG_COMP_EXACT = 64u,     /* range_from[0] is `after` itself */
+  QW_AGG_COMP_AFTER_ALL = 128u, /* every non-null key of the split comes before `after` */
+  QW_AGG_COMP_AFTER_HOST = 256u /* the request has `after` but the walk does not filter (HAS_AFTER cleared): the
+                                   device does not cut the composite either, the host filters and cuts */
+};
+#define QW_AGG_COMP_MAX_SIZE 65000u /* the reference's default aggregation_bucket_limit */
+
 /* One aggregation node. Bucket aggregations may have children (sub-aggregations):
  * nodes [first_child, first_child+num_children). Top-level aggs have parent == 0xFFFFFFFF. */
 typedef struct QwAggNode {
@@ -272,8 +301,8 @@ typedef struct QwAggNode {
   /* RANGE: bucket i = [range_from[i], range_to[i]) in mapped-u64 space */
   uint64_t range_from[QW_MAX_AGG_RANGES], range_to[QW_MAX_AGG_RANGES];
   /* TERMS on numeric columns: dense index = raw value; on STR: ordinal */
-  uint32_t has_missing;  /* `missing` parameter present */
-  uint32_t reserved;
+  uint32_t has_missing;  /* `missing` parameter present (composite: `missing_bucket`) */
+  uint32_t reserved;     /* TRACE_IDS: the timestamp column; TERMS / HISTOGRAM: QW_AGG_COMP_* flags */
   uint64_t missing_value; /* mapped-u64 (numeric) or ordinal==dict_num_terms for "new key" */
 } QwAggNode;
 
@@ -341,7 +370,7 @@ typedef struct QwAggEntry {
   QwAggCell cell;
 } QwAggEntry; /* 56 bytes */
 
-/* 1 when the plan's aggregation tree takes the hashed layout: a node below two bucket ancestors that is not a
+/* 1 when the plan's aggregation tree takes the hashed layout: a composite source node, a node below two bucket ancestors that is not a
  * metric (or any node below three), the dense cells of all nodes adding up to more than QW_AGG_DENSE_MAX_CELLS,
  * or a TERMS node whose dense space (num_buckets without the `missing` slot) exceeds QW_AGG_DENSE_MAX_TERMS.
  * Reads only the plan; the caller has checked every parent index. */
@@ -349,6 +378,7 @@ static inline int qw_agg_hashed(const QwAggNode* nodes, uint32_t n) {
   uint64_t total = 0;
   for (uint32_t i = 0; i < n; i++) {
     const QwAggNode* g = &nodes[i];
+    if ((g->kind == QW_AGG_TERMS || g->kind == QW_AGG_HISTOGRAM) && (g->reserved & QW_AGG_COMP_LEVEL)) return 1;
     if (g->kind == QW_AGG_TERMS && (uint64_t)g->num_buckets - (g->has_missing ? 1u : 0u) > QW_AGG_DENSE_MAX_TERMS) return 1;
     uint32_t depth = 0;
     uint64_t cells = g->kind == QW_AGG_STATS ? 1 : g->num_buckets;

@@ -10,6 +10,7 @@
 //   * final: into_final_result (quickwit-search/src/root.rs:1105-1135): buckets cut to `size`,
 //     histogram gaps filled when min_doc_count == 0, extended_bounds, key_as_string.
 #include <algorithm>
+#include <cerrno>
 #include <cmath>
 #include <map>
 #include <set>
@@ -51,6 +52,103 @@ static double num_or(const Json& j, const char* k, double d) {
   return d;
 }
 
+// `after` value of a composite source: type-tagged strings ("str:…", "i64:…", "u64:…", "f64:…", "bool:…", the form
+// after_key is written in) or plain JSON strings, numbers, booleans and null
+static CompKey parse_after_value(const Json& v, const std::string& src) {
+  CompKey k;
+  auto bad = [&]() { fail(QWGPU_EINVALID_AGG, "composite `after` value of source `%s` is not a valid key", src.c_str()); };
+  switch (v.type) {
+    case Json::Null: k.t = CompKey::Null; return k;
+    case Json::Bool: k.t = CompKey::Bool; k.u = v.b ? 1 : 0; return k;
+    case Json::U64: k.t = CompKey::U64; k.u = v.u; return k;
+    case Json::I64: k.t = CompKey::I64; k.i = v.i; return k;
+    case Json::F64: k.t = CompKey::F64; k.f = v.f; return k;
+    case Json::Str: break;
+    default: bad();
+  }
+  const std::string& s = v.s;
+  const size_t colon = s.find(':');
+  const std::string tag = colon == std::string::npos ? "" : s.substr(0, colon), rest = colon == std::string::npos ? "" : s.substr(colon + 1);
+  char* end = nullptr;
+  errno = 0;
+  if (tag == "str") { k.t = CompKey::Str; k.s = rest; }
+  else if (tag == "i64") { k.t = CompKey::I64; k.i = strtoll(rest.c_str(), &end, 10); if (rest.empty() || *end || errno) bad(); }
+  else if (tag == "u64") { k.t = CompKey::U64; k.u = strtoull(rest.c_str(), &end, 10); if (rest.empty() || rest[0] == '-' || *end || errno) bad(); }
+  else if (tag == "f64") { k.t = CompKey::F64; k.f = strtod(rest.c_str(), &end); if (rest.empty() || *end) bad(); }
+  else if (tag == "bool") { k.t = CompKey::Bool; if (rest != "true" && rest != "false") bad(); k.u = rest == "true"; }
+  else { k.t = CompKey::Str; k.s = s; }
+  return k;
+}
+
+// composite: {"size": n, "sources": [{name: {terms | histogram | date_histogram: {...}}}, ...], "after": {...}}
+static void parse_composite(const Json& spec, AggReq& a, int depth) {
+  if (depth > 0) fail(QWGPU_EUNSUPPORTED, "composite aggregation `%s` below another aggregation is not implemented on the GPU path", a.name.c_str());
+  if (!spec.is_obj()) fail(QWGPU_EINVALID_AGG, "composite aggregation `%s` must be a JSON object", a.name.c_str());
+  a.kind = AggReq::Composite;
+  const double size = num_or(spec, "size", 10);
+  if (!(size >= 1) || size != std::floor(size)) fail(QWGPU_EINVALID_AGG, "composite `size` must be a positive integer");
+  if (size > QW_AGG_COMP_MAX_SIZE) fail(QWGPU_EUNSUPPORTED, "composite `size` %g exceeds the bucket limit %u", size, QW_AGG_COMP_MAX_SIZE);
+  a.size = (uint32_t)size;
+  const Json* srcs = spec.get("sources");
+  if (!srcs || !srcs->is_arr() || srcs->arr.empty()) fail(QWGPU_EINVALID_AGG, "composite aggregation `%s` requires a non-empty `sources` list", a.name.c_str());
+  for (const Json& e : srcs->arr) {
+    if (!e.is_obj() || e.obj.size() != 1 || !e.obj[0].second.is_obj() || e.obj[0].second.obj.size() != 1)
+      fail(QWGPU_EINVALID_AGG, "a composite source must be an object {name: {type: {...}}}");
+    AggReq s;
+    s.name = e.obj[0].first;
+    for (const AggReq& o : a.sources) if (o.name == s.name) fail(QWGPU_EINVALID_AGG, "duplicate composite source name `%s`", s.name.c_str());
+    const std::string& t = e.obj[0].second.obj[0].first;
+    const Json& p = e.obj[0].second.obj[0].second;
+    if (!p.is_obj()) fail(QWGPU_EINVALID_AGG, "composite source `%s` must be a JSON object", s.name.c_str());
+    for (const char* k : {"missing_order", "format", "script", "calendar_interval", "time_zone"})
+      if (p.get(k)) fail(QWGPU_EUNSUPPORTED, "`%s` of composite source `%s` is not implemented on the GPU path", k, s.name.c_str());
+    const Json* f = p.get("field");
+    if (!f || !f->is_str()) fail(QWGPU_EINVALID_AGG, "composite source `%s` requires a `field`", s.name.c_str());
+    s.field = f->s;
+    if (t == "terms") s.kind = AggReq::Terms;
+    else if (t == "histogram") {
+      s.kind = AggReq::Histogram;
+      s.interval = num_or(p, "interval", 0);
+      s.offset = num_or(p, "offset", 0);
+    } else if (t == "date_histogram") {
+      s.kind = AggReq::DateHistogram;
+      const Json* fi = p.get("fixed_interval");
+      if (p.get("interval") || !fi || !fi->is_str()) fail(QWGPU_EINVALID_AGG, "composite date_histogram source `%s` requires `fixed_interval`", s.name.c_str());
+      s.interval = parse_duration_ms(fi->s, false);
+      if (const Json* off = p.get("offset")) s.offset = off->is_str() ? parse_duration_ms(off->s, true) : off->as_f64();
+    } else fail(QWGPU_EINVALID_AGG, "unknown composite source type `%s`", t.c_str());
+    if (s.kind != AggReq::Terms && !(s.interval > 0)) fail(QWGPU_EINVALID_AGG, "histogram interval must be larger than 0");
+    s.order_desc = false;
+    if (const Json* o = p.get("order")) {
+      if (!o->is_str() || (o->s != "asc" && o->s != "desc")) fail(QWGPU_EINVALID_AGG, "composite source `%s`: `order` must be \"asc\" or \"desc\"", s.name.c_str());
+      s.order_desc = o->s == "desc";
+    }
+    s.has_missing = p.bool_or("missing_bucket", false);
+    a.sources.push_back(std::move(s));
+  }
+  if (const Json* af = spec.get("after")) {
+    if (!af->is_obj()) fail(QWGPU_EINVALID_AGG, "composite `after` must be an object");
+    a.has_after = true;
+    a.after.resize(a.sources.size());
+    std::vector<bool> seen(a.sources.size(), false);
+    for (auto& kv : af->obj) {
+      size_t i = 0;
+      while (i < a.sources.size() && a.sources[i].name != kv.first) i++;
+      if (i == a.sources.size()) fail(QWGPU_EINVALID_AGG, "composite `after` names `%s`, which is not a source", kv.first.c_str());
+      if (seen[i]) fail(QWGPU_EINVALID_AGG, "composite `after` names `%s` twice", kv.first.c_str());
+      seen[i] = true;
+      const AggReq& s = a.sources[i];
+      CompKey k = parse_after_value(kv.second, s.name);
+      if (k.t == CompKey::Null && !s.has_missing) fail(QWGPU_EINVALID_AGG, "composite `after` is null for source `%s`, which has no missing_bucket", s.name.c_str());
+      if (s.kind != AggReq::Terms && k.t != CompKey::Null && !k.numeric())
+        fail(QWGPU_EINVALID_AGG, "composite `after` value of histogram source `%s` must be a number", s.name.c_str());
+      a.after[i] = std::move(k);
+    }
+    for (size_t i = 0; i < seen.size(); i++)
+      if (!seen[i]) fail(QWGPU_EINVALID_AGG, "composite `after` lacks source `%s`", a.sources[i].name.c_str());
+  }
+}
+
 static void parse_agg_map(const Json& j, std::vector<AggReq>& out, int depth) {
   if (!j.is_obj()) fail(QWGPU_EINVALID_AGG, "aggregation request must be a JSON object");
   if (depth > 8) fail(QWGPU_EINVALID_AGG, "aggregation nesting too deep");
@@ -66,7 +164,8 @@ static void parse_agg_map(const Json& j, std::vector<AggReq>& out, int depth) {
       if (found) fail(QWGPU_EINVALID_AGG, "aggregation `%s` has more than one type", a.name.c_str());
       found = true;
       a.field = spec.str_or("field", "");
-      if (t == "terms") {
+      if (t == "composite") parse_composite(spec, a, depth);
+      else if (t == "terms") {
         a.kind = AggReq::Terms;
         a.size = (uint32_t)num_or(spec, "size", 10);
         double ss = -1;
@@ -118,7 +217,7 @@ static void parse_agg_map(const Json& j, std::vector<AggReq>& out, int depth) {
       else if (t == "min") a.kind = AggReq::Min;
       else if (t == "max") a.kind = AggReq::Max;
       else if (t == "value_count" || t == "count") a.kind = AggReq::Count;
-      else if (t == "percentiles" || t == "cardinality" || t == "extended_stats" || t == "composite" || t == "top_hits" || t == "filter")
+      else if (t == "percentiles" || t == "cardinality" || t == "extended_stats" || t == "top_hits" || t == "filter")
         fail(QWGPU_EUNSUPPORTED, "`%s` aggregations are not implemented on the GPU path yet", t.c_str());
       else fail(QWGPU_EINVALID_AGG, "unknown aggregation type `%s`", t.c_str());
     }
@@ -173,7 +272,174 @@ static uint64_t f64_bound_to_mapped(uint32_t type, double v) {  // smallest mapp
   }
 }
 
-static QwAggNode lower_one(const AggReq& a, const ImageView& img, AggBinding& b) {
+// Exact order between two non-null integers / floats of any of the three numeric key types: -1, 0, 1
+static int num_cmp(const CompKey& x, const CompKey& y) {
+  auto ld = [](const CompKey& k) { return k.t == CompKey::I64 ? (long double)k.i : k.t == CompKey::U64 ? (long double)k.u : (long double)k.f; };
+  if (x.t == CompKey::F64 || y.t == CompKey::F64) {
+    const long double a = ld(x), b = ld(y);  // (64-bit mantissa: every i64 / u64 is exact)
+    if (std::isnan(a) || std::isnan(b)) return std::isnan(a) - std::isnan(b);
+    return a < b ? -1 : (a > b ? 1 : 0);
+  }
+  if (x.t == y.t) return x.t == CompKey::I64 ? (x.i < y.i ? -1 : x.i > y.i) : (x.u < y.u ? -1 : x.u > y.u);
+  if (x.t == CompKey::I64) return x.i < 0 ? -1 : ((uint64_t)x.i < y.u ? -1 : (uint64_t)x.i > y.u);
+  return y.i < 0 ? 1 : (x.u < (uint64_t)y.i ? -1 : x.u > (uint64_t)y.i);
+}
+// Ascending order of one key position: null first, then bool, string (bytes), number (by value); keys of
+// different columns types only meet when one field has different types in different splits
+static int key_cmp(const CompKey& x, const CompKey& y) {
+  const int rx = x.numeric() ? 3 : (int)x.t, ry = y.numeric() ? 3 : (int)y.t;
+  if (rx != ry) return rx < ry ? -1 : 1;
+  switch (rx) {
+    case CompKey::Null: return 0;
+    case CompKey::Bool: return x.u < y.u ? -1 : x.u > y.u;
+    case CompKey::Str: { const int c = x.s.compare(y.s); return c < 0 ? -1 : c > 0; }
+    default: return num_cmp(x, y);
+  }
+}
+
+// The key of histogram position `pos` of a composite source: the histogram aggregation's bucket key
+// (pos * interval + offset, in request units); a date_histogram key is the i64 of its epoch milliseconds
+static CompKey comp_hist_key(const QwAggNode& n, uint32_t col_type, bool date, int64_t pos) {
+  const double unit = col_type == QW_COL_DATETIME ? 1e6 : 1.0;
+  CompKey c;
+  c.f = ((double)pos * n.interval + n.offset) / unit;
+  if (date) { c.t = CompKey::I64; c.i = (int64_t)std::llround(c.f); }
+  else c.t = CompKey::F64;
+  return c;
+}
+
+// The key space bound of one composite source node for its `after` value on this split (QwAggNode doc in
+// qwgpu_format.h): false when the split's column cannot hold a key of after's type (the host filters alone then).
+static bool comp_after_bound(const QwAggNode& n, const QwImgColumn* col, const ImageView& img, const AggReq& s, const CompKey& k,
+                             uint64_t& bound, uint32_t& flags) {
+  const bool desc = s.order_desc;
+  bound = 0;
+  if (k.t == CompKey::Null) { flags |= QW_AGG_COMP_AFTER_NULL; return true; }
+  const uint64_t nb = n.num_buckets - (n.has_missing ? 1u : 0u);
+  if (!col || !col->num_vals || nb == 0) { flags |= QW_AGG_COMP_AFTER_ALL; return true; }  // only null keys here
+  bool exact = false;
+  if (n.kind == QW_AGG_HISTOGRAM) {
+    const double unit = col->type == QW_COL_DATETIME ? 1e6 : 1.0;
+    auto key = [&](int64_t p) { return comp_hist_key(n, col->type, s.kind == AggReq::DateHistogram, p); };
+    const double pos = std::floor(((k.t == CompKey::F64 ? k.f : k.t == CompKey::I64 ? (double)k.i : (double)k.u) * unit - n.offset) / n.interval);
+    if (!std::isfinite(pos) || std::fabs(pos) > 9e15) return false;
+    // the position from the formula, corrected by a few steps for the rounding of key(); keys that stay equal over
+    // more positions than that (an offset far larger than the interval) leave the filter to the host
+    int64_t q = (int64_t)pos;
+    int steps = 0;
+    if (!desc) {  // smallest position whose key is >= after
+      while (num_cmp(key(q), k) < 0 && steps++ < 4) q++;
+      while (num_cmp(key(q - 1), k) >= 0 && steps++ < 8) q--;
+      if (num_cmp(key(q), k) < 0 || num_cmp(key(q - 1), k) >= 0) return false;
+    } else {      // largest position whose key is <= after
+      while (num_cmp(key(q), k) > 0 && steps++ < 4) q--;
+      while (num_cmp(key(q + 1), k) <= 0 && steps++ < 8) q++;
+      if (num_cmp(key(q), k) > 0 || num_cmp(key(q + 1), k) <= 0) return false;
+    }
+    exact = num_cmp(key(q), k) == 0;
+    const int64_t idx = q - n.base_pos;
+    if (!desc) {
+      if (idx < 0) { bound = 0; exact = false; }
+      else if ((uint64_t)idx >= nb) { flags |= QW_AGG_COMP_AFTER_ALL; return true; }
+      else bound = (uint64_t)idx;
+    } else {
+      if (idx < 0) { flags |= QW_AGG_COMP_AFTER_ALL; return true; }
+      else if ((uint64_t)idx >= nb) { bound = nb - 1; exact = false; }
+      else bound = (uint64_t)idx;
+    }
+    if (exact) flags |= QW_AGG_COMP_EXACT;
+    return true;
+  }
+  // TERMS: the after value in the column's mapped space (desc: the largest mapped value <= after, else the smallest >=)
+  uint64_t m = 0;
+  if (col->type == QW_COL_STR) {
+    if (k.t != CompKey::Str) return false;
+    const uint32_t lb = img.dict_lower_bound(*col, (const uint8_t*)k.s.data(), (uint32_t)k.s.size(), &exact);
+    if (!desc) { if (lb >= col->dict_num_terms) { flags |= QW_AGG_COMP_AFTER_ALL; return true; } m = lb; }
+    else if (exact) m = lb;
+    else { if (lb == 0) { flags |= QW_AGG_COMP_AFTER_ALL; return true; } m = lb - 1; }
+  } else if (col->type == QW_COL_BOOL) {
+    if (k.t != CompKey::Bool) return false;
+    m = k.u;
+    exact = true;
+  } else {
+    if (!k.numeric()) return false;
+    // the key type of the column's values, and the mapped value of the nearest one on the side that is kept
+    const bool is_f = col->type == QW_COL_F64, is_i = col->type == QW_COL_I64 || col->type == QW_COL_DATETIME;
+    CompKey lo_t, hi_t;  // the column type's range
+    if (is_f) {
+      if (k.t == CompKey::F64 && std::isnan(k.f)) return false;
+      const double v = k.t == CompKey::F64 ? k.f : (k.t == CompKey::I64 ? (double)k.i : (double)k.u);
+      CompKey c; c.t = CompKey::F64; c.f = v;
+      const int cmp = num_cmp(c, k);  // the double nearest `after`, and where it lies
+      double w = v;
+      if (!desc && cmp < 0) w = std::nextafter(v, INFINITY);
+      if (desc && cmp > 0) w = std::nextafter(v, -INFINITY);
+      m = f64_to_u64(w == 0.0 ? 0.0 : w);
+      exact = cmp == 0;
+    } else {
+      // integers: clamp `after` into the type's range, rounding towards the kept side
+      long double v = k.t == CompKey::I64 ? (long double)k.i : k.t == CompKey::U64 ? (long double)k.u : (long double)k.f;
+      const long double lo = is_i ? -9223372036854775808.0L : 0.0L, hi = is_i ? 9223372036854775807.0L : 18446744073709551615.0L;
+      long double r = desc ? std::floor(v) : std::ceil(v);
+      exact = r == v && v >= lo && v <= hi;
+      if (r < lo) { if (desc) { flags |= QW_AGG_COMP_AFTER_ALL; return true; } r = lo; }
+      if (r > hi) { if (!desc) { flags |= QW_AGG_COMP_AFTER_ALL; return true; } r = hi; }
+      m = is_i ? i64_to_u64((int64_t)r) : (uint64_t)r;
+    }
+  }
+  // mapped -> bit-packed raw (raw = (mapped - min) / gcd), rounding towards the kept side
+  if (!desc) {
+    if (m > col->max_value) { flags |= QW_AGG_COMP_AFTER_ALL; return true; }
+    if (m < col->min_value) { bound = 0; exact = false; }
+    else {
+      const uint64_t d = m - col->min_value;
+      bound = d / col->gcd + (d % col->gcd ? 1 : 0);
+      exact = exact && d % col->gcd == 0;
+    }
+  } else {
+    if (m < col->min_value) { flags |= QW_AGG_COMP_AFTER_ALL; return true; }
+    if (m > col->max_value) { bound = (col->max_value - col->min_value) / col->gcd; exact = false; }
+    else {
+      const uint64_t d = m - col->min_value;
+      bound = d / col->gcd;
+      exact = exact && d % col->gcd == 0;
+    }
+  }
+  if (exact) flags |= QW_AGG_COMP_EXACT;
+  return true;
+}
+
+static QwAggNode lower_one(const AggReq& a, const ImageView& img, AggBinding& b, uint32_t comp_level = 0);
+// source `level` of composite `a`: the source's own node, with the composite descriptor
+static QwAggNode lower_comp_source(const AggReq& a, const ImageView& img, AggBinding& b, uint32_t level) {
+  const AggReq& s = a.sources[level];
+  QwAggNode n = lower_one(s, img, b);
+  b.req = &a;
+  b.comp_level = level;
+  if (s.has_missing && n.kind == QW_AGG_HISTOGRAM) n.num_buckets++;  // the missing bucket, last (as terms)
+  n.has_missing = s.has_missing;
+  uint32_t flags = QW_AGG_COMP_LEVEL | (level + 1 == a.sources.size() ? (uint32_t)QW_AGG_COMP_LAST : 0u) |
+                   (s.order_desc ? (uint32_t)QW_AGG_COMP_DESC : 0u) | (s.has_missing ? (uint32_t)QW_AGG_COMP_MISSING : 0u);
+  if (a.has_after && b.column >= 0 && a.after[level].t != CompKey::Null) {
+    // a terms source's `after` value must have its column's key type (histogram sources were checked at parse time)
+    const uint32_t ct = img.columns[b.column].type;
+    const CompKey& k = a.after[level];
+    if ((ct == QW_COL_STR && k.t != CompKey::Str) || (ct == QW_COL_BOOL && k.t != CompKey::Bool) ||
+        (ct != QW_COL_STR && ct != QW_COL_BOOL && !k.numeric()))
+      fail(QWGPU_EINVALID_AGG, "composite `after` value of source `%s` does not match the type of field `%s`", s.name.c_str(), s.field.c_str());
+  }
+  uint64_t bound = 0;
+  if (a.has_after && comp_after_bound(n, b.column >= 0 ? &img.columns[b.column] : nullptr, img, s, a.after[level], bound, flags))
+    flags |= QW_AGG_COMP_HAS_AFTER;
+  n.reserved = flags;
+  n.range_from[0] = bound;
+  n.range_to[0] = a.size;
+  return n;
+}
+
+static QwAggNode lower_one(const AggReq& a, const ImageView& img, AggBinding& b, uint32_t comp_level) {
+  if (a.kind == AggReq::Composite) return lower_comp_source(a, img, b, comp_level);
   QwAggNode n;
   memset(&n, 0, sizeof n);
   n.parent = 0xFFFFFFFFu;
@@ -246,16 +512,28 @@ static QwAggNode lower_one(const AggReq& a, const ImageView& img, AggBinding& b)
 std::vector<QwAggNode> lower_aggs(const std::vector<AggReq>& reqs, const ImageView& img, std::vector<AggBinding>& bindings) {
   std::vector<QwAggNode> out;
   bindings.clear();
-  struct Pending { const AggReq* a; uint32_t idx; };
+  struct Pending { const AggReq* a; uint32_t idx, level; };
   std::vector<Pending> queue;
   for (auto& a : reqs) {
     AggBinding b;
     out.push_back(lower_one(a, img, b));
     bindings.push_back(b);
-    queue.push_back({&a, (uint32_t)out.size() - 1});
+    queue.push_back({&a, (uint32_t)out.size() - 1, 0});
   }
   for (size_t qi = 0; qi < queue.size(); qi++) {
     Pending p = queue[qi];
+    if (p.a->kind == AggReq::Composite && p.level + 1 < p.a->sources.size()) {
+      // a composite's sources form a chain: the next source is the only child
+      out[p.idx].first_child = (uint32_t)out.size();
+      out[p.idx].num_children = 1;
+      AggBinding b;
+      QwAggNode n = lower_one(*p.a, img, b, p.level + 1);
+      n.parent = p.idx;
+      out.push_back(n);
+      bindings.push_back(b);
+      queue.push_back({p.a, (uint32_t)out.size() - 1, p.level + 1});
+      continue;
+    }
     if (p.a->children.empty()) continue;
     out[p.idx].first_child = (uint32_t)out.size();
     out[p.idx].num_children = (uint32_t)p.a->children.size();
@@ -265,8 +543,19 @@ std::vector<QwAggNode> lower_aggs(const std::vector<AggReq>& reqs, const ImageVi
       n.parent = p.idx;
       out.push_back(n);
       bindings.push_back(b);
-      queue.push_back({&c, (uint32_t)out.size() - 1});
+      queue.push_back({&c, (uint32_t)out.size() - 1, 0});
     }
+  }
+  // the walk filters a composite only when the split places `after` in the key space of every source; otherwise the
+  // host alone filters and cuts it (AFTER_HOST)
+  for (size_t i = 0; i < out.size(); i++) {
+    const AggReq* r = bindings[i].req;
+    if (r->kind != AggReq::Composite || bindings[i].comp_level != 0) continue;
+    bool all = true;
+    for (size_t j = i; j < out.size(); j++) if (bindings[j].req == r && !(out[j].reserved & QW_AGG_COMP_HAS_AFTER)) all = false;
+    if (r->has_after && !all)
+      for (size_t j = i; j < out.size(); j++)
+        if (bindings[j].req == r) out[j].reserved = (out[j].reserved & ~(uint32_t)QW_AGG_COMP_HAS_AFTER) | QW_AGG_COMP_AFTER_HOST;
   }
   return out;
 }
@@ -292,6 +581,7 @@ struct IAgg;
 struct IBucket {
   IKey key;        // terms
   double hkey = 0;  // histogram (column units) / range index
+  std::vector<CompKey> ckey;  // composite: one key per source
   uint64_t count = 0;
   std::vector<IAgg> subs;
 };
@@ -332,6 +622,26 @@ struct BR {
 static void ser_aggs(BW& w, const std::vector<IAgg>& v);
 static void ser_agg(BW& w, const IAgg& a) {
   w.varint(a.kind);
+  if (a.kind == AggReq::Composite) {
+    // per bucket: the key tuple (type, value per source), doc_count, sub-aggregations
+    w.varint(a.buckets.size());
+    for (auto& b : a.buckets) {
+      w.varint(b.ckey.size());
+      for (const CompKey& k : b.ckey) {
+        w.varint(k.t);
+        switch (k.t) {
+          case CompKey::Null: break;
+          case CompKey::Str: w.str(k.s); break;
+          case CompKey::I64: w.varint((uint64_t)k.i); break;
+          case CompKey::F64: w.f64(k.f); break;
+          default: w.varint(k.u);
+        }
+      }
+      w.varint(b.count);
+      ser_aggs(w, b.subs);
+    }
+    return;
+  }
   if (a.kind >= AggReq::Stats) { w.varint(a.m_count); w.f64(a.m_sum); w.f64(a.m_min); w.f64(a.m_max); return; }
   w.varint(a.is_date);
   w.varint(a.sum_other);
@@ -354,6 +664,31 @@ static std::vector<IAgg> de_aggs(BR& r);
 static IAgg de_agg(BR& r) {
   IAgg a;
   a.kind = (uint8_t)r.varint();
+  if (a.kind == AggReq::Composite) {
+    const uint64_t n = r.varint();
+    for (uint64_t i = 0; i < n; i++) {
+      IBucket b;
+      const uint64_t nk = r.varint();
+      if (nk > (uint64_t)(r.e - r.p)) fail(QWGPU_EINTERNAL, "failed to merge intermediate aggregation results: truncated buffer");
+      b.ckey.resize(nk);
+      for (CompKey& k : b.ckey) {
+        const uint64_t t = r.varint();
+        if (t > CompKey::F64) fail(QWGPU_EINTERNAL, "failed to merge intermediate aggregation results: bad composite key");
+        k.t = (CompKey::T)t;
+        switch (k.t) {
+          case CompKey::Null: break;
+          case CompKey::Str: k.s = r.str(); break;
+          case CompKey::I64: k.i = (int64_t)r.varint(); break;
+          case CompKey::F64: k.f = r.f64(); break;
+          default: k.u = r.varint();
+        }
+      }
+      b.count = r.varint();
+      b.subs = de_aggs(r);
+      a.buckets.push_back(std::move(b));
+    }
+    return a;
+  }
   if (a.kind >= AggReq::Stats) { a.m_count = r.varint(); a.m_sum = r.f64(); a.m_min = r.f64(); a.m_max = r.f64(); return a; }
   a.is_date = (uint8_t)r.varint();
   a.sum_other = r.varint();
@@ -504,10 +839,35 @@ static void cut_terms(const AggReq& req, IAgg& a) {
   }
 }
 
+// ---- composite: key order, the `after` filter and the cut to `size` (per split and after every merge) ---------
+static int comp_cmp(const AggReq& req, const std::vector<CompKey>& x, const std::vector<CompKey>& y) {
+  for (size_t i = 0; i < x.size() && i < y.size(); i++) {
+    const int c = key_cmp(x[i], y[i]);
+    if (c) return req.sources[i].order_desc ? -c : c;
+  }
+  return x.size() < y.size() ? -1 : x.size() > y.size();
+}
+struct CompKeyLess {  // source-order-free total order (merging by key tuple)
+  bool operator()(const std::vector<CompKey>& x, const std::vector<CompKey>& y) const {
+    for (size_t i = 0; i < x.size() && i < y.size(); i++) if (const int c = key_cmp(x[i], y[i])) return c < 0;
+    return x.size() < y.size();
+  }
+};
+static void comp_sort_cut(const AggReq& req, IAgg& a) {
+  for (const IBucket& b : a.buckets)
+    if (b.ckey.size() != req.sources.size()) fail(QWGPU_EINTERNAL, "intermediate aggregation result does not match the request");
+  if (req.has_after)
+    a.buckets.erase(std::remove_if(a.buckets.begin(), a.buckets.end(), [&](const IBucket& b) { return comp_cmp(req, b.ckey, req.after) <= 0; }),
+                    a.buckets.end());
+  std::sort(a.buckets.begin(), a.buckets.end(), [&](const IBucket& x, const IBucket& y) { return comp_cmp(req, x.ckey, y.ckey) < 0; });
+  if (a.buckets.size() > req.size) a.buckets.resize(req.size);
+}
+
 static IAgg build_node(const BuildCtx& c, uint32_t ni, uint64_t parent_cell) {
   const QwAggNode& n = c.nodes[ni];
   const AggBinding& b = c.cp.agg_bindings[ni];
   const AggReq& req = *b.req;
+  if (req.kind == AggReq::Composite) fail(QWGPU_EINVALID_ARG, "composite aggregation results are given as entries");
   const QwAggCell* base = c.cells + c.bases[ni];
   if (req.is_metric()) return metric_from_cell(c.cp, c.img, c.nodes, ni, base[parent_cell]);
   IAgg a;
@@ -541,10 +901,60 @@ struct EntryCtx {
 };
 static const uint32_t kNoEntry = 0xFFFFFFFEu;  // the parent of an empty range bucket: has no entries below it
 
+static IAgg build_node_e(const EntryCtx& c, uint32_t ni, uint32_t parent);
+
+// the typed key of a composite source's entry: strings through the dictionary, numbers through the column mapping,
+// histogram positions to the histogram key (date_histogram: epoch milliseconds)
+static CompKey comp_entry_key(const EntryCtx& c, uint32_t ni, const QwAggEntry& x) {
+  const QwAggNode& n = c.nodes[ni];
+  const AggBinding& b = c.cp.agg_bindings[ni];
+  CompKey k;
+  if (x.flags & QW_AGG_ENTRY_MISSING) return k;
+  const QwImgColumn& col = c.img.columns[b.column];
+  if (n.kind == QW_AGG_HISTOGRAM) return comp_hist_key(n, col.type, b.req->sources[b.comp_level].kind == AggReq::DateHistogram, n.base_pos + (int64_t)x.key);
+  const uint64_t mapped = col.min_value + col.gcd * x.key;
+  switch (col.type) {
+    case QW_COL_STR: { const uint8_t* p; uint32_t len; c.img.dict_term(col, (uint32_t)mapped, &p, &len); k.t = CompKey::Str; k.s.assign((const char*)p, len); break; }
+    case QW_COL_F64: k.t = CompKey::F64; k.f = u64_to_f64(mapped); break;
+    case QW_COL_I64: case QW_COL_DATETIME: k.t = CompKey::I64; k.i = u64_to_i64(mapped); break;
+    case QW_COL_BOOL: k.t = CompKey::Bool; k.u = mapped; break;
+    default: k.t = CompKey::U64; k.u = mapped; break;
+  }
+  return k;
+}
+// composite rooted at source node ni0: one bucket per leaf entry of the source chain, keyed by the chain's keys;
+// then the `after` filter, the sort and the cut to `size`
+static IAgg build_composite_e(const EntryCtx& c, uint32_t ni0, uint32_t parent0) {
+  const AggReq& req = *c.cp.agg_bindings[ni0].req;
+  IAgg a;
+  a.kind = AggReq::Composite;
+  std::vector<CompKey> path(req.sources.size());
+  auto walk = [&](auto&& self, uint32_t ni, uint32_t parent, size_t level) -> void {
+    auto it = c.kids.find({parent, ni});
+    if (it == c.kids.end()) return;
+    const QwAggNode& n = c.nodes[ni];
+    for (uint32_t e : it->second) {
+      const QwAggEntry& x = c.entries[e];
+      if (x.cell.count == 0) continue;
+      path[level] = comp_entry_key(c, ni, x);
+      if (level + 1 < path.size()) { self(self, n.first_child, e, level + 1); continue; }
+      IBucket bk;
+      bk.ckey = path;
+      bk.count = x.cell.count;
+      for (uint32_t k = 0; k < n.num_children; k++) bk.subs.push_back(build_node_e(c, n.first_child + k, e));
+      a.buckets.push_back(std::move(bk));
+    }
+  };
+  walk(walk, ni0, parent0, 0);
+  comp_sort_cut(req, a);
+  return a;
+}
+
 static IAgg build_node_e(const EntryCtx& c, uint32_t ni, uint32_t parent) {
   const QwAggNode& n = c.nodes[ni];
   const AggBinding& b = c.cp.agg_bindings[ni];
   const AggReq& req = *b.req;
+  if (req.kind == AggReq::Composite) return build_composite_e(c, ni, parent);
   static const std::vector<uint32_t> none;
   auto it = c.kids.find({parent, ni});
   const std::vector<uint32_t>& es = it == c.kids.end() ? none : it->second;
@@ -605,12 +1015,12 @@ static std::vector<IAgg> build_top_entries(const CompiledPlan& cp, const ImageVi
       fail(QWGPU_EINVALID_ARG, "aggregation entry %zu does not match the plan's tree", e);
     const QwAggNode& n = nodes[x.node];
     const AggBinding& b = cp.agg_bindings[x.node];
-    bool ok = x.flags == 0 || (n.kind == QW_AGG_TERMS && x.flags == QW_AGG_ENTRY_MISSING);
+    bool ok = x.flags == 0 || ((n.kind == QW_AGG_TERMS || n.kind == QW_AGG_HISTOGRAM) && x.flags == QW_AGG_ENTRY_MISSING);
     if (ok && (x.flags & QW_AGG_ENTRY_MISSING)) ok = n.has_missing && x.key == 0;
     else if (ok) {
       switch (n.kind) {
         case QW_AGG_STATS: ok = x.key == 0; break;
-        case QW_AGG_HISTOGRAM: ok = x.key < n.num_buckets; break;
+        case QW_AGG_HISTOGRAM: ok = x.key < (uint64_t)n.num_buckets - (n.has_missing ? 1u : 0u); break;
         case QW_AGG_RANGE: ok = x.key < n.num_ranges; break;
         case QW_AGG_TERMS: {
           ok = b.column >= 0 && img.columns[b.column].num_vals > 0 && img.columns[b.column].gcd &&
@@ -768,6 +1178,19 @@ static void merge_lists(const std::vector<AggReq>& reqs, std::vector<IAgg>& acc,
 }
 static void merge_into(const AggReq& req, IAgg& acc, IAgg&& other) {
   if (acc.kind != other.kind) fail(QWGPU_EINTERNAL, "failed to merge intermediate aggregation results: kind mismatch");
+  if (acc.kind == AggReq::Composite) {
+    // union by key tuple, then the same filter / sort / cut as each split's. Exact: a bucket among the first `size`
+    // of the merge has fewer than `size` buckets before it in any part, so no part's cut dropped it
+    std::map<std::vector<CompKey>, size_t, CompKeyLess> index;
+    for (size_t i = 0; i < acc.buckets.size(); i++) index.emplace(acc.buckets[i].ckey, i);
+    for (auto& b : other.buckets) {
+      auto it = index.find(b.ckey);
+      if (it == index.end()) { index.emplace(b.ckey, acc.buckets.size()); acc.buckets.push_back(std::move(b)); }
+      else { IBucket& t = acc.buckets[it->second]; t.count += b.count; merge_lists(req.children, t.subs, std::move(b.subs)); }
+    }
+    comp_sort_cut(req, acc);
+    return;
+  }
   if (acc.kind >= AggReq::Stats) {
     acc.m_count += other.m_count;
     acc.m_sum += other.m_sum;
@@ -869,6 +1292,42 @@ static void fin_key(const IKey& k, std::string& out) {
     default: out += std::to_string(k.u);
   }
 }
+// an f64 the way Rust's Display writes it: the shortest digits that read back the same value, never an exponent,
+// no ".0" on whole numbers (100 -> "100", 0.1 -> "0.1", 1e21 -> "1000000000000000000000")
+static std::string rust_display_f64(double v) {
+  if (std::isnan(v)) return "NaN";
+  if (std::isinf(v)) return v > 0 ? "inf" : "-inf";
+  char buf[64];
+  for (int p = 0; p < 17; p++) {
+    snprintf(buf, sizeof buf, "%.*e", p, v);
+    if (strtod(buf, nullptr) == v) break;
+  }
+  std::string s(buf);
+  const bool neg = s[0] == '-';
+  if (neg) s.erase(0, 1);
+  const size_t e = s.find('e');
+  const int exp = atoi(s.c_str() + e + 1);
+  std::string digits;
+  for (size_t i = 0; i < e; i++) if (s[i] != '.') digits += s[i];
+  while (digits.size() > 1 && digits.back() == '0') digits.pop_back();
+  const int point = exp + 1;  // digits before the decimal point
+  std::string out;
+  if (point <= 0) out = "0." + std::string((size_t)-point, '0') + digits;
+  else if ((size_t)point >= digits.size()) out = digits + std::string((size_t)point - digits.size(), '0');
+  else out = digits.substr(0, (size_t)point) + "." + digits.substr((size_t)point);
+  return (neg ? "-" : "") + out;
+}
+// the type-tagged form of a composite key (tantivy's AfterKey): "str:…", "i64:…", "u64:…", "f64:…", "bool:…"
+static std::string comp_key_tagged(const CompKey& k) {
+  switch (k.t) {
+    case CompKey::Bool: return k.u ? "bool:true" : "bool:false";
+    case CompKey::Str: return "str:" + k.s;
+    case CompKey::I64: return "i64:" + std::to_string(k.i);
+    case CompKey::U64: return "u64:" + std::to_string(k.u);
+    case CompKey::F64: return "f64:" + rust_display_f64(k.f);
+    default: return "";
+  }
+}
 static void opt_f64(bool some, double v, std::string& out) { if (some) json_f64(v, out); else out += "null"; }
 static std::string range_num(double v) {
   std::string s;
@@ -908,6 +1367,52 @@ static void fin_agg(const AggReq& req, const IAgg* a, std::string& out) {
     fin_aggs(req.children, b ? &b->subs : nullptr, inner);
     out += inner.substr(1, inner.size() - 2);  // splice the members of {...}
   };
+  if (req.kind == AggReq::Composite) {
+    // {"after_key": {source: tagged key}, "buckets": [{"doc_count", "key": {source: key}, sub-aggregations}]};
+    // after_key is the last bucket's key ({} without buckets), type-tagged so that it pages back exactly
+    IAgg c;
+    c.kind = a->kind;
+    c.buckets = a->buckets;
+    comp_sort_cut(req, c);
+    auto plain = [&](const CompKey& k) {
+      switch (k.t) {
+        case CompKey::Null: out += "null"; break;
+        case CompKey::Bool: out += k.u ? "true" : "false"; break;
+        case CompKey::Str: json_escape(k.s, out); break;
+        case CompKey::I64: out += std::to_string(k.i); break;
+        case CompKey::U64: out += std::to_string(k.u); break;
+        default: json_f64(k.f, out);
+      }
+    };
+    out += "{\"after_key\":{";
+    if (!c.buckets.empty()) {
+      const std::vector<CompKey>& last = c.buckets.back().ckey;
+      for (size_t i = 0; i < req.sources.size(); i++) {
+        if (i) out += ",";
+        json_escape(req.sources[i].name, out);
+        out += ":";
+        if (last[i].t == CompKey::Null) out += "null";
+        else json_escape(comp_key_tagged(last[i]), out);
+      }
+    }
+    out += "},\"buckets\":[";
+    for (size_t bi = 0; bi < c.buckets.size(); bi++) {
+      const IBucket& b = c.buckets[bi];
+      if (bi) out += ",";
+      out += "{\"doc_count\":" + std::to_string(b.count) + ",\"key\":{";
+      for (size_t i = 0; i < req.sources.size(); i++) {
+        if (i) out += ",";
+        json_escape(req.sources[i].name, out);
+        out += ":";
+        plain(b.ckey[i]);
+      }
+      out += "}";
+      subs(&b);
+      out += "}";
+    }
+    out += "]}";
+    return;
+  }
   if (req.kind == AggReq::Terms) {
     std::vector<IBucket> bs = a->buckets;
     sort_term_buckets(req, bs);

@@ -24,10 +24,25 @@ bool parse_datetime_str(const std::string& s, int64_t* nanos);
 
 // ---- aggregation request (tantivy::aggregation::agg_req::Aggregations, Elasticsearch-shaped JSON;
 // semantics per docs/reference/aggregation.md) --------------------------------------------------------
+// One value of a composite key tuple (CompositeKey, quickwit-query/src/aggregations.rs)
+struct CompKey {
+  enum T : uint8_t { Null = 0, Bool = 1, Str = 2, I64 = 3, U64 = 4, F64 = 5 } t = Null;
+  std::string s;
+  uint64_t u = 0;  // Bool (0 / 1), U64
+  int64_t i = 0;
+  double f = 0;
+  bool numeric() const { return t >= I64; }
+};
 struct AggReq {
   // TraceIds: quickwit's FindTraceIdsCollector (find_trace_ids_collector.rs), which takes the place of the whole
   // aggregation request (`size` = num_traces, `field` = trace_id_field_name, `ts_field` = span_timestamp_field_name)
-  enum Kind { Terms, Histogram, DateHistogram, Range, Stats, Avg, Sum, Min, Max, Count, TraceIds } kind = Terms;
+  // Composite: `sources` are Terms / Histogram / DateHistogram requests (their `name`, `field`, interval / offset,
+  // `order_desc` and `has_missing` = missing_bucket), `size` the page size, `after` one key per source when
+  // `has_after`; `children` hang below the last source
+  enum Kind { Terms, Histogram, DateHistogram, Range, Stats, Avg, Sum, Min, Max, Count, TraceIds, Composite } kind = Terms;
+  std::vector<AggReq> sources;
+  std::vector<CompKey> after;
+  bool has_after = false;
   std::string ts_field;
   uint64_t num_traces = 0;
   std::string name, field;
@@ -68,6 +83,7 @@ struct AggBinding {
   const AggReq* req = nullptr;
   int column = -1;
   uint32_t col_type = 0;
+  uint32_t comp_level = 0;  // req is a Composite: the node is source `comp_level` of its chain
 };
 // Flattens the request against one split (column lookup, dense bucket space); nodes are emitted
 // breadth-first so that the children of a node are contiguous.

@@ -70,7 +70,7 @@ struct DAgg {
   uint32_t col, num_buckets, has_bounds, num_ranges;
   uint32_t has_missing, cell_base;
   uint32_t is_f64;  // STATS: 1 = sum doubles, 0 = the exact u64 sum of raw offsets (qw_stats_sum_exact, host-decided)
-  uint32_t pad;
+  uint32_t comp;    // TERMS / HISTOGRAM: QW_AGG_COMP_* flags (QwAggNode.reserved), read by the hashed walk only
   double interval, offset, bound_min, bound_max;
   int64_t base_pos;
   // fast path (flat bucket aggregations over single-valued columns, see lower_plan): histogram
@@ -80,7 +80,8 @@ struct DAgg {
   uint64_t bounds;       // device address of uint64[num_buckets + 1] (HISTOGRAM only)
   float inv_step;        // ~ num_buckets / (bounds[nb] - bounds[0]): first guess of the bucket
   uint32_t stat_base;    // STATS on the fast path: first of this node's {sum, ~min, max} triples in shared memory
-  uint32_t pad3[2];      // keeps sizeof(DAgg) a multiple of 16 (copied to shared memory as uint4)
+  uint64_t comp_after;   // composite source: the split's `after` bound (QwAggNode.range_from[0]); keeps sizeof(DAgg) a
+                         // multiple of 16 (copied to shared memory as uint4)
   uint64_t range_from[QW_MAX_AGG_RANGES], range_to[QW_MAX_AGG_RANGES];
 };
 static_assert(sizeof(DInstr) % 16 == 0 && sizeof(DCol) % 16 == 0 && sizeof(DAgg) % 16 == 0, "uint4-copied structs");

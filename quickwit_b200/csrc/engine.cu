@@ -15,6 +15,7 @@
 #include "driver_kernel.cuh"
 #include "agg_kernel.cuh"
 #include "trace_kernel.cuh"
+#include "composite_kernel.cuh"
 
 namespace qw {
 
@@ -338,7 +339,7 @@ uint64_t agg_hashed_bound(const QwAggNode* aggs, uint32_t n, const ImageView& im
       if (g.kind == QW_AGG_RANGE) reps = sat_mul(reps, g.num_ranges);
       if (g.column < img.hdr->num_columns && img.columns[g.column].cardinality == QW_CARD_MULTI) {
         any_multi = true;
-        multi = sat_mul(multi, img.columns[g.column].num_vals + (g.kind == QW_AGG_TERMS && g.has_missing ? num_docs : 0));
+        multi = sat_mul(multi, img.columns[g.column].num_vals + ((g.kind == QW_AGG_TERMS || g.kind == QW_AGG_HISTOGRAM) && g.has_missing ? num_docs : 0));
       }
     }
     total = std::min<uint64_t>(total + std::min(dense, sat_mul(any_multi ? multi : num_docs, reps)), 1ull << 62);
@@ -772,6 +773,10 @@ static void lower_plan(Lowered& L, const SplitDev& sp, const uint8_t* plan, size
     d.base_pos = a.base_pos;
     memcpy(d.range_from, a.range_from, sizeof d.range_from);
     memcpy(d.range_to, a.range_to, sizeof d.range_to);
+    if ((a.kind == QW_AGG_TERMS || a.kind == QW_AGG_HISTOGRAM) && (a.reserved & QW_AGG_COMP_LEVEL)) {
+      d.comp = a.reserved;
+      d.comp_after = a.range_from[0];
+    }
     if (a.parent != 0xFFFFFFFFu && aggs[a.parent].kind == QW_AGG_STATS) fail(QWGPU_EINVALID_AGG, "metric aggregations cannot have sub-aggregations");
     if (a.kind == QW_AGG_RANGE && a.num_ranges > QW_MAX_AGG_RANGES) fail(QWGPU_EUNSUPPORTED, "more than %d ranges", QW_MAX_AGG_RANGES);
     L.aggs.push_back(d);
@@ -1227,11 +1232,12 @@ bool Engine::search_once(const std::vector<std::shared_ptr<SplitDev>>& sp, const
   // cells, or at the bound when the batch runs again after an overflow
   const size_t s_hash = al(s_trace_data + tr_off[n]);
   std::vector<size_t> h_off(n + 1, 0);
-  bool any_hashed = false;
+  bool any_hashed = false, any_composite = false;
   for (uint32_t i = 0; i < n; i++) {
     DSplitPlan& P = low[i].P;
     if (P.hashed) {
       any_hashed = true;
+      for (const DAgg& d : low[i].aggs) if (d.comp & QW_AGG_COMP_LEVEL) any_composite = true;
       P.h_cap = (uint32_t)(at_bound ? low[i].h_bound : std::min<uint64_t>(low[i].h_bound, QWGPU_HASHED_INIT_CELLS));
       P.h_mask = agg_hashed_slots(P.h_cap) - 1;
     }
@@ -1481,6 +1487,12 @@ bool Engine::search_once(const std::vector<std::shared_ptr<SplitDev>>& sp, const
     CUDA_CHECK(cudaEventRecord(slot->ev2, st));
     launch_window(qwk::MODE_COLLECT, false, 0, 0, flags);
     CUDA_CHECK(cudaEventRecord(slot->ev3, st));
+    if (any_composite && !(flags & F_CANDS_ONLY)) {
+      // each composite's first `size` leaves with their chains and sub-aggregation entries, before the copy-back
+      qwk::k_composite_cut<<<n, QC_THREADS, 0, st>>>(kp.plans, kp.aggs);
+      stats.launches++;
+      stats.kernel_mask |= QWGPU_KERNEL_COMPOSITE_CUT;
+    }
     if (any_trace && !(flags & F_CANDS_ONLY)) {
       // top N of the per-trace maxima; splits whose N-th and (N+1)-th maxima tie replay the reference's selection
       qwk::k_trace_select<<<n, 1024, 0, st>>>(kp.plans);

@@ -707,9 +707,23 @@ __device__ __forceinline__ uint32_t hcell_count(const DSplitPlan& P, uint32_t no
   id = __shfl_sync(QW_FULL, id, lead);
   return on ? id : QW_HSLOT_EMPTY;
 }
+// Where the key of composite source g lies against the source's `after` value, in the source's order (null first
+// when ascending, last when descending): -1 before, 0 equal, 1 after.
+__device__ __forceinline__ int comp_vs_after(const DAgg& g, uint64_t key, bool missing) {
+  const bool desc = g.comp & QW_AGG_COMP_DESC;
+  if (g.comp & QW_AGG_COMP_AFTER_NULL) return missing ? 0 : (desc ? -1 : 1);
+  if (missing) return desc ? 1 : -1;
+  if (g.comp & QW_AGG_COMP_AFTER_ALL) return -1;
+  if (key == g.comp_after) return (g.comp & QW_AGG_COMP_EXACT) ? 0 : 1;
+  return (desc ? key > g.comp_after : key < g.comp_after) ? -1 : 1;
+}
 // Every matched doc walks the tree depth-first, visiting every value of a multi-valued column at every level (the
 // cartesian product, as agg_collect_doc). Loop bounds are warp-uniform; the per-level state lives in local memory
 // (the walk only runs for hashed plans).
+// Composite sources with an `after` tuple: a lane is "tight" at level d while its path through the levels above
+// equals the tuple's prefix. A tight lane drops a key before the level's `after` value, stays tight on an equal key
+// (drops it at the last level: pages start strictly after `after`) and is free below a key after it, so keys before
+// `after` never enter the table.
 __device__ __forceinline__ void agg_collect_hashed(const DSplitPlan& P, const DAgg* aggs, const DCol* cols, const uint8_t* base,
                                                 uint32_t doc, bool on, uint32_t lane) {
   // a split whose table overflowed runs again at its bound: the rest of this pass is wasted work
@@ -719,13 +733,15 @@ __device__ __forceinline__ void agg_collect_hashed(const DSplitPlan& P, const DA
   uint32_t node[QW_MAX_DAGGS], k[QW_MAX_DAGGS], r[QW_MAX_DAGGS], maxv[QW_MAX_DAGGS], child[QW_MAX_DAGGS];
   uint64_t a[QW_MAX_DAGGS];
   uint32_t nv[QW_MAX_DAGGS], parent[QW_MAX_DAGGS], cell[QW_MAX_DAGGS];
-  uint32_t flags = 0;  // per lane, bit d: the lane is live at level d; bit 8 + d: level d is the `missing` bucket
+  // per lane, bit d: the lane is live at level d; bit 8 + d: level d is the `missing` bucket; bit 16 + d: the lane is
+  // tight entering level d; bit 24 + d: the current key of level d keeps it tight
+  uint32_t flags = 0;
   for (uint32_t top = 0; top < P.n_aggs; top++) {
     if (aggs[top].parent != 0xFFFFFFFFu) continue;
     int d = 0;
     node[0] = top;
     parent[0] = QW_AGG_NO_PARENT;
-    flags = on ? 1u : 0u;
+    flags = (on ? 1u : 0u) | 0x10000u;
     bool fresh = true;
     while (d >= 0) {
       const DAgg& g = aggs[node[d]];
@@ -744,6 +760,7 @@ __device__ __forceinline__ void agg_collect_hashed(const DSplitPlan& P, const DA
         }
         bool missing;
         nv[d] = agg_values(g, cols, base, doc, live, a[d], missing);
+        if (g.kind == QW_AGG_HISTOGRAM && g.has_missing && live && nv[d] == 0) { missing = true; nv[d] = 1; }  // composite missing_bucket
         flags = (flags & ~(0x100u << d)) | (missing ? 0x100u << d : 0u);
         maxv[d] = __reduce_max_sync(QW_FULL, nv[d]);
         k[d] = 0;
@@ -764,6 +781,15 @@ __device__ __forceinline__ void agg_collect_hashed(const DSplitPlan& P, const DA
             key = bk;
           }
         }
+        if (g.comp & QW_AGG_COMP_HAS_AFTER) {
+          bool tight = false;
+          if (ok && ((flags >> (16 + d)) & 1u)) {
+            const int c = comp_vs_after(g, key, missing);
+            if (c < 0 || (c == 0 && (g.comp & QW_AGG_COMP_LAST))) ok = false;
+            tight = c == 0;
+          }
+          flags = (flags & ~(0x1000000u << d)) | (tight ? 0x1000000u << d : 0u);
+        }
         cell[d] = hcell_count(P, node[d] | (missing ? QW_AGG_ENTRY_MISSING << 8 : 0u), parent[d], key, ok, true, lane);
         child[d] = 0;
         if (++r[d] >= (g.kind == QW_AGG_RANGE ? g.num_ranges : 1u)) { r[d] = 0; k[d]++; }
@@ -775,6 +801,7 @@ __device__ __forceinline__ void agg_collect_hashed(const DSplitPlan& P, const DA
         node[d] = c;
         parent[d] = cell[d - 1];
         flags = (flags & ~(1u << d)) | (child_live ? 1u << d : 0u);
+        flags = (flags & ~(0x10000u << d)) | (((flags >> (23 + d)) & 1u) << (16 + d));
         fresh = true;
         continue;
       }

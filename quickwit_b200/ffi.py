@@ -31,12 +31,17 @@ ABSENT = 0xFFFFFFFF
 # qwgpu_split_result.kernel_mask (qwgpu.h)
 KERNEL_UNION, KERNEL_DRIVER, KERNEL_AGGSCAN, KERNEL_WINDOW, KERNEL_PHRASE = 1, 2, 4, 8, 16
 KERNEL_TRACE_SELECT, KERNEL_TRACE_REPLAY, KERNEL_FAST_AGGS = 32, 64, 128
-KERNEL_HASHED_AGGS, KERNEL_HASHED_AGGS_RETRY = 256, 512
+KERNEL_HASHED_AGGS, KERNEL_HASHED_AGGS_RETRY, KERNEL_COMPOSITE_CUT = 256, 512, 1024
 # hashed aggregation cells (qwgpu_format.h qw_agg_hashed, qwgpu.h): dense-layout limits, the initial capacity of a
 # split's table, the largest table a split may need, the `missing` flag of an entry
 AGG_DENSE_MAX_CELLS, AGG_DENSE_MAX_TERMS = 1 << 26, 1 << 24
 HASHED_INIT_CELLS, HASHED_MAX_BYTES = 65536, 8 << 30
 AGG_NO_PARENT, AGG_ENTRY_MISSING = 0xFFFFFFFF, 1
+# composite source nodes (qwgpu_format.h QW_AGG_COMP_*): QwAggNode.reserved flags, range_from[0] = the split's
+# `after` bound, range_to[0] = size
+AGG_COMP_LEVEL, AGG_COMP_LAST, AGG_COMP_DESC, AGG_COMP_MISSING = 1, 2, 4, 8
+AGG_COMP_HAS_AFTER, AGG_COMP_AFTER_NULL, AGG_COMP_EXACT, AGG_COMP_AFTER_ALL, AGG_COMP_AFTER_HOST = 16, 32, 64, 128, 256
+AGG_COMP_MAX_SIZE = 65000
 PLAN_MAGIC = 0x4E4C5051
 MAX_AGG_RANGES = 16
 

@@ -154,6 +154,26 @@ class Agg:
         self.kind, self.column, self.num_buckets, self.children = kind, column, num_buckets, list(children)
         self.interval, self.offset, self.base_pos, self.bounds = interval, offset, base_pos, bounds
         self.ranges, self.missing = list(ranges), missing
+        # composite source (see composite()): QW_AGG_COMP_* flags, the split's `after` bound, the page size
+        self.comp, self.comp_after, self.comp_size = 0, 0, 0
+
+
+def composite(sources: Sequence[Agg], size: int, children: Sequence[Agg] = (), desc: Sequence[int] = (),
+              after: Optional[Sequence[Tuple[int, int]]] = None) -> Agg:
+    """A composite aggregation as the plan holds it: `sources` (TERMS / HISTOGRAM nodes, `missing` set for a
+    missing_bucket source) chained, each the only child of the one before, `children` below the last. `desc`: indices
+    of the descending sources. `after`: per source (bound, QW_AGG_COMP_* after flags) in the node's key space, as
+    the lowering resolves it for a split. Returns the first source."""
+    for i, s in enumerate(sources):
+        last = i == len(sources) - 1
+        s.comp = ffi.AGG_COMP_LEVEL | (ffi.AGG_COMP_LAST if last else 0) | (ffi.AGG_COMP_DESC if i in desc else 0) | \
+            (ffi.AGG_COMP_MISSING if s.missing is not None else 0)
+        if after is not None:
+            s.comp_after = after[i][0]
+            s.comp |= ffi.AGG_COMP_HAS_AFTER | after[i][1]
+        s.comp_size = size
+        s.children = list(children) if last else [sources[i + 1]]
+    return sources[0]
 
 
 def _flatten_aggs(tops: Sequence[Agg]) -> List[ffi.QwAggNode]:
@@ -171,6 +191,8 @@ def _flatten_aggs(tops: Sequence[Agg]) -> List[ffi.QwAggNode]:
             g.range_from[i], g.range_to[i] = f, t
         if a.missing is not None:
             g.has_missing, g.missing_value = 1, a.missing
+        if a.comp:
+            g.reserved, g.range_from[0], g.range_to[0] = a.comp, a.comp_after, a.comp_size
         out.append(g)
         return idx
 
