@@ -196,7 +196,7 @@ struct KParams {
   uint32_t n_splits;
   uint32_t total_work;
   uint32_t stride;   // sampling stride over windows (1 = all)
-  uint32_t W;        // window size in docs (power of two, <= 8192)
+  uint32_t W;        // window size in docs (<= 32768; a power of two, except 15360 in BM25-union batches)
   uint32_t level;    // MODE_HIST: radix level being histogrammed
   uint32_t use_prefix;  // MODE_HIST: restrict to docs whose key matches thresh prefix
   uint32_t smem_aggs;   // 1: aggregation counts privatised in shared memory

@@ -379,7 +379,6 @@ struct Lowered {
   std::vector<DInstr> instrs;
   std::vector<DCol> cols;
   std::vector<uint64_t> bounds;  // raw-space histogram boundary tables of the fast aggregation path
-  uint32_t bounds_base = 0;      // position of `bounds` in the batch's table region
   std::vector<uint64_t> col_max_raw;  // parallel to cols: largest bit-packed raw value present in the column
   std::vector<DAgg> aggs;
   std::vector<int> col_map;  // image column -> DCol index
@@ -868,6 +867,13 @@ static void lower_plan(Lowered& L, const SplitDev& sp, const uint8_t* plan, size
   P.fast_aggs = fast ? 1 : 0;
 }
 
+// Consecutive regions of one buffer or shared-memory block: each starts where the one before ends, rounded up to
+// `align` bytes
+struct Arena {
+  size_t align, off = 0;
+  size_t take(size_t bytes) { const size_t o = off; off = (off + bytes + align - 1) & ~(align - 1); return o; }
+};
+
 // shared-memory arena for a batch (max over the batch's plans)
 static uint32_t stage_bytes_for(uint32_t W) {
   return std::min<uint32_t>(std::max<uint32_t>(W, 8192), 24576);
@@ -877,34 +883,33 @@ static SmemLayout make_layout(uint32_t W, uint32_t n_levels, uint32_t need_cnt, 
                               uint32_t max_instr, uint32_t max_cols, uint32_t max_aggs, uint32_t n_fn, bool rec_l0, bool rangeq) {
   SmemLayout L;
   memset(&L, 0xFF, sizeof L);
-  uint32_t off = 0;
-  auto take = [&](uint32_t bytes) { uint32_t o = off; off = (off + bytes + 15) & ~15u; return o; };
-  L.misc = take(32 + 4 * QW_MAX_TERMS + QW_MAX_TERMS);  // counters, per-term block bases, per-term instruction index
-  L.instr = take(std::max(max_instr, 1u) * sizeof(DInstr));
-  L.cols = take(std::max(max_cols, 1u) * sizeof(DCol));
-  L.aggs = take(std::max(max_aggs, 1u) * sizeof(DAgg));
-  L.key = take(sizeof(DKeySpec));
+  Arena a{16};
+  L.misc = a.take(32 + 4 * QW_MAX_TERMS + QW_MAX_TERMS);  // counters, per-term block bases, per-term instruction index
+  L.instr = a.take(std::max(max_instr, 1u) * sizeof(DInstr));
+  L.cols = a.take(std::max(max_cols, 1u) * sizeof(DCol));
+  L.aggs = a.take(std::max(max_aggs, 1u) * sizeof(DAgg));
+  L.key = a.take(sizeof(DKeySpec));
 
   for (uint32_t l = 0; l < n_levels; l++) {
-    L.lvl[l].req = take(W / 8);
-    L.lvl[l].shd = take(W / 8);
-    L.lvl[l].nt = take(W / 8);
-    if ((need_cnt >> l) & 1) L.lvl[l].cnt = take(W);
-    if ((need_msum >> l) & 1) L.lvl[l].msum = take(W * 4);
-    if ((need_ssum >> l) & 1) L.lvl[l].ssum = take(W * 4);
+    L.lvl[l].req = a.take(W / 8);
+    L.lvl[l].shd = a.take(W / 8);
+    L.lvl[l].nt = a.take(W / 8);
+    if ((need_cnt >> l) & 1) L.lvl[l].cnt = a.take(W);
+    if ((need_msum >> l) & 1) L.lvl[l].msum = a.take(W * 4);
+    if ((need_ssum >> l) & 1) L.lvl[l].ssum = a.take(W * 4);
     L.lvl[l].rsc = L.lvl[l].msum != 0xFFFFFFFFu ? L.lvl[l].msum : L.lvl[l].ssum;
   }
-  L.tmp = take(W / 8);
-  for (uint32_t s = 0; s < n_fn; s++) L.fn[s] = take(W);  // BM25 tables stay in global memory (L1-resident)
-  L.rng = take(QW_MAX_TERMS * 16);
+  L.tmp = a.take(W / 8);
+  for (uint32_t s = 0; s < n_fn; s++) L.fn[s] = a.take(W);  // BM25 tables stay in global memory (L1-resident)
+  L.rng = a.take(QW_MAX_TERMS * 16);
   L.hitq = L.rng;  // the collect-time hit queues alias rng / blkrec / termblk (contiguous, dead after the program)
-  L.blkrec = take(QW_MAX_WBLK * 8);
-  L.termblk = take(QW_MAX_TERMS * 8);
-  L.stage = take(stage_bytes_for(W));
+  L.blkrec = a.take(QW_MAX_WBLK * 8);
+  L.termblk = a.take(QW_MAX_TERMS * 8);
+  L.stage = a.take(stage_bytes_for(W));
   L.hist = L.stage;  // histogram / privatised aggregation counters reuse the staging area at collect time
-  if (rec_l0) L.l0hist = take(QW_HIST_BINS * 4);
-  if (rangeq) L.rangeq = take(QW_WARPS * (32 + 32 * 4) * 2);  // QW_WARPS x QW_HITQ_CAP uint16 (kernels.cuh)
-  L.total = off;
+  if (rec_l0) L.l0hist = a.take(QW_HIST_BINS * 4);
+  if (rangeq) L.rangeq = a.take(QW_WARPS * (32 + 32 * 4) * 2);  // QW_WARPS x QW_HITQ_CAP uint16 (kernels.cuh)
+  L.total = a.off;
   return L;
 }
 
@@ -913,13 +918,12 @@ static SmemLayout make_layout(uint32_t W, uint32_t n_levels, uint32_t need_cnt, 
 static qwk::USmem make_union_layout(uint32_t W, bool hist, uint32_t budget) {
   qwk::USmem L;
   memset(&L, 0, sizeof L);
-  uint32_t off = 0;
-  auto take = [&](uint32_t bytes) { uint32_t o = off; off = (off + bytes + 15) & ~15u; return o; };
-  L.score = take(W * 4);
-  L.bars = take(8 * (2 * QU_SLOTS + QU_CHAIN));
-  if (hist) L.hist = take(QW_HIST_BINS * 4);
-  L.cands = take(QU_NCW * QU_CANDS * 8 + QU_NCW * 4);
-  const uint32_t fixed = QU_MAXBLK * 16 + QU_MAX_TERMS * 16 + 32 + QU_PAD;
+  Arena a{16};
+  L.score = a.take(W * 4);
+  L.bars = a.take(8 * (2 * QU_SLOTS + QU_CHAIN));
+  if (hist) L.hist = a.take(QW_HIST_BINS * 4);
+  L.cands = a.take(QU_NCW * QU_CANDS * 8 + QU_NCW * 4);
+  const uint32_t off = (uint32_t)a.off, fixed = QU_MAXBLK * 16 + QU_MAX_TERMS * 16 + 32 + QU_PAD;
   const uint32_t cap = budget > off + QU_SLOTS * (fixed + 2048) ? ((budget - off) / QU_SLOTS - fixed) & ~15u : 2048;
   L.cap = cap;
   L.payload = 0;
@@ -927,26 +931,747 @@ static qwk::USmem make_union_layout(uint32_t W, bool hist, uint32_t budget) {
   L.ttab = L.recs + QU_MAXBLK * 16;
   L.hdr = L.ttab + QU_MAX_TERMS * 16;
   L.slot_stride = L.hdr + 48;  // header (32 B) + block hand-out counter
-  L.slot0 = take(QU_SLOTS * L.slot_stride);
-  L.total = off;
+  L.slot0 = a.take(QU_SLOTS * L.slot_stride);
+  L.total = a.off;
   return L;
 }
 
-bool Engine::search_once(const std::vector<std::shared_ptr<SplitDev>>& sp, const std::vector<const uint8_t*>& plans,
-                         const std::vector<size_t>& plan_lens, std::vector<SplitOutput>& outs, BatchStats& stats,
-                         const MergeSpec* merge, std::vector<MergedHit>* merged, const GatherSpec* gather,
-                         std::vector<RankHeader>* rank_headers, bool at_bound) {
-  const uint32_t n_in = (uint32_t)sp.size();
-  outs.assign(n_in, SplitOutput());
-  static const bool trace = getenv("QWGPU_TRACE") != nullptr;  // host phase timings on stderr
-  using tclock = std::chrono::steady_clock;
-  const auto t_begin = tclock::now();
-  CUDA_CHECK(cudaSetDevice(device));
-  // ---- lower every plan; splits whose plan cannot be lowered fail individually ----------------------
+// the BM25 top-K shape, [BOOL_BEGIN, TERM x n, BOOL_END] ranked by _score: the BM25-union pipeline (k_union)
+static bool union_eligible(const Lowered& L) {
+  return L.P.fused_score_root && L.P.max_hits && !L.P.sa.present && !L.P.n_aggs && L.P.key.kind[0] == QW_SORT_SCORE &&
+         L.P.key.order[0] == QW_ORDER_DESC && L.P.n_terms <= QU_MAX_TERMS && L.P.n_instr == L.P.n_terms + 2;
+}
+
+// one driving posting list + required column filters, no aggregations: the posting-driven kernel
+// (driver_kernel.cuh). [BOOL_BEGIN, TERM, (RANGE | EXISTS) x 0..4, BOOL_END] at level 0.
+static bool driver_eligible(const Lowered& L) {
+  const std::vector<DInstr>& I = L.instrs;
+  if (!(L.P.n_aggs == 0 && I.size() >= 3 && I.size() <= 3 + QD_MAX_FILTERS && I[0].op == OP_BOOL_BEGIN && I[1].op == OP_TERM &&
+        I.back().op == OP_BOOL_END && I.back().level == 0))
+    return false;
+  const bool req = I[1].occur == QW_OCCUR_MUST || I[1].occur == QW_OCCUR_FILTER;
+  if (!req && !(I[1].occur == QW_OCCUR_SHOULD && I.size() == 3 && I.back().r == 1 && I.back().n == 0)) return false;
+  for (size_t k = 2; k + 1 < I.size(); k++) {
+    const bool colpred = I[k].op == OP_RANGE || I[k].op == OP_EXISTS;
+    const bool unscored_req = I[k].occur == QW_OCCUR_FILTER || (I[k].occur == QW_OCCUR_MUST && !(I[k].flags & IF_SCORED));
+    if (!colpred || !unscored_req || I[k].level != 0) return false;
+  }
+  return true;
+}
+
+// match_all + flat terms / histogram aggregations, no hits: the streaming column kernel (agg_kernel.cuh). Lays out
+// its shared memory; false when a plan does not qualify or the layout does not fit.
+static bool aggscan_layout(const std::vector<Lowered>& low, int max_smem_optin, qwk::ASmem* alay) {
+  uint32_t maxbits[QW_MAX_DAGGS] = {0}, a_cells = 1;
+  for (const Lowered& L : low) {
+    if (!(L.P.n_instr == 3 && L.instrs[1].op == OP_ALL && L.P.max_hits == 0 && L.P.n_aggs > 0 && L.P.n_cells <= QA_MAX_CELLS)) return false;
+    for (uint32_t gi = 0; gi < L.P.n_aggs; gi++) {
+      const DAgg& d = L.aggs[gi];
+      const bool flat = d.parent == 0xFFFFFFFFu && d.num_children == 0 && (d.kind == QW_AGG_TERMS || d.kind == QW_AGG_HISTOGRAM) && !d.has_missing;
+      if (!flat || !L.P.fast_aggs || d.col == 0xFFFFFFFFu || L.cols[d.col].card != QW_CARD_FULL || L.cols[d.col].bits > 32) return false;
+      maxbits[gi] = std::max(maxbits[gi], L.cols[d.col].bits);
+    }
+    a_cells = std::max(a_cells, L.P.n_cells);
+  }
+  memset(alay, 0, sizeof *alay);
+  Arena slot{16};
+  for (uint32_t gi = 0; gi < QW_MAX_DAGGS; gi++) alay->col_off[gi] = slot.take(maxbits[gi] ? QA_CHUNK / 8 * maxbits[gi] + 16 : 0);
+  alay->hdr = slot.take(16);
+  alay->slot_stride = slot.off;
+  Arena a{16};
+  alay->bars = a.take(8 * 2 * QA_SLOTS);
+  alay->atab = a.take(QW_MAX_DAGGS * sizeof(qwk::AggRow));
+  alay->bcache = a.take(QA_CW * QW_MAX_DAGGS * 16);
+  alay->cells = a.take(a_cells * 4);
+  alay->slot0 = a.take(QA_SLOTS * alay->slot_stride);
+  alay->total = a.off;
+  return (int)alay->total + 1024 <= max_smem_optin;
+}
+
+// The kernel route of a batch and everything it fixes: window sizes, the threshold sample, the work lists and the
+// shared-memory layouts. A pass that the route's own kernel does not serve runs on k_window with `lay`.
+struct Route {
+  enum Kind { WINDOW, DRIVER, UNION, AGGSCAN } kind = WINDOW;
+  uint32_t W = 0, W_h = 0;   // docs per window: collect and exact radix passes / sampled threshold pass
+  uint32_t stride = 1;       // threshold sample: every stride-th window (driver: posting block)
+  bool edge_sample = false;  // the sample is the explicit list `sample_win`: strided windows + each split's first and last
+  bool rec_l0 = false;       // the collect pass records the exact level-0 histogram (second-chance top-K)
+  SmemLayout lay;             // k_window
+  qwk::USmem ulay_c, ulay_h;  // k_union collect / histogram
+  qwk::ASmem alay;            // k_aggscan
+  // prefix sums over splits: windows, sampled windows; driver: posting blocks, sampled blocks ([n + 1] or empty)
+  std::vector<uint32_t> fw_all, fw_smp, fw_drv, fw_dsm, sample_win;  // sample_win: window | edge << 31 per work item
+  // k_driver runs every pass without refine flags, at any radix level; k_union the collect pass and the level-0
+  // histogram without a prefix; k_aggscan the plain collect pass
+  bool serves(int mode, uint32_t level, uint32_t use_prefix, uint32_t flags) const {
+    return !flags && (kind == DRIVER || (kind == UNION && (mode == qwk::MODE_COLLECT || (level == 0 && !use_prefix))) ||
+                      (kind == AGGSCAN && mode == qwk::MODE_COLLECT));
+  }
+};
+
+// the threshold sample and the work lists of the route's window size
+static void plan_sample(Route& r, const std::vector<Lowered>& low, int sm_count) {
+  const uint32_t n = (uint32_t)low.size();
+  auto windows = [](const Lowered& L, uint32_t W) { return L.empty ? 0u : (L.P.num_docs + W - 1) / W; };
+  // BM25-union batches sample the threshold over the collect pass's window size rounded down to 1024 docs. Finer
+  // windows (the same fraction of the docs in more work items) were measured on the bench workload, one H100 80GB HBM3
+  // (400 W power limit): W gives 1.175-1.183 ms per 4-query step, W / 2 gives 1.194-1.203 ms and W / 4 gives
+  // 1.216-1.231 ms (the per-window clause chain does not shrink with the window).
+  r.W_h = r.kind == Route::UNION ? std::max(1024u, r.W & ~1023u) : r.W;
+  uint32_t mw = 0, tw = 0;
+  for (const Lowered& L : low) { mw = std::max(mw, windows(L, r.W_h)); tw += windows(L, r.W_h); }
+  // sampling stride of the threshold-estimation pass: 1/16 of the windows (a coarser sample shortens the histogram
+  // pass, but the looser threshold lets more candidates through the collect pass)
+  const uint32_t stride_cap = 16;
+  r.stride = std::min(stride_cap, std::max(1u, mw / 8));
+  if (r.kind == Route::UNION) {
+    // Large requests: at most ONE sampled window per resident block (the sampled pass is latency bound — a block
+    // that gets two windows doubles its duration), up to a stride of 32. Bench workload on one H100 80GB HBM3 (400 W
+    // power limit; 6528 windows, 132 SMs x 2 = 264 blocks): stride 25 instead of 16, 1.175-1.183 against 1.209-1.211 ms
+    // per 4-query step (a fixed stride of 32: 1.174-1.181 ms, no better).
+    const uint32_t per_block = (tw + (uint32_t)(sm_count * QU_MINB) - 1) / (uint32_t)(sm_count * QU_MINB);
+    r.stride = std::max(r.stride, std::min({per_block, 32u, std::max(1u, mw / 8)}));
+  }
+  if (r.kind == Route::DRIVER) {
+    // posting-driven kernel: the work list is the driving term's posting blocks; the threshold sample takes every
+    // stride-th BLOCK (128 postings, fine enough for keys that follow doc order: what lies between two sampled
+    // blocks is < 2K postings)
+    uint32_t max_blocks = 0;
+    for (const Lowered& L : low) max_blocks = std::max(max_blocks, L.empty ? 0u : L.instrs[1].n);
+    r.stride = std::min(stride_cap, std::max(1u, max_blocks / 64));
+    r.fw_drv.assign(n + 1, 0);
+    r.fw_dsm.assign(n + 1, 0);
+    for (uint32_t i = 0; i < n; i++) {
+      const uint32_t nb = low[i].empty ? 0u : low[i].instrs[1].n, phase = r.stride > 1 ? i % r.stride : 0;
+      r.fw_drv[i + 1] = r.fw_drv[i] + nb;
+      r.fw_dsm[i + 1] = r.fw_dsm[i] + (nb > phase ? (nb - phase + r.stride - 1) / r.stride : 0);
+    }
+  }
+  // the generic kernels sample an explicit window list: strided windows + the first and last window of each
+  // split (weight 1 in the histogram); the union pipeline keeps the plain strided sample (scores do not
+  // follow doc order)
+  r.edge_sample = r.kind != Route::UNION && r.kind != Route::DRIVER && r.stride > 1;
+  r.fw_all.assign(n + 1, 0);
+  r.fw_smp.assign(n + 1, 0);
+  for (uint32_t i = 0; i < n; i++) {
+    const uint32_t nw = windows(low[i], r.W_h), phase = r.stride > 1 ? i % r.stride : 0;
+    r.fw_all[i + 1] = r.fw_all[i] + windows(low[i], r.W);
+    if (r.edge_sample) {
+      uint32_t cnt = 0;
+      for (uint32_t w = 0; w < nw; w++) {
+        const bool edge = w == 0 || w + 1 == nw, strided = w % r.stride == phase;
+        if (edge || strided) { r.sample_win.push_back(w | (edge ? 0x80000000u : 0u)); cnt++; }
+      }
+      r.fw_smp[i + 1] = r.fw_smp[i] + cnt;
+    } else r.fw_smp[i + 1] = r.fw_smp[i] + (nw > phase ? (nw - phase + r.stride - 1) / r.stride : 0);
+  }
+}
+
+static Route choose_route(const std::vector<Lowered>& low, int max_smem_optin, int sm_count) {
+  Route r;
+  uint32_t n_levels = 1, need_cnt = 0, need_ssum = 0, need_msum = 0, max_instr = 0, max_cols = 0, max_aggs = 0, n_fn = 0;
+  // second-chance top-K: when no plan ranks by _score first, the collect pass also records the exact
+  // level-0 histogram and every window's best digit, so that a failed sampled threshold is repaired
+  // by a candidates-only pass over the few windows that can hold candidates
+  bool rec_l0 = true, rangeq = false, any_topk = false, all_union = true, all_driver = true;
+  for (const Lowered& L : low) {
+    all_union = all_union && union_eligible(L);
+    all_driver = all_driver && driver_eligible(L);
+    if (L.P.max_hits && L.P.key.kind[0] == QW_SORT_SCORE) rec_l0 = false;
+    for (const DInstr& in : L.instrs)
+      if ((in.op == OP_RANGE || in.op == OP_EXISTS) && (in.occur == QW_OCCUR_MUST || in.occur == QW_OCCUR_FILTER)) rangeq = true;
+    n_levels = std::max(n_levels, L.P.n_levels);
+    need_cnt |= L.need_cnt; need_ssum |= L.need_ssum; need_msum |= L.need_msum;
+    max_instr = std::max(max_instr, L.P.n_instr); max_cols = std::max(max_cols, L.P.n_cols); max_aggs = std::max(max_aggs, L.P.n_aggs);
+    n_fn = std::max(n_fn, L.P.n_fn_slots);
+    any_topk |= L.P.max_hits > 0;
+  }
+  if (all_driver) r.kind = Route::DRIVER;
+  else if (all_union) r.kind = Route::UNION;
+  else if (aggscan_layout(low, max_smem_optin, &r.alay)) r.kind = Route::AGGSCAN;
+  r.rec_l0 = rec_l0 && any_topk && r.kind != Route::DRIVER;
+  // (union batches: k_window is only the rare exact-radix fallback)
+  const int smem_per_block = max_smem_optin / (r.kind == Route::UNION ? 1 : QW_MIN_BLOCKS_PER_SM);
+  auto layout = [&](uint32_t W) {
+    return make_layout(W, n_levels, need_cnt, need_msum, need_ssum, max_instr, max_cols, max_aggs, n_fn, r.rec_l0, rangeq);
+  };
+  // k_aggscan's flat work list is the list of QA_CHUNK-doc chunks: the generic layout must take a whole chunk
+  if (r.kind == Route::AGGSCAN && (int)layout(QA_CHUNK).total + 1024 > smem_per_block) r.kind = Route::WINDOW;
+  // window size: as large as shared memory allows for the configured blocks/SM (per-window fixed
+  // costs — staging, program interpretation, barriers — amortise over more postings). BM25-union batches run the
+  // TMA + mbarrier pipeline (union_kernel.cuh): fixed 15360-doc windows, two blocks per SM
+  r.W = r.kind == Route::AGGSCAN ? QA_CHUNK : r.kind == Route::UNION ? 15360u * 2 / QU_MINB : 32768u;
+  for (;; r.W >>= 1) {
+    r.lay = layout(r.W);
+    if ((int)r.lay.total + 1024 <= smem_per_block || r.W == 1024) break;
+  }
+  if ((int)r.lay.total > max_smem_optin) fail(QWGPU_EUNSUPPORTED, "query needs %u bytes of shared memory per block", r.lay.total);
+  if (r.kind == Route::UNION) {
+    // (the generic layout above stays valid for the same W: exact radix passes below level 0 use k_window)
+    const uint32_t u_budget = (uint32_t)(max_smem_optin + 1024) / QU_MINB - 1024 - 64;
+    r.ulay_c = make_union_layout(r.W, false, u_budget);
+    r.ulay_h = make_union_layout(r.W, true, u_budget);
+  }
+  plan_sample(r, low, sm_count);
+  return r;
+}
+
+// A call slot from the pool, behind the admission gate; both are given back when the call ends, on every path.
+// Admission: at most QWGPU_MAX_IN_FLIGHT (default 16) searches drive the device at once; further callers wait here
+// on a condition variable (no CUDA calls, no spinning). Measured on the mixed config-5 query set from 64 host threads,
+// one H100 80GB HBM3 (400 W power limit): with the limit at 16, 1643 queries/s (p99 66-72 ms) in both of two runs;
+// with it at 64, 894 and 1517 queries/s (p99 341 and 174 ms) — the driver's per-context lock and 64 interleaved
+// streams cost more than the extra overlap brings.
+struct SlotLease {
+  Engine& e;
+  CallSlot* slot = nullptr;
+  explicit SlotLease(Engine& eng) : e(eng) {
+    static const int max_in_flight = getenv("QWGPU_MAX_IN_FLIGHT") ? std::max(1, atoi(getenv("QWGPU_MAX_IN_FLIGHT"))) : 16;
+    {
+      std::unique_lock<std::mutex> g(e.mu);
+      e.cv_admit.wait(g, [&] { return e.admitted < max_in_flight; });
+      e.admitted++;
+      if (!e.free_slots.empty()) { slot = e.free_slots.back(); e.free_slots.pop_back(); }
+    }
+    if (!slot) {
+      try {
+        slot = new CallSlot();
+        CUDA_CHECK(cudaStreamCreateWithFlags(&slot->stream, cudaStreamNonBlocking));
+        for (cudaEvent_t* ev : {&slot->ev0, &slot->ev1, &slot->ev2, &slot->ev3}) CUDA_CHECK(cudaEventCreate(ev));
+        CUDA_CHECK(cudaEventCreateWithFlags(&slot->ev_block, cudaEventBlockingSync | cudaEventDisableTiming));
+      } catch (...) {
+        delete slot;
+        { std::lock_guard<std::mutex> g(e.mu); e.admitted--; }
+        e.cv_admit.notify_one();
+        throw;
+      }
+    }
+    e.in_flight.fetch_add(1);
+  }
+  // the slot goes back to the pool only once its stream is idle: on an error path copies / kernels of this
+  // call may still be in flight, and the next call would reuse the pinned buffers under them
+  ~SlotLease() {
+    cudaStreamSynchronize(slot->stream);
+    e.in_flight.fetch_sub(1);
+    {
+      std::lock_guard<std::mutex> g(e.mu);
+      e.free_slots.push_back(slot);
+      e.admitted--;
+    }
+    e.cv_admit.notify_one();
+  }
+};
+
+// Waiting for the call's stream: cudaStreamSynchronize spins on a CPU core, which is the fastest wake-up while a
+// few calls are in flight (single-query latency) and a disaster when more host threads wait than there are cores
+// to spare — the spinners starve the threads that still have plans to compile. Beyond a quarter of the cores the
+// wait goes through a blocking event instead (the thread sleeps until the driver's interrupt).
+static void wait_call(Engine& e, CallSlot& slot) {
+  static const uint32_t spin_limit = getenv("QWGPU_SPIN_LIMIT") ? (uint32_t)atoi(getenv("QWGPU_SPIN_LIMIT")) : std::max(2u, std::thread::hardware_concurrency() / 4);
+  if (e.in_flight.load(std::memory_order_relaxed) > (int)spin_limit) {
+    CUDA_CHECK(cudaEventRecord(slot.ev_block, slot.stream));
+    CUDA_CHECK(cudaEventSynchronize(slot.ev_block));
+  } else CUDA_CHECK(cudaStreamSynchronize(slot.stream));
+}
+
+enum { F_REC = 1, F_REFINE = 2, F_CANDS_ONLY = 4 };  // collect / histogram pass flags
+// One device run of a lowered batch on the call's slot. lay_out() places every region in the slot's buffers: blob
+// (copied to the device: plans, programs, work lists), scratch (device only) and out (copied back); stage() gives the
+// run's copies of the plans their addresses and copies the blob over; run() issues the passes.
+struct Run {
+  Engine& e;
+  CallSlot& slot;
+  BatchStats& stats;
+  const std::vector<Lowered>& low;
+  const std::vector<uint32_t>& idx;
+  const Route& r;
+  const MergeSpec* merge;
+  const GatherSpec* gather;
+  const bool do_merge, do_gather;
+  const uint32_t n;
+  const cudaStream_t st;
+  std::vector<DSplitPlan> plans;      // copies of the lowered plans with the run's positions, capacities and addresses
+  std::vector<uint32_t> bounds_base;  // per split: position of its histogram bounds in the batch's table
+  struct Split { size_t out, tr_best, tr_match, h_table, h_keys, h_cells; };  // offsets of a split's regions
+  std::vector<Split> at;
+  bool any_topk, any_trace, any_hashed, any_composite, any_fast_aggs;
+  uint32_t kmax, n_phrases, phrase_blocks, tie_max_n;
+  size_t n_phrase_exp;
+  size_t o_plans, o_instr, o_cols, o_aggs, o_fwa, o_fws, o_bounds, o_rank, o_smp, o_phr, o_pexp, o_fwd, o_fwds, blob_bytes;
+  size_t s_thr, s_hist, s_state, s_wmax, s_cand, s_hits, s_cut, s_grecv, s_vblk, s_trace_state, s_trace_data, s_hash, scratch_bytes;
+  size_t rec_bytes, o_merged, o_ghdr, o_final, out_bytes;
+  std::vector<std::vector<DHKey>> h_keys;  // per hashed split: the used cells, copied back
+  std::vector<std::vector<QwAggCell>> h_cells;
+  KParams kp;
+  int occ;
+  float main_ms;  // device time of the run's collect passes
+
+  // at_bound: every hashed table is sized at its bound (the re-run after an overflow), else at
+  // min(bound, QWGPU_HASHED_INIT_CELLS) cells
+  void lay_out(bool at_bound) {
+    plans.resize(n);
+    bounds_base.resize(n);
+    at.assign(n, Split{});
+    any_topk = any_trace = any_hashed = any_composite = any_fast_aggs = false;
+    kmax = 1;
+    n_phrases = phrase_blocks = tie_max_n = 0;
+    n_phrase_exp = 0;
+  h_keys.assign(n, {});
+  h_cells.assign(n, {});
+    uint32_t tot_instr = 0, tot_cols = 0, tot_aggs = 0, tot_bounds = 0;
+    for (uint32_t i = 0; i < n; i++) {
+      const Lowered& L = low[i];
+      DSplitPlan& P = plans[i] = L.P;
+      P.num_windows = r.fw_all[i + 1] - r.fw_all[i];
+      P.instr_base = tot_instr; P.col_base = tot_cols; P.agg_base = tot_aggs;
+      bounds_base[i] = tot_bounds;
+      tot_instr += P.n_instr; tot_cols += P.n_cols; tot_aggs += P.n_aggs; tot_bounds += (uint32_t)L.bounds.size();
+      // privatised counters + stats triples must fit the (dead at collect time) staging area
+      if (P.fast_aggs && (((size_t)P.n_cells * 4 + 7) & ~(size_t)7) + (size_t)P.n_stat_cells * 24 > stage_bytes_for(r.W)) P.fast_aggs = 0;
+      if (P.hashed) {
+        any_hashed = true;
+        for (const DAgg& d : L.aggs) if (d.comp & QW_AGG_COMP_LEVEL) any_composite = true;
+        P.h_cap = (uint32_t)(at_bound ? L.h_bound : std::min<uint64_t>(L.h_bound, QWGPU_HASHED_INIT_CELLS));
+        P.h_mask = agg_hashed_slots(P.h_cap) - 1;
+      }
+      // phrases: one uncompressed posting block per block of each phrase's driver term (phrase_kernel.cuh)
+      for (size_t k = 0; k < L.phrases.size(); k++) { n_phrases++; phrase_blocks += L.instrs[L.phrase_instr[k]].n; }
+      n_phrase_exp += L.phrase_exp.size();
+      kmax = std::max(kmax, P.max_hits);
+      any_topk |= P.max_hits > 0;
+      any_trace |= P.tr_on != 0;
+    }
+    Arena blob{256};
+    o_plans = blob.take(n * sizeof(DSplitPlan));
+    o_instr = blob.take(tot_instr * sizeof(DInstr));
+    o_cols = blob.take(std::max(tot_cols, 1u) * sizeof(DCol));
+    o_aggs = blob.take(std::max(tot_aggs, 1u) * sizeof(DAgg));
+    o_fwa = blob.take((n + 1) * 4);
+    o_fws = blob.take((n + 1) * 4);
+    o_bounds = blob.take((size_t)tot_bounds * 8);
+    o_rank = blob.take((size_t)n * 4);
+    o_smp = blob.take(r.sample_win.size() * 4);
+    o_phr = blob.take((size_t)n_phrases * sizeof(DPhrase));
+    o_pexp = blob.take(n_phrase_exp * sizeof(DPhraseTerm));
+    o_fwd = blob.take(r.fw_drv.size() * 4);
+    o_fwds = blob.take(r.fw_dsm.size() * 4);
+    blob_bytes = blob.off;
+    rec_bytes = do_merge ? 64 + (size_t)merge->k * sizeof(qwk::DMergedHit) : 0;  // a rank's gather record
+    Arena s{256};
+    s_thr = s.take(n * sizeof(DThresh));
+    s_hist = s.take((size_t)n * QW_HIST_BINS * 4);
+    s_state = s.take((size_t)n * 4);
+    s_wmax = s.take(r.rec_l0 ? (size_t)r.fw_all[n] * 2 : 0);
+    s_cand = s.take(any_topk ? (size_t)n * QW_CAND_CAP * 24 : 0);
+    s_hits = s.take(do_merge ? (size_t)n * kmax * sizeof(QwHit) : 0);
+    s_cut = s.take((size_t)std::max<uint32_t>(n, 64) * 4 + 1024);  // split merge's cut, then the gathered merge's
+    s_grecv = s.take(gather && gather->world > 1 && do_merge ? (size_t)gather->world * rec_bytes : 0);
+    s_vblk = s.take((size_t)phrase_blocks * sizeof(VBlk));
+    // find_trace_ids: per split a DTraceState (one region, set to 0xFF bytes), then best[] + match bitmap (zeroed)
+    s_trace_state = s.take(any_trace ? (size_t)n * sizeof(qwk::DTraceState) : 0);
+    s_trace_data = s.off;
+    for (uint32_t i = 0; i < n; i++)
+      if (plans[i].tr_on) {
+        at[i].tr_best = s.take((size_t)plans[i].tr_num_ords * 8);
+        at[i].tr_match = s.take((size_t)((plans[i].num_docs + 31) / 32) * 4);
+      }
+    // hashed aggregation cells: per split [slot table][key records][cells]
+    s_hash = s.off;
+    for (uint32_t i = 0; i < n; i++) {
+      const DSplitPlan& P = plans[i];
+      if (!P.hashed) continue;
+      at[i].h_table = s.take((size_t)(P.h_mask + 1) * 4);
+      at[i].h_keys = s.take((size_t)P.h_cap * sizeof(DHKey));
+      at[i].h_cells = s.take((size_t)P.h_cap * sizeof(QwAggCell));
+    }
+    scratch_bytes = s.off;
+    Arena o{256};
+    for (uint32_t i = 0; i < n; i++)
+      at[i].out = o.take(32 + (do_merge ? 0 : (size_t)plans[i].max_hits * sizeof(QwHit)) + (size_t)plans[i].n_cells * sizeof(QwAggCell));
+    // [RankHeader 64 B (n_hits first)][DMergedHit x k]: the batch's merged top-k = this rank's gather record
+    o_merged = o.take(rec_bytes);
+    if (do_gather) {
+      o_ghdr = o.take((size_t)gather->world * 64);  // (compacted copy of the gathered headers)
+      o_final = o.take(16 + (size_t)merge->k * sizeof(qwk::DMergedHit));
+    }
+    out_bytes = o.off;
+  }
+
+  // slots are sized to the largest request the context has seen: a slot that meets a bigger request later would
+  // have to cudaFree / cudaMalloc (device-synchronising) in the middle of concurrent searches
+  void size_slot() {
+    size_t want_blob, want_scratch, want_out;
+    {
+      std::lock_guard<std::mutex> g(e.mu);
+      e.hw_blob = std::max(e.hw_blob, blob_bytes); e.hw_scratch = std::max(e.hw_scratch, scratch_bytes); e.hw_out = std::max(e.hw_out, out_bytes);
+      // (only while the marks stay moderate: one huge aggregation request must not size every slot after itself)
+      auto sized = [](size_t hw, size_t need) { return hw <= ((size_t)64 << 20) ? hw : need; };
+      want_blob = sized(e.hw_blob, blob_bytes); want_scratch = sized(e.hw_scratch, scratch_bytes); want_out = sized(e.hw_out, out_bytes);
+    }
+    slot.ensure(want_blob, want_scratch, want_out);
+  }
+
+  // Cross-rank phase (after this rank's result is final: a verification fallback must not repeat a collective the
+  // other ranks run once): the rank's record at out + o_merged -> every rank (one NCCL all-gather on the call's
+  // stream) -> merged again on the device -> [gathered headers][final hits] copied back
+  void exchange() {
+    const MergeSpec& m = *merge;
+    const GatherSpec& g = *gather;
+    uint8_t* g_recv = slot.d_scratch + s_grecv;
+    if (g.allgather(g.comm, slot.d_out + o_merged, g_recv, rec_bytes, (void*)st)) fail(QWGPU_EINTERNAL, "ncclAllGather failed");
+    const qwk::SrcGathered gsrc{g_recv, (uint32_t)rec_bytes, 64u};
+    uint32_t* g_cut = (uint32_t*)(slot.d_scratch + s_cut) + std::max<uint32_t>(n, 64);
+    qwk::k_merge_prep<qwk::SrcGathered><<<1, 1024, 0, st>>>(gsrc, (uint32_t)g.world, m.k, m.order1, m.order2, g_cut);
+    qwk::k_merge<qwk::SrcGathered><<<(uint32_t)(((uint64_t)g.world * m.k * 32 + 255) / 256), 256, 0, st>>>(gsrc, g_cut, (uint32_t)g.world, m.k, m.k, m.order1, m.order2,
+                                                                                    (qwk::DMergedHit*)(slot.d_out + o_final + 16), (uint32_t*)(slot.d_out + o_final));
+    CUDA_CHECK(cudaMemcpy2DAsync(slot.d_out + o_ghdr, 64, g_recv, rec_bytes, 64, (size_t)g.world, cudaMemcpyDeviceToDevice, st));
+    CUDA_CHECK(cudaMemcpyAsync(slot.h_out + o_ghdr, slot.d_out + o_ghdr, out_bytes - o_ghdr, cudaMemcpyDeviceToHost, st));
+  }
+
+  // the run's plans get the slot's addresses; everything the kernels read goes to the device in one copy
+  void stage() {
+    uint8_t *hb = slot.h_blob, *db = slot.d_blob;
+    uint32_t phr_done = 0, phr_blocks_done = 0;
+    size_t pexp_done = 0;
+    for (uint32_t i = 0; i < n; i++) {
+      const Lowered& L = low[i];
+      DSplitPlan& P = plans[i];
+      any_fast_aggs |= P.fast_aggs != 0;
+      if (P.tr_on) tie_max_n = std::max(tie_max_n, P.tr_n);
+      uint8_t* ob = slot.d_out + at[i].out;
+      P.out_num_hits = (uint64_t)ob;            // [0] hits, [1] eligible
+      P.out_nhits = (uint64_t)(ob + 16);
+      P.out_cand_count = (uint64_t)(ob + 20);
+      P.out_hits = do_merge ? (uint64_t)(slot.d_scratch + s_hits + (size_t)i * kmax * sizeof(QwHit)) : (uint64_t)(ob + 32);
+      P.out_cells = (uint64_t)(ob + 32 + (do_merge ? 0 : (size_t)P.max_hits * sizeof(QwHit)));
+      P.out_hist = (uint64_t)(slot.d_scratch + s_hist + (size_t)i * QW_HIST_BINS * 4);
+      P.out_cands = (uint64_t)(slot.d_scratch + s_cand + (size_t)i * QW_CAND_CAP * 24);
+      if (P.tr_on) {
+        P.tr_state = (uint64_t)(slot.d_scratch + s_trace_state + (size_t)i * sizeof(qwk::DTraceState));
+        P.tr_best = (uint64_t)(slot.d_scratch + at[i].tr_best);
+        P.tr_match = (uint64_t)(slot.d_scratch + at[i].tr_match);
+        P.tr_tie = (uint64_t)(ob + 24);
+      }
+      if (P.hashed) {
+        P.h_table = (uint64_t)(slot.d_scratch + at[i].h_table);
+        P.h_keys = (uint64_t)(slot.d_scratch + at[i].h_keys);
+        P.h_cells = (uint64_t)(slot.d_scratch + at[i].h_cells);
+        P.h_ctr = (uint64_t)(ob + 28);
+      }
+      DInstr* instrs = (DInstr*)(hb + o_instr) + P.instr_base;
+      memcpy(instrs, L.instrs.data(), P.n_instr * sizeof(DInstr));
+      for (size_t k = 0; k < L.phrases.size(); k++) {
+        DPhrase ph = L.phrases[k];
+        ph.first_work = phr_blocks_done;
+        ph.out = (uint64_t)(slot.d_scratch + s_vblk + (size_t)phr_blocks_done * sizeof(VBlk));
+        if (ph.n_exp) {
+          memcpy(hb + o_pexp + pexp_done * sizeof(DPhraseTerm), L.phrase_exp.data() + ph.exp, (size_t)ph.n_exp * sizeof(DPhraseTerm));
+          ph.exp = (uint64_t)(db + o_pexp + pexp_done * sizeof(DPhraseTerm));
+          pexp_done += ph.n_exp;
+        }
+        instrs[L.phrase_instr[k]].a = ph.out;
+        phr_blocks_done += instrs[L.phrase_instr[k]].n;
+        memcpy(hb + o_phr + (size_t)phr_done++ * sizeof(DPhrase), &ph, sizeof ph);
+      }
+      memcpy(hb + o_plans + i * sizeof(DSplitPlan), &P, sizeof P);
+      if (P.n_cols) memcpy(hb + o_cols + P.col_base * sizeof(DCol), L.cols.data(), P.n_cols * sizeof(DCol));
+      DAgg* aggs = (DAgg*)(hb + o_aggs) + P.agg_base;
+      if (P.n_aggs) memcpy(aggs, L.aggs.data(), P.n_aggs * sizeof(DAgg));
+      if (P.fast_aggs)  // (lowering left each histogram's bounds as an index into the split's table)
+        for (uint32_t a = 0; a < P.n_aggs; a++)
+          if (aggs[a].kind == QW_AGG_HISTOGRAM) aggs[a].bounds = (uint64_t)(db + o_bounds) + (bounds_base[i] + aggs[a].bounds) * 8;
+      if (!L.bounds.empty()) memcpy(hb + o_bounds + (size_t)bounds_base[i] * 8, L.bounds.data(), L.bounds.size() * 8);
+    }
+    if (do_merge) for (uint32_t i = 0; i < n; i++) ((uint32_t*)(hb + o_rank))[i] = merge->rank[idx[i]];
+    if (!r.sample_win.empty()) memcpy(hb + o_smp, r.sample_win.data(), r.sample_win.size() * 4);
+    if (!r.fw_drv.empty()) { memcpy(hb + o_fwd, r.fw_drv.data(), (n + 1) * 4); memcpy(hb + o_fwds, r.fw_dsm.data(), (n + 1) * 4); }
+    memcpy(hb + o_fwa, r.fw_all.data(), (n + 1) * 4);
+    memcpy(hb + o_fws, r.fw_smp.data(), (n + 1) * 4);
+    CUDA_CHECK(cudaMemcpyAsync(db, hb, blob_bytes, cudaMemcpyHostToDevice, st));
+    stats.h2d_bytes += blob_bytes;
+
+    kp = KParams{};
+    kp.plans = (const DSplitPlan*)(db + o_plans);
+    kp.instrs = (const DInstr*)(db + o_instr);
+    kp.cols = (const DCol*)(db + o_cols);
+    kp.aggs = (const DAgg*)(db + o_aggs);
+    kp.thresh = (DThresh*)(slot.d_scratch + s_thr);
+    kp.n_splits = n;
+    kp.W = r.W;
+    kp.stage_bytes = stage_bytes_for(r.W);
+    // privatised aggregation counters (and the radix histogram, 8 KB) live in the staging area
+    uint32_t max_cells = 0;
+    bool any_aggs = false;
+    for (const DSplitPlan& P : plans) { max_cells = std::max(max_cells, P.n_cells); any_aggs |= P.n_aggs > 0; }
+    kp.smem_aggs = (any_aggs && max_cells * 4 <= kp.stage_bytes && max_cells <= QW_SMEM_AGG_CELLS) ? 1 : 0;
+    kp.sm = r.lay;
+    kp.wmax = (uint16_t*)(slot.d_scratch + s_wmax);
+    kp.split_state = (const uint32_t*)(slot.d_scratch + s_state);
+    CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, qwk::k_window<qwk::MODE_COLLECT>, QW_THREADS, r.lay.total));
+    occ = std::max(occ, 1);
+  }
+
+  // one pass over the batch on the route's kernel when it serves the pass, else on k_window
+  void launch(int mode, bool sampled, uint32_t level, uint32_t use_prefix, uint32_t flags) {
+    const Route::Kind kind = r.serves(mode, level, use_prefix, flags) ? r.kind : Route::WINDOW;
+    const uint32_t stride = sampled ? r.stride : 1;
+    auto launched = [&](uint32_t kernel) { stats.launches++; stats.kernel_mask |= kernel; };
+    if (kind == Route::DRIVER) {
+      qwk::DrvParams d{};
+      d.plans = kp.plans; d.instrs = kp.instrs; d.cols = kp.cols; d.thresh = kp.thresh;
+      d.first_work = (const uint32_t*)(slot.d_blob + (sampled ? o_fwds : o_fwd)); d.n_splits = n; d.total_work = sampled ? r.fw_dsm[n] : r.fw_drv[n];
+      d.level = level; d.use_prefix = use_prefix; d.stride = stride;
+      if (d.total_work == 0) return;
+      const uint32_t dgrid = std::min<uint32_t>((d.total_work + QD_WARPS - 1) / QD_WARPS, (uint32_t)(e.sm_count * 4));
+      if (mode == qwk::MODE_HIST) qwk::k_driver<qwk::MODE_HIST><<<dgrid, QD_WARPS * 32, 0, st>>>(d);
+      else qwk::k_driver<qwk::MODE_COLLECT><<<dgrid, QD_WARPS * 32, 0, st>>>(d);
+      launched(QWGPU_KERNEL_DRIVER);
+      return;
+    }
+    const uint32_t* first_work = (const uint32_t*)(slot.d_blob + (sampled ? o_fws : o_fwa));
+    const uint32_t total_work = sampled ? r.fw_smp[n] : r.fw_all[n];
+    if (total_work == 0) return;
+    if (kind == Route::AGGSCAN) {
+      qwk::AParams a{};
+      a.plans = kp.plans; a.cols = kp.cols; a.aggs = kp.aggs;
+      a.first_work = first_work; a.n_splits = n; a.total_work = total_work;
+      a.sm = r.alay;
+      int aocc = 1;
+      CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&aocc, qwk::k_aggscan, QA_THREADS, r.alay.total));
+      const uint32_t agrid = std::min<uint32_t>(total_work, (uint32_t)(e.sm_count * std::max(aocc, 1)));
+      qwk::k_aggscan<<<agrid, QA_THREADS, r.alay.total, st>>>(a);
+      launched(QWGPU_KERNEL_AGGSCAN);
+      return;
+    }
+    if (kind == Route::UNION) {
+      qwk::UParams u{};
+      u.plans = kp.plans; u.instrs = kp.instrs; u.cols = kp.cols; u.thresh = kp.thresh;
+      u.first_work = first_work; u.n_splits = n; u.total_work = total_work; u.stride = stride; u.W = sampled ? r.W_h : r.W;
+      u.sm = mode == qwk::MODE_HIST ? r.ulay_h : r.ulay_c;
+      // cross-rank calls leave a few block slots free: the persistent grid would otherwise hold every SM's shared
+      // memory, a concurrent call's NCCL kernel would take the place of one of its blocks, and that block — with its
+      // static share of the windows — would only start when another one has finished (twice the kernel time)
+      const uint32_t ugrid = std::min<uint32_t>(total_work, (uint32_t)(e.sm_count * QU_MINB) - (do_gather ? 4u : 0u));
+      if (mode == qwk::MODE_HIST) qwk::k_union<qwk::MODE_HIST><<<ugrid, QU_THREADS, u.sm.total, st>>>(u);
+      else qwk::k_union<qwk::MODE_COLLECT><<<ugrid, QU_THREADS, u.sm.total, st>>>(u);
+      launched(QWGPU_KERNEL_UNION);
+      return;
+    }
+    KParams q = kp;
+    q.first_work = first_work;
+    q.total_work = total_work;
+    q.stride = stride;
+    q.sample_win = (sampled && r.edge_sample) ? (const uint32_t*)(slot.d_blob + o_smp) : nullptr;
+    q.level = level;
+    q.use_prefix = use_prefix;
+    q.rec_l0 = (flags & F_REC) ? 1 : 0;
+    q.refine = (flags & F_REFINE) ? 1 : 0;
+    q.cands_only = (flags & F_CANDS_ONLY) ? 1 : 0;
+    const uint32_t grid = std::min<uint32_t>(total_work, (uint32_t)(e.sm_count * occ));
+    if (mode == qwk::MODE_HIST) qwk::k_window<qwk::MODE_HIST><<<grid, QW_THREADS, r.lay.total, st>>>(q);
+    else if (any_hashed) qwk::k_window<qwk::MODE_COLLECT, true><<<grid, QW_THREADS, r.lay.total, st>>>(q);
+    else qwk::k_window<qwk::MODE_COLLECT><<<grid, QW_THREADS, r.lay.total, st>>>(q);
+    launched(QWGPU_KERNEL_WINDOW);
+    // (k_window aggregates on the fast path where the plan's and the launch's flags both allow it)
+    if (mode == qwk::MODE_COLLECT && !(flags & F_CANDS_ONLY) && any_fast_aggs && kp.smem_aggs) stats.kernel_mask |= QWGPU_KERNEL_FAST_AGGS;
+    if (mode == qwk::MODE_COLLECT && !(flags & F_CANDS_ONLY) && any_hashed) stats.kernel_mask |= QWGPU_KERNEL_HASHED_AGGS;
+  }
+
+  // the collect pass and the kernels that finish the split results (composite cut, trace ids, top-K selection, the
+  // batch's merge), then the copy-back, waited for; a candidates-only repair keeps the counts and aggregations out
+  void collect(uint32_t flags) {
+    const bool full = !(flags & F_CANDS_ONLY);
+    if (full) {
+      CUDA_CHECK(cudaMemsetAsync(slot.d_out, 0, out_bytes, st));
+      if (any_trace) {
+        CUDA_CHECK(cudaMemsetAsync(slot.d_scratch + s_trace_state, 0xFF, (size_t)n * sizeof(qwk::DTraceState), st));
+        CUDA_CHECK(cudaMemsetAsync(slot.d_scratch + s_trace_data, 0, s_hash - s_trace_data, st));
+      }
+      for (uint32_t i = 0; i < n; i++)
+        if (plans[i].hashed) {
+          CUDA_CHECK(cudaMemsetAsync(slot.d_scratch + at[i].h_table, 0xFF, (size_t)(plans[i].h_mask + 1) * 4, st));
+          CUDA_CHECK(cudaMemsetAsync(slot.d_scratch + at[i].h_cells, 0, (size_t)plans[i].h_cap * sizeof(QwAggCell), st));
+        }
+    }
+    CUDA_CHECK(cudaEventRecord(slot.ev2, st));
+    launch(qwk::MODE_COLLECT, false, 0, 0, flags);
+    CUDA_CHECK(cudaEventRecord(slot.ev3, st));
+    if (any_composite && full) {
+      // each composite's first `size` leaves with their chains and sub-aggregation entries, before the copy-back
+      qwk::k_composite_cut<<<n, QC_THREADS, 0, st>>>(kp.plans, kp.aggs);
+      stats.launches++;
+      stats.kernel_mask |= QWGPU_KERNEL_COMPOSITE_CUT;
+    }
+    if (any_trace && full) {
+      // top N of the per-trace maxima; splits whose N-th and (N+1)-th maxima tie replay the reference's selection
+      qwk::k_trace_select<<<n, 1024, 0, st>>>(kp.plans);
+      qwk::k_trace_replay<<<n, QT_TILE, trace_replay_smem(tie_max_n), st>>>(kp.plans, kp.cols);
+      stats.launches += 2;
+      stats.kernel_mask |= QWGPU_KERNEL_TRACE_SELECT;
+    }
+    const uint32_t sel_smem = 3 * 8 * QW_CAND_CAP;  // [all first words | 3 x QW_SEL_MAX survivors] or 3 x all (degenerate ties)
+    if (any_topk) { qwk::k_select<<<n, 1024, sel_smem, st>>>(kp.plans, kp.cols); stats.launches++; }
+    if (do_merge) {
+      uint32_t* d_cut = (uint32_t*)(slot.d_scratch + s_cut);
+      const qwk::SrcSplits src{kp.plans, (const uint32_t*)(slot.d_blob + o_rank), do_gather ? 1u : 0u};
+      qwk::k_merge_prep<qwk::SrcSplits><<<1, 1024, 0, st>>>(src, n, merge->k, merge->order1, merge->order2, d_cut);
+      const uint64_t threads = (uint64_t)n * kmax * 32;  // one warp per hit (warps of pruned hits leave at once)
+      qwk::k_merge<qwk::SrcSplits><<<(uint32_t)((threads + 255) / 256), 256, 0, st>>>(src, d_cut, n, kmax, merge->k, merge->order1, merge->order2,
+                                                          (qwk::DMergedHit*)(slot.d_out + o_merged + 64), (uint32_t*)(slot.d_out + o_merged));
+      stats.launches += 2;
+    }
+    const size_t back = do_gather ? o_ghdr : out_bytes;  // (gathering: the final hits follow in the cross-rank phase)
+    CUDA_CHECK(cudaMemcpyAsync(slot.h_out, slot.d_out, back, cudaMemcpyDeviceToHost, st));
+    stats.d2h_bytes += back;
+    CUDA_CHECK(cudaEventRecord(slot.ev1, st));
+    wait_call(e, slot);
+  }
+
+  // a split's candidate set is good when it holds at least min(K, eligible) and did not overflow
+  bool verify(std::vector<uint32_t>& state) const {
+    bool all = true;
+    for (uint32_t i = 0; i < n; i++) {
+      state[i] = 0;
+      if (low[i].P.max_hits == 0) continue;
+      const uint8_t* ob = slot.h_out + at[i].out;
+      const uint64_t eligible = ((const uint64_t*)ob)[1], cand = *(const uint32_t*)(ob + 20);
+      if (cand > QW_CAND_CAP || cand < std::min<uint64_t>(low[i].P.max_hits, eligible)) { state[i] = 1; all = false; }
+    }
+    return all;
+  }
+
+  // exact radix select over the composite key: one histogram pass per 11-bit digit until the
+  // candidate set of every split fits QW_CAND_CAP. After a failed sampled threshold with the
+  // level-0 histogram on record (refine), level 0 needs no pass at all, only the failing splits are
+  // revisited, and windows whose best digit is below the threshold digit are skipped.
+  void exact_select(bool refine, std::vector<uint32_t>& state) {
+    const uint32_t* d_state = refine ? kp.split_state : nullptr;
+    std::vector<DThresh> th(n);
+    auto all_done = [&]() {
+      for (uint32_t i = 0; i < n; i++) if (low[i].P.max_hits && (!refine || state[i]) && !th[i].done) return false;
+      return true;
+    };
+    uint32_t max_key_bits = 1, level = 0;
+    for (const Lowered& L : low) max_key_bits = std::max(max_key_bits, L.P.key.total_bits);
+    bool done = false;
+    if (refine) {
+      CUDA_CHECK(cudaMemcpyAsync(slot.d_scratch + s_state, state.data(), n * 4, cudaMemcpyHostToDevice, st));
+      qwk::k_pick<<<n, 256, 0, st>>>(kp.plans, kp.thresh, 0, 0, 1, d_state);
+      stats.launches++;
+      CUDA_CHECK(cudaMemcpyAsync(th.data(), slot.d_scratch + s_thr, n * sizeof(DThresh), cudaMemcpyDeviceToHost, st));
+      wait_call(e, slot);
+      done = all_done();
+      level = 1;
+    } else {
+      CUDA_CHECK(cudaMemsetAsync(slot.d_scratch, 0, s_cand, st));
+    }
+    for (; !done && level * QW_DIGIT_BITS < max_key_bits; level++) {
+      CUDA_CHECK(cudaMemsetAsync(slot.d_scratch + s_hist, 0, (size_t)n * QW_HIST_BINS * 4, st));
+      launch(qwk::MODE_HIST, false, level, level > 0 ? 1 : 0, refine ? F_REFINE : 0);
+      qwk::k_pick<<<n, 256, 0, st>>>(kp.plans, kp.thresh, level, 0, 1, d_state);
+      stats.launches++;
+      stats.radix_passes++;
+      CUDA_CHECK(cudaMemcpyAsync(th.data(), slot.d_scratch + s_thr, n * sizeof(DThresh), cudaMemcpyDeviceToHost, st));
+      wait_call(e, slot);
+      done = all_done();
+    }
+    stats.refined = refine ? 1 : 0;
+    collect(refine ? (F_REFINE | F_CANDS_ONLY) : 0);
+    if (!verify(state)) fail(QWGPU_EINTERNAL, "top-K candidate selection failed verification");
+  }
+
+  // device time up to ev1 since ev0, and of the collect pass between ev2 and ev3
+  void add_device_time() {
+    float ms = 0, main = 0;
+    cudaEventElapsedTime(&ms, slot.ev0, slot.ev1);
+    cudaEventElapsedTime(&main, slot.ev2, slot.ev3);
+    stats.gpu_time_us += ms * 1000.f;
+    main_ms += main;
+  }
+
+  // The device part of a call: the threshold and collect passes, the hashed copy-back and the cross-rank exchange.
+  // False, with nothing returned, when a split's hashed aggregation cells overflowed their capacity.
+  bool run(bool at_bound) {
+    main_ms = 0;
+    CUDA_CHECK(cudaEventRecord(slot.ev0, st));
+    CUDA_CHECK(cudaMemsetAsync(slot.d_scratch, 0, s_cand, st));  // thresholds, histograms, refinement state
+    if (phrase_blocks) {
+      // phrase pre-pass (inside the timed device region): every phrase of the batch becomes a posting list in
+      // scratch (beyond s_cand: never cleared), read by every later pass
+      uint32_t max_terms = 1;
+      for (const Lowered& L : low) for (const DPhrase& ph : L.phrases) max_terms = std::max(max_terms, ph.n_terms);
+      const size_t psm = (size_t)QP_WARPS * QP_SMEM_WORDS(max_terms) * 4;
+      const uint32_t pgrid = (phrase_blocks + QP_WARPS - 1) / QP_WARPS;
+      const DPhrase* d_phr = (const DPhrase*)(slot.d_blob + o_phr);
+      // the suffix stage of phrase prefixes lives in its own instantiation: plain phrases keep the lean kernel
+      if (n_phrase_exp) qwk::k_phrase<true><<<pgrid, QP_WARPS * 32, psm, slot.stream>>>(d_phr, n_phrases, phrase_blocks, max_terms);
+      else qwk::k_phrase<false><<<pgrid, QP_WARPS * 32, psm, slot.stream>>>(d_phr, n_phrases, phrase_blocks, max_terms);
+      stats.launches++;
+      stats.kernel_mask |= QWGPU_KERNEL_PHRASE;
+    }
+    stats.window_docs = r.kind == Route::DRIVER ? QW_BLOCK_LEN : r.W;
+    std::vector<uint32_t> state(n, 0);  // per split: 1 = its sampled threshold failed
+    bool ok = true;
+    if (any_topk && r.stride > 1) {
+      // fast path: threshold from a 1/stride sample of the windows, verified after the collect pass
+      stats.sample_stride = r.stride;
+      launch(qwk::MODE_HIST, true, 0, 0, 0);
+      qwk::k_pick<<<n, 256, 0, st>>>(kp.plans, kp.thresh, 0, r.edge_sample ? 2 : 1, r.stride, nullptr);
+      stats.launches++;
+      if (r.rec_l0) CUDA_CHECK(cudaMemsetAsync(slot.d_scratch + s_hist, 0, (size_t)n * QW_HIST_BINS * 4, st));
+      collect(r.rec_l0 ? F_REC : 0);
+      ok = verify(state);
+      if (!ok) {
+        add_device_time();
+        stats.exact_fallbacks++;
+        CUDA_CHECK(cudaEventRecord(slot.ev0, st));
+      }
+    }
+    if (!any_topk) collect(0);
+    else if (r.stride == 1 || !ok) exact_select(!ok && r.rec_l0, state);
+    // hashed cells: a split that outgrew its capacity sends the batch round again at the bound (before any
+    // cross-rank collective, which must run once); otherwise only the used cells come back
+    auto used = [&](uint32_t i) { return *(const uint32_t*)(slot.h_out + at[i].out + 28); };
+    bool overflow = false;
+    for (uint32_t i = 0; i < n; i++) overflow |= plans[i].hashed && (used(i) >> 31);
+    if (overflow && at_bound) fail(QWGPU_EINTERNAL, "hashed aggregation cells overflowed their bound");
+    if (!overflow) {
+      if (any_hashed) {
+        for (uint32_t i = 0; i < n; i++) {
+          if (!plans[i].hashed) continue;
+          const uint32_t nu = std::min(used(i), plans[i].h_cap);
+          h_keys[i].resize(nu);
+          h_cells[i].resize(nu);
+          if (!nu) continue;
+          CUDA_CHECK(cudaMemcpyAsync(h_keys[i].data(), slot.d_scratch + at[i].h_keys, (size_t)nu * sizeof(DHKey), cudaMemcpyDeviceToHost, st));
+          CUDA_CHECK(cudaMemcpyAsync(h_cells[i].data(), slot.d_scratch + at[i].h_cells, (size_t)nu * sizeof(QwAggCell), cudaMemcpyDeviceToHost, st));
+          stats.d2h_bytes += (size_t)nu * (sizeof(DHKey) + sizeof(QwAggCell));
+        }
+        wait_call(e, slot);
+      }
+      if (do_gather) {
+        qwk::k_rank_header<<<1, 32, 0, st>>>(kp.plans, n, (qwk::DRankHeader*)(slot.d_out + o_merged), gather->attempted, gather->successful, gather->n_failed);
+        exchange();
+        CUDA_CHECK(cudaEventRecord(slot.ev1, st));
+        wait_call(e, slot);
+        stats.launches += 4;
+        stats.d2h_bytes += out_bytes - o_ghdr;
+      }
+      CUDA_CHECK(cudaGetLastError());
+    }
+    add_device_time();
+    stats.main_kernel_us = main_ms * 1000.f;
+    return !overflow;
+  }
+};
+
+// Lowers every plan once per call; a split whose plan cannot be lowered fails alone. idx: position of each lowered
+// plan in the caller's arrays.
+static std::vector<Lowered> lower_batch(const std::vector<std::shared_ptr<SplitDev>>& sp, const std::vector<const uint8_t*>& plans,
+                                        const std::vector<size_t>& plan_lens, std::vector<SplitOutput>& outs, std::vector<uint32_t>& idx) {
   std::vector<Lowered> low;
-  std::vector<uint32_t> idx;  // position in the caller's arrays
-  low.reserve(n_in);
-  for (uint32_t i = 0; i < n_in; i++) {
+  low.reserve(sp.size());
+  for (uint32_t i = 0; i < (uint32_t)sp.size(); i++) {
     try {
       if (!sp[i]) fail(QWGPU_ENOTFOUND, "split not registered");
       Lowered L;
@@ -958,822 +1683,180 @@ bool Engine::search_once(const std::vector<std::shared_ptr<SplitDev>>& sp, const
       outs[i].error = e.what();
     }
   }
-  {
-    // a re-run after an overflow sizes every hashed table of the call at its bound: the call's tables together must
-    // fit QWGPU_HASHED_MAX_BYTES, else every hashed split of the call fails here, before any launch
-    uint64_t total = 0;
-    uint32_t n_hashed = 0;
-    for (const Lowered& L : low)
-      if (L.P.hashed) { total += agg_hashed_table_bytes(L.h_bound); n_hashed++; }
-    if (total > QWGPU_HASHED_MAX_BYTES) {
-      std::vector<Lowered> keep;
-      std::vector<uint32_t> keep_idx;
-      for (size_t k = 0; k < low.size(); k++) {
-        if (!low[k].P.hashed) { keep.push_back(std::move(low[k])); keep_idx.push_back(idx[k]); continue; }
-        char msg[512];
-        snprintf(msg, sizeof msg, "split `%s`: the aggregation may create up to %llu buckets; the hashed tables of the call's %u "
-                 "hashed splits need %llu bytes at their bounds, more than the GPU limit of %llu bytes per call",
-                 sp[idx[k]]->id.c_str(), (unsigned long long)low[k].h_bound, n_hashed, (unsigned long long)total,
-                 (unsigned long long)QWGPU_HASHED_MAX_BYTES);
-        outs[idx[k]].status = QWGPU_EUNSUPPORTED;
-        outs[idx[k]].error = msg;
-      }
-      low.swap(keep);
-      idx.swap(keep_idx);
-    }
+  // a re-run after an overflow sizes every hashed table of the call at its bound: the call's tables together must
+  // fit QWGPU_HASHED_MAX_BYTES, else every hashed split of the call fails here, before any launch
+  uint64_t total = 0;
+  uint32_t n_hashed = 0;
+  for (const Lowered& L : low)
+    if (L.P.hashed) { total += agg_hashed_table_bytes(L.h_bound); n_hashed++; }
+  if (total <= QWGPU_HASHED_MAX_BYTES) return low;
+  std::vector<Lowered> keep;
+  std::vector<uint32_t> keep_idx;
+  for (size_t k = 0; k < low.size(); k++) {
+    if (!low[k].P.hashed) { keep.push_back(std::move(low[k])); keep_idx.push_back(idx[k]); continue; }
+    char msg[512];
+    snprintf(msg, sizeof msg, "split `%s`: the aggregation may create up to %llu buckets; the hashed tables of the call's %u "
+             "hashed splits need %llu bytes at their bounds, more than the GPU limit of %llu bytes per call",
+             sp[idx[k]]->id.c_str(), (unsigned long long)low[k].h_bound, n_hashed, (unsigned long long)total,
+             (unsigned long long)QWGPU_HASHED_MAX_BYTES);
+    outs[idx[k]].status = QWGPU_EUNSUPPORTED;
+    outs[idx[k]].error = msg;
   }
-  const uint32_t n = (uint32_t)low.size();
-  if (n == 0) {
-    // no searchable split on this rank: it still takes part in the collective with an empty record
-    if (merge && merged && gather && gather->allgather && gather->world > 1 && rank_headers && merge->k) {
-      const size_t rec = 64 + (size_t)merge->k * sizeof(qwk::DMergedHit), W8 = (size_t)gather->world;
-      uint8_t *d = nullptr;
-      const size_t o_recv = 256 * ((rec + 255) / 256), o_fin = o_recv + 256 * ((W8 * rec + 255) / 256), o_cut = o_fin + 256 * ((16 + rec + 255) / 256), o_hd = o_cut + 1024, total = o_hd + W8 * 64;
-      CUDA_CHECK(cudaMalloc(&d, total));
-      cudaStream_t st0 = nullptr;
-      CUDA_CHECK(cudaStreamCreateWithFlags(&st0, cudaStreamNonBlocking));
-      CUDA_CHECK(cudaMemsetAsync(d, 0, total, st0));
-      qwk::DRankHeader h;
-      memset(&h, 0, sizeof h);
-      h.attempted = gather->attempted; h.successful = gather->successful; h.n_failed = gather->n_failed;
-      CUDA_CHECK(cudaMemcpyAsync(d, &h, sizeof h, cudaMemcpyHostToDevice, st0));
-      if (gather->allgather(gather->comm, d, d + o_recv, rec, (void*)st0)) fail(QWGPU_EINTERNAL, "ncclAllGather failed");
-      const qwk::SrcGathered gsrc{d + o_recv, (uint32_t)rec, 64u};
-      qwk::k_merge_prep<qwk::SrcGathered><<<1, 1024, 0, st0>>>(gsrc, (uint32_t)gather->world, merge->k, merge->order1, merge->order2, (uint32_t*)(d + o_cut));
-      const uint64_t gthreads = (uint64_t)gather->world * merge->k * 32;
-      qwk::k_merge<qwk::SrcGathered><<<(uint32_t)((gthreads + 255) / 256), 256, 0, st0>>>(gsrc, (uint32_t*)(d + o_cut), (uint32_t)gather->world, merge->k, merge->k, merge->order1, merge->order2,
-                                                                                       (qwk::DMergedHit*)(d + o_fin + 16), (uint32_t*)(d + o_fin));
-      CUDA_CHECK(cudaMemcpy2DAsync(d + o_hd, 64, d + o_recv, rec, 64, W8, cudaMemcpyDeviceToDevice, st0));
-      std::vector<uint8_t> host(16 + (size_t)merge->k * sizeof(qwk::DMergedHit));
-      rank_headers->resize(gather->world);
-      CUDA_CHECK(cudaMemcpyAsync(host.data(), d + o_fin, host.size(), cudaMemcpyDeviceToHost, st0));
-      CUDA_CHECK(cudaMemcpyAsync(rank_headers->data(), d + o_hd, W8 * 64, cudaMemcpyDeviceToHost, st0));
-      CUDA_CHECK(cudaStreamSynchronize(st0));
-      const uint32_t nm = *(const uint32_t*)host.data();
-      const qwk::DMergedHit* mh = (const qwk::DMergedHit*)(host.data() + 16);
-      merged->resize(nm);
-      for (uint32_t j = 0; j < nm; j++) { (*merged)[j].hit = mh[j].hit; (*merged)[j].split = mh[j].split; (*merged)[j].pad = 0; }
-      cudaStreamDestroy(st0);
-      cudaFree(d);
-    }
-    return true;
-  }
-  const auto t_lowered = tclock::now();
+  idx.swap(keep_idx);
+  return keep;
+}
 
-  // ---- batch-wide parameters --------------------------------------------------------------------------
-  uint32_t n_levels = 1, need_cnt = 0, need_ssum = 0, need_msum = 0, max_instr = 0, max_cols = 0, max_aggs = 0, n_fn = 0;
-  bool scoring = false, any_topk = false, any_aggs = false, smem_aggs = true;
-  uint32_t max_cells = 0, max_key_bits = 0;
-  uint32_t tot_instr = 0, tot_cols = 0, tot_aggs = 0, tot_bounds = 0;
-  // second-chance top-K: when no plan ranks by _score first, the collect pass also records the exact
-  // level-0 histogram and every window's best digit, so that a failed sampled threshold is repaired
-  // by a candidates-only pass over the few windows that can hold candidates
-  bool rec_l0 = true, rangeq = false;
-  // every plan has the BM25 top-K shape => the BM25-union pipeline (k_union)
-  bool all_union = true, all_driver = true;
-  for (auto& L : low) {
-    if (!(L.P.fused_score_root && L.P.max_hits && !L.P.sa.present && !L.P.n_aggs && L.P.key.kind[0] == QW_SORT_SCORE &&
-          L.P.key.order[0] == QW_ORDER_DESC))
-      all_union = false;
-    if (L.P.n_terms > QU_MAX_TERMS || L.P.n_instr != L.P.n_terms + 2) all_union = false;  // [BOOL_BEGIN, TERM x n, BOOL_END]
-    {
-      // one driving posting list + required column filters, no aggregations: the posting-driven kernel
-      // (driver_kernel.cuh). [BOOL_BEGIN, TERM, (RANGE | EXISTS) x 0..4, BOOL_END] at level 0.
-      const std::vector<DInstr>& I = L.instrs;
-      bool d = L.P.n_aggs == 0 && I.size() >= 3 && I.size() <= 3 + QD_MAX_FILTERS && I[0].op == OP_BOOL_BEGIN && I[1].op == OP_TERM &&
-               I.back().op == OP_BOOL_END && I.back().level == 0;
-      if (d) {
-        const bool req = I[1].occur == QW_OCCUR_MUST || I[1].occur == QW_OCCUR_FILTER;
-        if (!req && !(I[1].occur == QW_OCCUR_SHOULD && I.size() == 3 && I.back().r == 1 && I.back().n == 0)) d = false;
-        for (size_t k = 2; k + 1 < I.size() && d; k++) {
-          const bool colpred = I[k].op == OP_RANGE || I[k].op == OP_EXISTS;
-          const bool unscored_req = I[k].occur == QW_OCCUR_FILTER || (I[k].occur == QW_OCCUR_MUST && !(I[k].flags & IF_SCORED));
-          if (!colpred || !unscored_req || I[k].level != 0) d = false;
-        }
-      }
-      if (!d) all_driver = false;
-    }
-    if (L.P.max_hits && L.P.key.kind[0] == QW_SORT_SCORE) rec_l0 = false;
-    max_key_bits = std::max(max_key_bits, L.P.key.total_bits);
-    for (const DInstr& in : L.instrs)
-      if ((in.op == OP_RANGE || in.op == OP_EXISTS) && (in.occur == QW_OCCUR_MUST || in.occur == QW_OCCUR_FILTER)) rangeq = true;
-    n_levels = std::max(n_levels, L.P.n_levels);
-    need_cnt |= L.need_cnt; need_ssum |= L.need_ssum; need_msum |= L.need_msum;
-    max_instr = std::max(max_instr, L.P.n_instr); max_cols = std::max(max_cols, L.P.n_cols); max_aggs = std::max(max_aggs, L.P.n_aggs);
-    n_fn = std::max(n_fn, L.P.n_fn_slots);
-    scoring |= L.P.scoring != 0; any_topk |= L.P.max_hits > 0; any_aggs |= L.P.n_aggs > 0;
-    max_cells = std::max(max_cells, L.P.n_cells);
-    L.P.instr_base = tot_instr; L.P.col_base = tot_cols; L.P.agg_base = tot_aggs;
-    L.bounds_base = tot_bounds;
-    tot_instr += L.P.n_instr; tot_cols += L.P.n_cols; tot_aggs += L.P.n_aggs; tot_bounds += (uint32_t)L.bounds.size();
-  }
-  rec_l0 = rec_l0 && any_topk;
-  // window size: as large as shared memory allows for the configured blocks/SM (per-window fixed
-  // costs — staging, program interpretation, barriers — amortise over more postings)
-  uint32_t W = 32768;
-  // BM25-union batches run the TMA + mbarrier pipeline (union_kernel.cuh): fixed 15360-doc windows,
-  // two blocks per SM
-  const bool use_driver = all_driver;
-  if (use_driver) rec_l0 = false;
-  const bool use_union = all_union && !use_driver;
-  const uint32_t u_budget = (uint32_t)(max_smem_optin + 1024) / QU_MINB - 1024 - 64;
-  // match_all + flat terms / histogram aggregations, no hits: the streaming column kernel (agg_kernel.cuh)
-  bool use_aggscan = true;
-  qwk::ASmem alay;
-  memset(&alay, 0, sizeof alay);
-  {
-    uint32_t maxbits[QW_MAX_DAGGS] = {0};
-    for (auto& L : low) {
-      if (!(L.P.n_instr == 3 && L.instrs[1].op == OP_ALL && L.P.max_hits == 0 && L.P.n_aggs > 0 && L.P.n_cells <= QA_MAX_CELLS)) { use_aggscan = false; break; }
-      for (uint32_t gi = 0; gi < L.P.n_aggs; gi++) {
-        const DAgg& d = L.aggs[gi];
-        const bool flat = d.parent == 0xFFFFFFFFu && d.num_children == 0 && (d.kind == QW_AGG_TERMS || d.kind == QW_AGG_HISTOGRAM) && !d.has_missing;
-        if (!flat || !L.P.fast_aggs || d.col == 0xFFFFFFFFu || L.cols[d.col].card != QW_CARD_FULL || L.cols[d.col].bits > 32) { use_aggscan = false; break; }
-        maxbits[gi] = std::max(maxbits[gi], L.cols[d.col].bits);
-      }
-      if (!use_aggscan) break;
-    }
-    if (use_aggscan) {
-      uint32_t off = 0;
-      auto take = [&](uint32_t bytes) { uint32_t o = off; off = (off + bytes + 15) & ~15u; return o; };
-      for (uint32_t gi = 0; gi < QW_MAX_DAGGS; gi++) alay.col_off[gi] = take(maxbits[gi] ? QA_CHUNK / 8 * maxbits[gi] + 16 : 0);
-      alay.hdr = take(16);
-      alay.slot_stride = off;
-      off = 0;
-      uint32_t a_cells = 1;
-      for (auto& L : low) a_cells = std::max(a_cells, L.P.n_cells);
-      alay.bars = take(8 * 2 * QA_SLOTS);
-      alay.atab = take(QW_MAX_DAGGS * sizeof(qwk::AggRow));
-      alay.bcache = take(QA_CW * QW_MAX_DAGGS * 16);
-      alay.cells = take(a_cells * 4);
-      alay.slot0 = take(QA_SLOTS * alay.slot_stride);
-      alay.total = off;
-      if ((int)alay.total + 1024 > max_smem_optin) use_aggscan = false;
-    }
-  }
-  if (use_aggscan) W = QA_CHUNK;  // the flat work list is the list of 8192-doc chunks
-  qwk::USmem ulay_c, ulay_h;
-  if (use_union) W = 15360u * 2 / QU_MINB;
-  SmemLayout lay;
-  for (;;) {
-    lay = make_layout(W, n_levels, need_cnt, need_msum, need_ssum, max_instr, max_cols, max_aggs, n_fn, rec_l0, rangeq);
-    if ((int)lay.total + 1024 <= max_smem_optin / (use_union ? 1 : QW_MIN_BLOCKS_PER_SM) || W == 1024) break;  // (union batches: k_window is only the rare exact-radix fallback)
-    W >>= 1;
-  }
-  (void)scoring;
-  if (use_aggscan && W != QA_CHUNK) use_aggscan = false;
-  if (use_union) {
-    // (the generic layout above stays valid for the same W: exact radix passes below level 0 use k_window)
-    ulay_c = make_union_layout(W, false, u_budget);
-    ulay_h = make_union_layout(W, true, u_budget);
-  }
-  if ((int)lay.total > max_smem_optin) fail(QWGPU_EUNSUPPORTED, "query needs %u bytes of shared memory per block", lay.total);
+static void strip_doc_key(QwHit& h) { h.flags &= ~1u; h.v1 = 0; }  // (the doc-id sort key's internal fields)
 
-  // ---- device blob: plans, programs, work maps ----------------------------------------------------------
-  std::vector<uint32_t> fw_all(n + 1), fw_smp(n + 1);
-  uint32_t max_windows = 0;
-  for (uint32_t i = 0; i < n; i++) {
-    low[i].P.num_windows = low[i].empty ? 0 : (low[i].P.num_docs + W - 1) / W;
-    max_windows = std::max(max_windows, low[i].P.num_windows);
+// one split's result out of its region of the copied-back buffer (and its hashed entries)
+static void unpack_split(SplitOutput& o, BatchStats& stats, const Lowered& L, const SplitDev& s, const uint8_t* plan, const uint8_t* ob,
+                         bool do_merge, const std::vector<DHKey>& keys, const std::vector<QwAggCell>& cells) {
+  const DSplitPlan& P = L.P;
+  o.num_hits = ((const uint64_t*)ob)[0];
+  uint32_t nh = *(const uint32_t*)(ob + 16);
+  if (!do_merge) {
+    o.hits.assign((const QwHit*)(ob + 32), (const QwHit*)(ob + 32) + nh);
+    if (P.key.kind[0] == QW_SORT_DOCID) for (auto& h : o.hits) strip_doc_key(h);
   }
-  // sampling stride of the threshold-estimation pass: 1/16 of the windows (a coarser sample shortens the histogram
-  // pass, but the looser threshold lets more candidates through the collect pass)
-  const uint32_t stride_cap = 16;
-  uint32_t stride = std::min(stride_cap, std::max(1u, max_windows / 8));
-  // BM25-union batches sample the threshold over the collect pass's window size rounded down to 1024 docs. Finer
-  // windows (the same fraction of the docs in more work items) were measured on the bench workload, one H100 80GB HBM3
-  // (400 W power limit): W gives 1.175-1.183 ms per 4-query step, W / 2 gives 1.194-1.203 ms and W / 4 gives
-  // 1.216-1.231 ms (the per-window clause chain does not shrink with the window).
-  const uint32_t W_h = use_union ? std::max(1024u, W & ~1023u) : W;
-  if (use_union) {
-    uint32_t mw = 0, tw = 0;
-    for (uint32_t i = 0; i < n; i++) {
-      const uint32_t nw = low[i].empty ? 0u : (low[i].P.num_docs + W_h - 1) / W_h;
-      mw = std::max(mw, nw);
-      tw += nw;
-    }
-    stride = std::min(stride_cap, std::max(1u, mw / 8));
-    // Large requests: at most ONE sampled window per resident block (the sampled pass is latency bound — a block
-    // that gets two windows doubles its duration), up to a stride of 32. Bench workload on one H100 80GB HBM3 (400 W
-    // power limit; 6528 windows, 132 SMs x 2 = 264 blocks): stride 25 instead of 16, 1.175-1.183 against 1.209-1.211 ms
-    // per 4-query step (a fixed stride of 32: 1.174-1.181 ms, no better).
-    const uint32_t per_block = (tw + (uint32_t)(sm_count * QU_MINB) - 1) / (uint32_t)(sm_count * QU_MINB);
-    stride = std::max(stride, std::min({per_block, 32u, std::max(1u, mw / 8)}));
-  }
-  // posting-driven kernel: the work list is the driving term's posting blocks; the threshold sample takes every
-  // stride-th BLOCK (128 postings, fine enough for keys that follow doc order: what lies between two sampled
-  // blocks is < 2K postings)
-  std::vector<uint32_t> fw_drv(n + 1, 0), fw_dsm(n + 1, 0);
-  if (use_driver) {
-    uint32_t max_blocks = 0;
-    for (uint32_t i = 0; i < n; i++) max_blocks = std::max(max_blocks, low[i].empty ? 0u : low[i].instrs[1].n);
-    stride = std::min(stride_cap, std::max(1u, max_blocks / 64));
-    for (uint32_t i = 0; i < n; i++) {
-      const uint32_t nb = low[i].empty ? 0u : low[i].instrs[1].n, phase = stride > 1 ? i % stride : 0;
-      fw_drv[i + 1] = fw_drv[i] + nb;
-      fw_dsm[i + 1] = fw_dsm[i] + (nb > phase ? (nb - phase + stride - 1) / stride : 0);
+  const QwAggCell* c = (const QwAggCell*)(ob + 32 + (do_merge ? 0 : (size_t)P.max_hits * sizeof(QwHit)));
+  o.cells.assign(c, c + P.n_cells);
+  for (auto& cell : o.cells) cell.min_mapped = ~cell.min_mapped;  // device keeps max(~m); see agg_stats
+  if (P.hashed) {
+    o.hashed = true;
+    o.entries.resize(keys.size());
+    for (size_t e = 0; e < o.entries.size(); e++) {
+      QwAggEntry& x = o.entries[e];
+      x.node = keys[e].node_flags & 0xFFu;
+      x.flags = keys[e].node_flags >> 8;
+      x.parent = keys[e].parent;
+      x.key = keys[e].key;
+      x.reserved = 0;
+      x.cell = cells[e];
+      x.cell.min_mapped = ~x.cell.min_mapped;
     }
   }
-  // the generic kernels sample an explicit window list: strided windows + the first and last window of each
-  // split (weight 1 in the histogram); the union pipeline keeps the plain strided sample (scores do not
-  // follow doc order)
-  const bool edge_sample = !use_union && !use_driver && stride > 1;
-  std::vector<uint32_t> sample_win;
-  fw_all[0] = fw_smp[0] = 0;
-  for (uint32_t i = 0; i < n; i++) {
-    uint32_t nw = low[i].P.num_windows, phase = stride > 1 ? i % stride : 0;
-    fw_all[i + 1] = fw_all[i] + nw;
-    if (use_union) nw = low[i].empty ? 0 : (low[i].P.num_docs + W_h - 1) / W_h;  // (the sampled pass has its own window size)
-    if (edge_sample) {
-      uint32_t cnt = 0;
-      for (uint32_t w = 0; w < nw; w++) {
-        const bool edge = w == 0 || w + 1 == nw, strided = w % stride == phase;
-        if (edge || strided) { sample_win.push_back(w | (edge ? 0x80000000u : 0u)); cnt++; }
+  if (P.tr_on) {
+    if (*(const uint32_t*)(ob + 24)) stats.kernel_mask |= QWGPU_KERNEL_TRACE_REPLAY;
+    // a matched doc without a trace id reads ordinal 0: with an empty dictionary the reference's ord_to_bytes fails
+    const QwImgColumn& tc = s.view.columns[L.tr_img_col];
+    for (const QwAggCell& cell : o.cells)
+      if (cell.count == 1 && cell.sum_bits >= tc.dict_num_terms) {
+        o.status = QWGPU_EINTERNAL;
+        o.error = "failed to look up a trace id in the column term dictionary";
+        o.cells.clear();
+        break;
       }
-      fw_smp[i + 1] = fw_smp[i] + cnt;
-    } else fw_smp[i + 1] = fw_smp[i] + (nw > phase ? (nw - phase + stride - 1) / stride : 0);
   }
-  // phrases: one uncompressed posting block per block of each phrase's driver term (phrase_kernel.cuh)
-  uint32_t n_phrases = 0, phrase_blocks = 0;
-  size_t n_phrase_exp = 0;  // expansions of the batch's phrase prefixes
-  for (auto& L : low) {
-    for (size_t k = 0; k < L.phrases.size(); k++) { n_phrases++; phrase_blocks += L.instrs[L.phrase_instr[k]].n; }
-    n_phrase_exp += L.phrase_exp.size();
-  }
-  auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
-  size_t o_plans = 0, o_instr = al(o_plans + n * sizeof(DSplitPlan)), o_cols = al(o_instr + tot_instr * sizeof(DInstr)),
-         o_aggs = al(o_cols + std::max(tot_cols, 1u) * sizeof(DCol)), o_fwa = al(o_aggs + std::max(tot_aggs, 1u) * sizeof(DAgg)),
-         o_fws = al(o_fwa + (n + 1) * 4), o_bounds = al(o_fws + (n + 1) * 4), o_rank = al(o_bounds + (size_t)tot_bounds * 8),
-         o_smp = al(o_rank + (size_t)n * 4), o_phr = al(o_smp + sample_win.size() * 4), o_pexp = al(o_phr + (size_t)n_phrases * sizeof(DPhrase)),
-         o_fwd = al(o_pexp + n_phrase_exp * sizeof(DPhraseTerm)),
-         o_fwds = al(o_fwd + (use_driver ? (size_t)(n + 1) * 4 : 0)), blob_bytes = al(o_fwds + (use_driver ? (size_t)(n + 1) * 4 : 0));
-  // device-side cross-split merge: the per-split hit lists stay in scratch, only the merged top-K comes back
-  const bool do_merge = merge && merged && merge->k > 0 && any_topk && merge->rank.size() == n_in;
-  uint32_t kmax = 1;
-  for (auto& L : low) kmax = std::max(kmax, L.P.max_hits);
-  // scratch: thresholds, histograms, candidates
-  size_t s_thr = 0, s_hist = al(s_thr + n * sizeof(DThresh)), s_state = al(s_hist + (size_t)n * QW_HIST_BINS * 4),
-         s_wmax = al(s_state + (size_t)n * 4), s_cand = al(s_wmax + (rec_l0 ? (size_t)fw_all[n] * 2 : 0)),
-         s_hits = al(s_cand + (any_topk ? (size_t)n * QW_CAND_CAP * 24 : 0)),
-         s_cut = al(s_hits + (do_merge ? (size_t)n * kmax * sizeof(QwHit) : 0)),
-         s_grecv = al(s_cut + (size_t)std::max<uint32_t>(n, 64) * 4 + 1024),
-         s_vblk = al(s_grecv + (gather && gather->world > 1 && do_merge ? (size_t)gather->world * (64 + (size_t)merge->k * sizeof(qwk::DMergedHit)) : 0)),
-         s_trace = al(s_vblk + (size_t)phrase_blocks * sizeof(VBlk));
-  // find_trace_ids: per split a DTraceState (one region, set to 0xFF bytes), then best[] + match bitmap (zeroed)
-  std::vector<size_t> tr_off(n + 1, 0);
-  bool any_trace = false;
-  for (uint32_t i = 0; i < n; i++) {
-    const DSplitPlan& P = low[i].P;
-    tr_off[i + 1] = tr_off[i] + (P.tr_on ? al((size_t)P.tr_num_ords * 8) + al((size_t)((P.num_docs + 31) / 32) * 4) : 0);
-    any_trace |= P.tr_on != 0;
-  }
-  const size_t s_trace_state = s_trace, s_trace_data = al(s_trace + (any_trace ? (size_t)n * sizeof(qwk::DTraceState) : 0));
-  // hashed aggregation cells: per split [slot table][key records][cells], at min(bound, QWGPU_HASHED_INIT_CELLS)
-  // cells, or at the bound when the batch runs again after an overflow
-  const size_t s_hash = al(s_trace_data + tr_off[n]);
-  std::vector<size_t> h_off(n + 1, 0);
-  bool any_hashed = false, any_composite = false;
-  for (uint32_t i = 0; i < n; i++) {
-    DSplitPlan& P = low[i].P;
-    if (P.hashed) {
-      any_hashed = true;
-      for (const DAgg& d : low[i].aggs) if (d.comp & QW_AGG_COMP_LEVEL) any_composite = true;
-      P.h_cap = (uint32_t)(at_bound ? low[i].h_bound : std::min<uint64_t>(low[i].h_bound, QWGPU_HASHED_INIT_CELLS));
-      P.h_mask = agg_hashed_slots(P.h_cap) - 1;
-    }
-    h_off[i + 1] = h_off[i] + (P.hashed ? al((size_t)(P.h_mask + 1) * 4) + al((size_t)P.h_cap * sizeof(DHKey)) + al((size_t)P.h_cap * sizeof(QwAggCell)) : 0);
-  }
-  const size_t scratch_bytes = al(s_hash + h_off[n]);
-  // out: per split [hdr 32B][hits][cells]
-  std::vector<size_t> out_off(n + 1);
-  out_off[0] = 0;
-  for (uint32_t i = 0; i < n; i++)
-    out_off[i + 1] = al(out_off[i] + 32 + (do_merge ? 0 : (size_t)low[i].P.max_hits * sizeof(QwHit)) + (size_t)low[i].P.n_cells * sizeof(QwAggCell));
-  // [RankHeader 64 B (n_hits first)][DMergedHit x k]: the batch's merged top-k = this rank's gather record
-  const size_t o_merged = out_off[n];
-  const size_t rec_bytes = do_merge ? 64 + (size_t)merge->k * sizeof(qwk::DMergedHit) : 0;
-  const bool do_gather = do_merge && gather && gather->allgather && gather->world > 1 && rank_headers;
-  // gathered: [world x RankHeader (compacted copy)][final count 16 B][final DMergedHit x k]
-  const size_t o_ghdr = al(o_merged + rec_bytes), o_final = al(o_ghdr + (do_gather ? (size_t)gather->world * 64 : 0));
-  size_t out_bytes = do_merge ? (do_gather ? al(o_final + 16 + (size_t)merge->k * sizeof(qwk::DMergedHit)) : al(o_merged + rec_bytes)) : out_off[n];
-
-  // Admission: at most QWGPU_MAX_IN_FLIGHT (default 16) searches drive the device at once; further callers wait here
-  // on a condition variable (no CUDA calls, no spinning). Measured on the mixed config-5 query set from 64 host threads,
-  // one H100 80GB HBM3 (400 W power limit): with the limit at 16, 1643 queries/s (p99 66-72 ms) in both of two runs;
-  // with it at 64, 894 and 1517 queries/s (p99 341 and 174 ms) — the driver's per-context lock and 64 interleaved
-  // streams cost more than the extra overlap brings.
-  static const int max_in_flight = getenv("QWGPU_MAX_IN_FLIGHT") ? std::max(1, atoi(getenv("QWGPU_MAX_IN_FLIGHT"))) : 16;
-  CallSlot* slot = nullptr;
-  {
-    std::unique_lock<std::mutex> g(mu);
-    cv_admit.wait(g, [&] { return admitted < max_in_flight; });
-    admitted++;
-    if (!free_slots.empty()) { slot = free_slots.back(); free_slots.pop_back(); }
-  }
-  struct Admit {  // (released on every path, including a throw before the slot guard below exists)
-    Engine* e;
-    ~Admit() {
-      { std::lock_guard<std::mutex> g(e->mu); e->admitted--; }
-      e->cv_admit.notify_one();
-    }
-  } admit{this};
-  if (!slot) {
-    slot = new CallSlot();
-    CUDA_CHECK(cudaStreamCreateWithFlags(&slot->stream, cudaStreamNonBlocking));
-    CUDA_CHECK(cudaEventCreate(&slot->ev0));
-    CUDA_CHECK(cudaEventCreate(&slot->ev1));
-    CUDA_CHECK(cudaEventCreate(&slot->ev2));
-    CUDA_CHECK(cudaEventCreate(&slot->ev3));
-    CUDA_CHECK(cudaEventCreateWithFlags(&slot->ev_block, cudaEventBlockingSync | cudaEventDisableTiming));
-  }
-  // the slot goes back to the pool only once its stream is idle: on an error path copies / kernels of this
-  // call may still be in flight, and the next call would reuse the pinned buffers under them
-  struct Release {
-    Engine* e; CallSlot* s;
-    ~Release() {
-      cudaStreamSynchronize(s->stream);
-      e->in_flight.fetch_sub(1);
-      std::lock_guard<std::mutex> g(e->mu);
-      e->free_slots.push_back(s);
-    }
-  } rel{this, slot};
-  in_flight.fetch_add(1);
-  // Waiting for the call's stream: cudaStreamSynchronize spins on a CPU core, which is the fastest wake-up while a
-  // few calls are in flight (single-query latency) and a disaster when more host threads wait than there are cores
-  // to spare — the spinners starve the threads that still have plans to compile. Beyond a quarter of the cores the
-  // wait goes through a blocking event instead (the thread sleeps until the driver's interrupt).
-  static const uint32_t spin_limit = getenv("QWGPU_SPIN_LIMIT") ? (uint32_t)atoi(getenv("QWGPU_SPIN_LIMIT")) : std::max(2u, std::thread::hardware_concurrency() / 4);
-  auto wait_stream = [&]() {
-    if (in_flight.load(std::memory_order_relaxed) > (int)spin_limit) {
-      CUDA_CHECK(cudaEventRecord(slot->ev_block, slot->stream));
-      CUDA_CHECK(cudaEventSynchronize(slot->ev_block));
-    } else CUDA_CHECK(cudaStreamSynchronize(slot->stream));
+  o.postings_scored = L.postings;
+  // SURVEY.md §8d algorithmic bytes: postings (+ fieldnorms, added at lowering) + column probes
+  uint64_t bytes = L.alg_bytes;
+  auto col_bytes = [&](uint32_t c, uint64_t probes) {
+    const QwImgColumn& ic = s.view.columns[c];
+    uint64_t full = ((uint64_t)ic.num_vals * ic.bits + 7) / 8;
+    return std::min<uint64_t>(probes * ((ic.bits + 7) / 8), full);
   };
-  size_t want_blob, want_scratch, want_out;
-  {
-    // slots are sized to the largest request the context has seen: a slot that meets a bigger request later would
-    // have to cudaFree / cudaMalloc (device-synchronising) in the middle of concurrent searches
-    std::lock_guard<std::mutex> g(mu);
-    hw_blob = std::max(hw_blob, blob_bytes); hw_scratch = std::max(hw_scratch, scratch_bytes); hw_out = std::max(hw_out, out_bytes);
-    // (only while the marks stay moderate: one huge aggregation request must not size every slot after itself)
-    auto sized = [](size_t hw, size_t need) { return hw <= ((size_t)64 << 20) ? hw : need; };
-    want_blob = sized(hw_blob, blob_bytes); want_scratch = sized(hw_scratch, scratch_bytes); want_out = sized(hw_out, out_bytes);
-  }
-  slot->ensure(want_blob, want_scratch, want_out);
-  cudaStream_t st = slot->stream;
+  uint64_t driver = L.min_required_df == ~0ull ? P.num_docs : L.min_required_df;
+  for (auto& rc : L.range_cols) bytes += col_bytes(rc.first, driver);
+  const QwPlanHeader* ph = (const QwPlanHeader*)plan;
+  for (int k = 0; k < 2; k++)
+    if (ph->sort[k].kind == QW_SORT_COLUMN && ph->sort[k].column != 0xFFFFFFFFu && P.max_hits) bytes += col_bytes(ph->sort[k].column, o.num_hits);
+  const QwAggNode* an = (const QwAggNode*)(plan + sizeof(QwPlanHeader) + (size_t)ph->num_nodes * sizeof(QwPlanNode));
+  for (uint32_t a = 0; a < ph->num_aggs; a++) if (an[a].column != 0xFFFFFFFFu) bytes += col_bytes(an[a].column, o.num_hits);
+  o.algorithmic_bytes = bytes;
+}
 
-  uint32_t phr_done = 0, phr_blocks_done = 0;
-  size_t pexp_done = 0;
-  bool any_fast_aggs = false;
-  for (uint32_t i = 0; i < n; i++) {
-    DSplitPlan& P = low[i].P;
-    // privatised counters + stats triples must fit the (dead at collect time) staging area
-    if (P.fast_aggs && (((size_t)P.n_cells * 4 + 7) & ~(size_t)7) + (size_t)P.n_stat_cells * 24 > stage_bytes_for(W)) P.fast_aggs = 0;
-    any_fast_aggs |= P.fast_aggs != 0;
-    uint8_t* ob = slot->d_out + out_off[i];
-    P.out_num_hits = (uint64_t)ob;            // [0] hits, [1] eligible
-    P.out_nhits = (uint64_t)(ob + 16);
-    P.out_cand_count = (uint64_t)(ob + 20);
-    P.out_hits = do_merge ? (uint64_t)(slot->d_scratch + s_hits + (size_t)i * kmax * sizeof(QwHit)) : (uint64_t)(ob + 32);
-    P.out_cells = (uint64_t)(ob + 32 + (do_merge ? 0 : (size_t)P.max_hits * sizeof(QwHit)));
-    P.out_hist = (uint64_t)(slot->d_scratch + s_hist + (size_t)i * QW_HIST_BINS * 4);
-    P.out_cands = (uint64_t)(slot->d_scratch + s_cand + (size_t)i * QW_CAND_CAP * 24);
-    if (P.tr_on) {
-      P.tr_state = (uint64_t)(slot->d_scratch + s_trace_state + (size_t)i * sizeof(qwk::DTraceState));
-      P.tr_best = (uint64_t)(slot->d_scratch + s_trace_data + tr_off[i]);
-      P.tr_match = P.tr_best + al((size_t)P.tr_num_ords * 8);
-      P.tr_tie = (uint64_t)(ob + 24);
-    }
-    if (P.hashed) {
-      P.h_table = (uint64_t)(slot->d_scratch + s_hash + h_off[i]);
-      P.h_keys = P.h_table + al((size_t)(P.h_mask + 1) * 4);
-      P.h_cells = P.h_keys + al((size_t)P.h_cap * sizeof(DHKey));
-      P.h_ctr = (uint64_t)(ob + 28);
-    }
-    for (size_t k = 0; k < low[i].phrases.size(); k++) {
-      DPhrase& ph = low[i].phrases[k];
-      DInstr& pin = low[i].instrs[low[i].phrase_instr[k]];
-      ph.first_work = phr_blocks_done;
-      ph.out = (uint64_t)(slot->d_scratch + s_vblk + (size_t)phr_blocks_done * sizeof(VBlk));
-      DPhrase staged = ph;  // (ph.exp stays an index into phrase_exp)
-      if (ph.n_exp) {
-        memcpy(slot->h_blob + o_pexp + pexp_done * sizeof(DPhraseTerm), low[i].phrase_exp.data() + ph.exp, (size_t)ph.n_exp * sizeof(DPhraseTerm));
-        staged.exp = (uint64_t)(slot->d_blob + o_pexp + pexp_done * sizeof(DPhraseTerm));
-        pexp_done += ph.n_exp;
-      }
-      pin.a = ph.out;
-      phr_blocks_done += pin.n;
-      memcpy(slot->h_blob + o_phr + (size_t)phr_done++ * sizeof(DPhrase), &staged, sizeof staged);
-    }
-    memcpy(slot->h_blob + o_plans + i * sizeof(DSplitPlan), &P, sizeof P);
-    memcpy(slot->h_blob + o_instr + P.instr_base * sizeof(DInstr), low[i].instrs.data(), P.n_instr * sizeof(DInstr));
-    if (P.n_cols) memcpy(slot->h_blob + o_cols + P.col_base * sizeof(DCol), low[i].cols.data(), P.n_cols * sizeof(DCol));
-    if (P.fast_aggs)
-      for (DAgg& d : low[i].aggs)
-        if (d.kind == QW_AGG_HISTOGRAM) d.bounds = (uint64_t)(slot->d_blob + o_bounds) + (low[i].bounds_base + d.bounds) * 8;
-    if (P.n_aggs) memcpy(slot->h_blob + o_aggs + P.agg_base * sizeof(DAgg), low[i].aggs.data(), P.n_aggs * sizeof(DAgg));
-    if (!low[i].bounds.empty()) memcpy(slot->h_blob + o_bounds + (size_t)low[i].bounds_base * 8, low[i].bounds.data(), low[i].bounds.size() * 8);
+// The device merge's hits (count at `cnt`, DMergedHit records at `recs`). A batch's own merge names positions in
+// `low`, which `idx` maps back to the caller's arrays; a cross-rank merge (idx null) carries GLOBAL split ranks (the
+// caller owns the rank -> split id table), and a rank with no searchable split does not know the sort.
+static void unpack_merged(const uint8_t* cnt, const uint8_t* recs, const std::vector<Lowered>& low, const std::vector<uint32_t>* idx,
+                          std::vector<MergedHit>& merged) {
+  const uint32_t nm = *(const uint32_t*)cnt;
+  const qwk::DMergedHit* mh = (const qwk::DMergedHit*)recs;
+  merged.resize(nm);
+  for (uint32_t j = 0; j < nm; j++) {
+    const Lowered* L = idx ? &low[mh[j].split] : low.empty() ? nullptr : &low[0];
+    MergedHit& m = merged[j];
+    m.hit = mh[j].hit; m.split = idx ? (*idx)[mh[j].split] : mh[j].split; m.pad = 0;
+    if (L && L->P.key.kind[0] == QW_SORT_DOCID) strip_doc_key(m.hit);
   }
-  if (do_merge) for (uint32_t i = 0; i < n; i++) ((uint32_t*)(slot->h_blob + o_rank))[i] = merge->rank[idx[i]];
-  if (!sample_win.empty()) memcpy(slot->h_blob + o_smp, sample_win.data(), sample_win.size() * 4);
-  if (use_driver) { memcpy(slot->h_blob + o_fwd, fw_drv.data(), (n + 1) * 4); memcpy(slot->h_blob + o_fwds, fw_dsm.data(), (n + 1) * 4); }
-  memcpy(slot->h_blob + o_fwa, fw_all.data(), (n + 1) * 4);
-  memcpy(slot->h_blob + o_fws, fw_smp.data(), (n + 1) * 4);
-  CUDA_CHECK(cudaMemcpyAsync(slot->d_blob, slot->h_blob, blob_bytes, cudaMemcpyHostToDevice, st));
-  stats.h2d_bytes += blob_bytes;
+}
 
-  KParams kp;
-  memset(&kp, 0, sizeof kp);
-  kp.plans = (const DSplitPlan*)(slot->d_blob + o_plans);
-  kp.instrs = (const DInstr*)(slot->d_blob + o_instr);
-  kp.cols = (const DCol*)(slot->d_blob + o_cols);
-  kp.aggs = (const DAgg*)(slot->d_blob + o_aggs);
-  kp.thresh = (DThresh*)(slot->d_scratch + s_thr);
-  kp.n_splits = n;
-  kp.W = W;
-  kp.stage_bytes = stage_bytes_for(W);
-  // privatised aggregation counters (and the radix histogram, 8 KB) live in the staging area
-  if (max_cells * 4 > kp.stage_bytes || max_cells > QW_SMEM_AGG_CELLS) smem_aggs = false;
-  kp.smem_aggs = (any_aggs && smem_aggs) ? 1 : 0;
-  kp.sm = lay;
-  kp.wmax = (uint16_t*)(slot->d_scratch + s_wmax);
-  kp.split_state = (const uint32_t*)(slot->d_scratch + s_state);
-  int occ = 1;
-  CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, qwk::k_window<qwk::MODE_COLLECT>, QW_THREADS, lay.total));
-  occ = std::max(occ, 1);
-  enum { F_REC = 1, F_REFINE = 2, F_CANDS_ONLY = 4 };
-  auto launch_window = [&](int mode, bool sampled, uint32_t level, uint32_t use_prefix, uint32_t flags) {
-    KParams q = kp;
-    q.first_work = (const uint32_t*)(slot->d_blob + (sampled ? o_fws : o_fwa));
-    q.total_work = sampled ? fw_smp[n] : fw_all[n];
-    q.stride = sampled ? stride : 1;
-    q.sample_win = (sampled && edge_sample) ? (const uint32_t*)(slot->d_blob + o_smp) : nullptr;
-    q.level = level;
-    q.use_prefix = use_prefix;
-    q.rec_l0 = (flags & F_REC) ? 1 : 0;
-    q.refine = (flags & F_REFINE) ? 1 : 0;
-    q.cands_only = (flags & F_CANDS_ONLY) ? 1 : 0;
-    if (use_driver && flags == 0) {
-      qwk::DrvParams d;
-      memset(&d, 0, sizeof d);
-      d.plans = kp.plans; d.instrs = kp.instrs; d.cols = kp.cols; d.thresh = kp.thresh;
-      d.first_work = (const uint32_t*)(slot->d_blob + (sampled ? o_fwds : o_fwd)); d.n_splits = n; d.total_work = sampled ? fw_dsm[n] : fw_drv[n];
-      d.level = level; d.use_prefix = use_prefix; d.stride = sampled ? stride : 1;
-      if (d.total_work == 0) return;
-      const uint32_t dgrid = std::min<uint32_t>((d.total_work + QD_WARPS - 1) / QD_WARPS, (uint32_t)(sm_count * 4));
-      if (mode == qwk::MODE_HIST) qwk::k_driver<qwk::MODE_HIST><<<dgrid, QD_WARPS * 32, 0, st>>>(d);
-      else qwk::k_driver<qwk::MODE_COLLECT><<<dgrid, QD_WARPS * 32, 0, st>>>(d);
-      stats.launches++;
-      stats.kernel_mask |= QWGPU_KERNEL_DRIVER;
-      return;
-    }
-    if (q.total_work == 0) return;
-    if (use_aggscan && mode == qwk::MODE_COLLECT && flags == 0) {
-      qwk::AParams a;
-      memset(&a, 0, sizeof a);
-      a.plans = kp.plans; a.cols = kp.cols; a.aggs = kp.aggs;
-      a.first_work = q.first_work; a.n_splits = n; a.total_work = q.total_work;
-      a.sm = alay;
-      int aocc = 1;
-      CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&aocc, qwk::k_aggscan, QA_THREADS, alay.total));
-      const uint32_t agrid = std::min<uint32_t>(q.total_work, (uint32_t)(sm_count * std::max(aocc, 1)));
-      qwk::k_aggscan<<<agrid, QA_THREADS, alay.total, st>>>(a);
-      stats.launches++;
-      stats.kernel_mask |= QWGPU_KERNEL_AGGSCAN;
-      return;
-    }
-    if (use_union && flags == 0 && (mode == qwk::MODE_COLLECT || (level == 0 && !use_prefix))) {
-      qwk::UParams u;
-      memset(&u, 0, sizeof u);
-      u.plans = kp.plans; u.instrs = kp.instrs; u.cols = kp.cols; u.thresh = kp.thresh;
-      u.first_work = q.first_work; u.n_splits = n; u.total_work = q.total_work; u.stride = q.stride; u.W = sampled ? W_h : W;
-      u.sm = mode == qwk::MODE_HIST ? ulay_h : ulay_c;
-      // cross-rank calls leave a few block slots free: the persistent grid would otherwise hold every SM's shared
-      // memory, a concurrent call's NCCL kernel would take the place of one of its blocks, and that block — with its
-      // static share of the windows — would only start when another one has finished (twice the kernel time)
-      const uint32_t ugrid = std::min<uint32_t>(q.total_work, (uint32_t)(sm_count * QU_MINB) - (do_gather ? 4u : 0u));
-      if (mode == qwk::MODE_HIST) qwk::k_union<qwk::MODE_HIST><<<ugrid, QU_THREADS, u.sm.total, st>>>(u);
-      else qwk::k_union<qwk::MODE_COLLECT><<<ugrid, QU_THREADS, u.sm.total, st>>>(u);
-      stats.launches++;
-      stats.kernel_mask |= QWGPU_KERNEL_UNION;
-      return;
-    }
-    uint32_t grid = std::min<uint32_t>(q.total_work, (uint32_t)(sm_count * occ));
-    if (mode == qwk::MODE_HIST) qwk::k_window<qwk::MODE_HIST><<<grid, QW_THREADS, lay.total, st>>>(q);
-    else if (any_hashed) qwk::k_window<qwk::MODE_COLLECT, true><<<grid, QW_THREADS, lay.total, st>>>(q);
-    else qwk::k_window<qwk::MODE_COLLECT><<<grid, QW_THREADS, lay.total, st>>>(q);
-    stats.launches++;
-    stats.kernel_mask |= QWGPU_KERNEL_WINDOW;
-    // (k_window aggregates on the fast path where the plan's and the launch's flags both allow it)
-    if (mode == qwk::MODE_COLLECT && !(flags & F_CANDS_ONLY) && any_fast_aggs && kp.smem_aggs) stats.kernel_mask |= QWGPU_KERNEL_FAST_AGGS;
-    if (mode == qwk::MODE_COLLECT && !(flags & F_CANDS_ONLY) && any_hashed) stats.kernel_mask |= QWGPU_KERNEL_HASHED_AGGS;
-  };
-  const uint32_t sel_smem = 3 * 8 * QW_CAND_CAP;  // [all first words | 3 x QW_SEL_MAX survivors] or 3 x all (degenerate ties)
-  uint32_t tie_max_n = 0;
-  for (auto& L : low) if (L.P.tr_on) tie_max_n = std::max(tie_max_n, L.P.tr_n);
-  auto run_collect = [&](uint32_t flags) {
-    if (!(flags & F_CANDS_ONLY)) CUDA_CHECK(cudaMemsetAsync(slot->d_out, 0, out_bytes, st));
-    if (any_trace && !(flags & F_CANDS_ONLY)) {
-      CUDA_CHECK(cudaMemsetAsync(slot->d_scratch + s_trace_state, 0xFF, (size_t)n * sizeof(qwk::DTraceState), st));
-      CUDA_CHECK(cudaMemsetAsync(slot->d_scratch + s_trace_data, 0, tr_off[n], st));
-    }
-    if (any_hashed && !(flags & F_CANDS_ONLY))
-      for (uint32_t i = 0; i < n; i++) {
-        const DSplitPlan& P = low[i].P;
-        if (!P.hashed) continue;
-        CUDA_CHECK(cudaMemsetAsync((void*)P.h_table, 0xFF, (size_t)(P.h_mask + 1) * 4, st));
-        CUDA_CHECK(cudaMemsetAsync((void*)P.h_cells, 0, (size_t)P.h_cap * sizeof(QwAggCell), st));
-      }
-    CUDA_CHECK(cudaEventRecord(slot->ev2, st));
-    launch_window(qwk::MODE_COLLECT, false, 0, 0, flags);
-    CUDA_CHECK(cudaEventRecord(slot->ev3, st));
-    if (any_composite && !(flags & F_CANDS_ONLY)) {
-      // each composite's first `size` leaves with their chains and sub-aggregation entries, before the copy-back
-      qwk::k_composite_cut<<<n, QC_THREADS, 0, st>>>(kp.plans, kp.aggs);
-      stats.launches++;
-      stats.kernel_mask |= QWGPU_KERNEL_COMPOSITE_CUT;
-    }
-    if (any_trace && !(flags & F_CANDS_ONLY)) {
-      // top N of the per-trace maxima; splits whose N-th and (N+1)-th maxima tie replay the reference's selection
-      qwk::k_trace_select<<<n, 1024, 0, st>>>(kp.plans);
-      qwk::k_trace_replay<<<n, QT_TILE, trace_replay_smem(tie_max_n), st>>>(kp.plans, kp.cols);
-      stats.launches += 2;
-      stats.kernel_mask |= QWGPU_KERNEL_TRACE_SELECT;
-    }
-    if (any_topk) { qwk::k_select<<<n, 1024, sel_smem, st>>>(kp.plans, kp.cols); stats.launches++; }
-    if (do_merge) {
-      uint32_t* d_cut = (uint32_t*)(slot->d_scratch + s_cut);
-      const qwk::SrcSplits src{kp.plans, (const uint32_t*)(slot->d_blob + o_rank), do_gather ? 1u : 0u};
-      qwk::k_merge_prep<qwk::SrcSplits><<<1, 1024, 0, st>>>(src, n, merge->k, merge->order1, merge->order2, d_cut);
-      const uint64_t threads = (uint64_t)n * kmax * 32;  // one warp per hit (warps of pruned hits leave at once)
-      qwk::k_merge<qwk::SrcSplits><<<(uint32_t)((threads + 255) / 256), 256, 0, st>>>(src, d_cut, n, kmax, merge->k, merge->order1, merge->order2,
-                                                          (qwk::DMergedHit*)(slot->d_out + o_merged + 64), (uint32_t*)(slot->d_out + o_merged));
-      stats.launches += 2;
-    }
-    const size_t back = do_gather ? o_ghdr : out_bytes;  // (gathering: the final hits follow in the cross-rank phase)
-    CUDA_CHECK(cudaMemcpyAsync(slot->h_out, slot->d_out, back, cudaMemcpyDeviceToHost, st));
-    stats.d2h_bytes += back;
-  };
-  // a split's candidate set is good when it holds at least min(K, eligible) and did not overflow
-  std::vector<uint32_t> state(n, 0);
-  auto verify = [&]() -> bool {
-    bool all = true;
-    for (uint32_t i = 0; i < n; i++) {
-      state[i] = 0;
-      if (low[i].P.max_hits == 0) continue;
-      const uint8_t* ob = slot->h_out + out_off[i];
-      uint64_t eligible = ((const uint64_t*)ob)[1];
-      uint32_t cand = *(const uint32_t*)(ob + 20);
-      if (cand > QW_CAND_CAP || cand < std::min<uint64_t>(low[i].P.max_hits, eligible)) { state[i] = 1; all = false; }
-    }
-    return all;
-  };
-
-  const auto t_staged = tclock::now();
-  CUDA_CHECK(cudaEventRecord(slot->ev0, st));
-  CUDA_CHECK(cudaMemsetAsync(slot->d_scratch, 0, s_cand, st));  // thresholds, histograms, refinement state
-  if (phrase_blocks) {
-    // phrase pre-pass (inside the timed device region): every phrase of the batch becomes a posting list in
-    // scratch (beyond s_cand: never cleared), read by every later pass
-    uint32_t max_terms = 1;
-    for (auto& L : low) for (auto& ph : L.phrases) max_terms = std::max(max_terms, ph.n_terms);
-    const size_t psm = (size_t)QP_WARPS * QP_SMEM_WORDS(max_terms) * 4;
-    const uint32_t pgrid = (phrase_blocks + QP_WARPS - 1) / QP_WARPS;
-    const DPhrase* d_phr = (const DPhrase*)(slot->d_blob + o_phr);
-    // the suffix stage of phrase prefixes lives in its own instantiation: plain phrases keep the lean kernel
-    if (n_phrase_exp) qwk::k_phrase<true><<<pgrid, QP_WARPS * 32, psm, st>>>(d_phr, n_phrases, phrase_blocks, max_terms);
-    else qwk::k_phrase<false><<<pgrid, QP_WARPS * 32, psm, st>>>(d_phr, n_phrases, phrase_blocks, max_terms);
-    stats.launches++;
-    stats.kernel_mask |= QWGPU_KERNEL_PHRASE;
-  }
-  stats.window_docs = use_driver ? QW_BLOCK_LEN : W;
-  bool ok = true;
-  float main_ms = 0;
-  auto add_main = [&]() { float ms = 0; cudaEventElapsedTime(&ms, slot->ev2, slot->ev3); main_ms += ms; };
-  if (any_topk && stride > 1) {
-    // fast path: threshold from a 1/stride sample of the windows, verified after the collect pass
-    stats.sample_stride = stride;
-    launch_window(qwk::MODE_HIST, true, 0, 0, 0);
-    qwk::k_pick<<<n, 256, 0, st>>>(kp.plans, kp.thresh, 0, edge_sample ? 2 : 1, stride, nullptr);
-    stats.launches++;
-    if (rec_l0) CUDA_CHECK(cudaMemsetAsync(slot->d_scratch + s_hist, 0, (size_t)n * QW_HIST_BINS * 4, st));
-    run_collect(rec_l0 ? F_REC : 0);
-    CUDA_CHECK(cudaEventRecord(slot->ev1, st));
-    wait_stream();
-    ok = verify();
-    if (!ok) {
-      float ms = 0;
-      cudaEventElapsedTime(&ms, slot->ev0, slot->ev1);
-      stats.gpu_time_us += ms * 1000.f;
-      add_main();
-      stats.exact_fallbacks++;
-      CUDA_CHECK(cudaEventRecord(slot->ev0, st));
-    }
-  }
-  if (!any_topk) {
-    run_collect(0);
-    CUDA_CHECK(cudaEventRecord(slot->ev1, st));
-    wait_stream();
-  } else if (stride == 1 || !ok) {
-    // exact radix select over the composite key: one histogram pass per 11-bit digit until the
-    // candidate set of every split fits QW_CAND_CAP. After a failed sampled threshold with the
-    // level-0 histogram on record (refine), level 0 needs no pass at all, only the failing splits are
-    // revisited, and windows whose best digit is below the threshold digit are skipped.
-    const bool refine = !ok && rec_l0;
-    const uint32_t* d_state = refine ? kp.split_state : nullptr;
-    std::vector<DThresh> th(n);
-    auto all_done = [&]() {
-      for (uint32_t i = 0; i < n; i++) if (low[i].P.max_hits && (!refine || state[i]) && !th[i].done) return false;
-      return true;
-    };
-    uint32_t level = 0;
-    bool done = false;
-    if (refine) {
-      CUDA_CHECK(cudaMemcpyAsync(slot->d_scratch + s_state, state.data(), n * 4, cudaMemcpyHostToDevice, st));
-      qwk::k_pick<<<n, 256, 0, st>>>(kp.plans, kp.thresh, 0, 0, 1, d_state);
-      stats.launches++;
-      CUDA_CHECK(cudaMemcpyAsync(th.data(), slot->d_scratch + s_thr, n * sizeof(DThresh), cudaMemcpyDeviceToHost, st));
-      wait_stream();
-      done = all_done();
-      level = 1;
-    } else {
-      CUDA_CHECK(cudaMemsetAsync(slot->d_scratch, 0, s_cand, st));
-    }
-    for (; !done && level * QW_DIGIT_BITS < std::max(max_key_bits, 1u); level++) {
-      CUDA_CHECK(cudaMemsetAsync(slot->d_scratch + s_hist, 0, (size_t)n * QW_HIST_BINS * 4, st));
-      launch_window(qwk::MODE_HIST, false, level, level > 0 ? 1 : 0, refine ? F_REFINE : 0);
-      qwk::k_pick<<<n, 256, 0, st>>>(kp.plans, kp.thresh, level, 0, 1, d_state);
-      stats.launches++;
-      stats.radix_passes++;
-      CUDA_CHECK(cudaMemcpyAsync(th.data(), slot->d_scratch + s_thr, n * sizeof(DThresh), cudaMemcpyDeviceToHost, st));
-      wait_stream();
-      done = all_done();
-    }
-    stats.refined = refine ? 1 : 0;
-    run_collect(refine ? (F_REFINE | F_CANDS_ONLY) : 0);
-    CUDA_CHECK(cudaEventRecord(slot->ev1, st));
-    wait_stream();
-    if (!verify()) fail(QWGPU_EINTERNAL, "top-K candidate selection failed verification");
-  }
-  // hashed cells: a split that outgrew its capacity sends the batch round again at the bound (before any
-  // cross-rank collective, which must run once); otherwise only the used cells come back
-  std::vector<std::vector<DHKey>> h_keys(n);
-  std::vector<std::vector<QwAggCell>> h_cells(n);
-  if (any_hashed) {
-    bool overflow = false;
-    for (uint32_t i = 0; i < n; i++)
-      if (low[i].P.hashed && (*(const uint32_t*)(slot->h_out + out_off[i] + 28) >> 31)) overflow = true;
-    if (overflow) {
-      if (at_bound) fail(QWGPU_EINTERNAL, "hashed aggregation cells overflowed their bound");
-      float ms = 0;
-      cudaEventElapsedTime(&ms, slot->ev0, slot->ev1);
-      stats.gpu_time_us += ms * 1000.f;
-      add_main();
-      return false;
-    }
-    for (uint32_t i = 0; i < n; i++) {
-      const DSplitPlan& P = low[i].P;
-      if (!P.hashed) continue;
-      const uint32_t used = std::min(*(const uint32_t*)(slot->h_out + out_off[i] + 28), P.h_cap);
-      h_keys[i].resize(used);
-      h_cells[i].resize(used);
-      if (!used) continue;
-      CUDA_CHECK(cudaMemcpyAsync(h_keys[i].data(), (const void*)P.h_keys, (size_t)used * sizeof(DHKey), cudaMemcpyDeviceToHost, st));
-      CUDA_CHECK(cudaMemcpyAsync(h_cells[i].data(), (const void*)P.h_cells, (size_t)used * sizeof(QwAggCell), cudaMemcpyDeviceToHost, st));
-      stats.d2h_bytes += (size_t)used * (sizeof(DHKey) + sizeof(QwAggCell));
-    }
-    wait_stream();
-  }
-  if (do_gather) {
-    // Cross-rank phase, after this rank's result is final (a verification fallback above must not repeat a
-    // collective the other ranks run once): the rank's record -> every rank (one NCCL all-gather on this
-    // call's stream) -> merged again on the device -> one more small copy back.
-    uint32_t* d_cut = (uint32_t*)(slot->d_scratch + s_cut);
-    qwk::k_rank_header<<<1, 32, 0, st>>>(kp.plans, n, (qwk::DRankHeader*)(slot->d_out + o_merged), gather->attempted, gather->successful, gather->n_failed);
-    uint8_t* g_recv = slot->d_scratch + s_grecv;
-    if (gather->allgather(gather->comm, slot->d_out + o_merged, g_recv, rec_bytes, (void*)st)) fail(QWGPU_EINTERNAL, "ncclAllGather failed");
-    const qwk::SrcGathered gsrc{g_recv, (uint32_t)rec_bytes, 64u};
-    uint32_t* g_cut = d_cut + std::max<uint32_t>(n, 64);
-    qwk::k_merge_prep<qwk::SrcGathered><<<1, 1024, 0, st>>>(gsrc, (uint32_t)gather->world, merge->k, merge->order1, merge->order2, g_cut);
-    const uint64_t gthreads = (uint64_t)gather->world * merge->k * 32;
-    qwk::k_merge<qwk::SrcGathered><<<(uint32_t)((gthreads + 255) / 256), 256, 0, st>>>(gsrc, g_cut, (uint32_t)gather->world, merge->k, merge->k, merge->order1, merge->order2,
-                                                                                    (qwk::DMergedHit*)(slot->d_out + o_final + 16), (uint32_t*)(slot->d_out + o_final));
-    CUDA_CHECK(cudaMemcpy2DAsync(slot->d_out + o_ghdr, 64, g_recv, rec_bytes, 64, (size_t)gather->world, cudaMemcpyDeviceToDevice, st));
-    CUDA_CHECK(cudaMemcpyAsync(slot->h_out + o_ghdr, slot->d_out + o_ghdr, out_bytes - o_ghdr, cudaMemcpyDeviceToHost, st));
-    CUDA_CHECK(cudaEventRecord(slot->ev1, st));
-    wait_stream();
-    stats.launches += 4;
-    stats.d2h_bytes += out_bytes - o_ghdr;
-  }
-  CUDA_CHECK(cudaGetLastError());
-  {
-    float ms = 0;
-    cudaEventElapsedTime(&ms, slot->ev0, slot->ev1);
-    stats.gpu_time_us += ms * 1000.f;
-    add_main();
-    stats.main_kernel_us = main_ms * 1000.f;
-  }
-
-  const auto t_searched = tclock::now();
-  // ---- unpack ---------------------------------------------------------------------------------------
-  for (uint32_t i = 0; i < n; i++) {
-    SplitOutput& o = outs[idx[i]];
-    const DSplitPlan& P = low[i].P;
-    const uint8_t* ob = slot->h_out + out_off[i];
-    o.num_hits = ((const uint64_t*)ob)[0];
-    uint32_t nh = *(const uint32_t*)(ob + 16);
-    if (!do_merge) {
-      o.hits.assign((const QwHit*)(ob + 32), (const QwHit*)(ob + 32) + nh);
-      if (P.key.kind[0] == QW_SORT_DOCID) for (auto& h : o.hits) { h.flags &= ~1u; h.v1 = 0; }
-    }
-    const QwAggCell* c = (const QwAggCell*)(ob + 32 + (do_merge ? 0 : (size_t)P.max_hits * sizeof(QwHit)));
-    o.cells.assign(c, c + P.n_cells);
-    for (auto& cell : o.cells) cell.min_mapped = ~cell.min_mapped;  // device keeps max(~m); see agg_stats
-    if (P.hashed) {
-      o.hashed = true;
-      o.entries.resize(h_keys[i].size());
-      for (size_t e = 0; e < o.entries.size(); e++) {
-        QwAggEntry& x = o.entries[e];
-        x.node = h_keys[i][e].node_flags & 0xFFu;
-        x.flags = h_keys[i][e].node_flags >> 8;
-        x.parent = h_keys[i][e].parent;
-        x.key = h_keys[i][e].key;
-        x.reserved = 0;
-        x.cell = h_cells[i][e];
-        x.cell.min_mapped = ~x.cell.min_mapped;
-      }
-    }
-    if (P.tr_on) {
-      if (*(const uint32_t*)(ob + 24)) stats.kernel_mask |= QWGPU_KERNEL_TRACE_REPLAY;
-      // a matched doc without a trace id reads ordinal 0: with an empty dictionary the reference's ord_to_bytes fails
-      const QwImgColumn& tc = sp[idx[i]]->view.columns[low[i].tr_img_col];
-      for (const QwAggCell& cell : o.cells)
-        if (cell.count == 1 && cell.sum_bits >= tc.dict_num_terms) {
-          o.status = QWGPU_EINTERNAL;
-          o.error = "failed to look up a trace id in the column term dictionary";
-          o.cells.clear();
-          break;
-        }
-    }
-    o.postings_scored = low[i].postings;
-    // SURVEY.md §8d algorithmic bytes: postings (+ fieldnorms, added at lowering) + column probes
-    uint64_t bytes = low[i].alg_bytes;
-    const SplitDev& s = *sp[idx[i]];
-    auto col_bytes = [&](uint32_t c, uint64_t probes) {
-      const QwImgColumn& ic = s.view.columns[c];
-      uint64_t full = ((uint64_t)ic.num_vals * ic.bits + 7) / 8;
-      return std::min<uint64_t>(probes * ((ic.bits + 7) / 8), full);
-    };
-    uint64_t driver = low[i].min_required_df == ~0ull ? P.num_docs : low[i].min_required_df;
-    for (auto& rc : low[i].range_cols) bytes += col_bytes(rc.first, driver);
-    const QwPlanHeader* ph = (const QwPlanHeader*)plans[idx[i]];
-    for (int k = 0; k < 2; k++)
-      if (ph->sort[k].kind == QW_SORT_COLUMN && ph->sort[k].column != 0xFFFFFFFFu && P.max_hits) bytes += col_bytes(ph->sort[k].column, o.num_hits);
-    const QwAggNode* an = (const QwAggNode*)(plans[idx[i]] + sizeof(QwPlanHeader) + (size_t)ph->num_nodes * sizeof(QwPlanNode));
-    for (uint32_t a = 0; a < ph->num_aggs; a++) if (an[a].column != 0xFFFFFFFFu) bytes += col_bytes(an[a].column, o.num_hits);
-    o.algorithmic_bytes = bytes;
-  }
-  if (do_gather) {
-    // the cross-rank result: hits carry GLOBAL split ranks (the caller owns the rank -> split id table)
-    const uint32_t nm = *(const uint32_t*)(slot->h_out + o_final);
-    const qwk::DMergedHit* mh = (const qwk::DMergedHit*)(slot->h_out + o_final + 16);
-    merged->resize(nm);
-    const bool by_doc = low[0].P.key.kind[0] == QW_SORT_DOCID;
-    for (uint32_t j = 0; j < nm; j++) {
-      MergedHit& m = (*merged)[j];
-      m.hit = mh[j].hit; m.split = mh[j].split; m.pad = 0;
-      if (by_doc) { m.hit.flags &= ~1u; m.hit.v1 = 0; }
-    }
-    rank_headers->resize(gather->world);
-    memcpy(rank_headers->data(), slot->h_out + o_ghdr, (size_t)gather->world * 64);
-  } else if (do_merge) {
-    const uint32_t nm = *(const uint32_t*)(slot->h_out + o_merged);
-    const qwk::DMergedHit* mh = (const qwk::DMergedHit*)(slot->h_out + o_merged + 64);
-    merged->resize(nm);
-    for (uint32_t j = 0; j < nm; j++) {
-      MergedHit& m = (*merged)[j];
-      m.hit = mh[j].hit;
-      m.split = idx[mh[j].split];
-      m.pad = 0;
-      if (low[mh[j].split].P.key.kind[0] == QW_SORT_DOCID) { m.hit.flags &= ~1u; m.hit.v1 = 0; }
-    }
-  }
-  if (trace) {
-    auto us = [](tclock::time_point a, tclock::time_point b) { return (long)std::chrono::duration_cast<std::chrono::microseconds>(b - a).count(); };
-    fprintf(stderr, "[qwgpu] search: lower %ld us, stage %ld us, launch+wait %ld us (device %.0f us), unpack %ld us\n", us(t_begin, t_lowered),
-            us(t_lowered, t_staged), us(t_staged, t_searched), stats.gpu_time_us, us(t_searched, tclock::now()));
-  }
-  return true;
+// A rank with no searchable split still takes part in the collective, with an empty record (and reports no device work)
+static void exchange_empty(Engine& e, const MergeSpec& merge, const GatherSpec& gather, std::vector<MergedHit>& merged,
+                           std::vector<RankHeader>& rank_headers) {
+  SlotLease lease(e);
+  const std::vector<Lowered> none;
+  const std::vector<uint32_t> no_idx;
+  const Route no_route{};
+  BatchStats unused;
+  Run run{e, *lease.slot, unused, none, no_idx, no_route, &merge, &gather, true, true, 0, lease.slot->stream};
+  run.lay_out(false);
+  run.size_slot();
+  CUDA_CHECK(cudaMemsetAsync(run.slot.d_out, 0, run.out_bytes, run.st));
+  qwk::DRankHeader h{};
+  h.attempted = gather.attempted;
+  h.successful = gather.successful;
+  h.n_failed = gather.n_failed;
+  CUDA_CHECK(cudaMemcpyAsync(run.slot.d_out + run.o_merged, &h, sizeof h, cudaMemcpyHostToDevice, run.st));
+  run.exchange();
+  wait_call(e, run.slot);
+  unpack_merged(run.slot.h_out + run.o_final, run.slot.h_out + run.o_final + 16, none, nullptr, merged);
+  rank_headers.resize(gather.world);
+  memcpy(rank_headers.data(), run.slot.h_out + run.o_ghdr, (size_t)gather.world * 64);
 }
 
 void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std::vector<const uint8_t*>& plans,
                     const std::vector<size_t>& plan_lens, std::vector<SplitOutput>& outs, BatchStats& stats,
                     const MergeSpec* merge, std::vector<MergedHit>* merged, const GatherSpec* gather, std::vector<RankHeader>* rank_headers) {
-  if (search_once(sp, plans, plan_lens, outs, stats, merge, merged, gather, rank_headers, false)) return;
-  // a split's hashed aggregation cells outgrew QWGPU_HASHED_INIT_CELLS: the batch runs again with every hashed
-  // split's table at its bound, where it cannot overflow (the first run's device time stays in the stats)
-  stats.kernel_mask |= QWGPU_KERNEL_HASHED_AGGS_RETRY;
-  search_once(sp, plans, plan_lens, outs, stats, merge, merged, gather, rank_headers, true);
+  outs.assign(sp.size(), SplitOutput());
+  static const bool trace = getenv("QWGPU_TRACE") != nullptr;  // host phase timings on stderr
+  using tclock = std::chrono::steady_clock;
+  const auto t_begin = tclock::now();
+  CUDA_CHECK(cudaSetDevice(device));
+  std::vector<uint32_t> idx;
+  const std::vector<Lowered> low = lower_batch(sp, plans, plan_lens, outs, idx);
+  const bool gathering = merge && merged && merge->k > 0 && gather && gather->allgather && gather->world > 1 && rank_headers;
+  if (low.empty()) {
+    if (gathering) exchange_empty(*this, *merge, *gather, *merged, *rank_headers);
+    return;
+  }
+  const auto t_lowered = tclock::now();
+  const Route r = choose_route(low, max_smem_optin, sm_count);
+  // device-side cross-split merge: the per-split hit lists stay in scratch, only the merged top-K comes back
+  const bool do_merge = merge && merged && merge->k > 0 && merge->rank.size() == sp.size() &&
+                        std::any_of(low.begin(), low.end(), [](const Lowered& L) { return L.P.max_hits > 0; });
+  SlotLease lease(*this);
+  Run run{*this, *lease.slot, stats, low, idx, r, merge, gather, do_merge, do_merge && gathering, (uint32_t)low.size(), lease.slot->stream};
+  tclock::time_point t_staged;
+  for (bool at_bound : {false, true}) {
+    run.lay_out(at_bound);
+    run.size_slot();
+    run.stage();
+    if (!at_bound) t_staged = tclock::now();
+    if (run.run(at_bound)) break;
+    // a split's hashed aggregation cells outgrew QWGPU_HASHED_INIT_CELLS: the batch runs again with every hashed
+    // split's table at its bound, where it cannot overflow (the first run's device time stays in the stats)
+    stats.kernel_mask |= QWGPU_KERNEL_HASHED_AGGS_RETRY;
+  }
+
+  const auto t_searched = tclock::now();
+  const uint8_t* h_out = lease.slot->h_out;
+  for (uint32_t i = 0; i < low.size(); i++)
+    unpack_split(outs[idx[i]], stats, low[i], *sp[idx[i]], plans[idx[i]], h_out + run.at[i].out, do_merge, run.h_keys[i], run.h_cells[i]);
+  if (run.do_gather) {
+    // the cross-rank result: hits carry GLOBAL split ranks (the caller owns the rank -> split id table)
+    unpack_merged(h_out + run.o_final, h_out + run.o_final + 16, low, nullptr, *merged);
+    rank_headers->resize(gather->world);
+    memcpy(rank_headers->data(), h_out + run.o_ghdr, (size_t)gather->world * 64);
+  } else if (do_merge) {
+    unpack_merged(h_out + run.o_merged, h_out + run.o_merged + 64, low, &idx, *merged);
+  }
+  if (trace) {
+    // (a call re-run after a hashed overflow counts the re-run's staging in launch+wait)
+    auto us =[](tclock::time_point a, tclock::time_point b) { return (long)std::chrono::duration_cast<std::chrono::microseconds>(b - a).count(); };
+    fprintf(stderr, "[qwgpu] search: lower %ld us, stage %ld us, launch+wait %ld us (device %.0f us), unpack %ld us\n", us(t_begin, t_lowered),
+            us(t_lowered, t_staged), us(t_staged, t_searched), stats.gpu_time_us, us(t_searched, tclock::now()));
+  }
 }
 
 }  // namespace qw

@@ -119,12 +119,6 @@ struct Engine {
               const std::vector<size_t>& plan_lens, std::vector<SplitOutput>& outs, BatchStats& stats,
               const MergeSpec* merge = nullptr, std::vector<MergedHit>* merged = nullptr,
               const GatherSpec* gather = nullptr, std::vector<RankHeader>* rank_headers = nullptr);
-  // one run of the batch; false (nothing returned yet) when a split's hashed aggregation cells overflowed their
-  // initial capacity. at_bound: every hashed split's table is sized at its bound.
-  bool search_once(const std::vector<std::shared_ptr<SplitDev>>& sp, const std::vector<const uint8_t*>& plans,
-                   const std::vector<size_t>& plan_lens, std::vector<SplitOutput>& outs, BatchStats& stats,
-                   const MergeSpec* merge, std::vector<MergedHit>* merged, const GatherSpec* gather,
-                   std::vector<RankHeader>* rank_headers, bool at_bound);
 };
 
 // plan validation helper shared with the compiler: total agg cells + per-node bases

@@ -189,6 +189,18 @@ def test_capacity_rerun(gpu_ctx, corpora):
         assert r.kernel_mask & HASHED and r.kernel_mask & RETRY, hex(r.kernel_mask)
 
 
+def test_capacity_rerun_keeps_fast_histogram(gpu_ctx, corpora):
+    """The re-run stages the call's plans again: a dense split whose histogram takes the fast path (a raw-space bounds
+    table in the staged blob) must give the same cells in a retried batch as searched alone."""
+    uid, main = corpora["uid"], corpora["main"]
+    hist = [H(main, "lat", 500.0)]
+    both = _run(gpu_ctx, [(uid, [T(uid, "uid", T(uid, "svc", ST(uid, "lat")))]), (main, hist)])
+    assert both[1].kernel_mask & RETRY and both[1].kernel_mask & ffi.KERNEL_FAST_AGGS, hex(both[1].kernel_mask)
+    alone = _run(gpu_ctx, [(main, hist)])
+    assert not alone[0].kernel_mask & RETRY and alone[0].cells
+    assert both[1].cells == alone[0].cells
+
+
 # ---- finalised JSON: entries builder, leaf_search, root merge ---------------------------------------------------------
 DM = {"field_mappings": [
     {"name": "svc", "type": "text", "tokenizer": "raw", "fast": True},
