@@ -314,11 +314,30 @@ typedef struct QwPlanHeader {
   uint32_t max_hits;  /* leaf_max_hits = max_hits + start_offset (collector.rs:772-774) */
   uint32_t scoring;   /* QuickwitCollector::requires_scoring (collector.rs:819-830) */
   uint32_t count_only; /* max_hits == 0 && no aggregation (collector.rs:723-725) */
-  uint32_t reserved;
+  uint32_t reserved;   /* QW_PLAN_* flags */
   QwSortSpec sort[2];
   QwSearchAfter search_after;
   /* followed by QwPlanNode[num_nodes], then QwAggNode[num_aggs] */
 } QwPlanHeader;
+
+/* QwPlanHeader.reserved: return the hits through full QwHit records from the device even where qw_plan_score_hits()
+ * holds (the results are the same; tests compare the two forms) */
+#define QW_PLAN_FULL_HITS 1u
+
+/* A hit of a plan ranked by _score descending alone, as the device hands it back: the rest of its QwHit follows
+ * from these two fields (v1 = f64_to_u64(score as f64), flags = 1, v2 = reserved = 0). */
+typedef struct QwScoreHit {
+  uint32_t doc_id;
+  float score;
+} QwScoreHit;
+
+/* 1 when the device returns the plan's hits as QwScoreHit records: sorted by _score descending with no second key
+ * (a `_doc` second key extracts None), no search_after, and QW_PLAN_FULL_HITS clear. */
+static inline int qw_plan_score_hits(const QwPlanHeader* h) {
+  return h->sort[0].kind == QW_SORT_SCORE && h->sort[0].order == QW_ORDER_DESC &&
+         (h->sort[1].kind == QW_SORT_NONE || h->sort[1].kind == QW_SORT_DOCID) && !h->search_after.present &&
+         !(h->reserved & QW_PLAN_FULL_HITS);
+}
 
 /* ---------------------------------------------------------------- result --------------------- */
 

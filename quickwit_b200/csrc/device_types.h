@@ -130,7 +130,8 @@ struct DSplitPlan {
   uint32_t fused_score_root;  // root bool is a pure OR of positive-weight scored terms
   uint32_t fast_aggs;         // every aggregation is a bucket aggregation (optionally with stats children)
                               // or a stats node over always-present single-valued columns
-  uint32_t n_stat_cells, pad1;  // fast path: number of privatised stats cells
+  uint32_t n_stat_cells;   // fast path: number of privatised stats cells
+  uint32_t score_hits;     // k_select writes QwScoreHit records (qw_plan_score_hits; never in a merged batch)
   uint64_t fn_off[2];      // data-relative fieldnorm arrays staged per window
   uint64_t bm25_tab[2];    // device addresses of float[256] BM25 norm tables, followed by the
                            // float[QW_TFF_ROWS][256] tf-factor table of the same field
@@ -141,7 +142,7 @@ struct DSplitPlan {
   uint64_t out_cand_count; // device address of a uint32 counter
   uint64_t out_cands;      // device address of uint64[3 * QW_CAND_CAP]
   uint64_t out_cells;      // device address of QwAggCell[n_cells]
-  uint64_t out_hits;       // device address of QwHit[max_hits]
+  uint64_t out_hits;       // device address of QwHit[max_hits] (score_hits: QwScoreHit[max_hits])
   uint64_t out_nhits;      // device address of uint32 (hits written by k_select)
   // find_trace_ids (trace_kernel.cuh); tr_on == 0 when the plan has no QW_AGG_TRACE_IDS node
   uint64_t tr_best;        // device address of uint64[tr_num_ords]: latest span per trace ordinal (0 = none)

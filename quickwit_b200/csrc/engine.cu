@@ -650,6 +650,7 @@ static void lower_plan(Lowered& L, const SplitDev& sp, const uint8_t* plan, size
   P.max_hits = ph->max_hits;
   P.scoring = ph->scoring;
   P.sa = ph->search_after;
+  P.score_hits = (uint32_t)qw_plan_score_hits(ph);
   const bool scoring = ph->scoring != 0;
   if (nodes[0].kind == QW_NODE_BOOL) {
     lower_node(L, sp, nodes, ph->num_nodes, 0, 0, QW_OCCUR_MUST, scoring);
@@ -1175,6 +1176,12 @@ static void wait_call(Engine& e, CallSlot& slot) {
 }
 
 enum { F_REC = 1, F_REFINE = 2, F_CANDS_ONLY = 4 };  // collect / histogram pass flags
+
+// bytes of a split's hit list in its output region (a merged batch keeps the lists in scratch)
+static size_t out_hit_bytes(const DSplitPlan& P, bool do_merge) {
+  return do_merge ? 0 : (size_t)P.max_hits * (P.score_hits ? sizeof(QwScoreHit) : sizeof(QwHit));
+}
+
 // One device run of a lowered batch on the call's slot. lay_out() places every region in the slot's buffers: blob
 // (copied to the device: plans, programs, work lists), scratch (device only) and out (copied back); stage() gives the
 // run's copies of the plans their addresses and copies the blob over; run() issues the passes.
@@ -1223,6 +1230,7 @@ struct Run {
       const Lowered& L = low[i];
       DSplitPlan& P = plans[i] = L.P;
       P.num_windows = r.fw_all[i + 1] - r.fw_all[i];
+      if (do_merge) P.score_hits = 0;  // (k_merge reads QwHit lists)
       P.instr_base = tot_instr; P.col_base = tot_cols; P.agg_base = tot_aggs;
       bounds_base[i] = tot_bounds;
       tot_instr += P.n_instr; tot_cols += P.n_cols; tot_aggs += P.n_aggs; tot_bounds += (uint32_t)L.bounds.size();
@@ -1287,7 +1295,7 @@ struct Run {
     scratch_bytes = s.off;
     Arena o{256};
     for (uint32_t i = 0; i < n; i++)
-      at[i].out = o.take(32 + (do_merge ? 0 : (size_t)plans[i].max_hits * sizeof(QwHit)) + (size_t)plans[i].n_cells * sizeof(QwAggCell));
+      at[i].out = o.take(32 + out_hit_bytes(plans[i], do_merge) + (size_t)plans[i].n_cells * sizeof(QwAggCell));
     // [RankHeader 64 B (n_hits first)][DMergedHit x k]: the batch's merged top-k = this rank's gather record
     o_merged = o.take(rec_bytes);
     if (do_gather) {
@@ -1343,7 +1351,7 @@ struct Run {
       P.out_nhits = (uint64_t)(ob + 16);
       P.out_cand_count = (uint64_t)(ob + 20);
       P.out_hits = do_merge ? (uint64_t)(slot.d_scratch + s_hits + (size_t)i * kmax * sizeof(QwHit)) : (uint64_t)(ob + 32);
-      P.out_cells = (uint64_t)(ob + 32 + (do_merge ? 0 : (size_t)P.max_hits * sizeof(QwHit)));
+      P.out_cells = (uint64_t)(ob + 32 + out_hit_bytes(P, do_merge));
       P.out_hist = (uint64_t)(slot.d_scratch + s_hist + (size_t)i * QW_HIST_BINS * 4);
       P.out_cands = (uint64_t)(slot.d_scratch + s_cand + (size_t)i * QW_CAND_CAP * 24);
       if (P.tr_on) {
@@ -1708,17 +1716,33 @@ static std::vector<Lowered> lower_batch(const std::vector<std::shared_ptr<SplitD
 
 static void strip_doc_key(QwHit& h) { h.flags &= ~1u; h.v1 = 0; }  // (the doc-id sort key's internal fields)
 
-// one split's result out of its region of the copied-back buffer (and its hashed entries)
-static void unpack_split(SplitOutput& o, BatchStats& stats, const Lowered& L, const SplitDev& s, const uint8_t* plan, const uint8_t* ob,
-                         bool do_merge, const std::vector<DHKey>& keys, const std::vector<QwAggCell>& cells) {
-  const DSplitPlan& P = L.P;
+// the QwHit that k_select writes for a hit ranked by _score descending alone
+static QwHit expand_score_hit(const QwScoreHit& s) {
+  QwHit h;
+  h.v1 = f64_to_u64((double)s.score);
+  h.v2 = 0;
+  h.doc_id = s.doc_id;
+  h.flags = 1;
+  h.score = s.score;
+  h.reserved = 0;
+  return h;
+}
+
+// one split's result out of its region of the copied-back buffer (and its hashed entries); P: the run's copy of
+// the split's plan
+static void unpack_split(SplitOutput& o, BatchStats& stats, const Lowered& L, const DSplitPlan& P, const SplitDev& s, const uint8_t* plan,
+                         const uint8_t* ob, bool do_merge, const std::vector<DHKey>& keys, const std::vector<QwAggCell>& cells) {
   o.num_hits = ((const uint64_t*)ob)[0];
   uint32_t nh = *(const uint32_t*)(ob + 16);
-  if (!do_merge) {
+  if (!do_merge && P.score_hits) {
+    const QwScoreHit* sh = (const QwScoreHit*)(ob + 32);
+    o.hits.resize(nh);
+    for (uint32_t j = 0; j < nh; j++) o.hits[j] = expand_score_hit(sh[j]);
+  } else if (!do_merge) {
     o.hits.assign((const QwHit*)(ob + 32), (const QwHit*)(ob + 32) + nh);
     if (P.key.kind[0] == QW_SORT_DOCID) for (auto& h : o.hits) strip_doc_key(h);
   }
-  const QwAggCell* c = (const QwAggCell*)(ob + 32 + (do_merge ? 0 : (size_t)P.max_hits * sizeof(QwHit)));
+  const QwAggCell* c = (const QwAggCell*)(ob + 32 + out_hit_bytes(P, do_merge));
   o.cells.assign(c, c + P.n_cells);
   for (auto& cell : o.cells) cell.min_mapped = ~cell.min_mapped;  // device keeps max(~m); see agg_stats
   if (P.hashed) {
@@ -1842,7 +1866,7 @@ void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std:
   const auto t_searched = tclock::now();
   const uint8_t* h_out = lease.slot->h_out;
   for (uint32_t i = 0; i < low.size(); i++)
-    unpack_split(outs[idx[i]], stats, low[i], *sp[idx[i]], plans[idx[i]], h_out + run.at[i].out, do_merge, run.h_keys[i], run.h_cells[i]);
+    unpack_split(outs[idx[i]], stats, low[i], run.plans[i], *sp[idx[i]], plans[idx[i]], h_out + run.at[i].out, do_merge, run.h_keys[i], run.h_cells[i]);
   if (run.do_gather) {
     // the cross-rank result: hits carry GLOBAL split ranks (the caller owns the rank -> split id table)
     unpack_merged(h_out + run.o_final, h_out + run.o_final + 16, low, nullptr, *merged);

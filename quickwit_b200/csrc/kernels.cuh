@@ -1584,7 +1584,7 @@ __global__ void __launch_bounds__(256) k_pick(const DSplitPlan* plans, DThresh* 
 }
 
 // Harvest (quickwit-search/src/top_k_collector.rs:404-410, binary_heap.rs:187-193): the best
-// min(K, n) candidates of a split, best first, decoded back to QwHit.
+// min(K, n) candidates of a split, best first, decoded back to QwHit (QwScoreHit where P.score_hits).
 //   1. exact radix select (8-bit digits, MSB first) of the K-th largest first key word;
 //   2. compaction of the candidates >= that word (all ties kept) — normally ~K of the ~2-3K candidates;
 //   3. bitonic sort of the survivors with the full 192-bit comparison (the reference total order).
@@ -1784,7 +1784,8 @@ __global__ void __launch_bounds__(1024) k_select(const DSplitPlan* plans, const 
     }
     hh.v1 = v[0];
     hh.v2 = v[1];
-    hits[i] = hh;
+    if (P.score_hits) reinterpret_cast<QwScoreHit*>(hits)[i] = QwScoreHit{hh.doc_id, hh.score};
+    else hits[i] = hh;
   }
   if (tid == 0) *(uint32_t*)P.out_nhits = out_n;
 }
