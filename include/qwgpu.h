@@ -90,6 +90,13 @@ int qwgpu_split_wait(qwgpu_ctx* ctx, const char* split_id);
 int qwgpu_residency_info(qwgpu_ctx* ctx, uint64_t* resident_bytes, uint64_t* budget_bytes, uint64_t* num_splits, uint64_t* evictions);
 int qwgpu_split_is_resident(qwgpu_ctx* ctx, const char* split_id);
 
+/* Largest max_hits + start_offset that a search on this context serves (1 .. 20 000; 4096 until set). A plan above it
+ * fails with QWGPU_EUNSUPPORTED (in a leaf response: a failed split, not retryable). Splits asked for more than 4096
+ * hits take the deep selection path (QWGPU_KERNEL_DEEP_SELECT); such a call needs call-slot scratch that grows with K
+ * — about 84 MB for 32 splits at K = 20 000 — and the context's slots keep that size for later calls, so a caller
+ * raises the limit when it expects such requests (the reference accepts max_hits and start_offset up to 10 000 each). */
+int qwgpu_set_max_hits(qwgpu_ctx* ctx, uint32_t max_hits);
+
 /* ---- seam A / B: protobuf in, protobuf out ---------------------------------------------------- */
 
 /* req = quickwit.search.LeafSearchRequest, resp = quickwit.search.LeafSearchResponse
@@ -153,6 +160,8 @@ typedef struct qwgpu_split_result {
                                                fallbacks, bytes) add up both runs. */
 #define QWGPU_KERNEL_COMPOSITE_CUT 1024u /* k_composite_cut cut the composite aggregations of the batch's hashed
                                             splits to their first `size` buckets before the copy-back */
+#define QWGPU_KERNEL_DEEP_SELECT 2048u /* a split of the batch asked for more than 4096 hits (max_hits + start_offset)
+                                          and took the deep selection path (k_deep_cut, k_deep_sort, k_deep_rank) */
 /* Initial capacity of a split's hashed cell table: min(this, the split's bound on distinct cells). */
 #define QWGPU_HASHED_INIT_CELLS 65536u
 /* Largest total of the hashed tables (cells, key records and slots, each at its split's bound) that one call may

@@ -37,6 +37,12 @@ impl GpuContext {
         check(unsafe { ffi::qwgpu_set_residency_budget(self.raw, bytes) })
     }
 
+    /// Largest `max_hits + start_offset` served (1 ..= 20 000; 4096 until set). A root that sends the reference's
+    /// limits (10 000 hits from offset up to 10 000) raises it to 20 000.
+    pub fn set_max_hits(&self, max_hits: u32) -> Result<(), SearchError> {
+        check(unsafe { ffi::qwgpu_set_max_hits(self.raw, max_hits) })
+    }
+
     /// Makes a split image (include/qwgpu_format.h) resident; the bytes may be dropped afterwards. The counterpart
     /// of `open_split_bundle` + `warmup` (quickwit-search/src/leaf.rs:210-251, 269-472).
     pub fn register_split(&self, split_id: &str, image: &[u8]) -> Result<(), SearchError> {

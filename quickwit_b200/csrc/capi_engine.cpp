@@ -1,5 +1,6 @@
 // capi_engine.cpp — C ABI entry points backed by the GPU engine (context, residency, seam C).
 #include "engine.h"
+#include "device_types.h"
 
 #define QW_API_BEGIN try {
 #define QW_API_END                                   \
@@ -64,6 +65,14 @@ int qwgpu_split_wait(qwgpu_ctx* ctx, const char* split_id) {
 int qwgpu_set_residency_budget(qwgpu_ctx* ctx, uint64_t bytes) {
   QW_API_BEGIN
   engine_of(ctx).set_budget(bytes);
+  return 0;
+  QW_API_END
+}
+
+int qwgpu_set_max_hits(qwgpu_ctx* ctx, uint32_t max_hits) {
+  QW_API_BEGIN
+  if (max_hits < 1 || max_hits > QW_MAX_HITS) qw::fail(QWGPU_EINVALID_ARG, "max_hits limit %u outside [1, 20 000]", max_hits);
+  engine_of(ctx).max_hits.store(max_hits, std::memory_order_relaxed);
   return 0;
   QW_API_END
 }

@@ -18,9 +18,19 @@
 #define QW_HIST_BINS 2048    /* 11-bit radix digits */
 #define QW_DIGIT_BITS 11
 #define QW_KEY_BITS 192
-#define QW_CAND_CAP 8192     /* candidates kept per split before the final sort */
-#define QW_MAX_TOPK 4096
+#define QW_CAND_CAP 8192     /* candidates kept per split before the final sort (K <= QW_MAX_TOPK) */
+#define QW_MAX_TOPK 4096     /* largest K that k_select sorts in one block (also the find_trace_ids limit) */
+#define QW_MAX_HITS 20000    /* largest max_hits + start_offset of a request: the reference's 10 000 + 10 000 */
 #define QW_SMEM_AGG_CELLS 4096
+
+#ifdef __CUDACC__
+#define QW_HOST_DEVICE __host__ __device__ __forceinline__
+#else
+#define QW_HOST_DEVICE static inline
+#endif
+// Candidate capacity of a split whose plan asks for K hits: QW_CAND_CAP up to QW_MAX_TOPK (k_select's shared
+// memory), above that 2K rounded up to a multiple of 1024 (the deep selection path, deep_select_kernel.cuh).
+QW_HOST_DEVICE uint32_t qw_cand_cap(uint32_t K) { return K <= QW_MAX_TOPK ? (uint32_t)QW_CAND_CAP : (2u * K + 1023u) & ~1023u; }
 
 enum { OP_TERM = 1, OP_RANGE = 2, OP_EXISTS = 3, OP_ALL = 4, OP_BOOL_BEGIN = 5, OP_BOOL_END = 6, OP_PHRASE = 7 };
 enum { IF_SCORED = 1u, IF_HAS_TF = 2u, IF_HAS_FN = 4u, IF_BITS_FROM_SCORE = 8u };
@@ -114,7 +124,7 @@ struct DThresh {  // per split, device-resident, written by k_pick
   uint64_t key[3];       // candidates are docs with composite key >= key
   uint32_t prefix_bits;  // number of leading bits of `key` that are fixed so far
   uint32_t above;        // docs strictly above the prefix (exact path bookkeeping)
-  uint32_t done;         // 1 when the candidate set fits QW_CAND_CAP
+  uint32_t done;         // 1 when the candidate set fits qw_cand_cap(K)
   uint32_t matched;      // docs matching the prefix at the last level
 };
 
@@ -140,7 +150,7 @@ struct DSplitPlan {
   uint64_t out_num_hits;   // device address of a uint64 counter
   uint64_t out_hist;       // device address of uint32[QW_HIST_BINS]
   uint64_t out_cand_count; // device address of a uint32 counter
-  uint64_t out_cands;      // device address of uint64[3 * QW_CAND_CAP]
+  uint64_t out_cands;      // device address of uint64[3 * qw_cand_cap(max_hits)]
   uint64_t out_cells;      // device address of QwAggCell[n_cells]
   uint64_t out_hits;       // device address of QwHit[max_hits] (score_hits: QwScoreHit[max_hits])
   uint64_t out_nhits;      // device address of uint32 (hits written by k_select)

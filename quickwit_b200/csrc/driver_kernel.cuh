@@ -151,14 +151,14 @@ __global__ void __launch_bounds__(QD_WARPS * 32) k_driver(const DrvParams p) {
               my_elig++;
               if (key_ge(dk.key, thr)) {
                 const uint32_t pos = atomicAdd((uint32_t*)P.out_cand_count, 1u);
-                if (pos < QW_CAND_CAP) { uint64_t* c = (uint64_t*)P.out_cands + 3ull * pos; c[0] = dk.key.w0; c[1] = dk.key.w1; c[2] = dk.key.w2; }
+                if (pos < qw_cand_cap(max_hits)) { uint64_t* c = (uint64_t*)P.out_cands + 3ull * pos; c[0] = dk.key.w0; c[1] = dk.key.w1; c[2] = dk.key.w2; }
               }
             }
           } else if (key_top11(P, ks, cols, base, doc[j], sc) >= thr_top) {
             const DocKey dk = doc_key(P, ks, cols, base, doc[j], sc);
             if (key_ge(dk.key, thr)) {
               const uint32_t pos = atomicAdd((uint32_t*)P.out_cand_count, 1u);
-              if (pos < QW_CAND_CAP) { uint64_t* c = (uint64_t*)P.out_cands + 3ull * pos; c[0] = dk.key.w0; c[1] = dk.key.w1; c[2] = dk.key.w2; }
+              if (pos < qw_cand_cap(max_hits)) { uint64_t* c = (uint64_t*)P.out_cands + 3ull * pos; c[0] = dk.key.w0; c[1] = dk.key.w1; c[2] = dk.key.w2; }
             }
           }
         } else {

@@ -16,6 +16,7 @@
 #include "agg_kernel.cuh"
 #include "trace_kernel.cuh"
 #include "composite_kernel.cuh"
+#include "deep_select_kernel.cuh"
 
 namespace qw {
 
@@ -633,13 +634,17 @@ static void lower_node(Lowered& L, const SplitDev& sp, const QwPlanNode* nodes, 
 
 static inline uint32_t bits_needed64(uint64_t v) { return v == 0 ? 0 : 64 - __builtin_clzll(v); }
 
-static void lower_plan(Lowered& L, const SplitDev& sp, const uint8_t* plan, size_t plan_len) {
+static void lower_plan(Lowered& L, const SplitDev& sp, const uint8_t* plan, size_t plan_len, uint32_t max_hits) {
   if (plan_len < sizeof(QwPlanHeader)) fail(QWGPU_EINVALID_ARG, "plan too short");
   const QwPlanHeader* ph = (const QwPlanHeader*)plan;
   if (ph->magic != QW_PLAN_MAGIC) fail(QWGPU_EINVALID_ARG, "bad plan magic");
   size_t need = sizeof(QwPlanHeader) + (size_t)ph->num_nodes * sizeof(QwPlanNode) + (size_t)ph->num_aggs * sizeof(QwAggNode);
   if (plan_len < need || ph->num_nodes == 0) fail(QWGPU_EINVALID_ARG, "plan truncated");
-  if (ph->max_hits > QW_MAX_TOPK) fail(QWGPU_EUNSUPPORTED, "max_hits + start_offset = %u exceeds the GPU top-K limit %d", ph->max_hits, QW_MAX_TOPK);
+  if (ph->max_hits > max_hits) {
+    if (max_hits >= QW_MAX_HITS) fail(QWGPU_EUNSUPPORTED, "max_hits + start_offset = %u exceeds the GPU top-K limit of 20 000", ph->max_hits);
+    fail(QWGPU_EUNSUPPORTED, "max_hits + start_offset = %u exceeds the context's GPU top-K limit %u (qwgpu_set_max_hits raises it up to 20 000)",
+         ph->max_hits, max_hits);
+  }
   const QwPlanNode* nodes = (const QwPlanNode*)(plan + sizeof(QwPlanHeader));
   const QwAggNode* aggs = (const QwAggNode*)(nodes + ph->num_nodes);
   memset(&L.P, 0, sizeof L.P);
@@ -1199,13 +1204,13 @@ struct Run {
   const cudaStream_t st;
   std::vector<DSplitPlan> plans;      // copies of the lowered plans with the run's positions, capacities and addresses
   std::vector<uint32_t> bounds_base;  // per split: position of its histogram bounds in the batch's table
-  struct Split { size_t out, tr_best, tr_match, h_table, h_keys, h_cells; };  // offsets of a split's regions
+  struct Split { size_t out, cand, tr_best, tr_match, h_table, h_keys, h_cells; };  // offsets of a split's regions
   std::vector<Split> at;
-  bool any_topk, any_trace, any_hashed, any_composite, any_fast_aggs;
-  uint32_t kmax, n_phrases, phrase_blocks, tie_max_n;
+  bool any_topk, any_deep, any_trace, any_hashed, any_composite, any_fast_aggs;
+  uint32_t kmax, deep_cap, n_phrases, phrase_blocks, tie_max_n;
   size_t n_phrase_exp;
   size_t o_plans, o_instr, o_cols, o_aggs, o_fwa, o_fws, o_bounds, o_rank, o_smp, o_phr, o_pexp, o_fwd, o_fwds, blob_bytes;
-  size_t s_thr, s_hist, s_state, s_wmax, s_cand, s_hits, s_cut, s_grecv, s_vblk, s_trace_state, s_trace_data, s_hash, scratch_bytes;
+  size_t s_thr, s_hist, s_state, s_wmax, s_cand, s_surv, s_deep_m, s_hits, s_cut, s_grecv, s_vblk, s_trace_state, s_trace_data, s_hash, scratch_bytes;
   size_t rec_bytes, o_merged, o_ghdr, o_final, out_bytes;
   std::vector<std::vector<DHKey>> h_keys;  // per hashed split: the used cells, copied back
   std::vector<std::vector<QwAggCell>> h_cells;
@@ -1219,8 +1224,9 @@ struct Run {
     plans.resize(n);
     bounds_base.resize(n);
     at.assign(n, Split{});
-    any_topk = any_trace = any_hashed = any_composite = any_fast_aggs = false;
+    any_topk = any_deep = any_trace = any_hashed = any_composite = any_fast_aggs = false;
     kmax = 1;
+    deep_cap = 0;
     n_phrases = phrase_blocks = tie_max_n = 0;
     n_phrase_exp = 0;
   h_keys.assign(n, {});
@@ -1247,6 +1253,7 @@ struct Run {
       n_phrase_exp += L.phrase_exp.size();
       kmax = std::max(kmax, P.max_hits);
       any_topk |= P.max_hits > 0;
+      if (P.max_hits > QW_MAX_TOPK) { any_deep = true; deep_cap = std::max(deep_cap, qw_cand_cap(P.max_hits)); }
       any_trace |= P.tr_on != 0;
     }
     Arena blob{256};
@@ -1270,7 +1277,13 @@ struct Run {
     s_hist = s.take((size_t)n * QW_HIST_BINS * 4);
     s_state = s.take((size_t)n * 4);
     s_wmax = s.take(r.rec_l0 ? (size_t)r.fw_all[n] * 2 : 0);
-    s_cand = s.take(any_topk ? (size_t)n * QW_CAND_CAP * 24 : 0);
+    // candidate lists: qw_cand_cap(K) keys of 24 bytes per split; with a deep plan in the batch, the survivor arrays
+    // of the deep selection path mirror them (same offsets from s_surv; used by the deep splits only)
+    size_t cand_bytes = 0;
+    for (uint32_t i = 0; i < n; i++) { at[i].cand = cand_bytes; cand_bytes += any_topk ? (size_t)qw_cand_cap(plans[i].max_hits) * 24 : 0; }
+    s_cand = s.take(cand_bytes);
+    s_surv = s.take(any_deep ? cand_bytes : 0);
+    s_deep_m = s.take(any_deep ? (size_t)n * 4 : 0);
     s_hits = s.take(do_merge ? (size_t)n * kmax * sizeof(QwHit) : 0);
     s_cut = s.take((size_t)std::max<uint32_t>(n, 64) * 4 + 1024);  // split merge's cut, then the gathered merge's
     s_grecv = s.take(gather && gather->world > 1 && do_merge ? (size_t)gather->world * rec_bytes : 0);
@@ -1353,7 +1366,7 @@ struct Run {
       P.out_hits = do_merge ? (uint64_t)(slot.d_scratch + s_hits + (size_t)i * kmax * sizeof(QwHit)) : (uint64_t)(ob + 32);
       P.out_cells = (uint64_t)(ob + 32 + out_hit_bytes(P, do_merge));
       P.out_hist = (uint64_t)(slot.d_scratch + s_hist + (size_t)i * QW_HIST_BINS * 4);
-      P.out_cands = (uint64_t)(slot.d_scratch + s_cand + (size_t)i * QW_CAND_CAP * 24);
+      P.out_cands = (uint64_t)(slot.d_scratch + s_cand + at[i].cand);
       if (P.tr_on) {
         P.tr_state = (uint64_t)(slot.d_scratch + s_trace_state + (size_t)i * sizeof(qwk::DTraceState));
         P.tr_best = (uint64_t)(slot.d_scratch + at[i].tr_best);
@@ -1519,6 +1532,16 @@ struct Run {
     }
     const uint32_t sel_smem = 3 * 8 * QW_CAND_CAP;  // [all first words | 3 x QW_SEL_MAX survivors] or 3 x all (degenerate ties)
     if (any_topk) { qwk::k_select<<<n, 1024, sel_smem, st>>>(kp.plans, kp.cols); stats.launches++; }
+    if (any_deep) {
+      // splits with K > QW_MAX_TOPK (k_select left them): cut, tile sort, rank (deep_select_kernel.cuh)
+      uint32_t* d_m = (uint32_t*)(slot.d_scratch + s_deep_m);
+      const size_t surv_off = s_surv - s_cand;
+      qwk::k_deep_cut<<<n, 1024, 0, st>>>(kp.plans, surv_off, d_m);
+      qwk::k_deep_sort<<<dim3((deep_cap + QD_TILE - 1) / QD_TILE, n), 1024, 3 * 8 * QD_TILE, st>>>(kp.plans, surv_off, d_m);
+      qwk::k_deep_rank<<<dim3(deep_cap / 256, n), 256, 0, st>>>(kp.plans, kp.cols, surv_off, d_m);
+      stats.launches += 3;
+      stats.kernel_mask |= QWGPU_KERNEL_DEEP_SELECT;
+    }
     if (do_merge) {
       uint32_t* d_cut = (uint32_t*)(slot.d_scratch + s_cut);
       const qwk::SrcSplits src{kp.plans, (const uint32_t*)(slot.d_blob + o_rank), do_gather ? 1u : 0u};
@@ -1543,13 +1566,13 @@ struct Run {
       if (low[i].P.max_hits == 0) continue;
       const uint8_t* ob = slot.h_out + at[i].out;
       const uint64_t eligible = ((const uint64_t*)ob)[1], cand = *(const uint32_t*)(ob + 20);
-      if (cand > QW_CAND_CAP || cand < std::min<uint64_t>(low[i].P.max_hits, eligible)) { state[i] = 1; all = false; }
+      if (cand > qw_cand_cap(low[i].P.max_hits) || cand < std::min<uint64_t>(low[i].P.max_hits, eligible)) { state[i] = 1; all = false; }
     }
     return all;
   }
 
   // exact radix select over the composite key: one histogram pass per 11-bit digit until the
-  // candidate set of every split fits QW_CAND_CAP. After a failed sampled threshold with the
+  // candidate set of every split fits its capacity (qw_cand_cap). After a failed sampled threshold with the
   // level-0 histogram on record (refine), level 0 needs no pass at all, only the failing splits are
   // revisited, and windows whose best digit is below the threshold digit are skipped.
   void exact_select(bool refine, std::vector<uint32_t>& state) {
@@ -1676,14 +1699,15 @@ struct Run {
 // Lowers every plan once per call; a split whose plan cannot be lowered fails alone. idx: position of each lowered
 // plan in the caller's arrays.
 static std::vector<Lowered> lower_batch(const std::vector<std::shared_ptr<SplitDev>>& sp, const std::vector<const uint8_t*>& plans,
-                                        const std::vector<size_t>& plan_lens, std::vector<SplitOutput>& outs, std::vector<uint32_t>& idx) {
+                                        const std::vector<size_t>& plan_lens, std::vector<SplitOutput>& outs, std::vector<uint32_t>& idx,
+                                        uint32_t max_hits) {
   std::vector<Lowered> low;
   low.reserve(sp.size());
   for (uint32_t i = 0; i < (uint32_t)sp.size(); i++) {
     try {
       if (!sp[i]) fail(QWGPU_ENOTFOUND, "split not registered");
       Lowered L;
-      lower_plan(L, *sp[i], plans[i], plan_lens[i]);
+      lower_plan(L, *sp[i], plans[i], plan_lens[i], max_hits);
       low.push_back(std::move(L));
       idx.push_back(i);
     } catch (const Error& e) {
@@ -1838,7 +1862,7 @@ void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std:
   const auto t_begin = tclock::now();
   CUDA_CHECK(cudaSetDevice(device));
   std::vector<uint32_t> idx;
-  const std::vector<Lowered> low = lower_batch(sp, plans, plan_lens, outs, idx);
+  const std::vector<Lowered> low = lower_batch(sp, plans, plan_lens, outs, idx, max_hits.load(std::memory_order_relaxed));
   const bool gathering = merge && merged && merge->k > 0 && gather && gather->allgather && gather->world > 1 && rank_headers;
   if (low.empty()) {
     if (gathering) exchange_empty(*this, *merge, *gather, *merged, *rank_headers);

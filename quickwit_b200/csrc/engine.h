@@ -99,6 +99,9 @@ struct Engine {
   // splits local and drops cold ones). Uploads can run in the background (register_split_async): `find` waits
   // for a split that is still loading.
   uint64_t budget = 0, tick = 0, evictions = 0;
+  // largest max_hits + start_offset a plan may ask for (qwgpu_set_max_hits): QW_MAX_TOPK unless the caller raised it,
+  // up to QW_MAX_HITS. Above QW_MAX_TOPK a call needs call-slot scratch that grows with K and stays allocated.
+  std::atomic<uint32_t> max_hits{4096};  // (QW_MAX_TOPK)
   std::condition_variable loaded_cv;
   struct Loader { std::thread t; std::shared_ptr<SplitDev> sp; };
   std::vector<Loader> loaders;

@@ -1344,7 +1344,7 @@ __global__ void __launch_bounds__(QW_THREADS, QW_MIN_BLOCKS_PER_SM) k_window(con
       if (!p.cands_only) for (uint32_t wd = tid; wd < NW; wd += QW_THREADS) my_hits += __popc(res[wd]);
       auto emit = [&](const Key& k) {
         const uint32_t pos = atomicAdd((uint32_t*)P.out_cand_count, 1u);
-        if (pos < QW_CAND_CAP) {
+        if (pos < qw_cand_cap(P.max_hits)) {
           uint64_t* c = (uint64_t*)P.out_cands + 3ull * pos;
           c[0] = k.w0; c[1] = k.w1; c[2] = k.w2;
         }
@@ -1578,9 +1578,52 @@ __global__ void __launch_bounds__(256) k_pick(const DSplitPlan* plans, DThresh* 
     else {
       T.above = base_above + s_sel[1];
       T.matched = h[digit];
-      T.done = (T.above + T.matched <= QW_CAND_CAP) ? 1 : 0;
+      T.done = (T.above + T.matched <= qw_cand_cap(K)) ? 1 : 0;
     }
   }
+}
+
+// Decodes a composite key back to the split's hit record at position i of its list: a QwHit, or the (doc id, score)
+// pair where P.score_hits (k_select and the deep selection path, deep_select_kernel.cuh).
+__device__ __forceinline__ void write_hit(const DSplitPlan& P, const DCol* cols, const Key& k, uint32_t i) {
+  const DKeySpec& ks = P.key;
+  const uint32_t docmask = ks.doc_bits >= 32 ? 0xFFFFFFFFu : ((1u << ks.doc_bits) - 1);
+  uint32_t pos = 0, has[2];
+  uint64_t r[2];
+#pragma unroll
+  for (int f = 0; f < 2; f++) {
+    has[f] = ks.hasbit[f] ? (uint32_t)key_get(k, pos, 1) : 0u;
+    pos += ks.hasbit[f];
+    r[f] = key_get(k, pos, ks.rbits[f]);
+    pos += ks.rbits[f];
+  }
+  const uint32_t docr = (uint32_t)key_get(k, pos, ks.doc_bits);
+  QwHit hh;
+  hh.doc_id = ks.order[0] == QW_ORDER_DESC ? docr : docmask - docr;
+  hh.flags = has[0] | (has[1] << 1);
+  hh.score = 0.0f;
+  hh.reserved = 0;
+  uint64_t v[2] = {0, 0};
+#pragma unroll
+  for (int f = 0; f < 2; f++) {
+    if (!has[f]) continue;
+    const bool desc = ks.order[f] == QW_ORDER_DESC;
+    if (ks.kind[f] == QW_SORT_SCORE) {
+      uint32_t o = (uint32_t)r[f];
+      if (!desc) o = ~o;
+      const uint32_t bits = (o & 0x80000000u) ? (o & 0x7FFFFFFFu) : ~o;
+      hh.score = __uint_as_float(bits);
+      v[f] = f64_to_u64_dev((double)hh.score);
+    } else {
+      const DCol& c = cols[ks.col[f]];
+      v[f] = c.min_value + c.gcd * (desc ? r[f] : ks.raw_max[f] - r[f]);
+    }
+  }
+  hh.v1 = v[0];
+  hh.v2 = v[1];
+  QwHit* hits = (QwHit*)P.out_hits;
+  if (P.score_hits) reinterpret_cast<QwScoreHit*>(hits)[i] = QwScoreHit{hh.doc_id, hh.score};
+  else hits[i] = hh;
 }
 
 // Harvest (quickwit-search/src/top_k_collector.rs:404-410, binary_heap.rs:187-193): the best
@@ -1593,6 +1636,7 @@ __global__ void __launch_bounds__(1024) k_select(const DSplitPlan* plans, const 
   const DSplitPlan& P = plans[blockIdx.x];
   const uint32_t tid = threadIdx.x;
   if (P.max_hits == 0) { if (tid == 0) *(uint32_t*)P.out_nhits = 0; return; }
+  if (P.max_hits > QW_MAX_TOPK) return;  // the deep selection path's split (deep_select_kernel.cuh)
   uint32_t n = *(const uint32_t*)P.out_cand_count;
   if (n > QW_CAND_CAP) n = QW_CAND_CAP;  // overflow is detected by the host (cand_count > cap)
   const uint32_t K = P.max_hits;
@@ -1745,48 +1789,8 @@ __global__ void __launch_bounds__(1024) k_select(const DSplitPlan* plans, const 
     }
   }
   const uint32_t out_n = m < K ? m : K;
-  QwHit* hits = (QwHit*)P.out_hits;
-  const DKeySpec& ks = P.key;
   const DCol* cols = all_cols + P.col_base;
-  const uint32_t docmask = ks.doc_bits >= 32 ? 0xFFFFFFFFu : ((1u << ks.doc_bits) - 1);
-  for (uint32_t i = tid; i < out_n; i += 1024) {
-    const Key k{k0[i], k1[i], k2[i]};
-    uint32_t pos = 0, has[2];
-    uint64_t r[2];
-#pragma unroll
-    for (int f = 0; f < 2; f++) {
-      has[f] = ks.hasbit[f] ? (uint32_t)key_get(k, pos, 1) : 0u;
-      pos += ks.hasbit[f];
-      r[f] = key_get(k, pos, ks.rbits[f]);
-      pos += ks.rbits[f];
-    }
-    const uint32_t docr = (uint32_t)key_get(k, pos, ks.doc_bits);
-    QwHit hh;
-    hh.doc_id = ks.order[0] == QW_ORDER_DESC ? docr : docmask - docr;
-    hh.flags = has[0] | (has[1] << 1);
-    hh.score = 0.0f;
-    hh.reserved = 0;
-    uint64_t v[2] = {0, 0};
-#pragma unroll
-    for (int f = 0; f < 2; f++) {
-      if (!has[f]) continue;
-      const bool desc = ks.order[f] == QW_ORDER_DESC;
-      if (ks.kind[f] == QW_SORT_SCORE) {
-        uint32_t o = (uint32_t)r[f];
-        if (!desc) o = ~o;
-        const uint32_t bits = (o & 0x80000000u) ? (o & 0x7FFFFFFFu) : ~o;
-        hh.score = __uint_as_float(bits);
-        v[f] = f64_to_u64_dev((double)hh.score);
-      } else {
-        const DCol& c = cols[ks.col[f]];
-        v[f] = c.min_value + c.gcd * (desc ? r[f] : ks.raw_max[f] - r[f]);
-      }
-    }
-    hh.v1 = v[0];
-    hh.v2 = v[1];
-    if (P.score_hits) reinterpret_cast<QwScoreHit*>(hits)[i] = QwScoreHit{hh.doc_id, hh.score};
-    else hits[i] = hh;
-  }
+  for (uint32_t i = tid; i < out_n; i += 1024) write_hit(P, cols, Key{k0[i], k1[i], k2[i]}, i);
   if (tid == 0) *(uint32_t*)P.out_nhits = out_n;
 }
 

@@ -133,7 +133,7 @@ __device__ __noinline__ void union_emit(const DSplitPlan* plans, const DThresh* 
   const DocKey dk = doc_key(P, P.key, cols + P.col_base, (const uint8_t*)P.data_base, doc, sc);
   if (key_ge(dk.key, thr)) {
     const uint32_t pos = atomicAdd((uint32_t*)P.out_cand_count, 1u);
-    if (pos < QW_CAND_CAP) {
+    if (pos < qw_cand_cap(P.max_hits)) {
       uint64_t* c = (uint64_t*)P.out_cands + 3ull * pos;
       c[0] = dk.key.w0; c[1] = dk.key.w1; c[2] = dk.key.w2;
     }
@@ -416,7 +416,7 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
         if (lane == 0) basepos = atomicAdd((uint32_t*)P.out_cand_count, (uint32_t)__popc(m));
         basepos = __shfl_sync(QW_FULL, basepos, 0);
         const uint32_t pos = basepos + __popc(m & ((1u << lane) - 1u));
-        if (pass && pos < QW_CAND_CAP) {
+        if (pass && pos < qw_cand_cap(P.max_hits)) {
           uint64_t* c = (uint64_t*)P.out_cands + 3ull * pos;
           c[0] = dk.key.w0; c[1] = dk.key.w1; c[2] = dk.key.w2;
         }

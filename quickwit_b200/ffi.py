@@ -32,6 +32,7 @@ ABSENT = 0xFFFFFFFF
 KERNEL_UNION, KERNEL_DRIVER, KERNEL_AGGSCAN, KERNEL_WINDOW, KERNEL_PHRASE = 1, 2, 4, 8, 16
 KERNEL_TRACE_SELECT, KERNEL_TRACE_REPLAY, KERNEL_FAST_AGGS = 32, 64, 128
 KERNEL_HASHED_AGGS, KERNEL_HASHED_AGGS_RETRY, KERNEL_COMPOSITE_CUT = 256, 512, 1024
+KERNEL_DEEP_SELECT = 2048
 # hashed aggregation cells (qwgpu_format.h qw_agg_hashed, qwgpu.h): dense-layout limits, the initial capacity of a
 # split's table, the largest table a split may need, the `missing` flag of an entry
 AGG_DENSE_MAX_CELLS, AGG_DENSE_MAX_TERMS = 1 << 26, 1 << 24
@@ -195,6 +196,7 @@ def lib() -> C.CDLL:
     bind("qwgpu_split_unregister", [vp, cp])
     bind("qwgpu_resident_bytes", [vp], u64)
     bind("qwgpu_set_residency_budget", [vp, u64])
+    bind("qwgpu_set_max_hits", [vp, C.c_uint32])
     bind("qwgpu_split_register_async", [vp, cp, vp, u64])
     bind("qwgpu_split_wait", [vp, cp])
     bind("qwgpu_residency_info", [vp, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)])

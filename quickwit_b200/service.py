@@ -90,6 +90,10 @@ class SearcherContext:
         """Cap on the split data kept in HBM; registrations beyond it evict the least recently searched splits."""
         ffi.check(self._L.qwgpu_set_residency_budget(self._ctx, nbytes))
 
+    def set_max_hits(self, max_hits: int):
+        """Largest max_hits + start_offset this context serves (1 .. 20 000; 4096 until set)."""
+        ffi.check(self._L.qwgpu_set_max_hits(self._ctx, max_hits))
+
     def register_split_async(self, img: SplitImage, split_id: Optional[str] = None):
         """Background upload; `img` must stay alive until wait_split() has returned."""
         ffi.check(self._L.qwgpu_split_register_async(self._ctx, (split_id or img.split_id).encode(), img.ptr, img.nbytes))
