@@ -32,6 +32,29 @@
 // memory), above that 2K rounded up to a multiple of 1024 (the deep selection path, deep_select_kernel.cuh).
 QW_HOST_DEVICE uint32_t qw_cand_cap(uint32_t K) { return K <= QW_MAX_TOPK ? (uint32_t)QW_CAND_CAP : (2u * K + 1023u) & ~1023u; }
 
+// First work item of block b of a `grid`-block persistent launch over `total` items: block b walks the contiguous
+// chunk [qw_chunk_begin(total, b, grid), qw_chunk_begin(total, b + 1, grid)).
+QW_HOST_DEVICE uint32_t qw_chunk_begin(uint32_t total, uint32_t b, uint32_t grid) { return (uint32_t)(((uint64_t)total * b) / grid); }
+
+// The threshold sample of a BM25-union collect pass that samples itself (k_union<MODE_SAMPLE_COLLECT>): the first
+// window of every block's chunk of the flat window list. first_work: prefix over the n splits of their windows
+// ([n + 1]); max_hits: per split. True when the pass may run: at least 4 windows per block, and every split that
+// has windows and asks for hits holds the first window of at least one block. Then stride[s] =
+// max(1, floor(windows_s / samples_s)) is the weight of split s's sample (rounded down: a more conservative threshold).
+static inline bool qw_fused_sample_plan(const uint32_t* first_work, const uint32_t* max_hits, uint32_t n, uint32_t grid, uint32_t* stride) {
+  const uint32_t total = first_work[n];
+  if (grid == 0 || total < 4ull * grid) return false;
+  uint32_t b = 0;
+  for (uint32_t s = 0; s < n; s++) {
+    const uint32_t windows = first_work[s + 1] - first_work[s];
+    uint32_t samples = 0;
+    for (; b < grid && qw_chunk_begin(total, b, grid) < first_work[s + 1]; b++) samples++;
+    if (windows && max_hits[s] && !samples) return false;
+    stride[s] = samples ? (windows / samples > 1 ? windows / samples : 1u) : 1u;
+  }
+  return true;
+}
+
 enum { OP_TERM = 1, OP_RANGE = 2, OP_EXISTS = 3, OP_ALL = 4, OP_BOOL_BEGIN = 5, OP_BOOL_END = 6, OP_PHRASE = 7 };
 enum { IF_SCORED = 1u, IF_HAS_TF = 2u, IF_HAS_FN = 4u, IF_BITS_FROM_SCORE = 8u };
 #define QW_TFF_ROWS 16 /* tf-factor table: tff[tf][fieldnorm_id] = tf / (tf + norm[id]) for tf < 16 */

@@ -103,6 +103,10 @@ Engine::Engine(int dev) : device(dev) {
   CUDA_CHECK(cudaFuncSetAttribute(qwk::k_window<qwk::MODE_COLLECT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem_optin));
   CUDA_CHECK(cudaFuncSetAttribute(qwk::k_union<qwk::MODE_HIST>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem_optin));
   CUDA_CHECK(cudaFuncSetAttribute(qwk::k_union<qwk::MODE_COLLECT>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem_optin));
+  CUDA_CHECK(cudaFuncSetAttribute(qwk::k_union<qwk::MODE_SAMPLE_COLLECT>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem_optin));
+  int coop = 0;
+  CUDA_CHECK(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
+  coop_launch = coop != 0;
   CUDA_CHECK(cudaFuncSetAttribute(qwk::k_aggscan, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem_optin));
   CUDA_CHECK(cudaFuncSetAttribute(qwk::k_select, cudaFuncAttributeMaxDynamicSharedMemorySize, 3 * 8 * QW_CAND_CAP));
   CUDA_CHECK(cudaFuncSetAttribute(qwk::k_trace_replay, cudaFuncAttributeMaxDynamicSharedMemorySize, trace_replay_smem(QW_MAX_TOPK)));
@@ -920,8 +924,9 @@ static SmemLayout make_layout(uint32_t W, uint32_t n_levels, uint32_t need_cnt, 
 }
 
 // shared-memory arena of the BM25-union pipeline (union_kernel.cuh): score array, QU_SLOTS staging slots
-// (block payload + records + per-term table + header), mbarriers, MODE_HIST histogram
-static qwk::USmem make_union_layout(uint32_t W, bool hist, uint32_t budget) {
+// (block payload + records + per-term table + header), mbarriers, MODE_HIST histogram, MODE_SAMPLE_COLLECT thresholds
+// (its sample histogram takes a held slot's payload)
+static qwk::USmem make_union_layout(uint32_t W, bool hist, bool sample, uint32_t budget) {
   qwk::USmem L;
   memset(&L, 0, sizeof L);
   Arena a{16};
@@ -929,6 +934,7 @@ static qwk::USmem make_union_layout(uint32_t W, bool hist, uint32_t budget) {
   L.bars = a.take(8 * (2 * QU_SLOTS + QU_CHAIN));
   if (hist) L.hist = a.take(QW_HIST_BINS * 4);
   L.cands = a.take(QU_NCW * QU_CANDS * 8 + QU_NCW * 4);
+  if (sample) L.thr = a.take(2 * sizeof(DThresh) + 2 * 4 + 2 * 4);
   const uint32_t off = (uint32_t)a.off, fixed = QU_MAXBLK * 16 + QU_MAX_TERMS * 16 + 32 + QU_PAD;
   const uint32_t cap = budget > off + QU_SLOTS * (fixed + 2048) ? ((budget - off) / QU_SLOTS - fixed) & ~15u : 2048;
   L.cap = cap;
@@ -1003,7 +1009,7 @@ struct Route {
   bool edge_sample = false;  // the sample is the explicit list `sample_win`: strided windows + each split's first and last
   bool rec_l0 = false;       // the collect pass records the exact level-0 histogram (second-chance top-K)
   SmemLayout lay;             // k_window
-  qwk::USmem ulay_c, ulay_h;  // k_union collect / histogram
+  qwk::USmem ulay_c, ulay_h, ulay_s;  // k_union collect / histogram / collect with its own sample
   qwk::ASmem alay;            // k_aggscan
   // prefix sums over splits: windows, sampled windows; driver: posting blocks, sampled blocks ([n + 1] or empty)
   std::vector<uint32_t> fw_all, fw_smp, fw_drv, fw_dsm, sample_win;  // sample_win: window | edge << 31 per work item
@@ -1115,8 +1121,9 @@ static Route choose_route(const std::vector<Lowered>& low, int max_smem_optin, i
   if (r.kind == Route::UNION) {
     // (the generic layout above stays valid for the same W: exact radix passes below level 0 use k_window)
     const uint32_t u_budget = (uint32_t)(max_smem_optin + 1024) / QU_MINB - 1024 - 64;
-    r.ulay_c = make_union_layout(r.W, false, u_budget);
-    r.ulay_h = make_union_layout(r.W, true, u_budget);
+    r.ulay_c = make_union_layout(r.W, false, false, u_budget);
+    r.ulay_h = make_union_layout(r.W, true, false, u_budget);
+    r.ulay_s = make_union_layout(r.W, false, true, u_budget);
   }
   plan_sample(r, low, sm_count);
   return r;
@@ -1180,7 +1187,9 @@ static void wait_call(Engine& e, CallSlot& slot) {
   } else CUDA_CHECK(cudaStreamSynchronize(slot.stream));
 }
 
-enum { F_REC = 1, F_REFINE = 2, F_CANDS_ONLY = 4 };  // collect / histogram pass flags
+// collect / histogram pass flags; F_SAMPLE: a BM25-union collect pass that samples its own threshold
+// (k_union<MODE_SAMPLE_COLLECT>, launched cooperatively)
+enum { F_REC = 1, F_REFINE = 2, F_CANDS_ONLY = 4, F_SAMPLE = 8 };
 
 // bytes of a split's hit list in its output region (a merged batch keeps the lists in scratch)
 static size_t out_hit_bytes(const DSplitPlan& P, bool do_merge) {
@@ -1209,9 +1218,13 @@ struct Run {
   bool any_topk, any_deep, any_trace, any_hashed, any_composite, any_fast_aggs;
   uint32_t kmax, deep_cap, n_phrases, phrase_blocks, tie_max_n;
   size_t n_phrase_exp;
-  size_t o_plans, o_instr, o_cols, o_aggs, o_fwa, o_fws, o_bounds, o_rank, o_smp, o_phr, o_pexp, o_fwd, o_fwds, blob_bytes;
-  size_t s_thr, s_hist, s_state, s_wmax, s_cand, s_surv, s_deep_m, s_hits, s_cut, s_grecv, s_vblk, s_trace_state, s_trace_data, s_hash, scratch_bytes;
-  size_t rec_bytes, o_merged, o_ghdr, o_final, out_bytes;
+  size_t o_plans, o_instr, o_cols, o_aggs, o_fwa, o_fws, o_sstr, o_bounds, o_rank, o_smp, o_phr, o_pexp, o_fwd, o_fwds, blob_bytes;
+  size_t s_thr, s_hist, s_state, s_wmax, s_sync, s_cand, s_surv, s_deep_m, s_hits, s_cut, s_grecv, s_vblk, s_trace_state, s_trace_data, s_hash, scratch_bytes;
+  size_t rec_bytes, o_merged, o_ghdr, o_final, o_err, out_bytes;
+  // the collect pass samples its own threshold (qw_fused_sample_plan): its cooperative grid and per-split sample weights
+  bool self_sample;
+  uint32_t sample_grid;
+  std::vector<uint32_t> sample_stride;
   std::vector<std::vector<DHKey>> h_keys;  // per hashed split: the used cells, copied back
   std::vector<std::vector<QwAggCell>> h_cells;
   KParams kp;
@@ -1256,6 +1269,20 @@ struct Run {
       if (P.max_hits > QW_MAX_TOPK) { any_deep = true; deep_cap = std::max(deep_cap, qw_cand_cap(P.max_hits)); }
       any_trace |= P.tr_on != 0;
     }
+    // BM25-union top-K calls sample the threshold inside the collect pass when the batch qualifies. Cross-rank calls
+    // keep the two-launch path: their cooperative grid could queue behind another lane's NCCL kernel that is itself
+    // waiting on a peer rank.
+    self_sample = false;
+    sample_grid = 0;
+    if (r.kind == Route::UNION && any_topk && !any_deep && !do_gather && e.coop_launch && r.ulay_s.cap >= QW_HIST_BINS * 4 + 64) {
+      int uocc = 0;
+      CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&uocc, qwk::k_union<qwk::MODE_SAMPLE_COLLECT>, QU_THREADS, r.ulay_s.total));
+      std::vector<uint32_t> mh(n);
+      for (uint32_t i = 0; i < n; i++) mh[i] = plans[i].max_hits;
+      sample_grid = (uint32_t)(e.sm_count * std::max(uocc, 0));
+      sample_stride.assign(n, 1);
+      self_sample = qw_fused_sample_plan(r.fw_all.data(), mh.data(), n, sample_grid, sample_stride.data());
+    }
     Arena blob{256};
     o_plans = blob.take(n * sizeof(DSplitPlan));
     o_instr = blob.take(tot_instr * sizeof(DInstr));
@@ -1263,6 +1290,7 @@ struct Run {
     o_aggs = blob.take(std::max(tot_aggs, 1u) * sizeof(DAgg));
     o_fwa = blob.take((n + 1) * 4);
     o_fws = blob.take((n + 1) * 4);
+    o_sstr = blob.take(self_sample ? (size_t)n * 4 : 0);
     o_bounds = blob.take((size_t)tot_bounds * 8);
     o_rank = blob.take((size_t)n * 4);
     o_smp = blob.take(r.sample_win.size() * 4);
@@ -1277,6 +1305,7 @@ struct Run {
     s_hist = s.take((size_t)n * QW_HIST_BINS * 4);
     s_state = s.take((size_t)n * 4);
     s_wmax = s.take(r.rec_l0 ? (size_t)r.fw_all[n] * 2 : 0);
+    s_sync = s.take(self_sample ? 4 : 0);  // the grid barrier's counter (zeroed with the prefix below s_cand)
     // candidate lists: qw_cand_cap(K) keys of 24 bytes per split; with a deep plan in the batch, the survivor arrays
     // of the deep selection path mirror them (same offsets from s_surv; used by the deep splits only)
     size_t cand_bytes = 0;
@@ -1315,6 +1344,7 @@ struct Run {
       o_ghdr = o.take((size_t)gather->world * 64);  // (compacted copy of the gathered headers)
       o_final = o.take(16 + (size_t)merge->k * sizeof(qwk::DMergedHit));
     }
+    o_err = o.take(self_sample ? 4 : 0);  // 1: the grid barrier timed out
     out_bytes = o.off;
   }
 
@@ -1408,6 +1438,7 @@ struct Run {
     if (!r.fw_drv.empty()) { memcpy(hb + o_fwd, r.fw_drv.data(), (n + 1) * 4); memcpy(hb + o_fwds, r.fw_dsm.data(), (n + 1) * 4); }
     memcpy(hb + o_fwa, r.fw_all.data(), (n + 1) * 4);
     memcpy(hb + o_fws, r.fw_smp.data(), (n + 1) * 4);
+    if (self_sample) memcpy(hb + o_sstr, sample_stride.data(), (size_t)n * 4);
     CUDA_CHECK(cudaMemcpyAsync(db, hb, blob_bytes, cudaMemcpyHostToDevice, st));
     stats.h2d_bytes += blob_bytes;
 
@@ -1434,7 +1465,7 @@ struct Run {
 
   // one pass over the batch on the route's kernel when it serves the pass, else on k_window
   void launch(int mode, bool sampled, uint32_t level, uint32_t use_prefix, uint32_t flags) {
-    const Route::Kind kind = r.serves(mode, level, use_prefix, flags) ? r.kind : Route::WINDOW;
+    const Route::Kind kind = (flags & F_SAMPLE) || r.serves(mode, level, use_prefix, flags) ? r.kind : Route::WINDOW;
     const uint32_t stride = sampled ? r.stride : 1;
     auto launched = [&](uint32_t kernel) { stats.launches++; stats.kernel_mask |= kernel; };
     if (kind == Route::DRIVER) {
@@ -1473,7 +1504,17 @@ struct Run {
       // memory, a concurrent call's NCCL kernel would take the place of one of its blocks, and that block — with its
       // static share of the windows — would only start when another one has finished (twice the kernel time)
       const uint32_t ugrid = std::min<uint32_t>(total_work, (uint32_t)(e.sm_count * QU_MINB) - (do_gather ? 4u : 0u));
-      if (mode == qwk::MODE_HIST) qwk::k_union<qwk::MODE_HIST><<<ugrid, QU_THREADS, u.sm.total, st>>>(u);
+      if (flags & F_SAMPLE) {
+        // one block per resident slot (occupancy x SMs, checked by qw_fused_sample_plan against the work): the grid
+        // barrier after the sample needs every block resident, which only a cooperative launch guarantees
+        u.sm = r.ulay_s;
+        u.sample_stride = (const uint32_t*)(slot.d_blob + o_sstr);
+        u.sync = (uint32_t*)(slot.d_scratch + s_sync);
+        u.err = (uint32_t*)(slot.d_out + o_err);
+        void* args[] = {&u};
+        CUDA_CHECK(cudaLaunchCooperativeKernel((const void*)qwk::k_union<qwk::MODE_SAMPLE_COLLECT>, dim3(sample_grid), dim3(QU_THREADS), args,
+                                               u.sm.total, st));
+      } else if (mode == qwk::MODE_HIST) qwk::k_union<qwk::MODE_HIST><<<ugrid, QU_THREADS, u.sm.total, st>>>(u);
       else qwk::k_union<qwk::MODE_COLLECT><<<ugrid, QU_THREADS, u.sm.total, st>>>(u);
       launched(QWGPU_KERNEL_UNION);
       return;
@@ -1643,14 +1684,23 @@ struct Run {
     stats.window_docs = r.kind == Route::DRIVER ? QW_BLOCK_LEN : r.W;
     std::vector<uint32_t> state(n, 0);  // per split: 1 = its sampled threshold failed
     bool ok = true;
-    if (any_topk && r.stride > 1) {
-      // fast path: threshold from a 1/stride sample of the windows, verified after the collect pass
-      stats.sample_stride = r.stride;
-      launch(qwk::MODE_HIST, true, 0, 0, 0);
-      qwk::k_pick<<<n, 256, 0, st>>>(kp.plans, kp.thresh, 0, r.edge_sample ? 2 : 1, r.stride, nullptr);
-      stats.launches++;
-      if (r.rec_l0) CUDA_CHECK(cudaMemsetAsync(slot.d_scratch + s_hist, 0, (size_t)n * QW_HIST_BINS * 4, st));
-      collect(r.rec_l0 ? F_REC : 0);
+    const bool sampled = self_sample || (any_topk && r.stride > 1);
+    if (sampled) {
+      if (self_sample) {
+        // fast path in one pass: the collect pass takes each block's first window as the threshold sample
+        stats.sample_stride = r.fw_all[n] / sample_grid;
+        collect(F_SAMPLE);
+        if (*(const uint32_t*)(slot.h_out + o_err)) fail(QWGPU_EINTERNAL, "k_union: the grid barrier after the threshold sample timed out");
+      } else {
+        // fast path: threshold from a 1/stride sample of the windows
+        stats.sample_stride = r.stride;
+        launch(qwk::MODE_HIST, true, 0, 0, 0);
+        qwk::k_pick<<<n, 256, 0, st>>>(kp.plans, kp.thresh, 0, r.edge_sample ? 2 : 1, r.stride, nullptr);
+        stats.launches++;
+        if (r.rec_l0) CUDA_CHECK(cudaMemsetAsync(slot.d_scratch + s_hist, 0, (size_t)n * QW_HIST_BINS * 4, st));
+        collect(r.rec_l0 ? F_REC : 0);
+      }
+      // verified after the collect pass
       ok = verify(state);
       if (!ok) {
         add_device_time();
@@ -1659,7 +1709,7 @@ struct Run {
       }
     }
     if (!any_topk) collect(0);
-    else if (r.stride == 1 || !ok) exact_select(!ok && r.rec_l0, state);
+    else if (!sampled || !ok) exact_select(!ok && r.rec_l0, state);
     // hashed cells: a split that outgrew its capacity sends the batch round again at the bound (before any
     // cross-rank collective, which must run once); otherwise only the used cells come back
     auto used = [&](uint32_t i) { return *(const uint32_t*)(slot.h_out + at[i].out + 28); };

@@ -107,6 +107,7 @@ struct Engine {
   std::vector<Loader> loaders;
   int sm_count = 0;  // set from cudaDeviceProp in Engine::Engine
   int max_smem_optin = 0;
+  bool coop_launch = false;  // cudaDevAttrCooperativeLaunch: k_union may sample its own threshold (grid barrier)
 
   explicit Engine(int dev);
   ~Engine();

@@ -810,7 +810,8 @@ __device__ __forceinline__ void agg_collect_hashed(const DSplitPlan& P, const DA
   }
 }
 
-enum { MODE_HIST = 0, MODE_COLLECT = 1 };
+// MODE_SAMPLE_COLLECT (k_union only): a collect pass that samples its own threshold from each block's first window
+enum { MODE_HIST = 0, MODE_COLLECT = 1, MODE_SAMPLE_COLLECT = 2 };
 
 // ---- warp-private helpers (each warp owns the doc sub-range [lo, lo + S) of the window) ------------
 __device__ __forceinline__ void wzero_u32(uint32_t* p, uint32_t first, uint32_t n, uint32_t lane) {
@@ -1505,38 +1506,39 @@ __global__ void __launch_bounds__(QW_THREADS, QW_MIN_BLOCKS_PER_SM) k_window(con
   }
 }
 
+__device__ __forceinline__ void pick_sync(uint32_t bar, uint32_t nt) {
+  if (bar == 0) __syncthreads();
+  else asm volatile("bar.sync %0, %1;" ::"r"(bar), "r"(nt) : "memory");
+}
+
 // Picks the radix digit of the top-K threshold from a split's histogram.
 //   sampled != 0: histogram comes from every `stride`-th window; pick the digit at a conservative
 //                 sample rank `k_sample` (verified afterwards against the true candidate count).
 //   sampled == 0: exact radix-select step at `level` (prefix / above bookkeeping in DThresh).
-//   split_state != null: only splits flagged for refinement are touched, and their candidate
-//                 counters are reset for the candidates-only collect pass that follows.
-__global__ void __launch_bounds__(256) k_pick(const DSplitPlan* plans, DThresh* thresh, uint32_t level, uint32_t sampled, uint32_t stride,
-                                              const uint32_t* split_state) {
-  __shared__ uint32_t s_part[256];
-  __shared__ uint32_t s_sel[2];
-  const uint32_t split = blockIdx.x, tid = threadIdx.x;
-  const DSplitPlan& P = plans[split];
-  DThresh& T = thresh[split];
-  if (P.max_hits == 0 || (split_state && split_state[split] == 0)) return;
-  if (split_state && tid == 0) *(uint32_t*)P.out_cand_count = 0;
-  if (!sampled && level > 0 && T.done) return;
-  const uint32_t* h = (const uint32_t*)P.out_hist;
-  // thread t owns the 8 bins [2048 - 8(t+1), 2048 - 8t), i.e. thread 0 owns the top bins
-  const uint32_t hi = QW_HIST_BINS - 8 * tid;
-  uint32_t loc[8], sum = 0;
+// Run by NT threads (tid < NT) that meet on barrier `bar` (0: the whole block, else a named barrier of exactly those
+// NT threads): k_pick, and k_union<MODE_SAMPLE_COLLECT> after its grid barrier. h: the split's histogram, read past
+// L1 (in k_union other blocks filled it during the same launch). s_part: NT / 32 words, s_sel: 2 words of shared
+// memory. Thread 0 writes T (global or shared memory).
+template <uint32_t NT>
+__device__ __forceinline__ void pick_digit(const DSplitPlan& P, DThresh& T, const uint32_t* h, uint32_t level, uint32_t sampled, uint32_t stride,
+                                           uint32_t tid, uint32_t bar, uint32_t* s_part, uint32_t* s_sel) {
+  constexpr uint32_t B = QW_HIST_BINS / NT;  // bins per thread
+  static_assert(QW_HIST_BINS % NT == 0 && NT % 32 == 0, "whole bins per thread, whole warps");
+  // thread t owns the B bins [2048 - B(t+1), 2048 - Bt), i.e. thread 0 owns the top bins
+  const uint32_t hi = QW_HIST_BINS - B * tid;
+  uint32_t loc[B], sum = 0;
 #pragma unroll
-  for (int j = 0; j < 8; j++) { loc[j] = h[hi - 1 - j]; sum += loc[j]; }
+  for (int j = 0; j < (int)B; j++) { loc[j] = __ldcg(h + hi - 1 - j); sum += loc[j]; }
   // exclusive prefix over threads (bins above mine): warp scan + the totals of the warps before mine
   uint32_t incl = sum;
 #pragma unroll
   for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, incl, o); if ((int)(tid & 31) >= o) incl += t; }
   if ((tid & 31) == 31) s_part[tid >> 5] = incl;
   if (tid == 0) { s_sel[0] = 0xFFFFFFFFu; s_sel[1] = 0; }
-  __syncthreads();
+  pick_sync(bar, NT);
   uint32_t above_me = incl - sum, total_all = 0;
 #pragma unroll
-  for (uint32_t w = 0; w < 8; w++) { const uint32_t t = s_part[w]; total_all += t; if (w < (tid >> 5)) above_me += t; }
+  for (uint32_t w = 0; w < NT / 32; w++) { const uint32_t t = s_part[w]; total_all += t; if (w < (tid >> 5)) above_me += t; }
   uint32_t K = P.max_hits;
   uint32_t target, base_above = 0;
   if (sampled == 2) {
@@ -1552,12 +1554,12 @@ __global__ void __launch_bounds__(256) k_pick(const DSplitPlan* plans, DThresh* 
   // find the largest digit t with suffix(t) >= target
   uint32_t run = above_me;
 #pragma unroll
-  for (int j = 0; j < 8; j++) {
+  for (int j = 0; j < (int)B; j++) {
     uint32_t before = run;
     run += loc[j];
     if (before < target && run >= target) { s_sel[0] = hi - 1 - j; s_sel[1] = before; }
   }
-  __syncthreads();
+  pick_sync(bar, NT);
   if (tid == 0) {
     uint32_t digit = s_sel[0];
     const uint32_t total = total_all;
@@ -1577,10 +1579,26 @@ __global__ void __launch_bounds__(256) k_pick(const DSplitPlan* plans, DThresh* 
     if (sampled) { T.above = 0; T.matched = 0; T.done = 1; }
     else {
       T.above = base_above + s_sel[1];
-      T.matched = h[digit];
+      T.matched = __ldcg(h + digit);
       T.done = (T.above + T.matched <= qw_cand_cap(K)) ? 1 : 0;
     }
   }
+}
+
+// One block per split.
+//   split_state != null: only splits flagged for refinement are touched, and their candidate
+//                 counters are reset for the candidates-only collect pass that follows.
+__global__ void __launch_bounds__(256) k_pick(const DSplitPlan* plans, DThresh* thresh, uint32_t level, uint32_t sampled, uint32_t stride,
+                                              const uint32_t* split_state) {
+  __shared__ uint32_t s_part[256 / 32];
+  __shared__ uint32_t s_sel[2];
+  const uint32_t split = blockIdx.x, tid = threadIdx.x;
+  const DSplitPlan& P = plans[split];
+  DThresh& T = thresh[split];
+  if (P.max_hits == 0 || (split_state && split_state[split] == 0)) return;
+  if (split_state && tid == 0) *(uint32_t*)P.out_cand_count = 0;
+  if (!sampled && level > 0 && T.done) return;
+  pick_digit<256>(P, T, (const uint32_t*)P.out_hist, level, sampled, stride, tid, 0, s_part, s_sel);
 }
 
 // Decodes a composite key back to the split's hit record at position i of its list: a QwHit, or the (doc id, score)

@@ -30,13 +30,16 @@
 //                   memory and no fence in the loop. The sweep of a finished window (count matches,
 //                   threshold test, clear) is one more stage of the same chain, so the next window's
 //                   decode overlaps the sweep of this one.
+//   own sample      MODE_SAMPLE_COLLECT: each block's first window is its share of the threshold sample; the
+//                   blocks meet at a grid barrier (cooperative launch), pick the threshold from the complete
+//                   histogram, sweep the first window against it, and collect the rest as MODE_COLLECT does.
 #pragma once
 #include "kernels.cuh"
 
 namespace qwk {
 
-/* 13 consumer warps + the producer, two blocks per SM: 72 registers per thread (sm_90a: 204 B of spill stores in the
- * COLLECT instantiation). Measured on one H100 80GB HBM3 (400 W power limit), k_union<COLLECT> per launch on the bench
+/* 13 consumer warps + the producer, two blocks per SM: 72 registers per thread (sm_90a: 40 B of spill stores in the
+ * COLLECT instantiation, 36 B in SAMPLE_COLLECT). Measured on one H100 80GB HBM3 (400 W power limit), k_union<COLLECT> per launch on the bench
  * workload: 201-202 us; 384 threads / 80 registers (56 B of spills): 204-205 us; 512 threads / 64 registers (292 B of
  * spills): 211-213 us. */
 #define QU_THREADS 448
@@ -60,6 +63,7 @@ struct USmem {
   uint32_t bars;                        // full[QU_SLOTS], empty[QU_SLOTS], chain[QU_CHAIN]
   uint32_t hist;                        // MODE_HIST: uint32[QW_HIST_BINS]
   uint32_t cands;                       // uint2[QU_NCW][QU_CANDS], then uint32 count[QU_NCW]
+  uint32_t thr;                         // MODE_SAMPLE_COLLECT: DThresh[2], then uint32 split[2] (the chunk's splits)
   uint32_t cap;                         // payload bytes per slot
   uint32_t total;
 };
@@ -68,8 +72,11 @@ struct UParams {
   const DSplitPlan* plans;
   const DInstr* instrs;
   const DCol* cols;
-  const DThresh* thresh;
+  DThresh* thresh;             // COLLECT: read; SAMPLE_COLLECT: written for the host by each split's first block
   const uint32_t* first_work;  // prefix over splits of (sampled) window counts; [n_splits + 1]
+  const uint32_t* sample_stride;  // SAMPLE_COLLECT: per split, the weight of its sample (qw_fused_sample_plan)
+  uint32_t* sync;                 // SAMPLE_COLLECT: grid barrier counter, zero at launch
+  uint32_t* err;                  // SAMPLE_COLLECT: set to 1 when the grid barrier timed out
   uint32_t n_splits, total_work, stride, W;
   USmem sm;
 };
@@ -77,8 +84,54 @@ struct UParams {
 struct UHdr {  // 32 bytes, written by the producer when it closes a slot
   uint32_t ws, wlen, split, flags;
   uint32_t n_blocks, n_terms, t_last;  // t_last: clause of the slot's last block (stages below it are final)
-  float s_lo;                          // COLLECT: f32 lower bound of the threshold bucket; HIST: score_scale
+  float s_lo;                          // COLLECT: f32 lower bound of the threshold bucket; HIST: score_scale (unused in SAMPLE_COLLECT)
 };
+
+// level-0 digit of a score's composite key: [1 | lin:10] (score_lin)
+__device__ __forceinline__ uint32_t score_digit(float s, float scale) {
+  const float x = __fmul_rn(s, scale);
+  const uint32_t l = x >= 1023.0f ? 1023u : (x > 0.0f ? (uint32_t)x : 0u);
+  return 1024u | l;
+}
+
+// f32 lower bound of a threshold's level-0 score bucket (conservative: one part in 2^20); -1: no threshold
+__device__ __forceinline__ float thresh_s_lo(const DThresh& T, float score_scale) {
+  const uint32_t thr_top = (uint32_t)(T.key[0] >> 53);
+  return thr_top >= 1024u ? __fmul_rn(__fdiv_rn((float)(thr_top & 1023u), score_scale), 0.999999f) : -1.0f;
+}
+
+__device__ __forceinline__ uint64_t globaltimer_ns() {
+  uint64_t t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+
+// Grid-wide barrier of k_union<MODE_SAMPLE_COLLECT>, called by one thread per block after the block's consumer warps
+// have met (so the fence below orders their global atomics before the arrival). False when the other blocks did not
+// all arrive within a second: the caller reports it, and the kernel still ends normally.
+//
+// Safe only because the kernel is launched cooperatively (cudaLaunchCooperativeKernel), with a grid of at most
+// occupancy x SM count blocks. The CUDA Programming Guide, on grid synchronization: "To guarantee the co-residency of
+// the thread blocks on the GPU, the number of blocks launched needs to be carefully considered." The runtime API
+// (cudaLaunchCooperativeKernel): "The total number of blocks launched cannot exceed the maximum number of blocks per
+// multiprocessor as returned by cudaOccupancyMaxActiveBlocksPerMultiprocessor (or
+// cudaOccupancyMaxActiveBlocksPerMultiprocessorWithFlags) times the number of multiprocessors as specified by the
+// device attribute cudaDevAttrMultiProcessorCount." A grid launched that way has all of its blocks resident together,
+// also while other calls' kernels run on other streams, so no block waits here for one that cannot start.
+__device__ __forceinline__ bool grid_barrier(uint32_t* ctr, uint32_t n_blocks) {
+  __threadfence();
+  atomicAdd(ctr, 1u);
+  const uint64_t t0 = globaltimer_ns();
+  for (;;) {
+    uint32_t v;
+    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(ctr) : "memory");
+    if (v >= n_blocks) break;
+    if (globaltimer_ns() - t0 > 1000000000ull) return false;
+    __nanosleep(500);
+  }
+  __threadfence();
+  return true;
+}
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
@@ -126,9 +179,8 @@ __device__ __forceinline__ uint32_t warp_incl_scan(uint32_t x) {
 
 // Rare path of the sweep: a doc that reaches the float lower bound builds its composite key and, if
 // it reaches the threshold key, joins the split's candidate list (k_select sorts it out).
-__device__ __noinline__ void union_emit(const DSplitPlan* plans, const DThresh* thresh, const DCol* cols, uint32_t split, uint32_t doc, float sc) {
+__device__ __noinline__ void union_emit(const DSplitPlan* plans, const DThresh& T, const DCol* cols, uint32_t split, uint32_t doc, float sc) {
   const DSplitPlan& P = plans[split];
-  const DThresh& T = thresh[split];
   const Key thr{T.key[0], T.key[1], T.key[2]};
   const DocKey dk = doc_key(P, P.key, cols + P.col_base, (const uint8_t*)P.data_base, doc, sc);
   if (key_ge(dk.key, thr)) {
@@ -161,8 +213,8 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
   // this block's chunk of the flat (split, window) list (handing windows out one at a time from a global counter was
   // slower: consecutive windows of a block then belong to different splits, and the plan switch sits on the
   // producer's critical path)
-  const uint32_t w_begin = (uint32_t)(((uint64_t)p.total_work * blockIdx.x) / gridDim.x);
-  const uint32_t w_end = (uint32_t)(((uint64_t)p.total_work * (blockIdx.x + 1)) / gridDim.x);
+  const uint32_t w_begin = qw_chunk_begin(p.total_work, blockIdx.x, gridDim.x);
+  const uint32_t w_end = qw_chunk_begin(p.total_work, blockIdx.x + 1, gridDim.x);
 
   if (warp == QU_NCW) {
     // ================================ producer ======================================================
@@ -217,12 +269,9 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
         t_fl = in.flags; t_w = in.f; t_sub16 = in.pad;
         t_tab = P.bm25_tab[in.r];
       }
-      if (MODE == MODE_COLLECT) {
-        // float lower bound of the threshold bucket (conservative: one part in 2^20)
-        const uint32_t thr_top = (uint32_t)(p.thresh[split].key[0] >> 53);
-        hdr_f = -1.0f;
-        if (thr_top >= 1024u) hdr_f = __fmul_rn(__fdiv_rn((float)(thr_top & 1023u), P.key.score_scale), 0.999999f);
-      } else hdr_f = P.key.score_scale;
+      // (SAMPLE_COLLECT: the consumers pick the threshold themselves, after the producer has moved on)
+      if (MODE == MODE_COLLECT) hdr_f = thresh_s_lo(p.thresh[split], P.key.score_scale);
+      else hdr_f = P.key.score_scale;
     };
     uint4 wa = make_uint4(0, 0, 0, 0), wb = wa;  // this lane's window-index entries (first / last index window)
     auto load_widx = [&](uint32_t window) {
@@ -347,6 +396,8 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
         }
         t = t2; tfl = tfl2; r = r2; ck = ck2; dat = dat2;
       }
+      // (the sample window reaches the consumers even without a block: they meet the other blocks after it)
+      if (MODE == MODE_SAMPLE_COLLECT && !open && work == w_begin) open_slot();
       if (open) close_slot(QU_F_LAST);
       if (have_next && nx_split != split) {
         split = nx_split;
@@ -380,6 +431,14 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
     uint2* cands = (uint2*)(qw_smem + p.sm.cands) + warp * QU_CANDS;
     uint32_t* ncand = (uint32_t*)(qw_smem + p.sm.cands + QU_NCW * QU_CANDS * 8) + warp;
     if (lane == 0) *ncand = 0;
+    // SAMPLE_COLLECT: the thresholds of the chunk's (one or two) splits, picked by the block itself
+    DThresh* s_thr = (DThresh*)(qw_smem + p.sm.thr);
+    uint32_t* s_thr_split = (uint32_t*)(s_thr + 2);
+    float* s_thr_lo = (float*)(s_thr_split + 2);
+    auto thr_of = [&](uint32_t split) -> const DThresh& {
+      if (MODE == MODE_SAMPLE_COLLECT) return s_thr[split == s_thr_split[0] ? 0 : 1];
+      return p.thresh[split];
+    };
     auto pass_to = [&](uint32_t st) {  // arrive at every stage below st
       if (my_stage < st) {
         __syncwarp();
@@ -400,7 +459,7 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
       const uint32_t n = min(*ncand, (uint32_t)QU_CANDS);
       if (n == 0) return;
       const DSplitPlan& P = p.plans[cur_split];
-      const DThresh& T = p.thresh[cur_split];
+      const DThresh& T = thr_of(cur_split);
       const Key thr{T.key[0], T.key[1], T.key[2]};
       bool pass = false;
       DocKey dk;
@@ -426,7 +485,7 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
       __syncwarp();
     };
     auto flush_hits = [&]() {
-      if (MODE != MODE_COLLECT || cur_split == 0xFFFFFFFFu) return;
+      if (MODE == MODE_HIST || cur_split == 0xFFFFFFFFu) return;
       flush_cands();
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) my_hits += __shfl_down_sync(QW_FULL, my_hits, o);
@@ -456,7 +515,7 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
             if (vv[j] > 0.0f && vv[j] >= s_lo) {
               const uint32_t pos = atomicAdd(ncand, 1u);
               if (pos < QU_CANDS) cands[pos] = make_uint2(ws + 4 * q + j, __float_as_uint(vv[j]));
-              else union_emit(p.plans, p.thresh, p.cols, split, ws + 4 * q + j, vv[j]);  // buffer full: slow road now
+              else union_emit(p.plans, thr_of(split), p.cols, split, ws + 4 * q + j, vv[j]);  // buffer full: slow road now
             }
           }
         }
@@ -638,9 +697,11 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
           if (half == 1) apply();
         }
       }
-      // this warp is done reading the slot
+      // this warp is done reading the slot (SAMPLE_COLLECT: the last slot of the block's first window -- wbase 1 -- is
+      // held: its payload takes the sample's histogram, and the producer stages ahead into the other slot meanwhile)
       __syncwarp();
-      if (lane == 0) mbar_arrive(bar_empty(slot));
+      const bool hold = MODE == MODE_SAMPLE_COLLECT && wbase == 1u && (flags & QU_F_LAST);
+      if (lane == 0 && !hold) mbar_arrive(bar_empty(slot));
       if (!(flags & QU_F_LAST)) {
         pass_to(wbase + t_last);  // the slot's last clause may continue in the next slot
         continue;
@@ -659,20 +720,64 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
         // ---- sweep: count matches (score > 0), test against the threshold, clear ----------------------
         next_base = end_stage + 1;
         collect_sweep(ws, split, hdr_f, end_stage);
+      } else if (MODE == MODE_SAMPLE_COLLECT) {
+        next_base = end_stage + 1;
+        if (hold) {
+          // ---- the block's first window is its share of the threshold sample ---------------------------------
+          wait_below(end_stage);  // every contribution is in, and no warp reads the slot any more
+          auto consumers_sync = [&]() { asm volatile("bar.sync 1, %0;" ::"n"(QU_NCT) : "memory"); };
+          uint32_t* shist = (uint32_t*)(qw_smem + sl + p.sm.payload);
+          for (uint32_t i = tid; i < QW_HIST_BINS; i += QU_NCT) shist[i] = 0;
+          consumers_sync();
+          const DSplitPlan& P = p.plans[split];
+          const float scale = P.key.score_scale;
+          for (uint32_t q = tid; q < (W >> 2); q += QU_NCT) {
+            const float4 v = sc4[q];  // (kept: the window is swept below, against the picked threshold)
+            const float vv[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+            for (int j = 0; j < 4; j++) if (vv[j] > 0.0f) atomicAdd(&shist[score_digit(vv[j], scale)], 1u);
+          }
+          consumers_sync();
+          uint32_t* gh = (uint32_t*)P.out_hist;
+          for (uint32_t i = tid; i < QW_HIST_BINS; i += QU_NCT) {
+            const uint32_t v = shist[i];
+            if (v) atomicAdd(&gh[i], v);
+          }
+          consumers_sync();
+          if (tid == 0 && !grid_barrier(p.sync, gridDim.x)) *p.err = 1;
+          consumers_sync();
+          // every block reads the same complete histograms: the same thresholds everywhere. The chunk touches the
+          // split of its first window and at most one more (qw_fused_sample_plan: every split holds a first window).
+          uint32_t split_b = split;
+          while (__ldg(p.first_work + split_b + 1) < w_end) split_b++;
+          for (uint32_t k = 0; k < (split_b != split ? 2u : 1u); k++) {
+            const uint32_t s = k ? split_b : split;
+            const DSplitPlan& Ps = p.plans[s];
+            if (Ps.max_hits == 0) { if (tid == 0) s_thr[k] = DThresh{}; }
+            else if (warp < 256 / 32)  // (s_part, s_sel in the histogram's place, dead now)
+              pick_digit<256>(Ps, s_thr[k], (const uint32_t*)Ps.out_hist, 0, 1, __ldg(p.sample_stride + s), tid, 2, shist, shist + 8);
+          }
+          consumers_sync();
+          if (tid < 2) {
+            const uint32_t s = tid ? split_b : split;
+            s_thr_split[tid] = s;
+            s_thr_lo[tid] = thresh_s_lo(s_thr[tid], p.plans[s].key.score_scale);
+            // for the host and later passes: written by the lowest block whose chunk touches the split
+            if (tid ? split_b != split : w_begin == __ldg(p.first_work + split)) p.thresh[s] = s_thr[tid];
+          }
+          consumers_sync();
+          if (lane == 0) mbar_arrive(bar_empty(slot));  // the held slot goes back to the producer
+        }
+        collect_sweep(ws, split, s_thr_lo[split == s_thr_split[0] ? 0 : 1], end_stage);
       } else {
         // level-0 digit histogram of the sampled windows: digit = [1 | lin:10] (score_lin)
         wait_below(end_stage);  // every contribution of the window is in
         const float scale = hdr_f;
-        auto lin = [&](float s) -> uint32_t {
-          const float x = __fmul_rn(s, scale);
-          const uint32_t l = x >= 1023.0f ? 1023u : (x > 0.0f ? (uint32_t)x : 0u);
-          return 1024u | l;
-        };
         for (uint32_t q = tid; q < (W >> 2); q += QU_NCT) {
           float vv[4];
           quad(q, vv);
 #pragma unroll
-          for (int j = 0; j < 4; j++) if (vv[j] > 0.0f) atomicAdd(&hist[lin(vv[j])], 1u);
+          for (int j = 0; j < 4; j++) if (vv[j] > 0.0f) atomicAdd(&hist[score_digit(vv[j], scale)], 1u);
         }
         __syncwarp();
         if (lane == 0) mbar_arrive(bar_chain(end_stage));
