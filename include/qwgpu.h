@@ -194,6 +194,14 @@ int qwgpu_build_leaf_response_entries(const uint8_t* img, uint64_t img_len, cons
  * QWGPU_EUNSUPPORTED when the table at that bound exceeds QWGPU_HASHED_MAX_BYTES, as a search would. */
 int qwgpu_agg_layout(const uint8_t* img, uint64_t img_len, const char* split_id, const uint8_t* plan, size_t plan_len,
                      uint32_t* hashed, uint64_t* bound_cells);
+/* The percentiles boundary table of column `column` of a split, host only (the table a search uploads for a
+ * QW_AGG_PERCENTILES node over it): *edges = uint64[*num_bins] (free with qwgpu_buf_free; NULL when the column has no
+ * values), edges[i] = the smallest bit-packed raw value whose DDSketch bin is >= bin i; *first_bin = the bin ordinal
+ * of index 0 (ordinals: 0 = the zero count, k - k0 + 1 = positive-store key k, -(k - k0 + 1) = negative-store key k,
+ * with k0 the key of the smallest double above 1e-9). Fails with QWGPU_EUNSUPPORTED for a column holding NaN or
+ * infinite values and QWGPU_EINVALID_AGG for a text or bytes column. */
+int qwgpu_percentiles_table(const uint8_t* img, uint64_t img_len, uint32_t column, uint64_t** edges, uint64_t* num_bins,
+                            int64_t* first_bin);
 
 /* Pre-search pruning (SURVEY.md 8a row a16), host only: what qwgpu_leaf_search does to the request of every
  * split before it searches — CanSplitDoBetter::{from_request, optimize_split_order, optimize}

@@ -242,13 +242,23 @@ enum {
   QW_AGG_HISTOGRAM = 2,      /* also date_histogram (interval/offset pre-scaled to column units) */
   QW_AGG_RANGE = 3,
   QW_AGG_STATS = 4,          /* stats / avg / sum / min / max / value_count share one collector */
-  QW_AGG_TRACE_IDS = 5       /* FindTraceIdsCollector (quickwit-search/src/find_trace_ids_collector.rs): the only node
+  QW_AGG_TRACE_IDS = 5,      /* FindTraceIdsCollector (quickwit-search/src/find_trace_ids_collector.rs): the only node
                                 of its plan. `column` = the trace-id QW_COL_BYTES column, `reserved` = the span timestamp
                                 column (0xFFFFFFFF when absent from the split: every timestamp reads 0),
                                 `num_buckets` = num_traces (N). Its N cells hold the split's result in no particular
                                 order: cell j is a span when `count` == 1, with `sum_bits` = the trace id's
                                 ordinal in the column dictionary and `max_mapped` = the span timestamp in the
                                 order-preserving i64 mapping. */
+  QW_AGG_PERCENTILES = 6     /* percentiles (a metric: no children). `column` = the value column; `num_buckets` = the bins
+                                of the split's DDSketch boundary table for that column (quickwit_b200/csrc/ddsketch.h:
+                                every bin between those of the column's minimum and maximum, in value order), plus one
+                                when `has_missing`; `missing_value` = the f64 bits of the `missing` value. A plan that
+                                holds one always takes the hashed layout (qw_agg_hashed). Its entries: key = the bin's
+                                index in that table (indices increase with the value: negative store, zero count,
+                                positive store), cell.count = the values in the bin, min_mapped / max_mapped = their
+                                smallest / largest value in the column's mapped space, sum_bits = 0; a matched doc
+                                without a value counts once in the entry with QW_AGG_ENTRY_MISSING (key 0) when
+                                `has_missing`, and nowhere otherwise. */
 };
 
 #define QW_MAX_AGG_RANGES 16
@@ -374,7 +384,8 @@ typedef struct QwAggCell {
  * layout when its tree is deeper than bucket -> bucket -> metric, its dense cells add up to more than
  * QW_AGG_DENSE_MAX_CELLS, or a TERMS node's dense space exceeds QW_AGG_DENSE_MAX_TERMS (qw_agg_hashed).
  *   key: TERMS = the bit-packed raw value (0 with QW_AGG_ENTRY_MISSING: the `missing` bucket); HISTOGRAM = the
- *        bucket index relative to base_pos (agg_bucket's f64 formula); RANGE = the range index; STATS = 0.
+ *        bucket index relative to base_pos (agg_bucket's f64 formula); RANGE = the range index; STATS = 0;
+ *        PERCENTILES = the index of the value's bin in the split's boundary table (QW_AGG_PERCENTILES).
  *   cell: as in the dense layout (bucket entries use `count` only). */
 #define QW_AGG_DENSE_MAX_CELLS (1ull << 26)
 #define QW_AGG_DENSE_MAX_TERMS (1ull << 24)
@@ -389,7 +400,7 @@ typedef struct QwAggEntry {
   QwAggCell cell;
 } QwAggEntry; /* 56 bytes */
 
-/* 1 when the plan's aggregation tree takes the hashed layout: a composite source node, a node below two bucket ancestors that is not a
+/* 1 when the plan's aggregation tree takes the hashed layout: a composite source node, a percentiles node, a node below two bucket ancestors that is not a
  * metric (or any node below three), the dense cells of all nodes adding up to more than QW_AGG_DENSE_MAX_CELLS,
  * or a TERMS node whose dense space (num_buckets without the `missing` slot) exceeds QW_AGG_DENSE_MAX_TERMS.
  * Reads only the plan; the caller has checked every parent index. */
@@ -398,6 +409,7 @@ static inline int qw_agg_hashed(const QwAggNode* nodes, uint32_t n) {
   for (uint32_t i = 0; i < n; i++) {
     const QwAggNode* g = &nodes[i];
     if ((g->kind == QW_AGG_TERMS || g->kind == QW_AGG_HISTOGRAM) && (g->reserved & QW_AGG_COMP_LEVEL)) return 1;
+    if (g->kind == QW_AGG_PERCENTILES) return 1;
     if (g->kind == QW_AGG_TERMS && (uint64_t)g->num_buckets - (g->has_missing ? 1u : 0u) > QW_AGG_DENSE_MAX_TERMS) return 1;
     uint32_t depth = 0;
     uint64_t cells = g->kind == QW_AGG_STATS ? 1 : g->num_buckets;

@@ -18,6 +18,7 @@
 #include <memory>
 
 #include "compile.h"
+#include "ddsketch.h"
 #include "device_types.h"
 
 namespace qw {
@@ -149,6 +150,29 @@ static void parse_composite(const Json& spec, AggReq& a, int depth) {
   }
 }
 
+// percentiles: {"field", "percents": [..] (default 1, 5, 25, 50, 75, 95, 99), "keyed" (default true), "missing": number}
+static void parse_percentiles(const Json& spec, AggReq& a) {
+  a.kind = AggReq::Percentiles;
+  if (a.field.empty()) fail(QWGPU_EINVALID_AGG, "percentiles aggregation `%s` requires a `field`", a.name.c_str());
+  a.percents = {1, 5, 25, 50, 75, 95, 99};
+  if (const Json* p = spec.get("percents")) {
+    if (!p->is_arr()) fail(QWGPU_EINVALID_AGG, "percentiles `percents` must be a list of numbers");
+    a.percents.clear();
+    for (const Json& x : p->arr) {
+      if (!x.is_num()) fail(QWGPU_EINVALID_AGG, "percentiles `percents` must be a list of numbers");
+      const double v = x.as_f64();
+      if (!(v >= 0 && v <= 100)) fail(QWGPU_EINVALID_AGG, "percent %g is not between 0 and 100", v);
+      a.percents.push_back(v);
+    }
+  }
+  a.keyed = spec.bool_or("keyed", true);
+  if (const Json* m = spec.get("missing")) {
+    if (!m->is_num()) fail(QWGPU_EINVALID_AGG, "percentiles `missing` must be a number");
+    a.has_missing = true;
+    a.missing = *m;
+  }
+}
+
 static void parse_agg_map(const Json& j, std::vector<AggReq>& out, int depth) {
   if (!j.is_obj()) fail(QWGPU_EINVALID_AGG, "aggregation request must be a JSON object");
   if (depth > 8) fail(QWGPU_EINVALID_AGG, "aggregation nesting too deep");
@@ -217,7 +241,8 @@ static void parse_agg_map(const Json& j, std::vector<AggReq>& out, int depth) {
       else if (t == "min") a.kind = AggReq::Min;
       else if (t == "max") a.kind = AggReq::Max;
       else if (t == "value_count" || t == "count") a.kind = AggReq::Count;
-      else if (t == "percentiles" || t == "cardinality" || t == "extended_stats" || t == "top_hits" || t == "filter")
+      else if (t == "percentiles") parse_percentiles(spec, a);
+      else if (t == "cardinality" || t == "extended_stats" || t == "top_hits" || t == "filter")
         fail(QWGPU_EUNSUPPORTED, "`%s` aggregations are not implemented on the GPU path yet", t.c_str());
       else fail(QWGPU_EINVALID_AGG, "unknown aggregation type `%s`", t.c_str());
     }
@@ -504,6 +529,19 @@ static QwAggNode lower_one(const AggReq& a, const ImageView& img, AggBinding& b,
       }
       break;
     }
+    case AggReq::Percentiles: {
+      // the bins of the split's boundary table for the column (the engine builds the table itself and checks the
+      // count), one more for the `missing` entry
+      n.kind = QW_AGG_PERCENTILES;
+      if (col && col->type == QW_COL_STR) fail(QWGPU_EINVALID_AGG, "percentiles on text field `%s`", a.field.c_str());
+      dds::Table t;
+      if (col && !dds::column_table(*col, false, &t))
+        fail(QWGPU_EUNSUPPORTED, "percentiles over field `%s`, which holds NaN or infinite values, are not implemented on the GPU path", a.field.c_str());
+      n.num_buckets = (uint32_t)t.num_bins + (a.has_missing ? 1u : 0u);
+      n.has_missing = a.has_missing;
+      if (a.has_missing) { const double m = a.missing.as_f64(); memcpy(&n.missing_value, &m, 8); }
+      break;
+    }
     default: n.kind = QW_AGG_STATS; n.num_buckets = 1; break;
   }
   return n;
@@ -593,6 +631,7 @@ struct IAgg {
   // metric
   uint64_t m_count = 0;
   double m_sum = 0, m_min = INFINITY, m_max = -INFINITY;
+  dds::Sketch sk;  // percentiles
   // key -> position in `buckets`, built on the first merge into this node and kept up to date, so that
   // folding n responses costs O(total buckets · log) instead of re-indexing the accumulator n times
   struct Index {
@@ -642,6 +681,14 @@ static void ser_agg(BW& w, const IAgg& a) {
     }
     return;
   }
+  if (a.kind == AggReq::Percentiles) {
+    // min, max, then (zigzag bin ordinal, count) per non-empty bin in value order; the count is their sum
+    w.f64(a.sk.min);
+    w.f64(a.sk.max);
+    w.varint(a.sk.bins.size());
+    for (const auto& kv : a.sk.bins) { w.varint(((uint64_t)kv.first << 1) ^ (uint64_t)(kv.first >> 63)); w.varint(kv.second); }
+    return;
+  }
   if (a.kind >= AggReq::Stats) { w.varint(a.m_count); w.f64(a.m_sum); w.f64(a.m_min); w.f64(a.m_max); return; }
   w.varint(a.is_date);
   w.varint(a.sum_other);
@@ -686,6 +733,19 @@ static IAgg de_agg(BR& r) {
       b.count = r.varint();
       b.subs = de_aggs(r);
       a.buckets.push_back(std::move(b));
+    }
+    return a;
+  }
+  if (a.kind == AggReq::Percentiles) {
+    a.sk.min = r.f64();
+    a.sk.max = r.f64();
+    const uint64_t n = r.varint();
+    if (n > (uint64_t)(r.e - r.p)) fail(QWGPU_EINTERNAL, "failed to merge intermediate aggregation results: truncated buffer");
+    for (uint64_t i = 0; i < n; i++) {
+      const uint64_t z = r.varint();
+      const uint64_t c = r.varint();
+      a.sk.bins[(int64_t)((z >> 1) ^ (~(z & 1) + 1))] += c;
+      a.sk.count += c;
     }
     return a;
   }
@@ -795,6 +855,8 @@ static void sort_term_buckets(const AggReq& req, std::vector<IBucket>& bs) {
   int ci = -1;
   for (size_t i = 0; i < req.children.size(); i++) if (req.children[i].name == name) ci = (int)i;
   if (ci < 0) fail(QWGPU_EINVALID_AGG, "could not find aggregation with name `%s` in metric sub_aggregations", name.c_str());
+  if (req.children[ci].kind == AggReq::Percentiles)
+    fail(QWGPU_EUNSUPPORTED, "ordering terms by the percentiles aggregation `%s` is not implemented on the GPU path", name.c_str());
   std::sort(bs.begin(), bs.end(), [&](const IBucket& a, const IBucket& b) {
     double x = metric_of(a.subs[ci], prop), y = metric_of(b.subs[ci], prop);
     if (x != y) return req.order_desc ? x > y : x < y;
@@ -868,6 +930,7 @@ static IAgg build_node(const BuildCtx& c, uint32_t ni, uint64_t parent_cell) {
   const AggBinding& b = c.cp.agg_bindings[ni];
   const AggReq& req = *b.req;
   if (req.kind == AggReq::Composite) fail(QWGPU_EINVALID_ARG, "composite aggregation results are given as entries");
+  if (req.kind == AggReq::Percentiles) fail(QWGPU_EINVALID_ARG, "percentiles aggregation results are given as entries");
   const QwAggCell* base = c.cells + c.bases[ni];
   if (req.is_metric()) return metric_from_cell(c.cp, c.img, c.nodes, ni, base[parent_cell]);
   IAgg a;
@@ -950,6 +1013,28 @@ static IAgg build_composite_e(const EntryCtx& c, uint32_t ni0, uint32_t parent0)
   return a;
 }
 
+// a percentiles node's entries under one parent bucket as a sketch in value space: table indices become bin ordinals
+// through the split's table for the column (tables differ per split, the ordinals do not); the `missing` entry counts
+// the missing value
+static IAgg build_percentiles_e(const EntryCtx& c, uint32_t ni, const std::vector<uint32_t>& es) {
+  const AggBinding& b = c.cp.agg_bindings[ni];
+  IAgg a;
+  a.kind = AggReq::Percentiles;
+  dds::Table t;
+  const QwImgColumn* col = b.column >= 0 ? &c.img.columns[b.column] : nullptr;
+  if (col) dds::column_table(*col, false, &t);
+  for (uint32_t e : es) {
+    const QwAggEntry& x = c.entries[e];
+    if (x.flags & QW_AGG_ENTRY_MISSING) {
+      const double m = b.req->missing.as_f64();
+      a.sk.add(dds::bin_ord(m), x.cell.count, m, m);
+    } else if (x.cell.count) {
+      a.sk.add(t.ord_lo + (int64_t)x.key, x.cell.count, dds::column_f64(col->type, x.cell.min_mapped), dds::column_f64(col->type, x.cell.max_mapped));
+    }
+  }
+  return a;
+}
+
 static IAgg build_node_e(const EntryCtx& c, uint32_t ni, uint32_t parent) {
   const QwAggNode& n = c.nodes[ni];
   const AggBinding& b = c.cp.agg_bindings[ni];
@@ -958,6 +1043,7 @@ static IAgg build_node_e(const EntryCtx& c, uint32_t ni, uint32_t parent) {
   static const std::vector<uint32_t> none;
   auto it = c.kids.find({parent, ni});
   const std::vector<uint32_t>& es = it == c.kids.end() ? none : it->second;
+  if (req.kind == AggReq::Percentiles) return build_percentiles_e(c, ni, es);
   if (req.is_metric()) {
     QwAggCell empty = {0, 0, ~0ull, 0};
     return metric_from_cell(c.cp, c.img, c.nodes, ni, es.empty() ? empty : c.entries[es[0]].cell);
@@ -1015,12 +1101,12 @@ static std::vector<IAgg> build_top_entries(const CompiledPlan& cp, const ImageVi
       fail(QWGPU_EINVALID_ARG, "aggregation entry %zu does not match the plan's tree", e);
     const QwAggNode& n = nodes[x.node];
     const AggBinding& b = cp.agg_bindings[x.node];
-    bool ok = x.flags == 0 || ((n.kind == QW_AGG_TERMS || n.kind == QW_AGG_HISTOGRAM) && x.flags == QW_AGG_ENTRY_MISSING);
+    bool ok = x.flags == 0 || ((n.kind == QW_AGG_TERMS || n.kind == QW_AGG_HISTOGRAM || n.kind == QW_AGG_PERCENTILES) && x.flags == QW_AGG_ENTRY_MISSING);
     if (ok && (x.flags & QW_AGG_ENTRY_MISSING)) ok = n.has_missing && x.key == 0;
     else if (ok) {
       switch (n.kind) {
         case QW_AGG_STATS: ok = x.key == 0; break;
-        case QW_AGG_HISTOGRAM: ok = x.key < (uint64_t)n.num_buckets - (n.has_missing ? 1u : 0u); break;
+        case QW_AGG_HISTOGRAM: case QW_AGG_PERCENTILES: ok = x.key < (uint64_t)n.num_buckets - (n.has_missing ? 1u : 0u); break;
         case QW_AGG_RANGE: ok = x.key < n.num_ranges; break;
         case QW_AGG_TERMS: {
           ok = b.column >= 0 && img.columns[b.column].num_vals > 0 && img.columns[b.column].gcd &&
@@ -1191,6 +1277,10 @@ static void merge_into(const AggReq& req, IAgg& acc, IAgg&& other) {
     comp_sort_cut(req, acc);
     return;
   }
+  if (acc.kind == AggReq::Percentiles) {  // bins add up; min and max of both
+    acc.sk.merge(other.sk);
+    return;
+  }
   if (acc.kind >= AggReq::Stats) {
     acc.m_count += other.m_count;
     acc.m_sum += other.m_sum;
@@ -1340,6 +1430,31 @@ static void fin_agg(const AggReq& req, const IAgg* a, std::string& out) {
   IAgg empty;
   empty.kind = (uint8_t)req.kind;
   if (!a) a = &empty;
+  if (req.kind == AggReq::Percentiles) {
+    // {"values": {"<percent>": value}} (keyed; the percent in Rust f64 Display form) or
+    // {"values": [{"key": percent, "value": value}]}; an empty sketch gives null
+    dds::Sketch s = a->sk;
+    s.collapse();
+    out += req.keyed ? "{\"values\":{" : "{\"values\":[";
+    for (size_t i = 0; i < req.percents.size(); i++) {
+      if (i) out += ",";
+      double v = 0;
+      const bool some = s.quantile(req.percents[i] / 100.0, &v);
+      if (req.keyed) {
+        json_escape(rust_display_f64(req.percents[i]), out);
+        out += ":";
+        opt_f64(some, v, out);
+      } else {
+        out += "{\"key\":";
+        json_f64(req.percents[i], out);
+        out += ",\"value\":";
+        opt_f64(some, v, out);
+        out += "}";
+      }
+    }
+    out += req.keyed ? "}}" : "]}";
+    return;
+  }
   if (req.is_metric()) {
     bool some = a->m_count > 0;
     double avg = some ? a->m_sum / (double)a->m_count : 0;

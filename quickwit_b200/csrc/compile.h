@@ -39,7 +39,9 @@ struct AggReq {
   // Composite: `sources` are Terms / Histogram / DateHistogram requests (their `name`, `field`, interval / offset,
   // `order_desc` and `has_missing` = missing_bucket), `size` the page size, `after` one key per source when
   // `has_after`; `children` hang below the last source
-  enum Kind { Terms, Histogram, DateHistogram, Range, Stats, Avg, Sum, Min, Max, Count, TraceIds, Composite } kind = Terms;
+  // Percentiles: `percents` (0..100), `keyed`, and `missing` (a number) when `has_missing`
+  enum Kind { Terms, Histogram, DateHistogram, Range, Stats, Avg, Sum, Min, Max, Count, TraceIds, Composite, Percentiles } kind = Terms;
+  std::vector<double> percents;
   std::vector<AggReq> sources;
   std::vector<CompKey> after;
   bool has_after = false;
@@ -61,7 +63,7 @@ struct AggReq {
   struct R { bool has_from = false, has_to = false; double from = 0, to = 0; std::string key; };
   std::vector<R> ranges;
   std::vector<AggReq> children;
-  bool is_metric() const { return kind >= Stats && kind <= Count; }
+  bool is_metric() const { return (kind >= Stats && kind <= Count) || kind == Percentiles; }
 };
 std::vector<AggReq> parse_agg_request(const std::string& json);
 inline bool is_trace_ids_request(const std::vector<AggReq>& r) { return r.size() == 1 && r[0].kind == AggReq::TraceIds; }

@@ -8,6 +8,7 @@
 #include <chrono>
 #include <cmath>
 
+#include "ddsketch.h"
 #include "engine.h"
 #include "kernels.cuh"
 #include "union_kernel.cuh"
@@ -344,7 +345,8 @@ uint64_t agg_hashed_bound(const QwAggNode* aggs, uint32_t n, const ImageView& im
       if (g.kind == QW_AGG_RANGE) reps = sat_mul(reps, g.num_ranges);
       if (g.column < img.hdr->num_columns && img.columns[g.column].cardinality == QW_CARD_MULTI) {
         any_multi = true;
-        multi = sat_mul(multi, img.columns[g.column].num_vals + ((g.kind == QW_AGG_TERMS || g.kind == QW_AGG_HISTOGRAM) && g.has_missing ? num_docs : 0));
+        multi = sat_mul(multi, img.columns[g.column].num_vals +
+                                   ((g.kind == QW_AGG_TERMS || g.kind == QW_AGG_HISTOGRAM || g.kind == QW_AGG_PERCENTILES) && g.has_missing ? num_docs : 0));
       }
     }
     total = std::min<uint64_t>(total + std::min(dense, sat_mul(any_multi ? multi : num_docs, reps)), 1ull << 62);
@@ -399,6 +401,20 @@ struct Lowered {
   uint32_t tr_img_col = 0;              // find_trace_ids: the trace-id column of the image
   uint64_t h_bound = 0;                 // hashed aggregation layout: upper bound on the split's distinct cells
 };
+
+// The boundary table of a percentiles node's column (ddsketch.h), built once per split and column: a column that
+// spans the whole double range takes a few million logarithms
+static std::shared_ptr<const std::vector<uint64_t>> percentiles_table(const SplitDev& sp, uint32_t c) {
+  std::lock_guard<std::mutex> g(sp.pct_mu);
+  auto it = sp.pct_tables.find(c);
+  if (it != sp.pct_tables.end()) return it->second;
+  dds::Table t;
+  if (!dds::column_table(sp.view.columns[c], true, &t))
+    fail(QWGPU_EUNSUPPORTED, "percentiles over a column holding NaN or infinite values are not implemented on the GPU path");
+  auto p = std::make_shared<const std::vector<uint64_t>>(std::move(t.edges));
+  sp.pct_tables.emplace(c, p);
+  return p;
+}
 
 static uint32_t use_col(Lowered& L, const SplitDev& sp, uint32_t c) {
   if (c == 0xFFFFFFFFu) return c;
@@ -786,8 +802,24 @@ static void lower_plan(Lowered& L, const SplitDev& sp, const uint8_t* plan, size
       d.comp = a.reserved;
       d.comp_after = a.range_from[0];
     }
-    if (a.parent != 0xFFFFFFFFu && aggs[a.parent].kind == QW_AGG_STATS) fail(QWGPU_EINVALID_AGG, "metric aggregations cannot have sub-aggregations");
+    if (a.parent != 0xFFFFFFFFu && (aggs[a.parent].kind == QW_AGG_STATS || aggs[a.parent].kind == QW_AGG_PERCENTILES))
+      fail(QWGPU_EINVALID_AGG, "metric aggregations cannot have sub-aggregations");
     if (a.kind == QW_AGG_RANGE && a.num_ranges > QW_MAX_AGG_RANGES) fail(QWGPU_EUNSUPPORTED, "more than %d ranges", QW_MAX_AGG_RANGES);
+    if (a.kind == QW_AGG_PERCENTILES) {
+      // the walk finds a value's bin in the column's boundary table (d.bounds: an index into L.bounds until the blob
+      // is laid out); the plan's bin count must be the table's
+      std::shared_ptr<const std::vector<uint64_t>> tab;
+      if (a.column != 0xFFFFFFFFu) {
+        const uint32_t t = sp.view.columns[a.column].type;
+        if (t == QW_COL_STR || t == QW_COL_BYTES) fail(QWGPU_EINVALID_AGG, "percentiles over a text or bytes column");
+        tab = percentiles_table(sp, a.column);
+      }
+      const uint64_t nb = tab ? tab->size() : 0;
+      if (a.num_buckets != nb + (a.has_missing ? 1u : 0u))
+        fail(QWGPU_EINVALID_ARG, "percentiles node %u: %u buckets, the split's column has %llu bins", i, a.num_buckets, (unsigned long long)nb);
+      d.bounds = L.bounds.size();
+      if (tab) L.bounds.insert(L.bounds.end(), tab->begin(), tab->end());
+    }
     L.aggs.push_back(d);
   }
   P.n_aggs = ph->num_aggs;
@@ -1428,9 +1460,10 @@ struct Run {
       if (P.n_cols) memcpy(hb + o_cols + P.col_base * sizeof(DCol), L.cols.data(), P.n_cols * sizeof(DCol));
       DAgg* aggs = (DAgg*)(hb + o_aggs) + P.agg_base;
       if (P.n_aggs) memcpy(aggs, L.aggs.data(), P.n_aggs * sizeof(DAgg));
-      if (P.fast_aggs)  // (lowering left each histogram's bounds as an index into the split's table)
-        for (uint32_t a = 0; a < P.n_aggs; a++)
-          if (aggs[a].kind == QW_AGG_HISTOGRAM) aggs[a].bounds = (uint64_t)(db + o_bounds) + (bounds_base[i] + aggs[a].bounds) * 8;
+      // (lowering left each fast-path histogram's and each percentiles node's table as an index into the split's tables)
+      for (uint32_t a = 0; a < P.n_aggs; a++)
+        if ((P.fast_aggs && aggs[a].kind == QW_AGG_HISTOGRAM) || aggs[a].kind == QW_AGG_PERCENTILES)
+          aggs[a].bounds = (uint64_t)(db + o_bounds) + (bounds_base[i] + aggs[a].bounds) * 8;
       if (!L.bounds.empty()) memcpy(hb + o_bounds + (size_t)bounds_base[i] * 8, L.bounds.data(), L.bounds.size() * 8);
     }
     if (do_merge) for (uint32_t i = 0; i < n; i++) ((uint32_t*)(hb + o_rank))[i] = merge->rank[idx[i]];

@@ -21,6 +21,9 @@ struct SplitDev {
   float* d_tabs = nullptr;   // device float[num_fields][256] BM25 norm tables
   uint64_t data_len = 0;
   std::vector<uint8_t> ids16;  // per column: 1 = a bytes column whose dictionary holds only 16-byte values
+  // per column: the percentiles boundary table (ddsketch.h column_table), built by the first search that needs it
+  mutable std::mutex pct_mu;
+  mutable std::map<uint32_t, std::shared_ptr<const std::vector<uint64_t>>> pct_tables;
   // residency: recency for the LRU, state of an asynchronous upload (0 loading, 1 ready, 2 failed)
   uint64_t last_use = 0;
   int state = 1;

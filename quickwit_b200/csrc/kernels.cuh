@@ -707,6 +707,17 @@ __device__ __forceinline__ uint32_t hcell_count(const DSplitPlan& P, uint32_t no
   id = __shfl_sync(QW_FULL, id, lead);
   return on ? id : QW_HSLOT_EMPTY;
 }
+// The bin of raw value `raw` of percentiles node g: the last entry of the column's boundary table that is <= raw
+// (DAgg::bounds, built on the host with the reference's logarithm: the device never evaluates one)
+__device__ __forceinline__ uint32_t pct_bin(const DAgg& g, uint64_t raw) {
+  const uint64_t* B = (const uint64_t*)g.bounds;
+  uint32_t lo = 0, hi = g.num_buckets - (g.has_missing ? 2u : 1u);
+  while (lo < hi) {
+    const uint32_t mid = (lo + hi + 1) >> 1;
+    if (__ldg(B + mid) <= raw) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
 // Where the key of composite source g lies against the source's `after` value, in the source's order (null first
 // when ascending, last when descending): -1 before, 0 equal, 1 after.
 __device__ __forceinline__ int comp_vs_after(const DAgg& g, uint64_t key, bool missing) {
@@ -760,7 +771,8 @@ __device__ __forceinline__ void agg_collect_hashed(const DSplitPlan& P, const DA
         }
         bool missing;
         nv[d] = agg_values(g, cols, base, doc, live, a[d], missing);
-        if (g.kind == QW_AGG_HISTOGRAM && g.has_missing && live && nv[d] == 0) { missing = true; nv[d] = 1; }  // composite missing_bucket
+        // composite missing_bucket, percentiles `missing`
+        if ((g.kind == QW_AGG_HISTOGRAM || g.kind == QW_AGG_PERCENTILES) && g.has_missing && live && nv[d] == 0) { missing = true; nv[d] = 1; }
         flags = (flags & ~(0x100u << d)) | (missing ? 0x100u << d : 0u);
         maxv[d] = __reduce_max_sync(QW_FULL, nv[d]);
         k[d] = 0;
@@ -772,10 +784,13 @@ __device__ __forceinline__ void agg_collect_hashed(const DSplitPlan& P, const DA
         if (k[d] >= maxv[d]) { d--; continue; }
         const bool missing = (flags >> (8 + d)) & 1u;
         bool ok = k[d] < nv[d];
-        uint64_t key = 0;
+        uint64_t key = 0, raw = 0;
         if (ok && !missing) {
           if (g.kind == QW_AGG_TERMS) key = col_raw(base, cols[g.col], a[d] + k[d]);
-          else {
+          else if (g.kind == QW_AGG_PERCENTILES) {
+            raw = col_raw(base, cols[g.col], a[d] + k[d]);
+            key = pct_bin(g, raw);
+          } else {
             uint32_t bk = 0;
             ok = agg_bucket(g, cols[g.col], base, a[d] + k[d], r[d], bk);
             key = bk;
@@ -791,6 +806,15 @@ __device__ __forceinline__ void agg_collect_hashed(const DSplitPlan& P, const DA
           flags = (flags & ~(0x1000000u << d)) | (tight ? 0x1000000u << d : 0u);
         }
         cell[d] = hcell_count(P, node[d] | (missing ? QW_AGG_ENTRY_MISSING << 8 : 0u), parent[d], key, ok, true, lane);
+        if (g.kind == QW_AGG_PERCENTILES && cell[d] != QW_HSLOT_EMPTY && !missing) {
+          // the bin's exact minimum and maximum (q = 0 and q = 1), kept as agg_stats keeps them: max(~m), max(m). Both
+          // only grow, so a value at or below what a load already sees cannot change them: the atomic is skipped
+          const DCol& c = cols[g.col];
+          const uint64_t m = c.min_value + c.gcd * raw;
+          unsigned long long* mm = (unsigned long long*)&cells[cell[d]].min_mapped;
+          if (~m > __ldcg(mm)) atomicMax(mm, (unsigned long long)~m);
+          if (m > __ldcg(mm + 1)) atomicMax(mm + 1, (unsigned long long)m);
+        }
         child[d] = 0;
         if (++r[d] >= (g.kind == QW_AGG_RANGE ? g.num_ranges : 1u)) { r[d] = 0; k[d]++; }
       }

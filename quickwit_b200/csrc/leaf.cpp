@@ -14,6 +14,7 @@
 #include <tuple>
 
 #include "compile.h"
+#include "ddsketch.h"
 #include "device_types.h"
 #include "engine.h"
 #include "comm.h"
@@ -910,6 +911,28 @@ int qwgpu_agg_layout(const uint8_t* img, uint64_t img_len, const char* split_id,
   }
   *hashed = qw_agg_hashed(aggs, ph->num_aggs) ? 1u : 0u;
   *bound_cells = *hashed ? qw::agg_hashed_layout(aggs, ph->num_aggs, v, split_id ? split_id : "") : 0;
+  return 0;
+  QW_API_END
+}
+
+int qwgpu_percentiles_table(const uint8_t* img, uint64_t img_len, uint32_t column, uint64_t** edges, uint64_t* num_bins,
+                            int64_t* first_bin) {
+  QW_API_BEGIN
+  qw::ImageView v;
+  v.open(img, img_len);
+  if (column >= v.hdr->num_columns) qw::fail(QWGPU_EINVALID_ARG, "column %u (split has %u)", column, v.hdr->num_columns);
+  const QwImgColumn& c = v.columns[column];
+  if (c.type == QW_COL_STR || c.type == QW_COL_BYTES) qw::fail(QWGPU_EINVALID_AGG, "percentiles over a text or bytes column");
+  qw::dds::Table t;
+  if (!qw::dds::column_table(c, true, &t)) qw::fail(QWGPU_EUNSUPPORTED, "percentiles over a column holding NaN or infinite values");
+  *edges = nullptr;
+  if (!t.edges.empty()) {
+    *edges = (uint64_t*)malloc(t.edges.size() * 8);
+    if (!*edges) qw::fail(QWGPU_EINTERNAL, "out of memory");
+    memcpy(*edges, t.edges.data(), t.edges.size() * 8);
+  }
+  *num_bins = t.num_bins;
+  *first_bin = t.ord_lo;
   return 0;
   QW_API_END
 }

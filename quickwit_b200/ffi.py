@@ -27,6 +27,7 @@ OCCUR_MUST, OCCUR_SHOULD, OCCUR_MUST_NOT, OCCUR_FILTER = range(4)
 SORT_NONE, SORT_DOCID, SORT_SCORE, SORT_COLUMN = range(4)
 ORDER_ASC, ORDER_DESC = 0, 1
 AGG_TERMS, AGG_HISTOGRAM, AGG_RANGE, AGG_STATS, AGG_TRACE_IDS = 1, 2, 3, 4, 5
+AGG_PERCENTILES = 6  # num_buckets = the bins of the split's boundary table (+1 with `missing`), missing_value = f64 bits
 ABSENT = 0xFFFFFFFF
 # qwgpu_split_result.kernel_mask (qwgpu.h)
 KERNEL_UNION, KERNEL_DRIVER, KERNEL_AGGSCAN, KERNEL_WINDOW, KERNEL_PHRASE = 1, 2, 4, 8, 16
@@ -210,6 +211,7 @@ def lib() -> C.CDLL:
     bind("qwgpu_build_leaf_response", [vp, u64, cp, vp, sz, cp, u64, vp, u32, vp, u32, C.POINTER(vp), C.POINTER(sz)])
     bind("qwgpu_build_leaf_response_entries", [vp, u64, cp, vp, sz, cp, u64, vp, u32, vp, u32, C.POINTER(vp), C.POINTER(sz)])
     bind("qwgpu_agg_layout", [vp, u64, cp, vp, sz, C.POINTER(u32), C.POINTER(u64)])
+    bind("qwgpu_percentiles_table", [vp, u64, u32, C.POINTER(vp), C.POINTER(u64), C.POINTER(C.c_int64)])
     bind("qwgpu_merge_leaf_responses", [vp, sz, u32, C.POINTER(vp), C.POINTER(sz),
                                         C.POINTER(vp), C.POINTER(sz)])
     bind("qwgpu_optimize_leaf_request", [vp, sz, C.POINTER(vp), C.POINTER(sz)])

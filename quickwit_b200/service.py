@@ -316,6 +316,20 @@ def agg_layout(img: SplitImage, plan: bytes, split_id: str = "") -> Tuple[bool, 
     return bool(hashed.value), int(bound.value)
 
 
+def percentiles_table(img: SplitImage, column: int) -> Tuple[int, List[int]]:
+    """(bin ordinal of index 0, edges) of the percentiles boundary table of a split's column (qwgpu_percentiles_table):
+    edges[i] = the smallest raw value whose DDSketch bin is >= bin i."""
+    L = ffi.lib()
+    out, nb, first = C.c_void_p(), C.c_uint64(), C.c_int64()
+    ffi.check(L.qwgpu_percentiles_table(img.ptr, img.nbytes, column, C.byref(out), C.byref(nb), C.byref(first)))
+    if not out.value:
+        return int(first.value), []
+    try:
+        return int(first.value), list(C.cast(out, C.POINTER(C.c_uint64))[:nb.value])
+    finally:
+        L.qwgpu_buf_free(out)
+
+
 # ---- multi-GPU partial exchange (SURVEY.md §8e): one fixed-size all-gather stands in for the root merge
 def partial_size(search_request_pb: bytes) -> int:
     L = ffi.lib()
