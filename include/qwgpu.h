@@ -162,6 +162,7 @@ typedef struct qwgpu_split_result {
                                             splits to their first `size` buckets before the copy-back */
 #define QWGPU_KERNEL_DEEP_SELECT 2048u /* a split of the batch asked for more than 4096 hits (max_hits + start_offset)
                                           and took the deep selection path (k_deep_cut, k_deep_sort, k_deep_rank) */
+#define QWGPU_KERNEL_TERM_SET 4096u /* k_term_set: the doc-set pre-pass of the batch's term-set (regex) nodes */
 /* Initial capacity of a split's hashed cell table: min(this, the split's bound on distinct cells). */
 #define QWGPU_HASHED_INIT_CELLS 65536u
 /* Largest total of the hashed tables (cells, key records and slots, each at its split's bound) that one call may
@@ -202,6 +203,13 @@ int qwgpu_agg_layout(const uint8_t* img, uint64_t img_len, const char* split_id,
  * infinite values and QWGPU_EINVALID_AGG for a text or bytes column. */
 int qwgpu_percentiles_table(const uint8_t* img, uint64_t img_len, uint32_t column, uint64_t** edges, uint64_t* num_bins,
                             int64_t* first_bin);
+
+/* The term ordinals of text field `field` whose whole term the regex `regex` matches (as given: no `(?i)` is added for
+ * the field's tokenizer), ascending, as the compiler expands a `regex` query (quickwit_b200/csrc/regex.h), and the
+ * automaton transitions the dictionary walk took. `ords` is freed with qwgpu_buf_free (null when none match). Host
+ * only; tests and tools/bench_regex.py use it to check and time the expansion. */
+int qwgpu_regex_terms(const uint8_t* img, uint64_t img_len, const char* field, const char* regex, uint32_t** ords,
+                      uint64_t* num_ords, uint64_t* transitions);
 
 /* Pre-search pruning (SURVEY.md 8a row a16), host only: what qwgpu_leaf_search does to the request of every
  * split before it searches — CanSplitDoBetter::{from_request, optimize_split_order, optimize}

@@ -172,6 +172,7 @@ typedef struct QwImgColumn {
 #define QW_MAX_PLAN_DEPTH 4
 #define QW_MAX_PHRASE_TERMS 8
 #define QW_MAX_PREFIX_EXPANSIONS 1024 /* expansion children of one PHRASE_PREFIX node */
+#define QW_MAX_SET_TERMS 65536 /* children of one TERM_SET node */
 
 enum {
   QW_NODE_TERM = 1,   /* tantivy TermQuery */
@@ -186,7 +187,7 @@ enum {
                          number of such b. Score = bm25_weight * tf-factor(phrase_count, fieldnorm) with
                          bm25_weight = (sum of the terms' idf, duplicates included) * (1 + K1) * boost
                          (Bm25Weight::for_terms). */
-  QW_NODE_PHRASE_PREFIX = 8 /* tantivy PhrasePrefixQuery with at least one exact term: children = the k exact TERM
+  QW_NODE_PHRASE_PREFIX = 8, /* tantivy PhrasePrefixQuery with at least one exact term: children = the k exact TERM
                                nodes in phrase order, then the E expansion TERM nodes of the last slot (the field's
                                first max_expansions terms, in byte order, that start with the prefix); the node's
                                `lo` = k; each child's `lo` = its position offset, so every expansion carries the last
@@ -195,6 +196,11 @@ enum {
                                term i at b + lo_i for every i and some expansion at b + lo_last. Never scored: the
                                node is only valid where its score is not read (filter / must_not, or any sort
                                other than _score). */
+  QW_NODE_TERM_SET = 9 /* a set of terms (tantivy AutomatonWeight of a regex query): children = E TERM nodes of one
+                          field with strictly increasing term_ord, 1 <= E <= QW_MAX_SET_TERMS. A doc matches when it holds
+                          any child. Positions are not needed, and the children do not count toward the plan's TERM
+                          clauses. Never scored: the node is only valid where its score is not read (filter / must_not,
+                          or any sort other than _score). */
 };
 enum { QW_OCCUR_MUST = 0, QW_OCCUR_SHOULD = 1, QW_OCCUR_MUST_NOT = 2, QW_OCCUR_FILTER = 3 };
 

@@ -13,7 +13,10 @@ namespace qw {
 // The subset of Quickwit's doc mapper JSON this path needs
 // (quickwit-doc-mapper/src/doc_mapper/{doc_mapper_builder.rs,field_mapping_entry.rs}).
 struct DocMapperInfo {
-  struct Field { std::string name, type, tokenizer, fast_precision; };
+  struct Field {
+    std::string name, type, tokenizer, fast_precision;
+    bool indexed = true;  // `indexed: false`: no term dictionary (a fast-only field)
+  };
   std::string timestamp_field;
   std::vector<Field> fields;
   std::vector<std::string> default_search_fields;

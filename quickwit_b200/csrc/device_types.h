@@ -55,13 +55,14 @@ static inline bool qw_fused_sample_plan(const uint32_t* first_work, const uint32
   return true;
 }
 
-enum { OP_TERM = 1, OP_RANGE = 2, OP_EXISTS = 3, OP_ALL = 4, OP_BOOL_BEGIN = 5, OP_BOOL_END = 6, OP_PHRASE = 7 };
+enum { OP_TERM = 1, OP_RANGE = 2, OP_EXISTS = 3, OP_ALL = 4, OP_BOOL_BEGIN = 5, OP_BOOL_END = 6, OP_PHRASE = 7, OP_TERM_SET = 8 };
 enum { IF_SCORED = 1u, IF_HAS_TF = 2u, IF_HAS_FN = 4u, IF_BITS_FROM_SCORE = 8u };
 #define QW_TFF_ROWS 16 /* tf-factor table: tff[tf][fieldnorm_id] = tf / (tf + norm[id]) for tf < 16 */
 
 struct DInstr {  // 64 bytes
   uint32_t op, level, occur, flags;
   uint64_t a, b, c;  // TERM: data_off, widx_off, skip_off | RANGE: lo, hi | PHRASE: a = VBlk[] (device address), c = driver skip_off
+                     // | TERM_SET: a = the node's doc bitmap (device address)
   uint32_t n;        // TERM: num_blocks   | BOOL_END: n_req
   uint32_t m;        // TERM: win_shift    | BOOL_END: n_should
   uint32_t r;        // TERM: fn slot      | RANGE/EXISTS: column | BOOL_END: required_should
@@ -91,6 +92,18 @@ struct DPhrase {
   uint32_t n_exp;       // phrase prefix: number of expansions of the last slot (0 = a plain phrase)
   uint64_t exp;         // phrase prefix: DPhraseTerm[n_exp] (device address; while lowering, index into Lowered)
   DPhraseTerm t[QW_MAX_PHRASE_TERMS];  // phrase prefix: the n_terms exact terms
+};
+
+// A term-set node evaluated by the pre-pass (termset_kernel.cuh) into a doc bitmap of ceil(num_docs / 32) words.
+struct DTermSetNode {
+  uint64_t bitmap;  // device address
+};
+struct DTermSetTerm {
+  uint64_t data, skip;  // the term's posting blocks and skip list (device addresses)
+  uint32_t nblk;        // its posting blocks
+  uint32_t first_block; // prefix of nblk over the batch's term-set terms (the pre-pass's flat block list)
+  uint32_t node;        // DTermSetNode of the batch (while lowering: of the plan)
+  uint32_t pad;
 };
 
 struct DCol {  // 48 bytes

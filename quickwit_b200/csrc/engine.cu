@@ -13,6 +13,7 @@
 #include "kernels.cuh"
 #include "union_kernel.cuh"
 #include "phrase_kernel.cuh"
+#include "termset_kernel.cuh"
 #include "driver_kernel.cuh"
 #include "agg_kernel.cuh"
 #include "trace_kernel.cuh"
@@ -398,6 +399,9 @@ struct Lowered {
   std::vector<DPhrase> phrases;         // phrase pre-pass descriptors (out / first_work filled per batch)
   std::vector<uint32_t> phrase_instr;   // instruction that consumes phrases[i]
   std::vector<DPhraseTerm> phrase_exp;  // expansions of the phrase prefixes (phrases[i].exp indexes it until staging)
+  std::vector<uint32_t> ts_instr;       // term-set nodes (pre-pass bitmaps): the instruction that reads each
+  std::vector<DTermSetTerm> ts_terms;   // their terms (first_block / node relative to this plan until staging)
+  uint32_t ts_blocks = 0;               // posting blocks of ts_terms
   uint32_t tr_img_col = 0;              // find_trace_ids: the trace-id column of the image
   uint64_t h_bound = 0;                 // hashed aggregation layout: upper bound on the split's distinct cells
 };
@@ -645,6 +649,41 @@ static void lower_node(Lowered& L, const SplitDev& sp, const QwPlanNode* nodes, 
       in.f = 0.f;
       L.phrase_instr.push_back((uint32_t)L.instrs.size());
       L.phrases.push_back(ph);
+      L.instrs.push_back(in);
+      break;
+    }
+    case QW_NODE_TERM_SET: {
+      // the pre-pass (termset_kernel.cuh) ORs the children's postings into a doc bitmap; the window program reads it
+      // (OP_TERM_SET), never scored
+      if (n.num_children < 1 || n.num_children > QW_MAX_SET_TERMS || n.first_child + n.num_children > nn)
+        fail(QWGPU_EINVALID_ARG, "term set node with %u terms", n.num_children);
+      if (scored)
+        fail(QWGPU_EUNSUPPORTED, "term set (regex) in a scoring clause of a query ranked by _score is not implemented on the GPU path");
+      uint64_t df = 0;
+      uint32_t field_id = 0;
+      for (uint32_t i = 0; i < n.num_children; i++) {
+        const QwPlanNode& c = nodes[n.first_child + i];
+        if (c.kind != QW_NODE_TERM || c.term_ord >= sp.view.hdr->num_terms) fail(QWGPU_EINVALID_ARG, "term set child %u is not a term of this split", i);
+        if (i && c.term_ord <= nodes[n.first_child + i - 1].term_ord) fail(QWGPU_EINVALID_ARG, "term set children not in increasing term order");
+        const QwImgTerm& t = sp.view.terms[c.term_ord];
+        if (i && t.field_id != field_id) fail(QWGPU_EINVALID_ARG, "term set terms of different fields");
+        field_id = t.field_id;
+        DTermSetTerm r;
+        memset(&r, 0, sizeof r);
+        r.data = (uint64_t)(sp.d_data + t.data_off);
+        r.skip = (uint64_t)(sp.d_data + t.skip_off);
+        r.nblk = t.num_blocks;
+        r.first_block = L.ts_blocks;
+        r.node = (uint32_t)L.ts_instr.size();
+        L.ts_blocks += t.num_blocks;
+        L.ts_terms.push_back(r);
+        df += t.doc_freq;
+        L.alg_bytes += t.data_len - t.fn_len;
+      }
+      L.postings += df;
+      if (occur == QW_OCCUR_MUST || occur == QW_OCCUR_FILTER) L.min_required_df = std::min<uint64_t>(L.min_required_df, std::min<uint64_t>(df, sp.view.hdr->num_docs));
+      in.op = OP_TERM_SET;
+      L.ts_instr.push_back((uint32_t)L.instrs.size());
       L.instrs.push_back(in);
       break;
     }
@@ -1250,6 +1289,9 @@ struct Run {
   bool any_topk, any_deep, any_trace, any_hashed, any_composite, any_fast_aggs;
   uint32_t kmax, deep_cap, n_phrases, phrase_blocks, tie_max_n;
   size_t n_phrase_exp;
+  uint32_t n_ts_nodes, n_ts_terms, ts_blocks;  // term-set pre-pass: nodes, terms and posting blocks of the batch
+  size_t o_tsn, o_tst, s_tsbm, ts_bm_bytes;    // its records (blob) and bitmaps (scratch, one region)
+  std::vector<size_t> ts_bm;                    // per split: offset of its first bitmap from s_tsbm
   size_t o_plans, o_instr, o_cols, o_aggs, o_fwa, o_fws, o_sstr, o_bounds, o_rank, o_smp, o_phr, o_pexp, o_fwd, o_fwds, blob_bytes;
   size_t s_thr, s_hist, s_state, s_wmax, s_sync, s_cand, s_surv, s_deep_m, s_hits, s_cut, s_grecv, s_vblk, s_trace_state, s_trace_data, s_hash, scratch_bytes;
   size_t rec_bytes, o_merged, o_ghdr, o_final, o_err, out_bytes;
@@ -1274,6 +1316,9 @@ struct Run {
     deep_cap = 0;
     n_phrases = phrase_blocks = tie_max_n = 0;
     n_phrase_exp = 0;
+    n_ts_nodes = n_ts_terms = ts_blocks = 0;
+    ts_bm_bytes = 0;
+    ts_bm.assign(n, 0);
   h_keys.assign(n, {});
   h_cells.assign(n, {});
     uint32_t tot_instr = 0, tot_cols = 0, tot_aggs = 0, tot_bounds = 0;
@@ -1296,6 +1341,12 @@ struct Run {
       // phrases: one uncompressed posting block per block of each phrase's driver term (phrase_kernel.cuh)
       for (size_t k = 0; k < L.phrases.size(); k++) { n_phrases++; phrase_blocks += L.instrs[L.phrase_instr[k]].n; }
       n_phrase_exp += L.phrase_exp.size();
+      // term sets: one doc bitmap per node
+      ts_bm[i] = ts_bm_bytes;
+      ts_bm_bytes += L.ts_instr.size() * (size_t)((P.num_docs + 31) / 32) * 4;
+      n_ts_nodes += (uint32_t)L.ts_instr.size();
+      n_ts_terms += (uint32_t)L.ts_terms.size();
+      ts_blocks += L.ts_blocks;
       kmax = std::max(kmax, P.max_hits);
       any_topk |= P.max_hits > 0;
       if (P.max_hits > QW_MAX_TOPK) { any_deep = true; deep_cap = std::max(deep_cap, qw_cand_cap(P.max_hits)); }
@@ -1328,6 +1379,8 @@ struct Run {
     o_smp = blob.take(r.sample_win.size() * 4);
     o_phr = blob.take((size_t)n_phrases * sizeof(DPhrase));
     o_pexp = blob.take(n_phrase_exp * sizeof(DPhraseTerm));
+    o_tsn = blob.take((size_t)n_ts_nodes * sizeof(DTermSetNode));
+    o_tst = blob.take((size_t)n_ts_terms * sizeof(DTermSetTerm));
     o_fwd = blob.take(r.fw_drv.size() * 4);
     o_fwds = blob.take(r.fw_dsm.size() * 4);
     blob_bytes = blob.off;
@@ -1349,6 +1402,8 @@ struct Run {
     s_cut = s.take((size_t)std::max<uint32_t>(n, 64) * 4 + 1024);  // split merge's cut, then the gathered merge's
     s_grecv = s.take(gather && gather->world > 1 && do_merge ? (size_t)gather->world * rec_bytes : 0);
     s_vblk = s.take((size_t)phrase_blocks * sizeof(VBlk));
+    // term-set bitmaps: beyond s_cand, since the exact top-K path clears the prefix again after the pre-pass
+    s_tsbm = s.take(ts_bm_bytes);
     // find_trace_ids: per split a DTraceState (one region, set to 0xFF bytes), then best[] + match bitmap (zeroed)
     s_trace_state = s.take(any_trace ? (size_t)n * sizeof(qwk::DTraceState) : 0);
     s_trace_data = s.off;
@@ -1414,7 +1469,7 @@ struct Run {
   // the run's plans get the slot's addresses; everything the kernels read goes to the device in one copy
   void stage() {
     uint8_t *hb = slot.h_blob, *db = slot.d_blob;
-    uint32_t phr_done = 0, phr_blocks_done = 0;
+    uint32_t phr_done = 0, phr_blocks_done = 0, tsn_done = 0, tst_done = 0, tsb_done = 0;
     size_t pexp_done = 0;
     for (uint32_t i = 0; i < n; i++) {
       const Lowered& L = low[i];
@@ -1456,6 +1511,19 @@ struct Run {
         phr_blocks_done += instrs[L.phrase_instr[k]].n;
         memcpy(hb + o_phr + (size_t)phr_done++ * sizeof(DPhrase), &ph, sizeof ph);
       }
+      for (size_t k = 0; k < L.ts_instr.size(); k++) {
+        DTermSetNode nd;
+        nd.bitmap = (uint64_t)(slot.d_scratch + s_tsbm + ts_bm[i] + k * (size_t)((P.num_docs + 31) / 32) * 4);
+        instrs[L.ts_instr[k]].a = nd.bitmap;
+        memcpy(hb + o_tsn + (size_t)(tsn_done + k) * sizeof(DTermSetNode), &nd, sizeof nd);
+      }
+      for (DTermSetTerm t : L.ts_terms) {
+        t.first_block += tsb_done;
+        t.node += tsn_done;
+        memcpy(hb + o_tst + (size_t)tst_done++ * sizeof(DTermSetTerm), &t, sizeof t);
+      }
+      tsn_done += (uint32_t)L.ts_instr.size();
+      tsb_done += L.ts_blocks;
       memcpy(hb + o_plans + i * sizeof(DSplitPlan), &P, sizeof P);
       if (P.n_cols) memcpy(hb + o_cols + P.col_base * sizeof(DCol), L.cols.data(), P.n_cols * sizeof(DCol));
       DAgg* aggs = (DAgg*)(hb + o_aggs) + P.agg_base;
@@ -1713,6 +1781,18 @@ struct Run {
       else qwk::k_phrase<false><<<pgrid, QP_WARPS * 32, psm, slot.stream>>>(d_phr, n_phrases, phrase_blocks, max_terms);
       stats.launches++;
       stats.kernel_mask |= QWGPU_KERNEL_PHRASE;
+    }
+    if (ts_bm_bytes) {
+      // term-set pre-pass (inside the timed device region): every term-set node of the batch becomes a doc bitmap in
+      // scratch, read by every later pass (cleared for every node, whether or not its terms hold a block)
+      CUDA_CHECK(cudaMemsetAsync(slot.d_scratch + s_tsbm, 0, ts_bm_bytes, st));
+    }
+    if (ts_blocks) {
+      const uint32_t tgrid = std::min<uint32_t>((ts_blocks + QS_WARPS - 1) / QS_WARPS, (uint32_t)e.sm_count * 8);
+      qwk::k_term_set<<<tgrid, QS_WARPS * 32, 0, st>>>((const DTermSetTerm*)(slot.d_blob + o_tst), n_ts_terms,
+                                                       (const DTermSetNode*)(slot.d_blob + o_tsn), ts_blocks);
+      stats.launches++;
+      stats.kernel_mask |= QWGPU_KERNEL_TERM_SET;
     }
     stats.window_docs = r.kind == Route::DRIVER ? QW_BLOCK_LEN : r.W;
     std::vector<uint32_t> state(n, 0);  // per split: 1 = its sampled threshold failed

@@ -1203,6 +1203,24 @@ __global__ void __launch_bounds__(QW_THREADS, QW_MIN_BLOCKS_PER_SM) k_window(con
             __syncthreads();
           }
           ip++;
+      } else if (op == OP_TERM_SET) {
+        // the node's doc bitmap from the pre-pass (termset_kernel.cuh): windows start on a word, and the words past
+        // num_docs are zero; never scored
+        const uint32_t* bm = (const uint32_t*)in.a + (ws >> 5);
+        const uint32_t nwv = (wlen + 31) >> 5;
+        const bool required = occur == QW_OCCUR_MUST || occur == QW_OCCUR_FILTER;
+        const bool init = (req_init >> level) & 1;
+        uint32_t* tgt = sm.u32(required ? LV.req : occur == QW_OCCUR_SHOULD ? LV.shd : LV.nt);
+        for (uint32_t wd = tid; wd < NW; wd += QW_THREADS) {
+          const uint32_t m = wd < nwv ? __ldg(bm + wd) : 0u;
+          if (required) tgt[wd] = init ? (tgt[wd] & m) : m;
+          else tgt[wd] |= m;
+          if (occur == QW_OCCUR_SHOULD && LV.cnt != 0xFFFFFFFFu)
+            for (uint32_t x = m; x; x &= x - 1) sm.u8(LV.cnt)[wd * 32 + __ffs(x) - 1]++;
+        }
+        if (required) req_init |= 1u << level;
+        __syncthreads();
+        ip++;
       } else if (op == OP_RANGE || op == OP_EXISTS || op == OP_ALL) {
         const bool required = occur == QW_OCCUR_MUST || occur == QW_OCCUR_FILTER;
         const bool init = (req_init >> level) & 1;

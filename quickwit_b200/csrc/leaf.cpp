@@ -13,6 +13,7 @@
 #include <chrono>
 #include <tuple>
 
+#include "regex.h"
 #include "compile.h"
 #include "ddsketch.h"
 #include "device_types.h"
@@ -911,6 +912,27 @@ int qwgpu_agg_layout(const uint8_t* img, uint64_t img_len, const char* split_id,
   }
   *hashed = qw_agg_hashed(aggs, ph->num_aggs) ? 1u : 0u;
   *bound_cells = *hashed ? qw::agg_hashed_layout(aggs, ph->num_aggs, v, split_id ? split_id : "") : 0;
+  return 0;
+  QW_API_END
+}
+
+int qwgpu_regex_terms(const uint8_t* img, uint64_t img_len, const char* field, const char* regex, uint32_t** ords, uint64_t* num_ords,
+                      uint64_t* transitions) {
+  QW_API_BEGIN
+  qw::ImageView v;
+  v.open(img, img_len);
+  const int f = v.find_field(field ? field : "");
+  if (f < 0) qw::fail(QWGPU_EINVALID_ARG, "no text field `%s` in the split", field ? field : "");
+  qw::rx::Regex re(regex ? regex : "");
+  const std::vector<uint32_t> out = re.matching_terms(v, (uint32_t)f);
+  *ords = nullptr;
+  if (!out.empty()) {
+    *ords = (uint32_t*)malloc(out.size() * 4);
+    if (!*ords) qw::fail(QWGPU_EINTERNAL, "out of host memory");
+    memcpy(*ords, out.data(), out.size() * 4);
+  }
+  *num_ords = out.size();
+  *transitions = re.transitions();
   return 0;
   QW_API_END
 }

@@ -18,6 +18,7 @@
 #include <climits>
 
 #include "compile.h"
+#include "regex.h"
 
 namespace qw {
 
@@ -102,6 +103,7 @@ DocMapperInfo parse_doc_mapper(const std::string& json) {
       fi.type = f.str_or("type", "text");
       fi.tokenizer = f.str_or("tokenizer", "default");
       fi.fast_precision = f.str_or("fast_precision", "seconds");
+      fi.indexed = f.bool_or("indexed", true);
       dm.fields.push_back(fi);
     }
   if (const Json* d = root->get("default_search_fields"))
@@ -127,9 +129,10 @@ static int64_t truncate_ns(int64_t ns, int64_t prec) {  // DateTime::truncate
 
 // ---- TantivyQueryAst mirror ------------------------------------------------------------------------
 struct TQ {
-  enum Kind { Bool, Term, Range, Exists, All, None, Phrase, PhrasePrefix } kind = None;
+  enum Kind { Bool, Term, Range, Exists, All, None, Phrase, PhrasePrefix, TermSet } kind = None;
   std::vector<uint32_t> phrase_terms;  // Phrase / PhrasePrefix: (exact) term ords in phrase order (offset k = position k)
-  std::vector<uint32_t> prefix_terms;  // PhrasePrefix: the expansions of the last slot (offset = phrase_terms.size())
+  std::vector<uint32_t> prefix_terms;  // PhrasePrefix: the expansions of the last slot (offset = phrase_terms.size());
+                                       // TermSet: the term ords of one field, ascending
   bool opaque = false;  // wrapped in a BoostQuery leaf: not subject to bool flattening / const folding
   std::vector<TQ> must, must_not, should, filter;
   bool has_msm = false;
@@ -414,6 +417,34 @@ static TQ phrase_prefix_leaf(const Ctx& cx, uint32_t f, const std::vector<std::s
   return outer;
 }
 
+// RegexQuery::to_resolved + build_tantivy_ast_impl (regex_query.rs): the field must be an indexed text field; a
+// tokenizer that lowercases prefixes `(?i)` unless the pattern's leading flags already hold an `i`. The pattern is
+// parsed before the split's terms are looked at, so a bad pattern fails on every split. The matching terms become one
+// TERM_SET node: tantivy's AutomatonWeight is constant-score, so it is served wherever its score is not read.
+static TQ regex_leaf(const Ctx& cx, const std::string& field, const std::string& regex) {
+  const int f = cx.img.find_field(field);
+  const DocMapperInfo::Field* fd = nullptr;
+  for (auto& d : cx.dm.fields) if (d.name == field) fd = &d;
+  const int c = cx.img.find_column(field);
+  if (f < 0) {
+    if ((c >= 0 && cx.img.columns[c].type != QW_COL_STR) || (fd && fd->type != "text" && fd->type != "json"))
+      fail(QWGPU_EINVALID_QUERY, "invalid query: trying to run a regex query on a non-text field");
+    if (c >= 0 || (fd && !fd->indexed)) fail(QWGPU_EINVALID_QUERY, "invalid query: field %s is not full-text searchable", field.c_str());
+    if (!fd) fail(QWGPU_EINVALID_QUERY, "invalid query: field does not exist: `%s`", field.c_str());
+  }
+  const bool lowercases = f >= 0 ? cx.img.fields[f].tokenizer != QW_TOK_RAW : fd->tokenizer != "raw";
+  rx::Regex re(lowercases && !rx::has_case_insensitive_flag(regex) ? "(?i)" + regex : regex);
+  if (f < 0) return tq_none();  // declared in the doc mapping but without a single term in this split
+  refuse_const_score_under_ranking(cx, "regex");
+  TQ t;
+  t.kind = TQ::TermSet;
+  t.prefix_terms = re.matching_terms(cx.img, (uint32_t)f);
+  if (t.prefix_terms.empty()) return tq_none();
+  if (t.prefix_terms.size() > QW_MAX_SET_TERMS)
+    fail(QWGPU_EUNSUPPORTED, "regex with %zu expansions in split (the GPU path takes at most %d)", t.prefix_terms.size(), QW_MAX_SET_TERMS);
+  return t;
+}
+
 static TQ range_leaf(uint32_t column, uint64_t lo, uint64_t hi) {
   TQ t;
   t.kind = TQ::Range;
@@ -694,8 +725,7 @@ static TQ build(const Ctx& cx, const Json& q, int depth) {
   }
   if (type == "user_input")
     fail(QWGPU_EINVALID_QUERY, "invalid query: user_input queries must be parsed by the root before reaching a leaf");
-  if (type == "regex")
-    fail(QWGPU_EUNSUPPORTED, "`%s` queries are not implemented on the GPU path yet", type.c_str());
+  if (type == "regex") return regex_leaf(cx, q.str_or("field", ""), q.str_or("regex", ""));
   fail(QWGPU_EINVALID_QUERY, "invalid query: unknown query type `%s`", type.c_str());
 }
 
@@ -765,6 +795,24 @@ static void emit(const TQ& t, uint32_t occur, const ImageView& img, std::vector<
         c.term_ord = i < k ? t.phrase_terms[i] : t.prefix_terms[i - k]; c.field_id = field_id; c.column = 0xFFFFFFFFu;
         c.bm25_weight = bm25_idf(img.terms[c.term_ord].doc_freq, img.hdr->num_docs) * (1.0f + BM25_K1);
         c.lo = i < k ? i : k;  // position offset inside the phrase; every expansion sits in the last slot
+      }
+      break;
+    }
+    case TQ::TermSet: {
+      // never scored (refused in scoring clauses under _score ranking): children = the terms, ascending
+      n.kind = QW_NODE_TERM_SET;
+      const uint32_t field_id = img.terms[t.prefix_terms[0]].field_id;
+      n.field_id = field_id;
+      const size_t first = out.size(), e = t.prefix_terms.size();  // (`n` dangles after the resize below)
+      out[idx].first_child = (uint32_t)first;
+      out[idx].num_children = (uint32_t)e;
+      out.resize(first + e);
+      for (size_t i = 0; i < e; i++) {
+        QwPlanNode& c = out[first + i];
+        memset(&c, 0, sizeof c);
+        c.kind = QW_NODE_TERM; c.occur = QW_OCCUR_SHOULD; c.boost = 1.0f; c.min_should_match = 0xFFFFFFFFu;
+        c.term_ord = t.prefix_terms[i]; c.field_id = field_id; c.column = 0xFFFFFFFFu;
+        c.bm25_weight = bm25_idf(img.terms[c.term_ord].doc_freq, img.hdr->num_docs) * (1.0f + BM25_K1);
       }
       break;
     }

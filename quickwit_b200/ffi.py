@@ -22,7 +22,9 @@ COL_U64, COL_I64, COL_F64, COL_BOOL, COL_DATETIME, COL_STR, COL_BYTES = range(7)
 CARD_FULL, CARD_OPTIONAL, CARD_MULTI = range(3)
 NODE_TERM, NODE_RANGE, NODE_BOOL, NODE_ALL, NODE_NONE, NODE_EXISTS, NODE_PHRASE = 1, 2, 3, 4, 5, 6, 7
 NODE_PHRASE_PREFIX = 8
+NODE_TERM_SET = 9  # children: 1..MAX_SET_TERMS TERM nodes of one field, increasing term_ord; never scored
 MAX_PHRASE_TERMS, MAX_PREFIX_EXPANSIONS = 8, 1024
+MAX_SET_TERMS = 65536
 OCCUR_MUST, OCCUR_SHOULD, OCCUR_MUST_NOT, OCCUR_FILTER = range(4)
 SORT_NONE, SORT_DOCID, SORT_SCORE, SORT_COLUMN = range(4)
 ORDER_ASC, ORDER_DESC = 0, 1
@@ -34,6 +36,7 @@ KERNEL_UNION, KERNEL_DRIVER, KERNEL_AGGSCAN, KERNEL_WINDOW, KERNEL_PHRASE = 1, 2
 KERNEL_TRACE_SELECT, KERNEL_TRACE_REPLAY, KERNEL_FAST_AGGS = 32, 64, 128
 KERNEL_HASHED_AGGS, KERNEL_HASHED_AGGS_RETRY, KERNEL_COMPOSITE_CUT = 256, 512, 1024
 KERNEL_DEEP_SELECT = 2048
+KERNEL_TERM_SET = 4096
 # hashed aggregation cells (qwgpu_format.h qw_agg_hashed, qwgpu.h): dense-layout limits, the initial capacity of a
 # split's table, the largest table a split may need, the `missing` flag of an entry
 AGG_DENSE_MAX_CELLS, AGG_DENSE_MAX_TERMS = 1 << 26, 1 << 24
@@ -211,6 +214,7 @@ def lib() -> C.CDLL:
     bind("qwgpu_build_leaf_response", [vp, u64, cp, vp, sz, cp, u64, vp, u32, vp, u32, C.POINTER(vp), C.POINTER(sz)])
     bind("qwgpu_build_leaf_response_entries", [vp, u64, cp, vp, sz, cp, u64, vp, u32, vp, u32, C.POINTER(vp), C.POINTER(sz)])
     bind("qwgpu_agg_layout", [vp, u64, cp, vp, sz, C.POINTER(u32), C.POINTER(u64)])
+    bind("qwgpu_regex_terms", [vp, u64, cp, cp, C.POINTER(vp), C.POINTER(u64), C.POINTER(u64)])
     bind("qwgpu_percentiles_table", [vp, u64, u32, C.POINTER(vp), C.POINTER(u64), C.POINTER(C.c_int64)])
     bind("qwgpu_merge_leaf_responses", [vp, sz, u32, C.POINTER(vp), C.POINTER(sz),
                                         C.POINTER(vp), C.POINTER(sz)])

@@ -103,6 +103,17 @@ def phrase_prefix_as_phrases(node: Node, occur: Optional[int] = None) -> Node:
     return Node(ffi.NODE_BOOL, node.occur if occur is None else occur, children=phrases)
 
 
+def term_set(img: SplitImage, field: str, ords: Sequence[int], occur=ffi.OCCUR_FILTER) -> Node:
+    """A TERM_SET node (the expansions of a regex query): a doc matches when it holds any of the term ords `ords` of
+    `field` (ascending). Never scored. No ords: matches nothing."""
+    if not ords:
+        return Node(ffi.NODE_NONE, occur)
+    fid = img.field_names().index(field)
+    kids = [Node(ffi.NODE_TERM, ffi.OCCUR_SHOULD, term_ord=o, field_id=fid, weight=bm25_weight(img.doc_freq(o), img.num_docs))
+            for o in ords]
+    return Node(ffi.NODE_TERM_SET, occur, children=kids, field_id=fid)
+
+
 def range_(img: SplitImage, column: str, lo: int, hi: int, occur=ffi.OCCUR_FILTER, boost=1.0) -> Node:
     c = img.column_ord(column)
     return Node(ffi.NODE_RANGE, occur, boost, column=c if c >= 0 else ffi.ABSENT, lo=lo, hi=hi)

@@ -330,6 +330,20 @@ def percentiles_table(img: SplitImage, column: int) -> Tuple[int, List[int]]:
         L.qwgpu_buf_free(out)
 
 
+def regex_terms(img: SplitImage, field: str, regex: str) -> Tuple[List[int], int]:
+    """(term ords of `field` whose whole term `regex` matches, ascending; automaton transitions of the dictionary walk)
+    (qwgpu_regex_terms: the pattern as given, without the tokenizer's `(?i)`)."""
+    L = ffi.lib()
+    out, n, steps = C.c_void_p(), C.c_uint64(), C.c_uint64()
+    ffi.check(L.qwgpu_regex_terms(img.ptr, img.nbytes, field.encode(), regex.encode(), C.byref(out), C.byref(n), C.byref(steps)))
+    if not out.value:
+        return [], int(steps.value)
+    try:
+        return list(C.cast(out, C.POINTER(C.c_uint32))[:n.value]), int(steps.value)
+    finally:
+        L.qwgpu_buf_free(out)
+
+
 # ---- multi-GPU partial exchange (SURVEY.md §8e): one fixed-size all-gather stands in for the root merge
 def partial_size(search_request_pb: bytes) -> int:
     L = ffi.lib()
