@@ -163,6 +163,9 @@ typedef struct qwgpu_split_result {
 #define QWGPU_KERNEL_DEEP_SELECT 2048u /* a split of the batch asked for more than 4096 hits (max_hits + start_offset)
                                           and took the deep selection path (k_deep_cut, k_deep_sort, k_deep_rank) */
 #define QWGPU_KERNEL_TERM_SET 4096u /* k_term_set: the doc-set pre-pass of the batch's term-set (regex) nodes */
+#define QWGPU_KERNEL_PHRASE_LONG 8192u /* k_phrase_long: the pre-pass of the batch's phrases of more than
+                                          QW_MAX_PHRASE_TERMS terms (k_phrase, and QWGPU_KERNEL_PHRASE, serve the
+                                          shorter ones) */
 /* Initial capacity of a split's hashed cell table: min(this, the split's bound on distinct cells). */
 #define QWGPU_HASHED_INIT_CELLS 65536u
 /* Largest total of the hashed tables (cells, key records and slots, each at its split's bound) that one call may

@@ -170,7 +170,9 @@ typedef struct QwImgColumn {
 
 #define QW_PLAN_MAGIC 0x4E4C5051u /* "QPLN" */
 #define QW_MAX_PLAN_DEPTH 4
-#define QW_MAX_PHRASE_TERMS 8
+#define QW_MAX_PHRASE_TERMS 8 /* exact terms of one PHRASE_PREFIX node (plus one); PHRASE nodes above it run the
+                                 long-phrase pre-pass */
+#define QW_MAX_PHRASE_LEN 256 /* TERM children of one PHRASE node */
 #define QW_MAX_PREFIX_EXPANSIONS 1024 /* expansion children of one PHRASE_PREFIX node */
 #define QW_MAX_SET_TERMS 65536 /* children of one TERM_SET node */
 
@@ -182,7 +184,8 @@ enum {
   QW_NODE_NONE = 5,   /* EmptyQuery */
   QW_NODE_EXISTS = 6, /* ExistsQuery on a column; const score 1 */
   QW_NODE_PHRASE = 7, /* tantivy PhraseQuery, slop 0: children = its TERM nodes in phrase order, all of one field
-                         with positions; child k's `lo` = position offset of the term inside the phrase. A doc
+                         with positions, 2 <= children <= QW_MAX_PHRASE_LEN; child k's `lo` = position offset of
+                         the term inside the phrase. A doc
                          matches when some base position b has term k at b + lo_k for every k; phrase_count =
                          number of such b. Score = bm25_weight * tf-factor(phrase_count, fieldnorm) with
                          bm25_weight = (sum of the terms' idf, duplicates included) * (1 + K1) * boost

@@ -90,8 +90,10 @@ struct DPhrase {
   uint32_t n_terms, driver, scored;
   uint32_t first_work;  // prefix of driver blocks over the batch's phrases
   uint32_t n_exp;       // phrase prefix: number of expansions of the last slot (0 = a plain phrase)
-  uint64_t exp;         // phrase prefix: DPhraseTerm[n_exp] (device address; while lowering, index into Lowered)
-  DPhraseTerm t[QW_MAX_PHRASE_TERMS];  // phrase prefix: the n_terms exact terms
+  uint64_t exp;         // phrase prefix: DPhraseTerm[n_exp]; phrase of more than QW_MAX_PHRASE_TERMS terms
+                        // (k_phrase_long): DPhraseTerm[n_terms], the driver first, then by ascending doc_freq
+                        // (device address; while lowering, index into Lowered::phrase_ext)
+  DPhraseTerm t[QW_MAX_PHRASE_TERMS];  // up to QW_MAX_PHRASE_TERMS terms (phrase prefix: the n_terms exact terms)
 };
 
 // A term-set node evaluated by the pre-pass (termset_kernel.cuh) into a doc bitmap of ceil(num_docs / 32) words.

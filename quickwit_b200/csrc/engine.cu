@@ -398,7 +398,8 @@ struct Lowered {
   bool empty = false;                   // a required clause of the root cannot match in this split: no work at all
   std::vector<DPhrase> phrases;         // phrase pre-pass descriptors (out / first_work filled per batch)
   std::vector<uint32_t> phrase_instr;   // instruction that consumes phrases[i]
-  std::vector<DPhraseTerm> phrase_exp;  // expansions of the phrase prefixes (phrases[i].exp indexes it until staging)
+  std::vector<DPhraseTerm> phrase_ext;  // term records outside DPhrase: the expansions of phrase prefixes and the terms
+                                        // of long phrases (phrases[i].exp indexes it until staging)
   std::vector<uint32_t> ts_instr;       // term-set nodes (pre-pass bitmaps): the instruction that reads each
   std::vector<DTermSetTerm> ts_terms;   // their terms (first_block / node relative to this plan until staging)
   uint32_t ts_blocks = 0;               // posting blocks of ts_terms
@@ -559,9 +560,12 @@ static void lower_node(Lowered& L, const SplitDev& sp, const QwPlanNode* nodes, 
       break;
     }
     case QW_NODE_PHRASE: {
-      // evaluated by the pre-pass (phrase_kernel.cuh) into one uncompressed posting block per block of its
-      // rarest term; the window program consumes those blocks (OP_PHRASE)
-      if (n.num_children < 2 || n.num_children > QW_MAX_PHRASE_TERMS || n.first_child + n.num_children > nn)
+      // evaluated by a pre-pass (phrase_kernel.cuh) into one uncompressed posting block per block of its rarest
+      // term; the window program consumes those blocks (OP_PHRASE). Up to QW_MAX_PHRASE_TERMS terms: k_phrase, the
+      // terms inline in DPhrase::t. Longer: k_phrase_long, the terms in phrase_ext, the driver first and then by
+      // ascending doc_freq so that candidates die as early as possible (the phrase count is an intersection of
+      // position sets: the order cannot change it)
+      if (n.num_children < 2 || n.num_children > QW_MAX_PHRASE_LEN || n.first_child + n.num_children > nn)
         fail(QWGPU_EINVALID_ARG, "phrase node with %u terms", n.num_children);
       DPhrase ph;
       memset(&ph, 0, sizeof ph);
@@ -572,6 +576,7 @@ static void lower_node(Lowered& L, const SplitDev& sp, const QwPlanNode* nodes, 
       uint64_t best_df = ~0ull;
       const QwImgField* fld = nullptr;
       uint32_t field_id = 0;
+      std::vector<std::pair<uint64_t, DPhraseTerm>> terms;  // (doc_freq, record) in phrase order
       for (uint32_t k = 0; k < n.num_children; k++) {
         const QwPlanNode& c = nodes[n.first_child + k];
         if (c.kind != QW_NODE_TERM || c.term_ord >= sp.view.hdr->num_terms) fail(QWGPU_EINVALID_ARG, "phrase term %u is not a term of this split", k);
@@ -580,12 +585,24 @@ static void lower_node(Lowered& L, const SplitDev& sp, const QwPlanNode* nodes, 
         if (k && t.field_id != field_id) fail(QWGPU_EINVALID_ARG, "phrase terms of different fields");
         field_id = t.field_id;
         fld = &sp.view.fields[t.field_id];
-        ph.t[k].data_off = t.data_off; ph.t[k].skip_off = t.skip_off; ph.t[k].pos_off = t.pos_off; ph.t[k].pidx_off = t.pidx_off;
-        ph.t[k].nblk = t.num_blocks; ph.t[k].offset = (uint32_t)c.lo;
+        DPhraseTerm pt;
+        memset(&pt, 0, sizeof pt);
+        pt.data_off = t.data_off; pt.skip_off = t.skip_off; pt.pos_off = t.pos_off; pt.pidx_off = t.pidx_off;
+        pt.nblk = t.num_blocks; pt.offset = (uint32_t)c.lo;
+        terms.push_back({t.doc_freq, pt});
         if (t.doc_freq < best_df) { best_df = t.doc_freq; ph.driver = k; }
         L.alg_bytes += t.data_len - t.fn_len;
       }
       const QwImgTerm& drv = sp.view.terms[nodes[n.first_child + ph.driver].term_ord];
+      if (n.num_children <= QW_MAX_PHRASE_TERMS) {
+        for (uint32_t k = 0; k < n.num_children; k++) ph.t[k] = terms[k].second;
+      } else {
+        // a stable sort keeps the first rarest term (the driver above) in front
+        std::stable_sort(terms.begin(), terms.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
+        ph.exp = L.phrase_ext.size();
+        ph.driver = 0;
+        for (const auto& x : terms) L.phrase_ext.push_back(x.second);
+      }
       L.postings += drv.doc_freq;
       L.alg_bytes += (uint64_t)drv.doc_freq * 4 * n.num_children;  // positions probed per candidate (lower bound)
       if (occur == QW_OCCUR_MUST || occur == QW_OCCUR_FILTER) L.min_required_df = std::min<uint64_t>(L.min_required_df, drv.doc_freq);
@@ -617,7 +634,7 @@ static void lower_node(Lowered& L, const SplitDev& sp, const QwPlanNode* nodes, 
       ph.data_base = (uint64_t)sp.d_data;
       ph.n_terms = k;
       ph.n_exp = n_exp;
-      ph.exp = L.phrase_exp.size();
+      ph.exp = L.phrase_ext.size();
       ph.fn_off = ~0ull;
       uint64_t best_df = ~0ull;
       uint32_t field_id = 0;
@@ -636,7 +653,7 @@ static void lower_node(Lowered& L, const SplitDev& sp, const QwPlanNode* nodes, 
         if (i < k) {
           ph.t[i] = pt;
           if (t.doc_freq < best_df) { best_df = t.doc_freq; ph.driver = i; }
-        } else L.phrase_exp.push_back(pt);
+        } else L.phrase_ext.push_back(pt);
         L.alg_bytes += t.data_len - t.fn_len;
       }
       const QwImgTerm& drv = sp.view.terms[nodes[n.first_child + ph.driver].term_ord];
@@ -1287,12 +1304,15 @@ struct Run {
   struct Split { size_t out, cand, tr_best, tr_match, h_table, h_keys, h_cells; };  // offsets of a split's regions
   std::vector<Split> at;
   bool any_topk, any_deep, any_trace, any_hashed, any_composite, any_fast_aggs;
-  uint32_t kmax, deep_cap, n_phrases, phrase_blocks, tie_max_n;
-  size_t n_phrase_exp;
+  uint32_t kmax, deep_cap, tie_max_n;
+  uint32_t n_phrases, phrase_blocks;            // k_phrase: phrases of up to QW_MAX_PHRASE_TERMS terms, their driver blocks
+  uint32_t n_phrases_long, phrase_blocks_long;  // k_phrase_long: the longer phrases
+  size_t n_phrase_ext;                          // DPhraseTerm records outside DPhrase (Lowered::phrase_ext)
+  bool any_prefix;                              // a phrase prefix: k_phrase<true>
   uint32_t n_ts_nodes, n_ts_terms, ts_blocks;  // term-set pre-pass: nodes, terms and posting blocks of the batch
   size_t o_tsn, o_tst, s_tsbm, ts_bm_bytes;    // its records (blob) and bitmaps (scratch, one region)
   std::vector<size_t> ts_bm;                    // per split: offset of its first bitmap from s_tsbm
-  size_t o_plans, o_instr, o_cols, o_aggs, o_fwa, o_fws, o_sstr, o_bounds, o_rank, o_smp, o_phr, o_pexp, o_fwd, o_fwds, blob_bytes;
+  size_t o_plans, o_instr, o_cols, o_aggs, o_fwa, o_fws, o_sstr, o_bounds, o_rank, o_smp, o_phr, o_phl, o_pext, o_fwd, o_fwds, blob_bytes;
   size_t s_thr, s_hist, s_state, s_wmax, s_sync, s_cand, s_surv, s_deep_m, s_hits, s_cut, s_grecv, s_vblk, s_trace_state, s_trace_data, s_hash, scratch_bytes;
   size_t rec_bytes, o_merged, o_ghdr, o_final, o_err, out_bytes;
   // the collect pass samples its own threshold (qw_fused_sample_plan): its cooperative grid and per-split sample weights
@@ -1314,8 +1334,9 @@ struct Run {
     any_topk = any_deep = any_trace = any_hashed = any_composite = any_fast_aggs = false;
     kmax = 1;
     deep_cap = 0;
-    n_phrases = phrase_blocks = tie_max_n = 0;
-    n_phrase_exp = 0;
+    n_phrases = phrase_blocks = n_phrases_long = phrase_blocks_long = tie_max_n = 0;
+    n_phrase_ext = 0;
+    any_prefix = false;
     n_ts_nodes = n_ts_terms = ts_blocks = 0;
     ts_bm_bytes = 0;
     ts_bm.assign(n, 0);
@@ -1339,8 +1360,13 @@ struct Run {
         P.h_mask = agg_hashed_slots(P.h_cap) - 1;
       }
       // phrases: one uncompressed posting block per block of each phrase's driver term (phrase_kernel.cuh)
-      for (size_t k = 0; k < L.phrases.size(); k++) { n_phrases++; phrase_blocks += L.instrs[L.phrase_instr[k]].n; }
-      n_phrase_exp += L.phrase_exp.size();
+      for (size_t k = 0; k < L.phrases.size(); k++) {
+        const bool lng = L.phrases[k].n_terms > QW_MAX_PHRASE_TERMS;
+        (lng ? n_phrases_long : n_phrases)++;
+        (lng ? phrase_blocks_long : phrase_blocks) += L.instrs[L.phrase_instr[k]].n;
+        any_prefix |= L.phrases[k].n_exp != 0;
+      }
+      n_phrase_ext += L.phrase_ext.size();
       // term sets: one doc bitmap per node
       ts_bm[i] = ts_bm_bytes;
       ts_bm_bytes += L.ts_instr.size() * (size_t)((P.num_docs + 31) / 32) * 4;
@@ -1378,7 +1404,8 @@ struct Run {
     o_rank = blob.take((size_t)n * 4);
     o_smp = blob.take(r.sample_win.size() * 4);
     o_phr = blob.take((size_t)n_phrases * sizeof(DPhrase));
-    o_pexp = blob.take(n_phrase_exp * sizeof(DPhraseTerm));
+    o_phl = blob.take((size_t)n_phrases_long * sizeof(DPhrase));
+    o_pext = blob.take(n_phrase_ext * sizeof(DPhraseTerm));
     o_tsn = blob.take((size_t)n_ts_nodes * sizeof(DTermSetNode));
     o_tst = blob.take((size_t)n_ts_terms * sizeof(DTermSetTerm));
     o_fwd = blob.take(r.fw_drv.size() * 4);
@@ -1401,7 +1428,7 @@ struct Run {
     s_hits = s.take(do_merge ? (size_t)n * kmax * sizeof(QwHit) : 0);
     s_cut = s.take((size_t)std::max<uint32_t>(n, 64) * 4 + 1024);  // split merge's cut, then the gathered merge's
     s_grecv = s.take(gather && gather->world > 1 && do_merge ? (size_t)gather->world * rec_bytes : 0);
-    s_vblk = s.take((size_t)phrase_blocks * sizeof(VBlk));
+    s_vblk = s.take((size_t)(phrase_blocks + phrase_blocks_long) * sizeof(VBlk));
     // term-set bitmaps: beyond s_cand, since the exact top-K path clears the prefix again after the pre-pass
     s_tsbm = s.take(ts_bm_bytes);
     // find_trace_ids: per split a DTraceState (one region, set to 0xFF bytes), then best[] + match bitmap (zeroed)
@@ -1469,8 +1496,9 @@ struct Run {
   // the run's plans get the slot's addresses; everything the kernels read goes to the device in one copy
   void stage() {
     uint8_t *hb = slot.h_blob, *db = slot.d_blob;
-    uint32_t phr_done = 0, phr_blocks_done = 0, tsn_done = 0, tst_done = 0, tsb_done = 0;
-    size_t pexp_done = 0;
+    uint32_t phr_done = 0, phl_done = 0, phr_blocks_done = 0, phl_blocks_done = 0, vblk_done = 0;
+    uint32_t tsn_done = 0, tst_done = 0, tsb_done = 0;
+    size_t pext_done = 0;
     for (uint32_t i = 0; i < n; i++) {
       const Lowered& L = low[i];
       DSplitPlan& P = plans[i];
@@ -1498,18 +1526,24 @@ struct Run {
       }
       DInstr* instrs = (DInstr*)(hb + o_instr) + P.instr_base;
       memcpy(instrs, L.instrs.data(), P.n_instr * sizeof(DInstr));
+      // short and long phrases go to their own kernel's array, each numbering its driver blocks from 0
       for (size_t k = 0; k < L.phrases.size(); k++) {
         DPhrase ph = L.phrases[k];
-        ph.first_work = phr_blocks_done;
-        ph.out = (uint64_t)(slot.d_scratch + s_vblk + (size_t)phr_blocks_done * sizeof(VBlk));
-        if (ph.n_exp) {
-          memcpy(hb + o_pexp + pexp_done * sizeof(DPhraseTerm), L.phrase_exp.data() + ph.exp, (size_t)ph.n_exp * sizeof(DPhraseTerm));
-          ph.exp = (uint64_t)(db + o_pexp + pexp_done * sizeof(DPhraseTerm));
-          pexp_done += ph.n_exp;
+        const bool lng = ph.n_terms > QW_MAX_PHRASE_TERMS;
+        const uint32_t nb = instrs[L.phrase_instr[k]].n;
+        ph.first_work = lng ? phl_blocks_done : phr_blocks_done;
+        ph.out = (uint64_t)(slot.d_scratch + s_vblk + (size_t)vblk_done * sizeof(VBlk));
+        const uint32_t n_ext = ph.n_exp ? ph.n_exp : lng ? ph.n_terms : 0;
+        if (n_ext) {
+          memcpy(hb + o_pext + pext_done * sizeof(DPhraseTerm), L.phrase_ext.data() + ph.exp, (size_t)n_ext * sizeof(DPhraseTerm));
+          ph.exp = (uint64_t)(db + o_pext + pext_done * sizeof(DPhraseTerm));
+          pext_done += n_ext;
         }
         instrs[L.phrase_instr[k]].a = ph.out;
-        phr_blocks_done += instrs[L.phrase_instr[k]].n;
-        memcpy(hb + o_phr + (size_t)phr_done++ * sizeof(DPhrase), &ph, sizeof ph);
+        vblk_done += nb;
+        (lng ? phl_blocks_done : phr_blocks_done) += nb;
+        if (lng) memcpy(hb + o_phl + (size_t)phl_done++ * sizeof(DPhrase), &ph, sizeof ph);
+        else memcpy(hb + o_phr + (size_t)phr_done++ * sizeof(DPhrase), &ph, sizeof ph);
       }
       for (size_t k = 0; k < L.ts_instr.size(); k++) {
         DTermSetNode nd;
@@ -1771,16 +1805,24 @@ struct Run {
     if (phrase_blocks) {
       // phrase pre-pass (inside the timed device region): every phrase of the batch becomes a posting list in
       // scratch (beyond s_cand: never cleared), read by every later pass
-      uint32_t max_terms = 1;
-      for (const Lowered& L : low) for (const DPhrase& ph : L.phrases) max_terms = std::max(max_terms, ph.n_terms);
+      uint32_t max_terms = 1;  // (over k_phrase's phrases only: a long phrase does not widen its shared memory)
+      for (const Lowered& L : low)
+        for (const DPhrase& ph : L.phrases) if (ph.n_terms <= QW_MAX_PHRASE_TERMS) max_terms = std::max(max_terms, ph.n_terms);
       const size_t psm = (size_t)QP_WARPS * QP_SMEM_WORDS(max_terms) * 4;
       const uint32_t pgrid = (phrase_blocks + QP_WARPS - 1) / QP_WARPS;
       const DPhrase* d_phr = (const DPhrase*)(slot.d_blob + o_phr);
       // the suffix stage of phrase prefixes lives in its own instantiation: plain phrases keep the lean kernel
-      if (n_phrase_exp) qwk::k_phrase<true><<<pgrid, QP_WARPS * 32, psm, slot.stream>>>(d_phr, n_phrases, phrase_blocks, max_terms);
+      if (any_prefix) qwk::k_phrase<true><<<pgrid, QP_WARPS * 32, psm, slot.stream>>>(d_phr, n_phrases, phrase_blocks, max_terms);
       else qwk::k_phrase<false><<<pgrid, QP_WARPS * 32, psm, slot.stream>>>(d_phr, n_phrases, phrase_blocks, max_terms);
       stats.launches++;
       stats.kernel_mask |= QWGPU_KERNEL_PHRASE;
+    }
+    if (phrase_blocks_long) {
+      // long-phrase pre-pass (phrase_kernel.cuh): the same output, shared memory independent of the phrase length
+      qwk::k_phrase_long<<<(phrase_blocks_long + QP_WARPS - 1) / QP_WARPS, QP_WARPS * 32, 0, slot.stream>>>(
+          (const DPhrase*)(slot.d_blob + o_phl), n_phrases_long, phrase_blocks_long);
+      stats.launches++;
+      stats.kernel_mask |= QWGPU_KERNEL_PHRASE_LONG;
     }
     if (ts_bm_bytes) {
       // term-set pre-pass (inside the timed device region): every term-set node of the batch becomes a doc bitmap in

@@ -340,4 +340,156 @@ __global__ void __launch_bounds__(QP_WARPS * 32) k_phrase(const DPhrase* phrases
   *reinterpret_cast<float4*>(&out->val[lane * 4]) = make_float4(oval[0], oval[1], oval[2], oval[3]);
 }
 
+// ---- phrases of more than QW_MAX_PHRASE_TERMS terms (k_phrase_long) ------------------------------------------------
+// k_phrase keeps every term's {first position index, tf} of all 128 candidates in shared memory, which grows with the
+// phrase. The long pre-pass keeps no per-term state: its terms (ph.exp, the driver first, then by ascending doc_freq)
+// are taken once each, and every present candidate at once narrows its surviving base positions to those where the
+// term lines up. The survivors are a 32-bit mask over one round of 32 driver positions; a candidate whose driver tf
+// exceeds 32 takes the term loop again for each further round of 32. A candidate dies when it lacks a term or its
+// mask empties, and a round ends as soon as no candidate of the warp holds a survivor, so a mismatch at an early term
+// costs that term only. Shared memory per warp: the decoded block of the term being probed, whatever the length.
+
+// the bits i of `mask` whose base pd[i] - off_d has a position base + off_t among the sorted pt[0, nt)
+__device__ __forceinline__ uint32_t phrase_narrow(const uint32_t* pd, uint32_t mask, uint32_t off_d, const uint32_t* pt,
+                                                  uint32_t nt, uint32_t off_t) {
+  uint32_t keep = 0, from = 0;
+  while (mask) {
+    const uint32_t i = __ffs(mask) - 1;
+    mask &= mask - 1;
+    const uint32_t p = __ldg(pd + i);
+    if (p < off_d) continue;  // the phrase would start before position 0
+    const uint32_t want = p - off_d + off_t;
+    uint32_t lo = from, hi = nt;  // the wanted positions ascend with i: search past the previous hit only
+    while (lo < hi) {
+      const uint32_t mid = (lo + hi) >> 1;
+      if (__ldg(pt + mid) < want) lo = mid + 1; else hi = mid;
+    }
+    if (lo == nt) break;
+    from = lo;
+    if (__ldg(pt + lo) == want) keep |= 1u << i;
+  }
+  return keep;
+}
+
+__global__ void __launch_bounds__(QP_WARPS * 32) k_phrase_long(const DPhrase* phrases, uint32_t n_phrases, uint32_t total_blocks) {
+  __shared__ __align__(16) uint32_t ql_smem[QP_WARPS][3 * QW_BLOCK_LEN];
+  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  uint32_t* bdoc = ql_smem[warp]; uint32_t* bpre = bdoc + QW_BLOCK_LEN; uint32_t* btf = bdoc + 2 * QW_BLOCK_LEN;
+  const uint32_t work = blockIdx.x * QP_WARPS + warp;
+  if (work >= total_blocks) return;
+  uint32_t pi = 0;
+  while (pi + 1 < n_phrases && phrases[pi + 1].first_work <= work) pi++;
+  const DPhrase& ph = phrases[pi];
+  const uint32_t b = work - ph.first_work;
+  const uint8_t* base = (const uint8_t*)ph.data_base;
+  const DPhraseTerm* terms = (const DPhraseTerm*)ph.exp;
+  const DPhraseTerm& D = terms[0];
+
+  // ---- 1. driver block ------------------------------------------------------------------------------------
+  const QwSkip* dsk = (const QwSkip*)(base + D.skip_off);
+  uint32_t cdoc[4], ctf[4], cpre[4], count;
+  phrase_decode(base + D.data_off + __ldg(&dsk[b].byte_off), lane, cdoc, ctf, count);
+  block_excl_prefix(ctf, lane, cpre);
+  const uint32_t* dpos = (const uint32_t*)(base + D.pos_off) + __ldg((const uint32_t*)(base + D.pidx_off) + b);
+  const uint32_t off_d = D.offset;
+  const uint32_t doc_first = __shfl_sync(0xFFFFFFFFu, cdoc[0], 0);
+  const uint32_t doc_last = __ldg(&dsk[b].last_doc);
+  uint32_t present = 0;  // bit j: candidate j holds every term looked up so far
+#pragma unroll
+  for (int j = 0; j < 4; j++) if (lane * 4 + j < count) present |= 1u << j;
+  uint32_t matches[4] = {0, 0, 0, 0};
+
+  // ---- 2. rounds of 32 driver positions, each narrowed by the other terms in order ------------------------------
+  for (uint32_t r0 = 0;; r0 += 32) {
+    uint32_t mask[4], live = 0;  // live bit j: candidate j still has a survivor in this round
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+      const uint32_t left = ((present >> j) & 1u) && ctf[j] > r0 ? ctf[j] - r0 : 0u;
+      mask[j] = left >= 32 ? 0xFFFFFFFFu : (1u << left) - 1u;
+      if (left) live |= 1u << j;
+    }
+    if (!__ballot_sync(0xFFFFFFFFu, live != 0)) break;
+    for (uint32_t t = 1; t < ph.n_terms; t++) {
+      const DPhraseTerm& T = terms[t];
+      const QwSkip* sk = (const QwSkip*)(base + T.skip_off);
+      const uint32_t* pidx = (const uint32_t*)(base + T.pidx_off);
+      const uint32_t* tpos = (const uint32_t*)(base + T.pos_off);
+      // the blocks of term t that can hold the driver block's docs: a short run [r_lo, r_hi] (as in k_phrase)
+      const uint32_t r_lo = phrase_first_block(sk, T.nblk, doc_first, lane);
+      const uint32_t r_hi = r_lo < T.nblk ? r_lo + phrase_first_block(sk + r_lo, T.nblk - r_lo, doc_last, lane) : T.nblk;
+      uint32_t need[4];
+#pragma unroll
+      for (int j = 0; j < 4; j++) {
+        need[j] = QP_NONE;
+        if ((live >> j) & 1u) {
+          uint32_t lo = r_lo, hi = min(r_hi + 1, T.nblk);
+          while (lo < hi) {
+            const uint32_t mid = (lo + hi) >> 1;
+            if (__ldg(&sk[mid].last_doc) < cdoc[j]) lo = mid + 1; else hi = mid;
+          }
+          if (lo < T.nblk) need[j] = lo;
+          else { present &= ~(1u << j); live &= ~(1u << j); mask[j] = 0; }
+        }
+      }
+      for (;;) {
+        uint32_t cur = min(min(need[0], need[1]), min(need[2], need[3]));
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) cur = min(cur, __shfl_xor_sync(0xFFFFFFFFu, cur, o));
+        if (cur == QP_NONE) break;
+        uint32_t d[4], f[4], pre[4], cnt;
+        phrase_decode(base + T.data_off + __ldg(&sk[cur].byte_off), lane, d, f, cnt);
+        block_excl_prefix(f, lane, pre);
+        __syncwarp();
+#pragma unroll
+        for (int j = 0; j < 4; j++) {
+          bdoc[lane * 4 + j] = lane * 4 + j < cnt ? d[j] : QP_NONE;  // (padding sorts last)
+          bpre[lane * 4 + j] = pre[j];
+          btf[lane * 4 + j] = f[j];
+        }
+        __syncwarp();
+        const uint32_t first = __ldg(pidx + cur);
+#pragma unroll
+        for (int j = 0; j < 4; j++) {
+          if (need[j] != cur) continue;
+          need[j] = QP_NONE;
+          uint32_t lo = 0, hi = cnt;
+          while (lo < hi) {
+            const uint32_t mid = (lo + hi) >> 1;
+            if (bdoc[mid] < cdoc[j]) lo = mid + 1; else hi = mid;
+          }
+          if (lo < cnt && bdoc[lo] == cdoc[j]) {
+            mask[j] = phrase_narrow(dpos + cpre[j] + r0, mask[j], off_d, tpos + first + bpre[lo], btf[lo], T.offset);
+            if (!mask[j]) live &= ~(1u << j);
+          } else { present &= ~(1u << j); live &= ~(1u << j); mask[j] = 0; }
+        }
+      }
+      if (!__ballot_sync(0xFFFFFFFFu, live != 0)) break;  // no survivor left in the warp: the later terms are moot
+    }
+#pragma unroll
+    for (int j = 0; j < 4; j++) matches[j] += __popc(mask[j]);
+  }
+
+  // ---- 3. output: k_phrase's scoring of phrase_count = matches ------------------------------------------------
+  VBlk* out = (VBlk*)ph.out + b;
+  uint32_t odoc[4];
+  float oval[4];
+#pragma unroll
+  for (int j = 0; j < 4; j++) {
+    odoc[j] = QP_NONE;
+    oval[j] = 0.f;
+    if (!matches[j]) continue;
+    odoc[j] = cdoc[j];
+    if (ph.scored) {
+      const float* tab = (const float*)ph.tab;
+      const uint32_t fn = ph.fn_off != ~0ull ? (uint32_t)__ldg(base + ph.fn_off + cdoc[j]) : 1u;
+      float tfn;
+      if (matches[j] < QW_TFF_ROWS) tfn = __ldg(tab + 256 + matches[j] * 256 + fn);
+      else { const float tff = (float)matches[j]; tfn = __fdiv_rn(tff, __fadd_rn(tff, __ldg(tab + fn))); }
+      oval[j] = __fmul_rn(ph.weight, tfn);
+    }
+  }
+  *reinterpret_cast<uint4*>(&out->doc[lane * 4]) = make_uint4(odoc[0], odoc[1], odoc[2], odoc[3]);
+  *reinterpret_cast<float4*>(&out->val[lane * 4]) = make_float4(oval[0], oval[1], oval[2], oval[3]);
+}
+
 }  // namespace qwk

@@ -492,7 +492,7 @@ static TQ full_text(const Ctx& cx, const std::string& field, const std::string& 
     if (!has_positions)
       fail(QWGPU_EINVALID_QUERY, "invalid query: Applied phrase query on field which does not have positions indexed");
     if (slop != 0) fail(QWGPU_EUNSUPPORTED, "phrase queries with slop > 0 are not implemented on the GPU path yet");
-    if (tokens.size() > QW_MAX_PHRASE_TERMS) fail(QWGPU_EUNSUPPORTED, "phrases of more than %d terms are not implemented on the GPU path", QW_MAX_PHRASE_TERMS);
+    if (tokens.size() > QW_MAX_PHRASE_LEN) fail(QWGPU_EUNSUPPORTED, "phrases of more than %d terms are not implemented on the GPU path", QW_MAX_PHRASE_LEN);
     // TantivyPhraseQuery::new_with_offset(terms) (full_text_query.rs:140-156): a term missing from the split
     // means no doc can match
     TQ ph;

@@ -24,6 +24,7 @@ NODE_TERM, NODE_RANGE, NODE_BOOL, NODE_ALL, NODE_NONE, NODE_EXISTS, NODE_PHRASE 
 NODE_PHRASE_PREFIX = 8
 NODE_TERM_SET = 9  # children: 1..MAX_SET_TERMS TERM nodes of one field, increasing term_ord; never scored
 MAX_PHRASE_TERMS, MAX_PREFIX_EXPANSIONS = 8, 1024
+MAX_PHRASE_LEN = 256  # TERM children of one NODE_PHRASE; above MAX_PHRASE_TERMS they run the long-phrase pre-pass
 MAX_SET_TERMS = 65536
 OCCUR_MUST, OCCUR_SHOULD, OCCUR_MUST_NOT, OCCUR_FILTER = range(4)
 SORT_NONE, SORT_DOCID, SORT_SCORE, SORT_COLUMN = range(4)
@@ -37,6 +38,7 @@ KERNEL_TRACE_SELECT, KERNEL_TRACE_REPLAY, KERNEL_FAST_AGGS = 32, 64, 128
 KERNEL_HASHED_AGGS, KERNEL_HASHED_AGGS_RETRY, KERNEL_COMPOSITE_CUT = 256, 512, 1024
 KERNEL_DEEP_SELECT = 2048
 KERNEL_TERM_SET = 4096
+KERNEL_PHRASE_LONG = 8192
 # hashed aggregation cells (qwgpu_format.h qw_agg_hashed, qwgpu.h): dense-layout limits, the initial capacity of a
 # split's table, the largest table a split may need, the `missing` flag of an entry
 AGG_DENSE_MAX_CELLS, AGG_DENSE_MAX_TERMS = 1 << 26, 1 << 24
