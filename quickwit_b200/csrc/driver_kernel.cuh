@@ -78,88 +78,38 @@ __global__ void __launch_bounds__(QD_WARPS * 32) k_driver(const DrvParams p) {
     for (uint32_t w = seg + warp; w < seg_end; w += QD_WARPS) {
       const uint32_t bb = (w - fw) * p.stride + (p.stride > 1 ? split % p.stride : 0);
       const uint8_t* blk = tdata + __ldg(&skips[bb].byte_off);
-      const uint4 h = __ldg(reinterpret_cast<const uint4*>(blk));  // QwSkip: last_doc, prev_last_doc, byte_off, bits/count
-      const uint32_t prev = h.y, doc_bits = h.w & 0xFF, tf_bits = (h.w >> 8) & 0xFF, count = h.w >> 16;
-      const uint4* dp = reinterpret_cast<const uint4*>(blk + 16);
-      uint32_t v[4] = {0, 0, 0, 0};
-      if (doc_bits) {
-        const uint32_t bitpos = lane * doc_bits, wi = bitpos >> 5, sh = bitpos & 31;
-        const uint4 A = __ldg(dp + wi);
-        const uint4 B = (sh + doc_bits > 32) ? __ldg(dp + wi + 1) : make_uint4(0, 0, 0, 0);
-        const uint32_t mask = 0xFFFFFFFFu >> (32 - doc_bits);
-        v[0] = __funnelshift_r(A.x, B.x, sh) & mask; v[1] = __funnelshift_r(A.y, B.y, sh) & mask;
-        v[2] = __funnelshift_r(A.z, B.z, sh) & mask; v[3] = __funnelshift_r(A.w, B.w, sh) & mask;
-      }
-      const uint32_t d0 = v[0] + 1, d1 = d0 + v[1] + 1, d2 = d1 + v[2] + 1, d3 = d2 + v[3] + 1;
-      uint32_t incl = d3;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t n = __shfl_up_sync(QW_FULL, incl, o);
-        if ((int)lane >= o) incl += n;
-      }
-      const uint32_t basev = prev + (incl - d3);  // mod 2^32
-      const uint32_t doc[4] = {basev + d0, basev + d1, basev + d2, basev + d3};
-      uint32_t tf[4] = {1, 1, 1, 1};
-      if (scored && has_tf && tf_bits) {
-        const uint4* tp = dp + doc_bits;
-        const uint32_t bitpos = lane * tf_bits, wi = bitpos >> 5, sh = bitpos & 31;
-        const uint4 A = __ldg(tp + wi);
-        const uint4 B = (sh + tf_bits > 32) ? __ldg(tp + wi + 1) : make_uint4(0, 0, 0, 0);
-        const uint32_t mask = 0xFFFFFFFFu >> (32 - tf_bits);
-        tf[0] = __funnelshift_r(A.x, B.x, sh) & mask; tf[1] = __funnelshift_r(A.y, B.y, sh) & mask;
-        tf[2] = __funnelshift_r(A.z, B.z, sh) & mask; tf[3] = __funnelshift_r(A.w, B.w, sh) & mask;
-      }
+      const BlkHdr h = blk_header<LdgLoad>(blk);
+      uint32_t doc[4], tf[4] = {1, 1, 1, 1};
+      blk_docs<LdgLoad>(blk, h, 0, lane, doc);
+      if (scored && has_tf) blk_tfs<LdgLoad>(blk, h, lane, tf);
       uint32_t fnw = 0x01010101u;  // no fieldnorms: constant fieldnorm id 1
-      if (scored && has_fn) fnw = __ldg(reinterpret_cast<const uint32_t*>(blk + 16u + 16u * (doc_bits + tf_bits)) + lane);
+      if (scored && has_fn) fnw = __ldg(reinterpret_cast<const uint32_t*>(blk + 16u + 16u * (h.doc_bits + h.tf_bits)) + lane);
 
 #pragma unroll
       for (int j = 0; j < 4; j++) {
-        bool on = lane * 4 + j < count;
+        bool on = lane * 4 + j < h.count;
         // ---- required column filters (FastFieldRangeQuery / ExistsQuery docsets) ------------------------------
         for (uint32_t f = 0; f < n_filters && on; f++) {
           const DInstr& fi = prog[2 + f];
           if (fi.r == 0xFFFFFFFFu) { on = false; break; }  // column absent from the split: nothing matches
-          const DCol& c = cols[fi.r];
-          uint64_t a, b;
-          col_range(base, c, doc[j], a, b);
-          if (fi.op == OP_EXISTS) on = a != b;
-          else {
-            bool hit = false;
-            for (uint64_t k = a; k < b && !hit; k++) {
-              const uint64_t mv = c.min_value + c.gcd * col_raw(base, c, k);
-              hit = mv >= fi.a && mv <= fi.b;
-            }
-            on = hit;
-          }
+          on = col_match(base, cols[fi.r], doc[j], fi.op, fi.a, fi.b);
         }
         my_hits += on ? 1u : 0u;
         if (!max_hits) continue;
-        // ---- BM25 of the posting: weight * tf-factor (Bm25Weight::score), same table / divide as fold_block -----
+        // ---- BM25 of the posting: weight * tf-factor (Bm25Weight::score) --------------------------------------
         float sc = 0.0f;
-        if (scored && on) {
-          const uint32_t fn = (fnw >> (8 * j)) & 0xFFu;
-          float tfn;
-          if (tf[j] < QW_TFF_ROWS) tfn = __ldg(tab + 256 + tf[j] * 256 + fn);
-          else { const float tff = (float)tf[j]; tfn = __fdiv_rn(tff, __fadd_rn(tff, __ldg(tab + fn))); }
-          sc = __fmul_rn(term.f, tfn);
-        }
+        if (scored && on) sc = __fmul_rn(term.f, tf_factor(tab, tf[j], (fnw >> (8 * j)) & 0xFFu));
         if (MODE == MODE_COLLECT) {
           if (!on) continue;
           if (sa_present) {
             const DocKey dk = doc_key(P, ks, cols, base, doc[j], sc);
             if (dk.eligible) {
               my_elig++;
-              if (key_ge(dk.key, thr)) {
-                const uint32_t pos = atomicAdd((uint32_t*)P.out_cand_count, 1u);
-                if (pos < qw_cand_cap(max_hits)) { uint64_t* c = (uint64_t*)P.out_cands + 3ull * pos; c[0] = dk.key.w0; c[1] = dk.key.w1; c[2] = dk.key.w2; }
-              }
+              if (key_ge(dk.key, thr)) push_cand(P, dk.key);
             }
           } else if (key_top11(P, ks, cols, base, doc[j], sc) >= thr_top) {
             const DocKey dk = doc_key(P, ks, cols, base, doc[j], sc);
-            if (key_ge(dk.key, thr)) {
-              const uint32_t pos = atomicAdd((uint32_t*)P.out_cand_count, 1u);
-              if (pos < qw_cand_cap(max_hits)) { uint64_t* c = (uint64_t*)P.out_cands + 3ull * pos; c[0] = dk.key.w0; c[1] = dk.key.w1; c[2] = dk.key.w2; }
-            }
+            if (key_ge(dk.key, thr)) push_cand(P, dk.key);
           }
         } else {
           uint32_t digit = 0;

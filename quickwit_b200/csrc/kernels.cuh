@@ -9,8 +9,8 @@
 //      staged with 16-byte cp.async copies at the same time;
 //   2. the packed posting bytes of ALL terms are staged with cp.async (16-byte, coalesced) while the
 //      same load round turns the terms' skip-list entries into the window's block table;
-//   3. terms are decoded block-per-warp (4-lane-interleaved bit-unpack -> warp-shuffle prefix scan ->
-//      doc ids), BM25 is applied in f32 and accumulated into per-window score arrays in the
+//   3. terms are decoded block-per-warp (posting.cuh: 4-lane-interleaved bit-unpack -> warp-shuffle
+//      prefix scan -> doc ids), BM25 is applied in f32 and accumulated into per-window score arrays in the
 //      reference's clause order (bit-reproducible sums, one barrier per clause; batches of the
 //      BM25-union shape run k_union in union_kernel.cuh instead) — and match sets are shared-memory
 //      bitmaps combined with AND / OR / AND-NOT exactly like tantivy's BooleanWeight;
@@ -24,6 +24,7 @@
 #include <cuda_runtime.h>
 
 #include "device_types.h"
+#include "posting.cuh"
 
 namespace qwk {
 
@@ -42,6 +43,15 @@ __device__ __forceinline__ bool key_ge(const Key& a, const Key& b) {
   return a.w2 >= b.w2;
 }
 __device__ __forceinline__ bool key_lt(const Key& a, const Key& b) { return !key_ge(a, b); }
+
+// appends a composite key to the split's candidate list for k_select; past qw_cand_cap(max_hits) only the count grows
+__device__ __forceinline__ void push_cand(const DSplitPlan& P, const Key& k) {
+  const uint32_t pos = atomicAdd((uint32_t*)P.out_cand_count, 1u);
+  if (pos < qw_cand_cap(P.max_hits)) {
+    uint64_t* c = (uint64_t*)P.out_cands + 3ull * pos;
+    c[0] = k.w0; c[1] = k.w1; c[2] = k.w2;
+  }
+}
 
 // ORs the low `nbits` bits of v (v < 2^nbits) into the key at bit position `pos`, counted from the
 // most significant bit of the 192-bit string
@@ -125,6 +135,18 @@ __device__ __forceinline__ void col_range(const uint8_t* base, const DCol& c, ui
   a = __ldg(start + d);
   b = __ldg(start + d + 1);
 }
+// OP_EXISTS: doc d has a value in column c; OP_RANGE: some value of doc d lies in [lo, hi]
+__device__ __forceinline__ bool col_match(const uint8_t* base, const DCol& c, uint32_t d, uint32_t op, uint64_t lo, uint64_t hi) {
+  uint64_t a, b;
+  col_range(base, c, d, a, b);
+  if (op == OP_EXISTS) return a != b;
+  bool hit = false;
+  for (uint64_t k = a; k < b && !hit; k++) {
+    const uint64_t mv = c.min_value + c.gcd * col_raw(base, c, k);
+    hit = mv >= lo && mv <= hi;
+  }
+  return hit;
+}
 
 __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc) {
   uint32_t s = (uint32_t)__cvta_generic_to_shared(smem_dst);
@@ -159,59 +181,26 @@ struct TermTarget {
   uint32_t cnt;
   uint32_t score;
   uint32_t fn;     // staged fieldnorm ids of the window (absent: constant fieldnorm id 1)
-  const float* gtab;  // global: float[256] BM25 norms then float[QW_TFF_ROWS][256] tf factors (read via L1)
+  const float* gtab;  // global: the BM25 table of tf_factor (posting.cuh), read via L1
   float weight;
   bool has_tf;
 };
 
-// Decode one posting block (header + 4-lane-interleaved bit-packed doc deltas + tfs) with one warp
-// and fold the postings that fall into [ws, we) into the target (all targets live in shared
-// memory). STAGED: the block bytes are in shared memory at qw_smem + blk_off; otherwise `gblk`
-// points to global memory.
+// Decode one posting block (posting.cuh) with one warp and fold the postings that fall into [ws, we)
+// into the target (all targets live in shared memory). STAGED: the block bytes are in shared memory at
+// qw_smem + blk_off; otherwise `gblk` points to global memory (direct mode). Both are read with plain loads.
 template <bool SCORED, bool CNT, bool STAGED, bool BITS = true>
 __device__ __forceinline__ void fold_block(uint32_t blk_off, const uint8_t* gblk, uint32_t ws, uint32_t rlo, uint32_t rlen, const TermTarget& tg, uint32_t lane) {
   const uint8_t* blk = STAGED ? (qw_smem + blk_off) : gblk;
-  const uint4 h = *reinterpret_cast<const uint4*>(blk);  // QwSkip: last_doc, prev_last_doc, byte_off, bits/count
-  const uint32_t last_doc = h.x, prev = h.y;
-  const uint32_t doc_bits = h.w & 0xFF, tf_bits = (h.w >> 8) & 0xFF, count = h.w >> 16;
+  const BlkHdr h = blk_header<PlainLoad>(blk);
   // accepted docs: ws + rlo <= doc < ws + rlo + rlen (targets are indexed by doc - ws)
-  if (last_doc < ws + rlo) return;
-  if (prev != QW_NO_PREV_DOC && prev + 1 >= ws + rlo + rlen) return;
-  const uint4* dp = reinterpret_cast<const uint4*>(blk + 16);
-  uint32_t v0 = 0, v1 = 0, v2 = 0, v3 = 0;
-  if (doc_bits) {
-    uint32_t bitpos = lane * doc_bits, wi = bitpos >> 5, sh = bitpos & 31;
-    uint4 A = dp[wi];
-    uint4 B = (sh + doc_bits > 32) ? dp[wi + 1] : make_uint4(0, 0, 0, 0);
-    uint32_t mask = 0xFFFFFFFFu >> (32 - doc_bits);
-    v0 = __funnelshift_r(A.x, B.x, sh) & mask;
-    v1 = __funnelshift_r(A.y, B.y, sh) & mask;
-    v2 = __funnelshift_r(A.z, B.z, sh) & mask;
-    v3 = __funnelshift_r(A.w, B.w, sh) & mask;
-  }
-  // strictly-sorted deltas: doc[i] = doc[i-1] + v[i] + 1
-  uint32_t d0 = v0 + 1, d1 = d0 + v1 + 1, d2 = d1 + v2 + 1, d3 = d2 + v3 + 1;
-  uint32_t incl = d3;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    uint32_t n = __shfl_up_sync(0xFFFFFFFFu, incl, o);
-    if ((int)lane >= o) incl += n;
-  }
-  const uint32_t basev = prev + (incl - d3) - ws;  // mod 2^32; window-relative
-  uint32_t rel[4] = {basev + d0, basev + d1, basev + d2, basev + d3};
-  const uint32_t nvalid = count > lane * 4 ? count - lane * 4 : 0;  // postings of this lane that exist
+  if (h.last_doc < ws + rlo) return;
+  if (h.prev != QW_NO_PREV_DOC && h.prev + 1 >= ws + rlo + rlen) return;
+  uint32_t rel[4];
+  blk_docs<PlainLoad>(blk, h, ws, lane, rel);  // window-relative
+  const uint32_t nvalid = h.count > lane * 4 ? h.count - lane * 4 : 0;  // postings of this lane that exist
   uint32_t tf[4] = {1, 1, 1, 1};
-  if (SCORED && tg.has_tf && tf_bits) {
-    const uint4* tp = dp + doc_bits;
-    uint32_t bitpos = lane * tf_bits, wi = bitpos >> 5, sh = bitpos & 31;
-    uint4 A = tp[wi];
-    uint4 B = (sh + tf_bits > 32) ? tp[wi + 1] : make_uint4(0, 0, 0, 0);
-    uint32_t mask = 0xFFFFFFFFu >> (32 - tf_bits);
-    tf[0] = __funnelshift_r(A.x, B.x, sh) & mask;
-    tf[1] = __funnelshift_r(A.y, B.y, sh) & mask;
-    tf[2] = __funnelshift_r(A.z, B.z, sh) & mask;
-    tf[3] = __funnelshift_r(A.w, B.w, sh) & mask;
-  }
+  if (SCORED && tg.has_tf) blk_tfs<PlainLoad>(blk, h, lane, tf);
   uint32_t* bits = reinterpret_cast<uint32_t*>(qw_smem + tg.bits);
   float* score = reinterpret_cast<float*>(qw_smem + tg.score);
   const float* tab = tg.gtab;
@@ -231,14 +220,11 @@ __device__ __forceinline__ void fold_block(uint32_t blk_off, const uint8_t* gblk
     float tfn[4], old[4];
 #pragma unroll
     for (int j = 0; j < 4; j++) {
-      // Bm25Weight::score: weight * (tf / (tf + cache[fieldnorm_id])), f32 round-to-nearest; the
-      // quotient comes from a table built with the same IEEE ops for tf < 16
-      const uint32_t t = tf[j];
+      // Bm25Weight::score: weight * tf-factor
       tfn[j] = 0.0f;
       old[j] = 0.0f;
       if (in[j]) {
-        if (t < QW_TFF_ROWS) tfn[j] = __ldg(tab + 256 + t * 256 + f[j]);
-        else { float tff = (float)t; tfn[j] = __fdiv_rn(tff, __fadd_rn(tff, __ldg(tab + f[j]))); }
+        tfn[j] = tf_factor(tab, tf[j], f[j]);
         old[j] = score[rel[j]];
       }
     }
@@ -939,24 +925,6 @@ __device__ __forceinline__ void warp_for_hits(const uint32_t* res, uint32_t NW, 
   if (cnt) body(lane < cnt ? (uint32_t)q[lane] : 0u, lane < cnt);
 }
 
-// Warp-cooperative 32-ary search of a term's skip list: ordinal of the first block whose last doc
-// is >= ws (nblk when there is none). All lanes return the same value.
-__device__ __forceinline__ uint32_t first_block_ge(const QwSkip* skips, uint32_t nblk, uint32_t ws, uint32_t lane) {
-  uint32_t a = 0, b = nblk;
-  while (b - a > 32) {
-    uint32_t step = (b - a + 31) >> 5;
-    uint32_t idx = a + lane * step;
-    bool ok = idx < b && __ldg(&skips[idx].last_doc) >= ws;
-    uint32_t m = __ballot_sync(0xFFFFFFFFu, ok);
-    if (m == 0) a = a + ((b - 1 - a) / step) * step + 1;
-    else { uint32_t f = __ffs(m) - 1; b = a + f * step + 1; if (f > 0) a = a + (f - 1) * step + 1; }
-  }
-  uint32_t idx = a + lane;
-  bool ok = idx < b && __ldg(&skips[idx].last_doc) >= ws;
-  uint32_t m = __ballot_sync(0xFFFFFFFFu, ok);
-  return m ? a + (__ffs(m) - 1) : nblk;
-}
-
 struct BlkRec {  // one staged posting block of the window
   uint16_t soff;  // byte offset of the block inside the stage area
   uint16_t lo;    // lower bound of its first doc, window-relative, clamped to [0, W]
@@ -1235,17 +1203,7 @@ __global__ void __launch_bounds__(QW_THREADS, QW_MIN_BLOCKS_PER_SM) k_window(con
           // 32 per warp step (compacted), and clear the bits of those that fail
           uint16_t* rq = (uint16_t*)sm.u8(p.sm.rangeq) + warp * QW_HITQ_CAP;
           warp_for_hits(req, NW, warp, lane, rq, [&](uint32_t i, bool on) {
-            bool hit = false;
-            if (on && has_col) {
-              const DCol& c = s_cols[col];
-              uint64_t a, b;
-              col_range(base, c, ws + i, a, b);
-              if (op == OP_EXISTS) hit = a != b;
-              else for (uint64_t k = a; k < b && !hit; k++) {
-                uint64_t mv = c.min_value + c.gcd * col_raw(base, c, k);
-                hit = mv >= lo && mv <= hi;
-              }
-            }
+            const bool hit = on && has_col && col_match(base, s_cols[col], ws + i, op, lo, hi);
             if (on && !hit) atomicAnd(&req[i >> 5], ~(1u << (i & 31)));
             if (hit && scored) sm.f32(LV.msum)[i] = __fadd_rn(sm.f32(LV.msum)[i], boost);
           });
@@ -1258,20 +1216,7 @@ __global__ void __launch_bounds__(QW_THREADS, QW_MIN_BLOCKS_PER_SM) k_window(con
             if (rw == 0) continue;  // warp-uniform
             cand = cand && ((rw >> lane) & 1);
           }
-          bool hit = false;
-          if (cand) {
-            if (op == OP_ALL) hit = true;
-            else {
-              const DCol& c = s_cols[col];
-              uint64_t a, b;
-              col_range(base, c, d, a, b);
-              if (op == OP_EXISTS) hit = a != b;
-              else for (uint64_t i = a; i < b && !hit; i++) {
-                uint64_t mv = c.min_value + c.gcd * col_raw(base, c, i);
-                hit = mv >= lo && mv <= hi;
-              }
-            }
-          }
+          const bool hit = cand && (op == OP_ALL || col_match(base, s_cols[col], d, op, lo, hi));
           const uint32_t word = __ballot_sync(0xFFFFFFFFu, hit);
           const uint32_t di = wd * 32 + lane;
           if (required) {
@@ -1385,18 +1330,11 @@ __global__ void __launch_bounds__(QW_THREADS, QW_MIN_BLOCKS_PER_SM) k_window(con
       uint32_t my_hits = 0, my_elig = 0, my_top = 0;
       // hit count: one popc per bitmap word
       if (!p.cands_only) for (uint32_t wd = tid; wd < NW; wd += QW_THREADS) my_hits += __popc(res[wd]);
-      auto emit = [&](const Key& k) {
-        const uint32_t pos = atomicAdd((uint32_t*)P.out_cand_count, 1u);
-        if (pos < qw_cand_cap(P.max_hits)) {
-          uint64_t* c = (uint64_t*)P.out_cands + 3ull * pos;
-          c[0] = k.w0; c[1] = k.w1; c[2] = k.w2;
-        }
-      };
       auto slow_path = [&](uint32_t i, float sc) {
         DocKey dk = doc_key(P, ks, s_cols, base, ws + i, sc);
         if (dk.eligible) {
           my_elig++;
-          if (key_ge(dk.key, thr)) emit(dk.key);
+          if (key_ge(dk.key, thr)) push_cand(P, dk.key);
         }
       };
       if (max_hits && ks.kind[0] == QW_SORT_SCORE && ks.order[0] == QW_ORDER_DESC && !sa_present && rscore && !n_aggs && !rec) {
@@ -1429,7 +1367,7 @@ __global__ void __launch_bounds__(QW_THREADS, QW_MIN_BLOCKS_PER_SM) k_window(con
                   ranked = true;
                   my_elig++;
                   top = (uint32_t)(dk.key.w0 >> 53);
-                  if (key_ge(dk.key, thr)) emit(dk.key);
+                  if (key_ge(dk.key, thr)) push_cand(P, dk.key);
                 }
               } else {
                 // cheap pre-filter on the key's first 11 bits; the composite key is only built for docs
@@ -1438,7 +1376,7 @@ __global__ void __launch_bounds__(QW_THREADS, QW_MIN_BLOCKS_PER_SM) k_window(con
                 top = key_top11(P, ks, s_cols, base, doc, sc);
                 if (top >= thr_top) {
                   const DocKey dk = doc_key(P, ks, s_cols, base, doc, sc);
-                  if (key_ge(dk.key, thr)) emit(dk.key);
+                  if (key_ge(dk.key, thr)) push_cand(P, dk.key);
                 }
               }
             }

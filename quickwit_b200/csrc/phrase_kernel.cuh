@@ -32,78 +32,115 @@ namespace qwk {
 #define QP_WARPS 4
 #define QP_NONE 0xFFFFFFFFu
 
-// block-wide unpack of one posting block by a warp: docs (absolute) and tfs of the lane's 4 postings
-__device__ __forceinline__ void phrase_decode(const uint8_t* blk, uint32_t lane, uint32_t (&doc)[4], uint32_t (&tf)[4], uint32_t& count) {
-  const uint4 h = __ldg(reinterpret_cast<const uint4*>(blk));  // QwSkip: last_doc, prev_last_doc, byte_off, bits/count
-  const uint32_t prev = h.y, doc_bits = h.w & 0xFF, tf_bits = (h.w >> 8) & 0xFF;
-  count = h.w >> 16;
-  const uint4* dp = reinterpret_cast<const uint4*>(blk + 16);
-  uint32_t v[4] = {0, 0, 0, 0};
-  if (doc_bits) {
-    const uint32_t bitpos = lane * doc_bits, wi = bitpos >> 5, sh = bitpos & 31;
-    const uint4 A = __ldg(dp + wi);
-    const uint4 B = (sh + doc_bits > 32) ? __ldg(dp + wi + 1) : make_uint4(0, 0, 0, 0);
-    const uint32_t mask = 0xFFFFFFFFu >> (32 - doc_bits);
-    v[0] = __funnelshift_r(A.x, B.x, sh) & mask; v[1] = __funnelshift_r(A.y, B.y, sh) & mask;
-    v[2] = __funnelshift_r(A.z, B.z, sh) & mask; v[3] = __funnelshift_r(A.w, B.w, sh) & mask;
-  }
-  const uint32_t d0 = v[0] + 1, d1 = d0 + v[1] + 1, d2 = d1 + v[2] + 1, d3 = d2 + v[3] + 1;
-  uint32_t incl = d3;
+// one posting block of a phrase term by a warp (posting.cuh): docs (absolute), tfs (0 for padding postings, which own
+// no positions) and their exclusive prefix over the block in lane-major order = each posting's first position index
+// relative to the block's; returns the block's posting count
+__device__ __forceinline__ uint32_t phrase_block(const uint8_t* blk, uint32_t lane, uint32_t (&doc)[4], uint32_t (&tf)[4], uint32_t (&pre)[4]) {
+  const BlkHdr h = blk_header<LdgLoad>(blk);
+  blk_docs<LdgLoad>(blk, h, 0, lane, doc);
+  blk_tfs<LdgLoad>(blk, h, lane, tf);
 #pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const uint32_t n = __shfl_up_sync(0xFFFFFFFFu, incl, o);
-    if ((int)lane >= o) incl += n;
-  }
-  const uint32_t basev = prev + (incl - d3);  // mod 2^32
-  doc[0] = basev + d0; doc[1] = basev + d1; doc[2] = basev + d2; doc[3] = basev + d3;
-  tf[0] = tf[1] = tf[2] = tf[3] = 1;
-  if (tf_bits) {
-    const uint4* tp = dp + doc_bits;
-    const uint32_t bitpos = lane * tf_bits, wi = bitpos >> 5, sh = bitpos & 31;
-    const uint4 A = __ldg(tp + wi);
-    const uint4 B = (sh + tf_bits > 32) ? __ldg(tp + wi + 1) : make_uint4(0, 0, 0, 0);
-    const uint32_t mask = 0xFFFFFFFFu >> (32 - tf_bits);
-    tf[0] = __funnelshift_r(A.x, B.x, sh) & mask; tf[1] = __funnelshift_r(A.y, B.y, sh) & mask;
-    tf[2] = __funnelshift_r(A.z, B.z, sh) & mask; tf[3] = __funnelshift_r(A.w, B.w, sh) & mask;
-  }
-#pragma unroll
-  for (int j = 0; j < 4; j++) if (lane * 4 + j >= count) tf[j] = 0;  // padding postings own no positions
-}
-
-// exclusive prefix of the lane's 4 values over the whole block (lane-major order)
-__device__ __forceinline__ void block_excl_prefix(const uint32_t (&x)[4], uint32_t lane, uint32_t (&pre)[4]) {
-  const uint32_t s = x[0] + x[1] + x[2] + x[3];
+  for (int j = 0; j < 4; j++) if (lane * 4 + j >= h.count) tf[j] = 0;
+  const uint32_t s = tf[0] + tf[1] + tf[2] + tf[3];
   uint32_t incl = s;
 #pragma unroll
   for (int o = 1; o < 32; o <<= 1) {
     const uint32_t n = __shfl_up_sync(0xFFFFFFFFu, incl, o);
     if ((int)lane >= o) incl += n;
   }
-  pre[0] = incl - s; pre[1] = pre[0] + x[0]; pre[2] = pre[1] + x[1]; pre[3] = pre[2] + x[2];
+  pre[0] = incl - s; pre[1] = pre[0] + tf[0]; pre[2] = pre[1] + tf[1]; pre[3] = pre[2] + tf[2];
+  return h.count;
 }
 
-// first index in [0, n) whose skip entry has last_doc >= doc (n if none): warp-cooperative 32-ary search, one round
-// of coalesced loads per factor 32
-__device__ __forceinline__ uint32_t phrase_first_block(const QwSkip* sk, uint32_t n, uint32_t doc, uint32_t lane) {
-  uint32_t lo = 0, hi = n;
-  while (lo < hi) {
-    const uint32_t step = (hi - lo + 31) / 32, idx = lo + lane * step;
-    const bool before = idx < hi && __ldg(&sk[idx].last_doc) < doc;  // true for a prefix of the probes
-    const uint32_t c = (uint32_t)__popc(__ballot_sync(0xFFFFFFFFu, before));
-    if (c == 0) { hi = lo; break; }
-    hi = min(hi, lo + c * step);
-    lo = lo + (c - 1) * step + 1;
+// Looks the live candidates of one driver block (bit j of `live`: doc cdoc[j]; the block spans [doc_first, doc_last])
+// up in term T. The candidates form one contiguous doc range, so the blocks of T that can hold them are a short run
+// [r_lo, r_hi]: two warp-cooperative searches find it (a handful of load rounds), and each candidate then searches
+// inside it (one or two steps for terms of comparable density) instead of the whole skip list. The warp decodes each
+// NEEDED block once, lowest first, into its shared arrays bdoc / bpre / btf (128 words each), and every candidate calls
+// found(j, first position index, tf) or missing(j).
+template <class Found, class Missing>
+__device__ __forceinline__ void phrase_probe(const uint8_t* base, const DPhraseTerm& T, uint32_t doc_first, uint32_t doc_last,
+                                             const uint32_t (&cdoc)[4], uint32_t live, uint32_t* bdoc, uint32_t* bpre,
+                                             uint32_t* btf, uint32_t lane, Found&& found, Missing&& missing) {
+  const QwSkip* sk = (const QwSkip*)(base + T.skip_off);
+  const uint32_t* pidx = (const uint32_t*)(base + T.pidx_off);
+  const uint32_t r_lo = first_block_ge(sk, T.nblk, doc_first, lane);
+  const uint32_t r_hi = r_lo < T.nblk ? r_lo + first_block_ge(sk + r_lo, T.nblk - r_lo, doc_last, lane) : T.nblk;  // first block that reaches doc_last
+  uint32_t need[4];
+#pragma unroll
+  for (int j = 0; j < 4; j++) {
+    need[j] = QP_NONE;
+    if ((live >> j) & 1u) {
+      // first block whose last_doc >= doc
+      uint32_t lo = r_lo, hi = min(r_hi + 1, T.nblk);
+      while (lo < hi) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (__ldg(&sk[mid].last_doc) < cdoc[j]) lo = mid + 1; else hi = mid;
+      }
+      if (lo < T.nblk) need[j] = lo; else missing(j);
+    }
   }
-  return lo;
+  for (;;) {
+    uint32_t cur = min(min(need[0], need[1]), min(need[2], need[3]));
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) cur = min(cur, __shfl_xor_sync(0xFFFFFFFFu, cur, o));
+    if (cur == QP_NONE) break;
+    // the warp decodes block `cur` of term T into shared memory
+    uint32_t d[4], f[4], pre[4];
+    const uint32_t cnt = phrase_block(base + T.data_off + __ldg(&sk[cur].byte_off), lane, d, f, pre);
+    __syncwarp();
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+      bdoc[lane * 4 + j] = lane * 4 + j < cnt ? d[j] : QP_NONE;  // (padding sorts last)
+      bpre[lane * 4 + j] = pre[j];
+      btf[lane * 4 + j] = f[j];
+    }
+    __syncwarp();
+    const uint32_t first = __ldg(pidx + cur);
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+      if (need[j] != cur) continue;
+      need[j] = QP_NONE;
+      uint32_t lo = 0, hi = cnt;
+      while (lo < hi) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (bdoc[mid] < cdoc[j]) lo = mid + 1; else hi = mid;
+      }
+      if (lo < cnt && bdoc[lo] == cdoc[j]) found(j, first + bpre[lo], btf[lo]);
+      else missing(j);
+    }
+  }
+}
+
+// A driver block's result as an uncompressed posting block: candidate j with phrase_count n[j] > 0 is {doc, weight *
+// tf-factor(n[j], fieldnorm)} (Bm25Weight::score with tf = phrase_count; val 0 when the phrase is unscored); the others
+// are {QP_NONE, 0}
+__device__ __forceinline__ void phrase_out(const DPhrase& ph, const uint8_t* base, uint32_t b, uint32_t lane, const uint32_t (&cdoc)[4],
+                                           const uint32_t (&n)[4]) {
+  uint32_t odoc[4];
+  float oval[4];
+#pragma unroll
+  for (int j = 0; j < 4; j++) {
+    odoc[j] = n[j] ? cdoc[j] : QP_NONE;
+    oval[j] = 0.f;
+    if (n[j] && ph.scored) {
+      const uint32_t fn = ph.fn_off != ~0ull ? (uint32_t)__ldg(base + ph.fn_off + cdoc[j]) : 1u;
+      oval[j] = __fmul_rn(ph.weight, tf_factor((const float*)ph.tab, n[j], fn));
+    }
+  }
+  VBlk* out = (VBlk*)ph.out + b;
+  *reinterpret_cast<uint4*>(&out->doc[lane * 4]) = make_uint4(odoc[0], odoc[1], odoc[2], odoc[3]);
+  *reinterpret_cast<float4*>(&out->val[lane * 4]) = make_float4(oval[0], oval[1], oval[2], oval[3]);
 }
 
 // shared memory per warp: 3 + 2 * max_terms arrays of 128 words (max_terms = the longest phrase of the batch), so that
 // short phrases — the usual case — leave room for three times as many warps per SM as a layout sized for 8 terms
 #define QP_SMEM_WORDS(max_terms) ((3u + 2u * (max_terms)) * QW_BLOCK_LEN)
 // kPrefix: the batch holds at least one phrase prefix (n_exp > 0); its plain phrases take the same path as in
-// k_phrase<false>
+// k_phrase<false>. k_phrase<false> asks for 10 blocks per SM (at most 48 registers): left to itself the compiler
+// takes 56 registers and no spills, and a batch of many short phrases then runs about 5% slower on an H100.
 template <bool kPrefix>
-__global__ void __launch_bounds__(QP_WARPS * 32) k_phrase(const DPhrase* phrases, uint32_t n_phrases, uint32_t total_blocks, uint32_t max_terms) {
+__global__ void __launch_bounds__(QP_WARPS * 32, kPrefix ? 0 : 10) k_phrase(const DPhrase* phrases, uint32_t n_phrases, uint32_t total_blocks, uint32_t max_terms) {
   // per warp: the decoded block of the term being probed + every term's {first position index, tf} per candidate
   extern __shared__ __align__(16) uint8_t qp_smem[];
   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -127,8 +164,7 @@ __global__ void __launch_bounds__(QP_WARPS * 32) k_phrase(const DPhrase* phrases
   uint32_t cdoc[4], ctf[4], cpre[4], count;
   {
     const QwSkip* sk = (const QwSkip*)(base + D.skip_off);
-    phrase_decode(base + D.data_off + __ldg(&sk[b].byte_off), lane, cdoc, ctf, count);
-    block_excl_prefix(ctf, lane, cpre);
+    count = phrase_block(base + D.data_off + __ldg(&sk[b].byte_off), lane, cdoc, ctf, cpre);
     const uint32_t first = __ldg((const uint32_t*)(base + D.pidx_off) + b);
 #pragma unroll
     for (int j = 0; j < 4; j++) {
@@ -143,67 +179,13 @@ __global__ void __launch_bounds__(QP_WARPS * 32) k_phrase(const DPhrase* phrases
   // ---- 2. the other terms ------------------------------------------------------------------------------------
   for (uint32_t t = 0; t < ph.n_terms; t++) {
     if (t == ph.driver) continue;
-    const DPhraseTerm& T = ph.t[t];
-    const QwSkip* sk = (const QwSkip*)(base + T.skip_off);
-    const uint32_t* pidx = (const uint32_t*)(base + T.pidx_off);
-    // The candidates are the postings of ONE driver block, i.e. a contiguous doc range: the blocks of term t that can
-    // hold them form a short run [r_lo, r_hi]. Two warp-cooperative searches find the run (a handful of load rounds);
-    // each candidate then searches inside it (one or two steps for terms of comparable density) instead of the whole
-    // skip list (14 dependent loads for 10 K blocks, four times per lane).
     const uint32_t doc_first = __shfl_sync(0xFFFFFFFFu, cdoc[0], 0);
     const uint32_t doc_last = __ldg(&((const QwSkip*)(base + D.skip_off))[b].last_doc);
-    const uint32_t r_lo = phrase_first_block(sk, T.nblk, doc_first, lane);
-    const uint32_t r_hi = r_lo < T.nblk ? r_lo + phrase_first_block(sk + r_lo, T.nblk - r_lo, doc_last, lane) : T.nblk;  // first block that reaches doc_last
-    uint32_t need[4];
-#pragma unroll
-    for (int j = 0; j < 4; j++) {
-      need[j] = QP_NONE;
-      if ((alive >> j) & 1u) {
-        // first block whose last_doc >= doc
-        uint32_t lo = r_lo, hi = min(r_hi + 1, T.nblk);
-        while (lo < hi) {
-          const uint32_t mid = (lo + hi) >> 1;
-          if (__ldg(&sk[mid].last_doc) < cdoc[j]) lo = mid + 1; else hi = mid;
-        }
-        if (lo < T.nblk) need[j] = lo; else alive &= ~(1u << j);
-      }
-    }
-    for (;;) {
-      uint32_t cur = min(min(need[0], need[1]), min(need[2], need[3]));
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) cur = min(cur, __shfl_xor_sync(0xFFFFFFFFu, cur, o));
-      if (cur == QP_NONE) break;
-      // the warp decodes block `cur` of term t into shared memory
-      uint32_t d[4], f[4], pre[4], cnt;
-      phrase_decode(base + T.data_off + __ldg(&sk[cur].byte_off), lane, d, f, cnt);
-      block_excl_prefix(f, lane, pre);
-      __syncwarp();
-#pragma unroll
-      for (int j = 0; j < 4; j++) {
-        bdoc[lane * 4 + j] = lane * 4 + j < cnt ? d[j] : QP_NONE;  // (padding sorts last)
-        bpre[lane * 4 + j] = pre[j];
-        btf[lane * 4 + j] = f[j];
-      }
-      __syncwarp();
-      const uint32_t first = __ldg(pidx + cur);
-#pragma unroll
-      for (int j = 0; j < 4; j++) {
-        if (need[j] != cur) continue;
-        need[j] = QP_NONE;
-        uint32_t lo = 0, hi = cnt;
-        while (lo < hi) {
-          const uint32_t mid = (lo + hi) >> 1;
-          if (bdoc[mid] < cdoc[j]) lo = mid + 1; else hi = mid;
-        }
-        if (lo < cnt && bdoc[lo] == cdoc[j]) {
-          S_POS(t, lane * 4 + j) = first + bpre[lo];
-          S_TF(t, lane * 4 + j) = btf[lo];
-        } else alive &= ~(1u << j);
-      }
-    }
+    phrase_probe(base, ph.t[t], doc_first, doc_last, cdoc, alive, bdoc, bpre, btf, lane,
+                 [&](uint32_t j, uint32_t pos, uint32_t tf) { S_POS(t, lane * 4 + j) = pos; S_TF(t, lane * 4 + j) = tf; },
+                 [&](uint32_t j) { alive &= ~(1u << j); });
   }
 
-  VBlk* out = (VBlk*)ph.out + b;
   if constexpr (kPrefix) {
     if (ph.n_exp) {
       // ---- 2b. phrase prefix: the expansions of the last slot ----------------------------------------------------
@@ -215,77 +197,34 @@ __global__ void __launch_bounds__(QP_WARPS * 32) k_phrase(const DPhrase* phrases
         const uint32_t open = alive & ~matched;
         if (!__ballot_sync(0xFFFFFFFFu, open != 0)) break;  // every alive candidate of the warp has matched
         const DPhraseTerm& T = X[e];
-        const QwSkip* sk = (const QwSkip*)(base + T.skip_off);
-        const uint32_t* pidx = (const uint32_t*)(base + T.pidx_off);
-        const uint32_t r_lo = phrase_first_block(sk, T.nblk, doc_first, lane);
-        if (r_lo >= T.nblk) continue;  // every posting of the expansion lies before the driver block
-        const uint32_t r_hi = r_lo + phrase_first_block(sk + r_lo, T.nblk - r_lo, doc_last, lane);
-        uint32_t need[4];
-#pragma unroll
-        for (int j = 0; j < 4; j++) {
-          need[j] = QP_NONE;
-          if ((open >> j) & 1u) {
-            uint32_t lo = r_lo, hi = min(r_hi + 1, T.nblk);
-            while (lo < hi) {
-              const uint32_t mid = (lo + hi) >> 1;
-              if (__ldg(&sk[mid].last_doc) < cdoc[j]) lo = mid + 1; else hi = mid;
-            }
-            if (lo < T.nblk) need[j] = lo;
-          }
-        }
-        for (;;) {
-          uint32_t cur = min(min(need[0], need[1]), min(need[2], need[3]));
-#pragma unroll
-          for (int o = 16; o > 0; o >>= 1) cur = min(cur, __shfl_xor_sync(0xFFFFFFFFu, cur, o));
-          if (cur == QP_NONE) break;
-          uint32_t d[4], f[4], pre[4], cnt;
-          phrase_decode(base + T.data_off + __ldg(&sk[cur].byte_off), lane, d, f, cnt);
-          block_excl_prefix(f, lane, pre);
-          __syncwarp();
-#pragma unroll
-          for (int j = 0; j < 4; j++) {
-            bdoc[lane * 4 + j] = lane * 4 + j < cnt ? d[j] : QP_NONE;
-            bpre[lane * 4 + j] = pre[j];
-            btf[lane * 4 + j] = f[j];
-          }
-          __syncwarp();
-          const uint32_t first = __ldg(pidx + cur);
-#pragma unroll
-          for (int j = 0; j < 4; j++) {
-            if (need[j] != cur) continue;
-            need[j] = QP_NONE;
-            uint32_t lo = 0, hi = cnt;
-            while (lo < hi) {
-              const uint32_t mid = (lo + hi) >> 1;
-              if (bdoc[mid] < cdoc[j]) lo = mid + 1; else hi = mid;
-            }
-            if (lo >= cnt || bdoc[lo] != cdoc[j]) continue;
-            const uint32_t c = lane * 4 + j;
-            const uint32_t* pe = (const uint32_t*)(base + T.pos_off) + first + bpre[lo];
-            const uint32_t ne = btf[lo];
-            for (uint32_t i = 0; i < ne; i++) {
-              const uint32_t q = __ldg(pe + i);
-              if (q < T.offset) continue;  // the phrase would start before position 0
-              const uint32_t start = q - T.offset;
-              bool all = true;
-              for (uint32_t t = 0; t < ph.n_terms && all; t++) {
-                const uint32_t want = start + ph.t[t].offset;
-                const uint32_t* pt = (const uint32_t*)(base + ph.t[t].pos_off) + S_POS(t, c);
-                uint32_t plo = 0, phi = S_TF(t, c);
-                while (plo < phi) {
-                  const uint32_t mid = (plo + phi) >> 1;
-                  if (__ldg(pt + mid) < want) plo = mid + 1; else phi = mid;
-                }
-                all = plo < S_TF(t, c) && __ldg(pt + plo) == want;
-              }
-              if (all) { matched |= 1u << j; break; }
-            }
-          }
-        }
+        phrase_probe(base, T, doc_first, doc_last, cdoc, open, bdoc, bpre, btf, lane,
+                     [&](uint32_t j, uint32_t pos, uint32_t ne) {
+                       const uint32_t c = lane * 4 + j;
+                       const uint32_t* pe = (const uint32_t*)(base + T.pos_off) + pos;
+                       for (uint32_t i = 0; i < ne; i++) {
+                         const uint32_t q = __ldg(pe + i);
+                         if (q < T.offset) continue;  // the phrase would start before position 0
+                         const uint32_t start = q - T.offset;
+                         bool all = true;
+                         for (uint32_t t = 0; t < ph.n_terms && all; t++) {
+                           const uint32_t want = start + ph.t[t].offset;
+                           const uint32_t* pt = (const uint32_t*)(base + ph.t[t].pos_off) + S_POS(t, c);
+                           uint32_t plo = 0, phi = S_TF(t, c);
+                           while (plo < phi) {
+                             const uint32_t mid = (plo + phi) >> 1;
+                             if (__ldg(pt + mid) < want) plo = mid + 1; else phi = mid;
+                           }
+                           all = plo < S_TF(t, c) && __ldg(pt + plo) == want;
+                         }
+                         if (all) { matched |= 1u << j; break; }
+                       }
+                     },
+                     [](uint32_t) {});
       }
       uint32_t odoc[4];
 #pragma unroll
       for (int j = 0; j < 4; j++) odoc[j] = (matched >> j) & 1u ? cdoc[j] : QP_NONE;
+      VBlk* out = (VBlk*)ph.out + b;
       *reinterpret_cast<uint4*>(&out->doc[lane * 4]) = make_uint4(odoc[0], odoc[1], odoc[2], odoc[3]);
       *reinterpret_cast<float4*>(&out->val[lane * 4]) = make_float4(0.f, 0.f, 0.f, 0.f);
       return;
@@ -294,17 +233,14 @@ __global__ void __launch_bounds__(QP_WARPS * 32) k_phrase(const DPhrase* phrases
 
   // ---- 3. positions: base positions at which every term lines up -----------------------------------------------
   const uint32_t off_d = D.offset;
-  uint32_t odoc[4];
-  float oval[4];
+  uint32_t matches[4];
 #pragma unroll
   for (int j = 0; j < 4; j++) {
-    odoc[j] = QP_NONE;
-    oval[j] = 0.f;
+    matches[j] = 0;
     if (!((alive >> j) & 1u)) continue;
     const uint32_t c = lane * 4 + j;
     const uint32_t* pd = (const uint32_t*)(base + D.pos_off) + S_POS(ph.driver, c);
     const uint32_t nd = ctf[j];
-    uint32_t matches = 0;
     for (uint32_t i = 0; i < nd; i++) {
       const uint32_t p = __ldg(pd + i);
       if (p < off_d) continue;  // the phrase would start before position 0
@@ -321,23 +257,10 @@ __global__ void __launch_bounds__(QP_WARPS * 32) k_phrase(const DPhrase* phrases
         }
         all = lo < S_TF(t, c) && __ldg(pt + lo) == want;
       }
-      matches += all ? 1u : 0u;
-    }
-    if (matches) {
-      odoc[j] = cdoc[j];
-      if (ph.scored) {
-        // Bm25Weight::score with tf = phrase_count: the same table / divide as a term posting
-        const float* tab = (const float*)ph.tab;
-        const uint32_t fn = ph.fn_off != ~0ull ? (uint32_t)__ldg(base + ph.fn_off + cdoc[j]) : 1u;
-        float tfn;
-        if (matches < QW_TFF_ROWS) tfn = __ldg(tab + 256 + matches * 256 + fn);
-        else { const float tff = (float)matches; tfn = __fdiv_rn(tff, __fadd_rn(tff, __ldg(tab + fn))); }
-        oval[j] = __fmul_rn(ph.weight, tfn);
-      }
+      matches[j] += all ? 1u : 0u;
     }
   }
-  *reinterpret_cast<uint4*>(&out->doc[lane * 4]) = make_uint4(odoc[0], odoc[1], odoc[2], odoc[3]);
-  *reinterpret_cast<float4*>(&out->val[lane * 4]) = make_float4(oval[0], oval[1], oval[2], oval[3]);
+  phrase_out(ph, base, b, lane, cdoc, matches);
 }
 
 // ---- phrases of more than QW_MAX_PHRASE_TERMS terms (k_phrase_long) ------------------------------------------------
@@ -387,9 +310,8 @@ __global__ void __launch_bounds__(QP_WARPS * 32) k_phrase_long(const DPhrase* ph
 
   // ---- 1. driver block ------------------------------------------------------------------------------------
   const QwSkip* dsk = (const QwSkip*)(base + D.skip_off);
-  uint32_t cdoc[4], ctf[4], cpre[4], count;
-  phrase_decode(base + D.data_off + __ldg(&dsk[b].byte_off), lane, cdoc, ctf, count);
-  block_excl_prefix(ctf, lane, cpre);
+  uint32_t cdoc[4], ctf[4], cpre[4];
+  const uint32_t count = phrase_block(base + D.data_off + __ldg(&dsk[b].byte_off), lane, cdoc, ctf, cpre);
   const uint32_t* dpos = (const uint32_t*)(base + D.pos_off) + __ldg((const uint32_t*)(base + D.pidx_off) + b);
   const uint32_t off_d = D.offset;
   const uint32_t doc_first = __shfl_sync(0xFFFFFFFFu, cdoc[0], 0);
@@ -411,58 +333,13 @@ __global__ void __launch_bounds__(QP_WARPS * 32) k_phrase_long(const DPhrase* ph
     if (!__ballot_sync(0xFFFFFFFFu, live != 0)) break;
     for (uint32_t t = 1; t < ph.n_terms; t++) {
       const DPhraseTerm& T = terms[t];
-      const QwSkip* sk = (const QwSkip*)(base + T.skip_off);
-      const uint32_t* pidx = (const uint32_t*)(base + T.pidx_off);
       const uint32_t* tpos = (const uint32_t*)(base + T.pos_off);
-      // the blocks of term t that can hold the driver block's docs: a short run [r_lo, r_hi] (as in k_phrase)
-      const uint32_t r_lo = phrase_first_block(sk, T.nblk, doc_first, lane);
-      const uint32_t r_hi = r_lo < T.nblk ? r_lo + phrase_first_block(sk + r_lo, T.nblk - r_lo, doc_last, lane) : T.nblk;
-      uint32_t need[4];
-#pragma unroll
-      for (int j = 0; j < 4; j++) {
-        need[j] = QP_NONE;
-        if ((live >> j) & 1u) {
-          uint32_t lo = r_lo, hi = min(r_hi + 1, T.nblk);
-          while (lo < hi) {
-            const uint32_t mid = (lo + hi) >> 1;
-            if (__ldg(&sk[mid].last_doc) < cdoc[j]) lo = mid + 1; else hi = mid;
-          }
-          if (lo < T.nblk) need[j] = lo;
-          else { present &= ~(1u << j); live &= ~(1u << j); mask[j] = 0; }
-        }
-      }
-      for (;;) {
-        uint32_t cur = min(min(need[0], need[1]), min(need[2], need[3]));
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) cur = min(cur, __shfl_xor_sync(0xFFFFFFFFu, cur, o));
-        if (cur == QP_NONE) break;
-        uint32_t d[4], f[4], pre[4], cnt;
-        phrase_decode(base + T.data_off + __ldg(&sk[cur].byte_off), lane, d, f, cnt);
-        block_excl_prefix(f, lane, pre);
-        __syncwarp();
-#pragma unroll
-        for (int j = 0; j < 4; j++) {
-          bdoc[lane * 4 + j] = lane * 4 + j < cnt ? d[j] : QP_NONE;  // (padding sorts last)
-          bpre[lane * 4 + j] = pre[j];
-          btf[lane * 4 + j] = f[j];
-        }
-        __syncwarp();
-        const uint32_t first = __ldg(pidx + cur);
-#pragma unroll
-        for (int j = 0; j < 4; j++) {
-          if (need[j] != cur) continue;
-          need[j] = QP_NONE;
-          uint32_t lo = 0, hi = cnt;
-          while (lo < hi) {
-            const uint32_t mid = (lo + hi) >> 1;
-            if (bdoc[mid] < cdoc[j]) lo = mid + 1; else hi = mid;
-          }
-          if (lo < cnt && bdoc[lo] == cdoc[j]) {
-            mask[j] = phrase_narrow(dpos + cpre[j] + r0, mask[j], off_d, tpos + first + bpre[lo], btf[lo], T.offset);
-            if (!mask[j]) live &= ~(1u << j);
-          } else { present &= ~(1u << j); live &= ~(1u << j); mask[j] = 0; }
-        }
-      }
+      phrase_probe(base, T, doc_first, doc_last, cdoc, live, bdoc, bpre, btf, lane,
+                   [&](uint32_t j, uint32_t pos, uint32_t tf) {
+                     mask[j] = phrase_narrow(dpos + cpre[j] + r0, mask[j], off_d, tpos + pos, tf, T.offset);
+                     if (!mask[j]) live &= ~(1u << j);
+                   },
+                   [&](uint32_t j) { present &= ~(1u << j); live &= ~(1u << j); mask[j] = 0; });
       if (!__ballot_sync(0xFFFFFFFFu, live != 0)) break;  // no survivor left in the warp: the later terms are moot
     }
 #pragma unroll
@@ -470,26 +347,7 @@ __global__ void __launch_bounds__(QP_WARPS * 32) k_phrase_long(const DPhrase* ph
   }
 
   // ---- 3. output: k_phrase's scoring of phrase_count = matches ------------------------------------------------
-  VBlk* out = (VBlk*)ph.out + b;
-  uint32_t odoc[4];
-  float oval[4];
-#pragma unroll
-  for (int j = 0; j < 4; j++) {
-    odoc[j] = QP_NONE;
-    oval[j] = 0.f;
-    if (!matches[j]) continue;
-    odoc[j] = cdoc[j];
-    if (ph.scored) {
-      const float* tab = (const float*)ph.tab;
-      const uint32_t fn = ph.fn_off != ~0ull ? (uint32_t)__ldg(base + ph.fn_off + cdoc[j]) : 1u;
-      float tfn;
-      if (matches[j] < QW_TFF_ROWS) tfn = __ldg(tab + 256 + matches[j] * 256 + fn);
-      else { const float tff = (float)matches[j]; tfn = __fdiv_rn(tff, __fadd_rn(tff, __ldg(tab + fn))); }
-      oval[j] = __fmul_rn(ph.weight, tfn);
-    }
-  }
-  *reinterpret_cast<uint4*>(&out->doc[lane * 4]) = make_uint4(odoc[0], odoc[1], odoc[2], odoc[3]);
-  *reinterpret_cast<float4*>(&out->val[lane * 4]) = make_float4(oval[0], oval[1], oval[2], oval[3]);
+  phrase_out(ph, base, b, lane, cdoc, matches);
 }
 
 }  // namespace qwk

@@ -3,12 +3,12 @@
 // program then ORs a window's words into the clause's target (OP_TERM_SET, kernels.cuh).
 //
 // One warp per 128-posting block, over the flat block list of every term-set term of the batch (grid-stride). A warp
-// finds its term by a 32-ary search of the block prefix, decodes the block with the phrase pre-pass's decode, and sets
+// finds its term by a 32-ary search of the block prefix, decodes the block's doc ids (posting.cuh), and sets
 // the doc bits with one atomicOr per distinct bitmap word: the block's postings are taken 32 at a time in doc order,
 // __match_any_sync groups the lanes of one word (a contiguous run, since doc ids ascend), a segmented shuffle ORs the
 // run into its first lane, and the run that ends a round is carried into the next round, which may continue the word.
 #pragma once
-#include "phrase_kernel.cuh"
+#include "posting.cuh"
 
 namespace qwk {
 
@@ -32,8 +32,9 @@ __global__ void __launch_bounds__(QS_WARPS * 32) k_term_set(const DTermSetTerm* 
     const DTermSetTerm& T = terms[lo];
     const QwSkip* skips = (const QwSkip*)__ldg(&T.skip);
     const uint8_t* blk = (const uint8_t*)__ldg(&T.data) + __ldg(&skips[b - __ldg(&T.first_block)].byte_off);
-    uint32_t doc[4], tf[4], count;
-    phrase_decode(blk, lane, doc, tf, count);
+    const BlkHdr h = blk_header<LdgLoad>(blk);
+    uint32_t doc[4];
+    blk_docs<LdgLoad>(blk, h, 0, lane, doc);
     uint32_t* bm = (uint32_t*)__ldg(&nodes[__ldg(&T.node)].bitmap);
     uint32_t carry = 0, carry_w = NONE;
 #pragma unroll
@@ -43,7 +44,7 @@ __global__ void __launch_bounds__(QS_WARPS * 32) k_term_set(const DTermSetTerm* 
       const uint32_t d0 = __shfl_sync(FULL, doc[0], src), d1 = __shfl_sync(FULL, doc[1], src);
       const uint32_t d2 = __shfl_sync(FULL, doc[2], src), d3 = __shfl_sync(FULL, doc[3], src);
       const uint32_t d = j == 0 ? d0 : j == 1 ? d1 : j == 2 ? d2 : d3;
-      const bool valid = r * 32 + lane < count;
+      const bool valid = r * 32 + lane < h.count;
       const uint32_t w = valid ? d >> 5 : NONE;
       uint32_t v = valid ? 1u << (d & 31) : 0u;
       const uint32_t grp = __match_any_sync(FULL, w);

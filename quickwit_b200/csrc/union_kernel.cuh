@@ -183,13 +183,7 @@ __device__ __noinline__ void union_emit(const DSplitPlan* plans, const DThresh& 
   const DSplitPlan& P = plans[split];
   const Key thr{T.key[0], T.key[1], T.key[2]};
   const DocKey dk = doc_key(P, P.key, cols + P.col_base, (const uint8_t*)P.data_base, doc, sc);
-  if (key_ge(dk.key, thr)) {
-    const uint32_t pos = atomicAdd((uint32_t*)P.out_cand_count, 1u);
-    if (pos < qw_cand_cap(P.max_hits)) {
-      uint64_t* c = (uint64_t*)P.out_cands + 3ull * pos;
-      c[0] = dk.key.w0; c[1] = dk.key.w1; c[2] = dk.key.w2;
-    }
-  }
+  if (key_ge(dk.key, thr)) push_cand(P, dk.key);
 }
 
 template <int MODE>
@@ -656,10 +650,7 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
 #pragma unroll
           for (int j = 0; j < 8; j++) {
             const uint32_t fn = ((j < 4 ? fnw.x : fnw.y) >> (8 * (j & 3))) & 0xFFu;
-            float tfn;
-            if (f[j] < QW_TFF_ROWS) tfn = __ldg(tab + 256 + f[j] * 256 + fn);
-            else { const float tff = (float)f[j]; tfn = __fdiv_rn(tff, __fadd_rn(tff, __ldg(tab + fn))); }
-            c[j] = __fmul_rn(weight, tfn);
+            c[j] = __fmul_rn(weight, tf_factor(tab, f[j], fn));
           }
         }
         // ---- ordered accumulate: everything of the earlier clauses must be in -------------------------

@@ -281,6 +281,15 @@ def boosted(group, boosts=(0.5, 3.0, 1.7, 1.0, 0.25)):
     return [Clause(cl.field, cl.terms, boosts[i % len(boosts)]) for i, cl in enumerate(group)]
 
 
+def term_set_groups(c):
+    """(field, terms) of the term sets over the sweep: one per doc width of `body` (its terms' blocks hold every
+    wide-delta position and the tails), the tf-width sweep, and each other field's terms."""
+    groups = [("body", c.terms_of("body", f"w{w:02d}_")) for w in range(23)]
+    groups.append(("body", c.terms_of("body", "tf")))
+    groups += [(f, c.terms_of(f)) for f in ("big", "nofn", "ph")]
+    return groups
+
+
 def driver_terms(c):
     return [(f, t) for (f, t) in sorted(c.postings) if f in ("body", "nofn", "big") and t != "dense"]
 

@@ -6,22 +6,27 @@ Each call is routed through one decoder, and the route is asserted from `kernel_
   * k_window: the same unions by `_score` ascending, with a `must` clause, and by doc id (unscored: no tfs read);
     a batch with an empty split and a split without the terms (plans k_union does not take);
   * k_driver: one term per call, scored, with and without a range filter;
-  * k_phrase: the phrase pairs by `_score` and by doc id, and one phrase prefix over expansions of every width.
+  * k_phrase: the phrase pairs by `_score` and by doc id, and one phrase prefix over expansions of every width;
+  * k_term_set: a term-set filter over the terms of each doc width, of the tf-width sweep and of each other field.
 Every result is compared bit for bit with scoring_ref's f32 restatement and with the oracle, and within the f64
 bound of scoring_ref.f64_bound."""
 import time
+
+import numpy as np
 
 import pytest
 
 from quickwit_b200 import ffi, plan as P
 from oracle import oracle as O
 from helpers import assert_same
+from regex_ref import oracle_search
 import posting_corpora as PC
 import scoring_ref as R
 
 pytestmark = pytest.mark.gpu
 
 UNION, WINDOW, DRIVER, PHRASE = ffi.KERNEL_UNION, ffi.KERNEL_WINDOW, ffi.KERNEL_DRIVER, ffi.KERNEL_PHRASE
+TERM_SET = ffi.KERNEL_TERM_SET
 
 
 @pytest.fixture(scope="module")
@@ -111,6 +116,27 @@ def test_phrase(gpu_ctx, sweep):
     assert len(want) > 0 and r.num_hits == len(want) and [h[0] for h in r.hits] == want[::-1].tolist()
     # (the oracle runs the same match set as an OR of one phrase per expansion)
     assert_same(r, O.split_search(sweep.img, P.make_plan(P.phrase_prefix_as_phrases(node), 4096, R.SORTS["doc_desc"])), ctx="phrase prefix")
+
+
+def test_term_set(gpu_ctx, sweep):
+    """A TERM_SET filter over each group's terms: its doc set is the union of the terms' postings, at most 16 517
+    docs, so one page of K = 20 000 holds all of it."""
+    img = sweep.img
+    gpu_ctx.set_max_hits(20_000)
+    try:
+        for field, terms in PC.term_set_groups(sweep):
+            want = np.unique(np.concatenate([sweep.postings[(field, t)][0] for t in terms]))
+            assert 0 < len(want) <= 20_000
+            node = P.bool_([P.term_set(img, field, sorted(img.term_ord(field, t) for t in terms))])
+            for sort, docs in (("doc_desc", want[::-1]), ("doc_asc", want)):
+                pl = P.make_plan(node, 20_000, R.SORTS[sort])
+                r = gpu_ctx.split_search([img.split_id], [pl])[0]
+                tag = f"term set {field}:{terms[0]}..{terms[-1]} ({len(terms)} terms) {sort} kernel_mask={r.kernel_mask:#x}"
+                assert r.kernel_mask & TERM_SET and r.kernel_mask & WINDOW, tag
+                assert r.num_hits == len(want) and [h[0] for h in r.hits] == docs.tolist(), tag
+                assert_same(r, oracle_search(img, pl), ctx=tag)
+    finally:
+        gpu_ctx.set_max_hits(4096)
 
 
 def test_large_split(gpu_ctx, others):
