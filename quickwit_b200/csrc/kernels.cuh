@@ -1339,9 +1339,11 @@ __global__ void __launch_bounds__(QW_THREADS, QW_MIN_BLOCKS_PER_SM) k_window(con
       };
       if (max_hits && ks.kind[0] == QW_SORT_SCORE && ks.order[0] == QW_ORDER_DESC && !sa_present && rscore && !n_aggs && !rec) {
         // fast path (BM25 top-K): a float lower bound of the threshold bucket filters 4 docs per lane
-        // per step; only survivors build the composite key. s_lo is conservative (one part in 2^20).
-        float s_lo = -1.0f;
-        if (thr_top >= 1024u) s_lo = __fmul_rn(__fdiv_rn((float)(thr_top & 1023u), ks.score_scale), 0.999999f);
+        // per step; only survivors build the composite key. s_lo is conservative (one part in 2^20). Bucket 0 holds
+        // every score below 1 / score_scale, negative ones included, and is the only bucket when score_scale is 0
+        // (score_max overflowed to +inf): it filters nothing.
+        float s_lo = -INFINITY;
+        if (thr_top >= 1024u && (thr_top & 1023u)) s_lo = __fmul_rn(__fdiv_rn((float)(thr_top & 1023u), ks.score_scale), 0.999999f);
         const float4* sc4 = reinterpret_cast<const float4*>(rscore);
         for (uint32_t q = tid; q < (W >> 2); q += QW_THREADS) {
           const uint32_t nib = (res[q >> 3] >> ((q & 7) * 4)) & 0xFu;

@@ -3,10 +3,10 @@ splits of column_corpora were built from (never from the image).
 
   * range: a doc matches when ANY of its mapped values lies in [lo, hi], compared in mapped u64 space (so -0.0 sorts
     below 0.0 and NaN above +inf, as the monotonic mapping orders them); exists: the doc has a value;
-  * bool: all required clauses, no must_not clause, and at least minimum_should_match (else 1 when there is no
-    required clause) should clauses;
-  * score: a range / exists clause scores its boost; a bool adds the scored MUST clauses in clause order, then the
-    matching SHOULD clauses in clause order, and sums the two, in f32;
+  * bool: bool_ref's rule (all required clauses, no must_not clause, at least minimum_should_match should clauses,
+    else 1 when there is no required clause; the f32 sum of the scored MUST clauses plus that of the matching SHOULD
+    clauses);
+  * score: a range / exists clause scores its boost, a term 0;
   * order (SegmentPartialHitSortingKey, collector.rs:1082-1118): sort value 1, sort value 2, None last in both
     directions, then the doc id in the direction of the first key; a column's sort value is the doc's first value in
     index order;
@@ -21,6 +21,7 @@ import numpy as np
 
 from quickwit_b200 import ffi, plan as P, splitgen as S
 from column_corpora import Col, Split
+import bool_ref
 
 MUST, SHOULD, MUST_NOT, FILTER = ffi.OCCUR_MUST, ffi.OCCUR_SHOULD, ffi.OCCUR_MUST_NOT, ffi.OCCUR_FILTER
 ASC, DESC = ffi.ORDER_ASC, ffi.ORDER_DESC
@@ -79,42 +80,25 @@ def range_mask(c: Col, lo: int, hi: int) -> np.ndarray:
     return out
 
 
-def evaluate(sp: Split, q: Q) -> Tuple[np.ndarray, np.ndarray]:
-    """(match mask, f32 score) of clause q over every doc of the split."""
+def _leaf(sp: Split, q: Q) -> Tuple[np.ndarray, np.ndarray]:
+    """(match mask, f32 score) of a term (unscored), range or exists clause over every doc of the split."""
     n = sp.num_docs
     f32 = np.float32
     if q.kind == "term":
         m = np.zeros(n, dtype=bool)
         m[sp.terms.get(q.term, np.zeros(0, dtype=np.int64))] = True
         return m, np.zeros(n, dtype=f32)
-    if q.kind in ("range", "exists"):
-        c = sp.cols.get(q.col)
-        if c is None:
-            m = np.zeros(n, dtype=bool)
-        else:
-            m = c.has.copy() if q.kind == "exists" else range_mask(c, q.lo, q.hi)
-        return m, np.where(m, f32(q.boost), f32(0)).astype(f32)
-    req = np.ones(n, dtype=bool)
-    n_req = 0
-    excl = np.zeros(n, dtype=bool)
-    cnt = np.zeros(n, dtype=np.int64)
-    msum = np.zeros(n, dtype=f32)
-    ssum = np.zeros(n, dtype=f32)
-    for ch in q.children:
-        m, s = evaluate(sp, ch)
-        if ch.occur in (MUST, FILTER):
-            req &= m
-            n_req += 1
-            if ch.occur == MUST:
-                msum = (msum + np.where(m, s, f32(0))).astype(f32)
-        elif ch.occur == SHOULD:
-            cnt += m
-            ssum = (ssum + np.where(m, s, f32(0))).astype(f32)
-        else:
-            excl |= m
-    need = q.msm if q.msm else (1 if n_req == 0 else 0)
-    m = req & ~excl & (cnt >= need)
-    return m, np.where(m, (msum + ssum).astype(f32), f32(0)).astype(f32)
+    c = sp.cols.get(q.col)
+    if c is None:
+        m = np.zeros(n, dtype=bool)
+    else:
+        m = c.has.copy() if q.kind == "exists" else range_mask(c, q.lo, q.hi)
+    return m, np.where(m, f32(q.boost), f32(0)).astype(f32)
+
+
+def evaluate(sp: Split, q: Q) -> Tuple[np.ndarray, np.ndarray]:
+    """(match mask, f32 score) of clause q over every doc of the split (bool_ref's rule over these leaves)."""
+    return bool_ref.evaluate(q, lambda x: _leaf(sp, x), sp.num_docs)
 
 
 class Sort:
@@ -205,10 +189,11 @@ def after(hit: Tuple) -> ffi.QwSearchAfter:
     return sa
 
 
-def check(got, sp: Split, q: Q, sort: Sort, K: int, sa=None, scored: bool = False, ctx: str = ""):
+def check(got, sp: Split, q: Q, sort: Sort, K: int, sa=None, scored: bool = False, ctx: str = "", ev=None):
     """`got` (a GPU or oracle result) against the brute force: num_hits and (doc, flags, v1, v2) of every hit, and the
-    f32 score bits of a plan ranked by _score."""
-    mask, score = evaluate(sp, q)
+    f32 score bits of a plan ranked by _score (`scored`). `ev(sp, q)` gives (match mask, f32 score); default:
+    `evaluate`."""
+    mask, score = (ev or evaluate)(sp, q)
     nh, want = top_k(sp, mask, score, sort, K, sa)
     assert got.num_hits == nh, f"{ctx}: num_hits {got.num_hits} != {nh}"
     g = [tuple(int(x) for x in h[:4]) for h in got.hits]

@@ -46,7 +46,7 @@ def weight(c, field, term, boost=1.0):
     df = len(c.postings[(field, term)][0])
     w = np.float32(P.bm25_weight(df, c.n, boost))
     ref = bm25_weight(df, c.n) * np.float32(boost)
-    assert abs(float(w) - float(ref)) <= 1e-6 * float(w), (term, float(w), float(ref))
+    assert abs(float(w) - float(ref)) <= 1e-6 * abs(float(w)), (term, float(w), float(ref))
     return w
 
 
@@ -89,7 +89,7 @@ class Clause:
         for df in dfs:  # Bm25Weight::for_terms: the idfs summed in phrase order
             idf = idf + np.log(f32(1) + (f32(c.n - df) + f32(0.5)) / (f32(df) + f32(0.5)), dtype=np.float32)
         ref = idf * (f32(1) + f32(K1)) * f32(self.boost)
-        assert abs(float(w) - float(ref)) <= 1e-6 * len(dfs) * float(w), (self.terms, float(w), float(ref))
+        assert abs(float(w) - float(ref)) <= 1e-6 * len(dfs) * abs(float(w)), (self.terms, float(w), float(ref))
         return w
 
     def idf64(self, c):
