@@ -97,6 +97,22 @@ int qwgpu_split_is_resident(qwgpu_ctx* ctx, const char* split_id);
  * raises the limit when it expects such requests (the reference accepts max_hits and start_offset up to 10 000 each). */
 int qwgpu_set_max_hits(qwgpu_ctx* ctx, uint32_t max_hits);
 
+/* Predicate cache (the reference's PredicateCache, quickwit-query/src/query_ast/cache_node.rs; DESIGN.md §4.9): per
+ * split, the doc set of each QW_NODE_CACHE subtree, one bitmap of ceil(num_docs / 32) uint32 words in HBM, keyed by
+ * the subtree's plan nodes. A search that misses evaluates the subtree once (QWGPU_KERNEL_PREDICATE_FILL) and
+ * publishes the bitmap when it has finished; later searches read it instead of evaluating the subtree. The leaf search
+ * wraps the query of an unscored request with search_after in such a node, so that each page of a paged search
+ * reads the doc set the first page computed. Entries go with their split (unregistered or evicted) and are evicted
+ * least recently used first within the budget.
+ *   qwgpu_set_predicate_cache_budget  bytes of HBM the entries may hold. 0 (the default) disables the cache and frees
+ *                                     every entry that no running search uses. Opt-in: the bytes come out of the HBM
+ *                                     that the splits use.
+ *   qwgpu_predicate_cache_info        budget, bytes held, entries, hits, misses, fills and evictions so far
+ *                                     (NULL = not wanted). */
+int qwgpu_set_predicate_cache_budget(qwgpu_ctx* ctx, uint64_t bytes);
+int qwgpu_predicate_cache_info(qwgpu_ctx* ctx, uint64_t* budget_bytes, uint64_t* used_bytes, uint64_t* entries, uint64_t* hits,
+                               uint64_t* misses, uint64_t* fills, uint64_t* evictions);
+
 /* ---- seam A / B: protobuf in, protobuf out ---------------------------------------------------- */
 
 /* req = quickwit.search.LeafSearchRequest, resp = quickwit.search.LeafSearchResponse
@@ -166,6 +182,9 @@ typedef struct qwgpu_split_result {
 #define QWGPU_KERNEL_PHRASE_LONG 8192u /* k_phrase_long: the pre-pass of the batch's phrases of more than
                                           QW_MAX_PHRASE_TERMS terms (k_phrase, and QWGPU_KERNEL_PHRASE, serve the
                                           shorter ones) */
+#define QWGPU_KERNEL_PREDICATE_FILL 16384u /* the call filled predicate-cache entries: its QW_NODE_CACHE subtrees that
+                                             missed ran first as one count-only k_window batch (with their own phrase /
+                                             term-set pre-passes), counted in the call's launches and device time */
 /* Initial capacity of a split's hashed cell table: min(this, the split's bound on distinct cells). */
 #define QWGPU_HASHED_INIT_CELLS 65536u
 /* Largest total of the hashed tables (cells, key records and slots, each at its split's bound) that one call may

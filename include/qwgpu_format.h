@@ -199,11 +199,16 @@ enum {
                                term i at b + lo_i for every i and some expansion at b + lo_last. Never scored: the
                                node is only valid where its score is not read (filter / must_not, or any sort
                                other than _score). */
-  QW_NODE_TERM_SET = 9 /* a set of terms (tantivy AutomatonWeight of a regex query): children = E TERM nodes of one
+  QW_NODE_TERM_SET = 9, /* a set of terms (tantivy AutomatonWeight of a regex query): children = E TERM nodes of one
                           field with strictly increasing term_ord, 1 <= E <= QW_MAX_SET_TERMS. A doc matches when it holds
                           any child. Positions are not needed, and the children do not count toward the plan's TERM
                           clauses. Never scored: the node is only valid where its score is not read (filter / must_not,
                           or any sort other than _score). */
+  QW_NODE_CACHE = 10 /* the reference's CacheNode (quickwit-query/src/query_ast/cache_node.rs): exactly one child, the
+                        inner subtree, matching the same docs. A context with a predicate cache
+                        (qwgpu_set_predicate_cache_budget) keeps the child's doc set per split and reads it instead of
+                        evaluating the child again. Never scored: in a scoring clause of a query ranked by _score, with
+                        the cache disabled, or around ALL / NONE, the engine lowers it as its child. */
 };
 enum { QW_OCCUR_MUST = 0, QW_OCCUR_SHOULD = 1, QW_OCCUR_MUST_NOT = 2, QW_OCCUR_FILTER = 3 };
 

@@ -43,6 +43,13 @@ impl GpuContext {
         check(unsafe { ffi::qwgpu_set_max_hits(self.raw, max_hits) })
     }
 
+    /// HBM the predicate cache may hold (0, the default, disables it): the doc sets of the queries of paged
+    /// (`search_after`) requests, kept per split so that later pages read them. Pass
+    /// the capacity of `searcher_config.predicate_cache` (256 MB by default in the reference).
+    pub fn set_predicate_cache_budget(&self, bytes: u64) -> Result<(), SearchError> {
+        check(unsafe { ffi::qwgpu_set_predicate_cache_budget(self.raw, bytes) })
+    }
+
     /// Makes a split image (include/qwgpu_format.h) resident; the bytes may be dropped afterwards. The counterpart
     /// of `open_split_bundle` + `warmup` (quickwit-search/src/leaf.rs:210-251, 269-472).
     pub fn register_split(&self, split_id: &str, image: &[u8]) -> Result<(), SearchError> {
@@ -62,6 +69,27 @@ impl GpuContext {
     pub fn resident_bytes(&self) -> u64 {
         unsafe { ffi::qwgpu_resident_bytes(self.raw) }
     }
+
+    /// The predicate cache's budget, bytes held, entries, and hits, misses, fills and evictions so far.
+    pub fn predicate_cache_info(&self) -> Result<PredicateCacheInfo, SearchError> {
+        let mut i = PredicateCacheInfo::default();
+        check(unsafe {
+            ffi::qwgpu_predicate_cache_info(self.raw, &mut i.budget_bytes, &mut i.used_bytes, &mut i.entries, &mut i.hits,
+                                            &mut i.misses, &mut i.fills, &mut i.evictions)
+        })?;
+        Ok(i)
+    }
+}
+
+#[derive(Clone, Copy, Debug, Default)]
+pub struct PredicateCacheInfo {
+    pub budget_bytes: u64,
+    pub used_bytes: u64,
+    pub entries: u64,
+    pub hits: u64,
+    pub misses: u64,
+    pub fills: u64,
+    pub evictions: u64,
 }
 
 impl Drop for GpuContext {

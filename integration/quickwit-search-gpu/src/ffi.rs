@@ -34,6 +34,9 @@ unsafe extern "C" {
     pub fn qwgpu_split_is_resident(ctx: *mut QwgpuCtx, split_id: *const c_char) -> i32;
     pub fn qwgpu_set_residency_budget(ctx: *mut QwgpuCtx, bytes: u64) -> i32;
     pub fn qwgpu_set_max_hits(ctx: *mut QwgpuCtx, max_hits: u32) -> i32;
+    pub fn qwgpu_set_predicate_cache_budget(ctx: *mut QwgpuCtx, bytes: u64) -> i32;
+    pub fn qwgpu_predicate_cache_info(ctx: *mut QwgpuCtx, budget_bytes: *mut u64, used_bytes: *mut u64, entries: *mut u64,
+                                      hits: *mut u64, misses: *mut u64, fills: *mut u64, evictions: *mut u64) -> i32;
     pub fn qwgpu_resident_bytes(ctx: *mut QwgpuCtx) -> u64;
 
     /// prost-encoded `LeafSearchRequest` in, prost-encoded `LeafSearchResponse` out (seam A).

@@ -77,6 +77,31 @@ int qwgpu_set_max_hits(qwgpu_ctx* ctx, uint32_t max_hits) {
   QW_API_END
 }
 
+int qwgpu_set_predicate_cache_budget(qwgpu_ctx* ctx, uint64_t bytes) {
+  QW_API_BEGIN
+  engine_of(ctx).set_pred_budget(bytes);
+  return 0;
+  QW_API_END
+}
+
+int qwgpu_predicate_cache_info(qwgpu_ctx* ctx, uint64_t* budget_bytes, uint64_t* used_bytes, uint64_t* entries, uint64_t* hits,
+                               uint64_t* misses, uint64_t* fills, uint64_t* evictions) {
+  QW_API_BEGIN
+  qw::PredCache& c = engine_of(ctx).pred;
+  std::lock_guard<std::mutex> g(c.mu);
+  uint64_t n = 0;
+  for (const auto& s : c.by_split) n += s.second.size();
+  if (budget_bytes) *budget_bytes = c.budget;
+  if (used_bytes) *used_bytes = c.used.load();
+  if (entries) *entries = n;
+  if (hits) *hits = c.hits;
+  if (misses) *misses = c.misses;
+  if (fills) *fills = c.fills;
+  if (evictions) *evictions = c.evictions;
+  return 0;
+  QW_API_END
+}
+
 int qwgpu_residency_info(qwgpu_ctx* ctx, uint64_t* resident_bytes, uint64_t* budget_bytes, uint64_t* num_splits, uint64_t* evictions) {
   QW_API_BEGIN
   qw::Engine& e = engine_of(ctx);

@@ -194,7 +194,9 @@ struct DSplitPlan {
   uint64_t out_nhits;      // device address of uint32 (hits written by k_select)
   // find_trace_ids (trace_kernel.cuh); tr_on == 0 when the plan has no QW_AGG_TRACE_IDS node
   uint64_t tr_best;        // device address of uint64[tr_num_ords]: latest span per trace ordinal (0 = none)
-  uint64_t tr_match;       // device address of uint32[ceil(num_docs / 32)]: the matched docs (read by the replay)
+  uint64_t match_out;      // 0, or the device address of uint32[ceil(num_docs / 32)] where k_window's collect pass
+                           // writes every window's final match words: the find_trace_ids replay's input, or the
+                           // predicate-cache entry that a fill plan fills
   uint64_t tr_state;       // device address of a DTraceState
   uint64_t tr_tie;         // device address of a uint32 in the split's output header: 1 = the replay ran
   uint32_t tr_on, tr_n;    // N = num_traces

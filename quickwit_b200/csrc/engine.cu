@@ -35,8 +35,77 @@ namespace qw {
 uint32_t id_to_fieldnorm(uint8_t id);  // image_builder.cpp
 
 SplitDev::~SplitDev() {
+  if (pred) pred->drop_split(this);
   if (d_data) cudaFree(d_data);
   if (d_tabs) cudaFree(d_tabs);
+}
+
+// ---- predicate cache (DESIGN.md §4.9) -------------------------------------------------------------
+PredEntry::~PredEntry() {
+  owner->used.fetch_sub(bytes);
+  if (!d_bits) return;
+  std::lock_guard<std::mutex> g(owner->free_mu);
+  owner->to_free.push_back(d_bits);
+}
+
+// Drops the least recently used published entries that no call holds until `limit` bytes or fewer are live (a pinned
+// entry stays: a running call reads it). Caller holds `mu`.
+bool PredCache::evict_to(uint64_t limit) {
+  while (used.load() > limit) {
+    std::unordered_map<std::string, std::shared_ptr<PredEntry>>* vm = nullptr;
+    std::unordered_map<std::string, std::shared_ptr<PredEntry>>::iterator victim;
+    for (auto& s : by_split)
+      for (auto e = s.second.begin(); e != s.second.end(); ++e)
+        if (e->second.use_count() == 1 && (!vm || e->second->last_use < victim->second->last_use)) { vm = &s.second; victim = e; }
+    if (!vm) return false;
+    vm->erase(victim);
+    evictions++;
+  }
+  return true;
+}
+
+std::shared_ptr<PredEntry> PredCache::acquire(const SplitDev* sp, const std::string& key, uint64_t bytes, bool* hit) {
+  std::lock_guard<std::mutex> g(mu);
+  auto& m = by_split[sp];
+  auto it = m.find(key);
+  if (it != m.end()) {
+    *hit = true;
+    hits++;
+    it->second->last_use = ++tick;
+    return it->second;
+  }
+  *hit = false;
+  misses++;
+  if (bytes > budget || !evict_to(budget - bytes)) return nullptr;
+  auto e = std::make_shared<PredEntry>();
+  e->owner = this;
+  e->key = key;
+  e->bytes = bytes;
+  e->last_use = ++tick;
+  used.fetch_add(bytes);
+  return e;
+}
+
+void PredCache::publish(const SplitDev* sp, const std::shared_ptr<PredEntry>& e) {
+  std::lock_guard<std::mutex> g(mu);
+  fills++;
+  if (!budget) return;  // (disabled while the call ran: the entry goes)
+  e->last_use = ++tick;
+  by_split[sp].emplace(e->key, e);  // (a concurrent fill of the same key that published first stays)
+}
+
+void PredCache::drop_split(const SplitDev* sp) {
+  std::lock_guard<std::mutex> g(mu);
+  by_split.erase(sp);
+}
+
+void PredCache::free_released(void* stream) {
+  std::vector<void*> v;
+  {
+    std::lock_guard<std::mutex> g(free_mu);
+    v.swap(to_free);
+  }
+  for (void* p : v) cudaFreeAsync(p, (cudaStream_t)stream);
 }
 
 struct CallSlot {
@@ -119,6 +188,42 @@ Engine::~Engine() {
   cudaSetDevice(device);
   for (CallSlot* s : free_slots) delete s;
   splits.clear();
+  pred.by_split.clear();
+  pred.free_released(nullptr);
+  if (pred.pool) {
+    cudaStreamSynchronize(nullptr);
+    cudaMemPoolDestroy((cudaMemPool_t)pred.pool);
+  }
+}
+
+// A budget of 0 disables the cache: every published entry is dropped (the bitmaps of entries a running call still
+// holds go when that call releases them). The bitmaps come from a pool of the engine's own that keeps freed memory
+// for reuse, so that no search allocates or frees device memory synchronously.
+void Engine::set_pred_budget(uint64_t bytes) {
+  CUDA_CHECK(cudaSetDevice(device));
+  {
+    std::lock_guard<std::mutex> g(pred.mu);
+    if (bytes && !pred.pool) {
+      cudaMemPoolProps props;
+      memset(&props, 0, sizeof props);
+      props.allocType = cudaMemAllocationTypePinned;
+      props.location.type = cudaMemLocationTypeDevice;
+      props.location.id = device;
+      cudaMemPool_t pool;
+      CUDA_CHECK(cudaMemPoolCreate(&pool, &props));
+      uint64_t keep = ~0ull;
+      CUDA_CHECK(cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep));
+      pred.pool = pool;
+    }
+    pred.budget = bytes;
+    if (!bytes) pred.by_split.clear();
+    else pred.evict_to(bytes);
+  }
+  if (!bytes && pred.pool) {
+    pred.free_released(nullptr);
+    CUDA_CHECK(cudaStreamSynchronize(nullptr));
+    CUDA_CHECK(cudaMemPoolTrimTo((cudaMemPool_t)pred.pool, 0));
+  }
 }
 
 // host half of a registration: directory copy + views (no device work)
@@ -203,6 +308,7 @@ static void publish(Engine& e, const std::shared_ptr<SplitDev>& sp) {
 void Engine::register_split(const char* id, const uint8_t* img, uint64_t len) {
   ImageView full;
   auto sp = open_split(id, img, len, &full);
+  sp->pred = &pred;
   {
     std::lock_guard<std::mutex> g(mu);
     if (budget && sp->data_len > budget) fail(QWGPU_EINVALID_ARG, "split `%s` needs %llu bytes, the residency budget is %llu", id, (unsigned long long)sp->data_len, (unsigned long long)budget);
@@ -224,6 +330,7 @@ void Engine::register_split(const char* id, const uint8_t* img, uint64_t len) {
 void Engine::register_split_async(const char* id, const uint8_t* img, uint64_t len) {
   ImageView full;
   auto sp = open_split(id, img, len, &full);
+  sp->pred = &pred;
   sp->state = 0;
   {
     std::lock_guard<std::mutex> g(mu);
@@ -297,6 +404,8 @@ void Engine::unregister_split(const char* id) {
   loaded_cv.wait(g, [&] { return sp->state != 0; });  // (its loader still writes the device buffer)
   it = splits.find(id);
   if (it != splits.end() && it->second == sp) { resident -= sp->data_len; splits.erase(it); }
+  sp.reset();  // (the last reference, unless a call still uses the split: its cache entries go with it)
+  pred.free_released(nullptr);
 }
 
 // A search takes the split in use: recency for the LRU; a split that is still loading is waited for.
@@ -405,6 +514,15 @@ struct Lowered {
   uint32_t ts_blocks = 0;               // posting blocks of ts_terms
   uint32_t tr_img_col = 0;              // find_trace_ids: the trace-id column of the image
   uint64_t h_bound = 0;                 // hashed aggregation layout: upper bound on the split's distinct cells
+  // predicate cache: `pc` is null when every QW_NODE_CACHE is lowered as its child (cache disabled, the plan's
+  // stripped lowering, a fill plan)
+  PredCache* pc = nullptr;
+  bool has_cache = false;                                   // the plan holds a QW_NODE_CACHE
+  std::map<uint32_t, std::shared_ptr<PredEntry>> cache_at;  // plan node -> the entry it reads (lower_node's input)
+  std::vector<std::pair<uint32_t, std::shared_ptr<PredEntry>>> cache_instr;  // instruction -> the entry it reads
+  std::vector<std::shared_ptr<PredEntry>> misses;           // entries this plan fills (published after the call)
+  std::shared_ptr<PredEntry> fill;                          // a fill plan: the entry its matches go to
+  std::shared_ptr<Lowered> stripped;  // a plan that reads entries: its lowering without the cache (the fallback)
 };
 
 // The boundary table of a percentiles node's column (ddsketch.h), built once per split and column: a column that
@@ -434,6 +552,50 @@ static uint32_t use_col(Lowered& L, const SplitDev& sp, uint32_t c) {
   L.cols.push_back(d);
   L.col_max_raw.push_back(ic.gcd ? (ic.max_value - ic.min_value) / ic.gcd : 0);
   return (uint32_t)L.col_map[c];
+}
+
+// The cache key of the subtree at `root`: its plan nodes in breadth-first order, children rebased onto that order,
+// the root's occur, every boost and bm25_weight zeroed (scores are never read through the cache). On one split these
+// nodes fix the doc set exactly. A fill plan's nodes are the key itself.
+static std::string pred_key(const QwPlanNode* nodes, uint32_t nn, uint32_t root) {
+  std::vector<QwPlanNode> out(1, nodes[root]);
+  for (size_t i = 0; i < out.size(); i++) {
+    QwPlanNode& n = out[i];
+    n.boost = 0.f;
+    n.bm25_weight = 0.f;
+    const bool parent = n.kind == QW_NODE_BOOL || n.kind == QW_NODE_PHRASE || n.kind == QW_NODE_PHRASE_PREFIX ||
+                        n.kind == QW_NODE_TERM_SET || n.kind == QW_NODE_CACHE;
+    if (!parent || !n.num_children) { n.first_child = n.num_children = 0; continue; }
+    if ((uint64_t)n.first_child + n.num_children > nn || out.size() + n.num_children > nn) fail(QWGPU_EINVALID_ARG, "plan children out of range");
+    const uint32_t first = n.first_child, cnt = n.num_children;
+    n.first_child = (uint32_t)out.size();
+    out.insert(out.end(), nodes + first, nodes + first + cnt);  // (`n` dangles from here)
+  }
+  out[0].occur = QW_OCCUR_MUST;
+  return std::string((const char*)out.data(), out.size() * sizeof(QwPlanNode));
+}
+
+// What the node at `idx` is lowered as, when it is a QW_NODE_CACHE: itself when it reads a cache entry (acquired
+// here into L.cache_at), else its child (the cache is off for this plan, the node's score is read, or the child is
+// ALL / NONE), followed through nested CACHE nodes. Any other node is itself.
+static uint32_t resolve_cache(Lowered& L, const SplitDev& sp, const QwPlanNode* nodes, uint32_t nn, uint32_t idx, bool scored) {
+  for (uint32_t hops = 0; idx < nn && nodes[idx].kind == QW_NODE_CACHE; hops++) {
+    const QwPlanNode& n = nodes[idx];
+    if (n.num_children != 1 || n.first_child >= nn || hops >= nn) fail(QWGPU_EINVALID_ARG, "cache node with %u children", n.num_children);
+    L.has_cache = true;
+    const uint32_t c = n.first_child;
+    if (L.pc && !scored && nodes[c].kind != QW_NODE_ALL && nodes[c].kind != QW_NODE_NONE) {
+      bool hit = false;
+      std::shared_ptr<PredEntry> e = L.pc->acquire(&sp, pred_key(nodes, nn, c), std::max<uint64_t>((sp.view.hdr->num_docs + 31) / 32, 1) * 4, &hit);
+      if (e) {
+        if (!hit) L.misses.push_back(e);
+        L.cache_at[idx] = std::move(e);
+        return idx;
+      }
+    }
+    idx = c;
+  }
+  return idx;
 }
 
 static void lower_node(Lowered& L, const SplitDev& sp, const QwPlanNode* nodes, uint32_t nn, uint32_t idx,
@@ -516,8 +678,12 @@ static void lower_node(Lowered& L, const SplitDev& sp, const QwPlanNode* nodes, 
       // only probe surviving candidates)
       std::vector<uint32_t> order;
       auto child = [&](uint32_t c) -> const QwPlanNode& { return nodes[n.first_child + c]; };
+      // what each child is lowered as (resolve_cache), with the child's own occur
+      std::vector<uint32_t> eff(n.num_children);
+      for (uint32_t c = 0; c < n.num_children; c++)
+        eff[c] = resolve_cache(L, sp, nodes, nn, n.first_child + c, scored && (child(c).occur == QW_OCCUR_MUST || child(c).occur == QW_OCCUR_SHOULD));
       auto is_req = [&](uint32_t c) { return child(c).occur == QW_OCCUR_MUST || child(c).occur == QW_OCCUR_FILTER; };
-      auto is_colpred = [&](uint32_t c) { return child(c).kind == QW_NODE_RANGE || child(c).kind == QW_NODE_EXISTS || child(c).kind == QW_NODE_ALL; };
+      auto is_colpred = [&](uint32_t c) { const uint32_t k = nodes[eff[c]].kind; return k == QW_NODE_RANGE || k == QW_NODE_EXISTS || k == QW_NODE_ALL; };
       const bool child_scored_ctx = scored_ctx;
       for (uint32_t c = 0; c < n.num_children; c++) if (is_req(c) && child_scored_ctx && child(c).occur == QW_OCCUR_MUST) order.push_back(c);
       for (int pass = 0; pass < 2; pass++)
@@ -532,10 +698,10 @@ static void lower_node(Lowered& L, const SplitDev& sp, const QwPlanNode* nodes, 
       for (uint32_t c = 0; c < n.num_children; c++) if (child(c).occur == QW_OCCUR_MUST_NOT) order.push_back(c);
       for (uint32_t c : order) {
         const QwPlanNode& cn = child(c);
-        uint32_t child_level = cn.kind == QW_NODE_BOOL ? level + 1 : level;
+        uint32_t child_level = nodes[eff[c]].kind == QW_NODE_BOOL ? level + 1 : level;
         if (scored && cn.occur == QW_OCCUR_MUST) L.need_msum |= 1u << level;
         if (scored && cn.occur == QW_OCCUR_SHOULD) L.need_ssum |= 1u << level;
-        lower_node(L, sp, nodes, nn, n.first_child + c, child_level, cn.occur, scored);
+        lower_node(L, sp, nodes, nn, eff[c], child_level, cn.occur, scored);
       }
       uint32_t msm = n.min_should_match == 0xFFFFFFFFu ? 0 : n.min_should_match;
       uint32_t need = msm > 0 ? msm : (n_req == 0 ? 1 : 0);
@@ -704,6 +870,14 @@ static void lower_node(Lowered& L, const SplitDev& sp, const QwPlanNode* nodes, 
       L.instrs.push_back(in);
       break;
     }
+    case QW_NODE_CACHE: {
+      // a subtree read from its predicate-cache entry (resolve_cache acquired it): the entry's doc bitmap, consumed
+      // like a term set's (OP_TERM_SET); a miss is filled by the call's fill pass first
+      in.op = OP_TERM_SET;
+      L.cache_instr.push_back({(uint32_t)L.instrs.size(), L.cache_at.at(idx)});
+      L.instrs.push_back(in);
+      break;
+    }
     default: fail(QWGPU_EINVALID_ARG, "unknown plan node kind %u", n.kind);
   }
 }
@@ -733,23 +907,24 @@ static void lower_plan(Lowered& L, const SplitDev& sp, const uint8_t* plan, size
   P.sa = ph->search_after;
   P.score_hits = (uint32_t)qw_plan_score_hits(ph);
   const bool scoring = ph->scoring != 0;
-  if (nodes[0].kind == QW_NODE_BOOL) {
-    lower_node(L, sp, nodes, ph->num_nodes, 0, 0, QW_OCCUR_MUST, scoring);
-  } else if (nodes[0].kind == QW_NODE_TERM && scoring) {
+  const uint32_t root = resolve_cache(L, sp, nodes, ph->num_nodes, 0, scoring);
+  if (nodes[root].kind == QW_NODE_BOOL) {
+    lower_node(L, sp, nodes, ph->num_nodes, root, 0, QW_OCCUR_MUST, scoring);
+  } else if (nodes[root].kind == QW_NODE_TERM && scoring) {
     // a scored single-term query is the one-clause case of the BM25 union: lower it as
     // bool{should: [term]} so that it takes k_union (same matches, same f32 score)
     QwPlanNode wrap[2];
     memset(wrap, 0, sizeof wrap);
     wrap[0].kind = QW_NODE_BOOL; wrap[0].occur = QW_OCCUR_MUST; wrap[0].boost = 1.0f;
     wrap[0].first_child = 1; wrap[0].num_children = 1; wrap[0].min_should_match = 0xFFFFFFFFu;
-    wrap[1] = nodes[0];
+    wrap[1] = nodes[root];
     wrap[1].occur = QW_OCCUR_SHOULD;
     lower_node(L, sp, wrap, 2, 0, 0, QW_OCCUR_MUST, scoring);
   } else {
     DInstr bg; memset(&bg, 0, sizeof bg); bg.op = OP_BOOL_BEGIN; L.instrs.push_back(bg);
     L.levels |= 1;
     if (scoring) L.need_msum |= 1;
-    lower_node(L, sp, nodes, ph->num_nodes, 0, 0, QW_OCCUR_MUST, scoring);
+    lower_node(L, sp, nodes, ph->num_nodes, root, 0, QW_OCCUR_MUST, scoring);
     DInstr en; memset(&en, 0, sizeof en); en.op = OP_BOOL_END; en.n = 1; en.flags = scoring ? IF_SCORED : 0; L.instrs.push_back(en);
   }
   {
@@ -1167,7 +1342,8 @@ static void plan_sample(Route& r, const std::vector<Lowered>& low, int sm_count)
   }
 }
 
-static Route choose_route(const std::vector<Lowered>& low, int max_smem_optin, int sm_count) {
+// fill: a predicate-cache fill batch, which only k_window serves (it writes the match words out)
+static Route choose_route(const std::vector<Lowered>& low, int max_smem_optin, int sm_count, bool fill = false) {
   Route r;
   uint32_t n_levels = 1, need_cnt = 0, need_ssum = 0, need_msum = 0, max_instr = 0, max_cols = 0, max_aggs = 0, n_fn = 0;
   // second-chance top-K: when no plan ranks by _score first, the collect pass also records the exact
@@ -1186,7 +1362,8 @@ static Route choose_route(const std::vector<Lowered>& low, int max_smem_optin, i
     n_fn = std::max(n_fn, L.P.n_fn_slots);
     any_topk |= L.P.max_hits > 0;
   }
-  if (all_driver) r.kind = Route::DRIVER;
+  if (fill) r.kind = Route::WINDOW;
+  else if (all_driver) r.kind = Route::DRIVER;
   else if (all_union) r.kind = Route::UNION;
   else if (aggscan_layout(low, max_smem_optin, &r.alay)) r.kind = Route::AGGSCAN;
   r.rec_l0 = rec_l0 && any_topk && r.kind != Route::DRIVER;
@@ -1515,7 +1692,7 @@ struct Run {
       if (P.tr_on) {
         P.tr_state = (uint64_t)(slot.d_scratch + s_trace_state + (size_t)i * sizeof(qwk::DTraceState));
         P.tr_best = (uint64_t)(slot.d_scratch + at[i].tr_best);
-        P.tr_match = (uint64_t)(slot.d_scratch + at[i].tr_match);
+        P.match_out = (uint64_t)(slot.d_scratch + at[i].tr_match);
         P.tr_tie = (uint64_t)(ob + 24);
       }
       if (P.hashed) {
@@ -1524,8 +1701,10 @@ struct Run {
         P.h_cells = (uint64_t)(slot.d_scratch + at[i].h_cells);
         P.h_ctr = (uint64_t)(ob + 28);
       }
+      if (L.fill) P.match_out = (uint64_t)L.fill->d_bits;
       DInstr* instrs = (DInstr*)(hb + o_instr) + P.instr_base;
       memcpy(instrs, L.instrs.data(), P.n_instr * sizeof(DInstr));
+      for (const auto& c : L.cache_instr) instrs[c.first].a = (uint64_t)c.second->d_bits;
       // short and long phrases go to their own kernel's array, each numbering its driver blocks from 0
       for (size_t k = 0; k < L.phrases.size(); k++) {
         DPhrase ph = L.phrases[k];
@@ -1901,11 +2080,39 @@ struct Run {
   }
 };
 
+// A plan with QW_NODE_CACHE nodes, lowered against the predicate cache: hits read their entries, misses get new
+// entries and, in `fills`, one count-only plan each (the subtree's key nodes as the whole query) whose collect pass
+// writes the entry. Nested CACHE nodes of a fill plan are lowered as their children.
+static Lowered lower_cached(PredCache* pc, const SplitDev& sp, const uint8_t* plan, size_t plan_len, uint32_t max_hits,
+                            std::vector<Lowered>& fills) {
+  Lowered C;
+  C.pc = pc;
+  lower_plan(C, sp, plan, plan_len, max_hits);
+  for (const std::shared_ptr<PredEntry>& m : C.misses) {
+    QwPlanHeader h;
+    memset(&h, 0, sizeof h);
+    h.magic = QW_PLAN_MAGIC;
+    h.version = 1;
+    h.num_nodes = (uint32_t)(m->key.size() / sizeof(QwPlanNode));
+    h.count_only = 1;
+    h.sort[0] = QwSortSpec{QW_SORT_DOCID, QW_ORDER_DESC, 0xFFFFFFFFu, 0};
+    h.sort[1] = QwSortSpec{QW_SORT_NONE, QW_ORDER_DESC, 0xFFFFFFFFu, 0};
+    std::string fp((const char*)&h, sizeof h);
+    fp += m->key;
+    Lowered F;
+    F.fill = m;
+    lower_plan(F, sp, (const uint8_t*)fp.data(), fp.size(), max_hits);
+    fills.push_back(std::move(F));
+  }
+  return C;
+}
+
 // Lowers every plan once per call; a split whose plan cannot be lowered fails alone. idx: position of each lowered
-// plan in the caller's arrays.
+// plan in the caller's arrays. pc: the predicate cache when it is enabled; the fill plans of the batch's misses go to
+// `fills`.
 static std::vector<Lowered> lower_batch(const std::vector<std::shared_ptr<SplitDev>>& sp, const std::vector<const uint8_t*>& plans,
                                         const std::vector<size_t>& plan_lens, std::vector<SplitOutput>& outs, std::vector<uint32_t>& idx,
-                                        uint32_t max_hits) {
+                                        uint32_t max_hits, PredCache* pc, std::vector<Lowered>& fills) {
   std::vector<Lowered> low;
   low.reserve(sp.size());
   for (uint32_t i = 0; i < (uint32_t)sp.size(); i++) {
@@ -1913,6 +2120,20 @@ static std::vector<Lowered> lower_batch(const std::vector<std::shared_ptr<SplitD
       if (!sp[i]) fail(QWGPU_ENOTFOUND, "split not registered");
       Lowered L;
       lower_plan(L, *sp[i], plans[i], plan_lens[i], max_hits);
+      // Route rule: the cache does not remove the work of k_driver's posting-driven walk, so a plan that k_driver
+      // serves with its CACHE nodes lowered as their children keeps that lowering. (k_union and k_aggscan plans never
+      // read an entry: a scored or ALL / NONE subtree is always lowered as itself.)
+      if (pc && L.has_cache && !driver_eligible(L)) {
+        std::vector<Lowered> f;
+        try {
+          Lowered C = lower_cached(pc, *sp[i], plans[i], plan_lens[i], max_hits, f);
+          C.stripped = std::make_shared<Lowered>(std::move(L));
+          L = std::move(C);
+          for (Lowered& x : f) fills.push_back(std::move(x));
+        } catch (const Error&) {
+          // (a subtree that does not lower on its own: the plan runs without the cache)
+        }
+      }
       low.push_back(std::move(L));
       idx.push_back(i);
     } catch (const Error& e) {
@@ -2067,18 +2288,64 @@ void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std:
   const auto t_begin = tclock::now();
   CUDA_CHECK(cudaSetDevice(device));
   std::vector<uint32_t> idx;
-  const std::vector<Lowered> low = lower_batch(sp, plans, plan_lens, outs, idx, max_hits.load(std::memory_order_relaxed));
+  PredCache* pc = nullptr;
+  {
+    std::lock_guard<std::mutex> g(pred.mu);
+    if (pred.budget) pc = &pred;
+  }
+  // (declared before the slot lease: the entries they pin are released only once the call's stream is idle)
+  std::vector<Lowered> fills;
+  std::vector<Lowered> low = lower_batch(sp, plans, plan_lens, outs, idx, max_hits.load(std::memory_order_relaxed), pc, fills);
   const bool gathering = merge && merged && merge->k > 0 && gather && gather->allgather && gather->world > 1 && rank_headers;
   if (low.empty()) {
     if (gathering) exchange_empty(*this, *merge, *gather, *merged, *rank_headers);
     return;
   }
   const auto t_lowered = tclock::now();
-  const Route r = choose_route(low, max_smem_optin, sm_count);
+  Route r = choose_route(low, max_smem_optin, sm_count);
   // device-side cross-split merge: the per-split hit lists stay in scratch, only the merged top-K comes back
   const bool do_merge = merge && merged && merge->k > 0 && merge->rank.size() == sp.size() &&
                         std::any_of(low.begin(), low.end(), [](const Lowered& L) { return L.P.max_hits > 0; });
   SlotLease lease(*this);
+  pred.free_released(lease.slot->stream);
+  if (!fills.empty()) {
+    // the entries' bitmaps, stream-ordered from the pool. The budget is a ceiling, not a reservation: when the device
+    // cannot provide a bitmap, the plans that needed it run without the cache (their stripped lowering) and their
+    // other fills are dropped — the optional cache never fails a search
+    const cudaStream_t st = lease.slot->stream;
+    for (Lowered& F : fills)
+      if (cudaMallocFromPoolAsync(&F.fill->d_bits, F.fill->bytes, (cudaMemPool_t)pred.pool, st) != cudaSuccess) {
+        cudaGetLastError();
+        F.fill->d_bits = nullptr;
+      }
+    bool fell_back = false;
+    for (Lowered& L : low)
+      if (std::any_of(L.misses.begin(), L.misses.end(), [](const std::shared_ptr<PredEntry>& m) { return !m->d_bits; })) {
+        Lowered s = std::move(*L.stripped);
+        L = std::move(s);
+        fell_back = true;
+      }
+    if (fell_back) r = choose_route(low, max_smem_optin, sm_count);
+    // (a fill whose entry no plan reads any more is the only holder of it)
+    fills.erase(std::remove_if(fills.begin(), fills.end(), [](const Lowered& F) { return !F.fill->d_bits || F.fill.use_count() == 1; }),
+                fills.end());
+    pred.free_released(st);
+  }
+  if (!fills.empty()) {
+    // the predicate-cache fill pass: every miss of the call as one count-only batch on k_window, before the call's
+    // own passes; each entry is zeroed first (windows that a fill plan skips as empty write nothing)
+    const cudaStream_t st = lease.slot->stream;
+    for (Lowered& F : fills) CUDA_CHECK(cudaMemsetAsync(F.fill->d_bits, 0, F.fill->bytes, st));
+    std::vector<uint32_t> fidx(fills.size());
+    for (uint32_t i = 0; i < (uint32_t)fills.size(); i++) fidx[i] = i;
+    const Route fr = choose_route(fills, max_smem_optin, sm_count, true);
+    Run fill{*this, *lease.slot, stats, fills, fidx, fr, nullptr, nullptr, false, false, (uint32_t)fills.size(), st};
+    fill.lay_out(false);
+    fill.size_slot();
+    fill.stage();
+    fill.run(false);
+    stats.kernel_mask |= QWGPU_KERNEL_PREDICATE_FILL;
+  }
   Run run{*this, *lease.slot, stats, low, idx, r, merge, gather, do_merge, do_merge && gathering, (uint32_t)low.size(), lease.slot->stream};
   tclock::time_point t_staged;
   for (bool at_bound : {false, true}) {
@@ -2092,6 +2359,9 @@ void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std:
     stats.kernel_mask |= QWGPU_KERNEL_HASHED_AGGS_RETRY;
   }
 
+  // the call has finished: its filled entries become visible to other calls
+  for (uint32_t i = 0; i < low.size(); i++)
+    for (const std::shared_ptr<PredEntry>& m : low[i].misses) pred.publish(sp[idx[i]].get(), m);
   const auto t_searched = tclock::now();
   const uint8_t* h_out = lease.slot->h_out;
   for (uint32_t i = 0; i < low.size(); i++)

@@ -6,12 +6,47 @@
 #include <memory>
 #include <mutex>
 #include <thread>
+#include <unordered_map>
 #include <string>
 #include <vector>
 
 #include "common.h"
 
 namespace qw {
+
+struct SplitDev;
+struct PredCache;
+
+// One predicate-cache entry: the doc set of a QW_NODE_CACHE subtree on one split, as uint32[ceil(num_docs / 32)] in
+// HBM. A call holds a reference to every entry it lowered against (a pin: eviction skips entries referenced
+// elsewhere); the last reference hands the bitmap back to the cache's pool.
+struct PredEntry {
+  PredCache* owner = nullptr;
+  std::string key;            // the subtree as plan nodes (pred_key)
+  void* d_bits = nullptr;     // allocated on the stream of the call that fills it
+  uint64_t bytes = 0, last_use = 0;
+  ~PredEntry();
+};
+
+// The context's predicate cache (DESIGN.md §4.9): the entries of every resident split, LRU within a byte budget.
+// Entries are published per split once the call that filled them has finished.
+struct PredCache {
+  std::mutex mu;  // guards everything below except `used` and the free list; never held while taking Engine::mu
+  uint64_t budget = 0, tick = 0;
+  uint64_t hits = 0, misses = 0, fills = 0, evictions = 0;
+  std::map<const SplitDev*, std::unordered_map<std::string, std::shared_ptr<PredEntry>>> by_split;
+  void* pool = nullptr;  // cudaMemPool_t, created with the first non-zero budget
+  std::atomic<uint64_t> used{0};  // bytes of every live entry, published or not
+  std::mutex free_mu;
+  std::vector<void*> to_free;  // bitmaps of released entries, freed stream-ordered by the next call
+  // a published entry for `key` (a hit, pinned), else a new unpublished entry of `bytes` (a miss); null when the
+  // miss does not fit the budget
+  std::shared_ptr<PredEntry> acquire(const SplitDev* sp, const std::string& key, uint64_t bytes, bool* hit);
+  void publish(const SplitDev* sp, const std::shared_ptr<PredEntry>& e);  // the first entry published for a key wins
+  bool evict_to(uint64_t limit);
+  void drop_split(const SplitDev* sp);
+  void free_released(void* stream);  // cudaFreeAsync of the released bitmaps on `stream`
+};
 
 struct SplitDev {
   std::string id;
@@ -28,6 +63,7 @@ struct SplitDev {
   uint64_t last_use = 0;
   int state = 1;
   std::string load_error;
+  PredCache* pred = nullptr;  // the context's predicate cache: this split's entries go with it
   ~SplitDev();
 };
 
@@ -89,6 +125,7 @@ struct BatchStats {
 struct Engine {
   int device = -1;
   std::mutex mu;
+  PredCache pred;  // (declared before `splits`: a split's destructor drops its entries here)
   std::map<std::string, std::shared_ptr<SplitDev>> splits;
   std::vector<CallSlot*> free_slots;
   std::atomic<int> in_flight{0};  // searches between slot acquisition and release
@@ -119,6 +156,8 @@ struct Engine {
   void register_split_async(const char* id, const uint8_t* img, uint64_t len);
   void wait_split(const char* id);  // throws the upload's error, if any
   void set_budget(uint64_t bytes);
+  // predicate cache budget (0 disables the cache and frees every entry that no call is using)
+  void set_pred_budget(uint64_t bytes);
   void unregister_split(const char* id);
   std::shared_ptr<SplitDev> find(const std::string& id);
   // Runs plan[i] on splits[i]; fills outs[i] (status per split). Throws only on whole-call errors.

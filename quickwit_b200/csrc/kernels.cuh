@@ -1408,10 +1408,11 @@ __global__ void __launch_bounds__(QW_THREADS, QW_MIN_BLOCKS_PER_SM) k_window(con
         if (rec && my_top) atomicMax(&s_misc[4], my_top);
       }
       __syncthreads();
-      if (P.tr_on && !p.cands_only) {
-        // find_trace_ids: the window's matches, for a replay of the reference's sentinel (trace_kernel.cuh)
+      if (P.match_out && !p.cands_only) {
+        // the window's matches: for find_trace_ids' replay of the reference's sentinel (trace_kernel.cuh), or into a
+        // predicate-cache entry (a fill plan)
         const uint32_t nwd = (P.num_docs + 31) >> 5;
-        for (uint32_t wd = tid; wd < NW && (ws >> 5) + wd < nwd; wd += QW_THREADS) ((uint32_t*)P.tr_match)[(ws >> 5) + wd] = res[wd];
+        for (uint32_t wd = tid; wd < NW && (ws >> 5) + wd < nwd; wd += QW_THREADS) ((uint32_t*)P.match_out)[(ws >> 5) + wd] = res[wd];
       }
       if (tid == 0 && !p.cands_only) {
         const uint32_t hits = s_misc[2];

@@ -321,11 +321,34 @@ static std::vector<SplitRequest> optimize_split_requests(const pb::SearchRequest
 // fails the same way on every node, and retrying would only run it twice.
 static inline bool retryable(int code) { return code != QWGPU_EUNSUPPORTED; }
 
+// add_top_cache_node (rewrite_request, leaf.rs:724-737): a request with search_after is a page of a paged search, and
+// the pages after it evaluate the same query again. With the context's predicate cache enabled, the query AST is
+// wrapped in a `cache` node, so that each split's doc set is computed once and read by every later page. A request
+// ranked by _score compiles the node as its inner query (compile_plan); with the cache disabled nothing is wrapped.
+// Like the reference, which wraps each split's request after the split-level decisions (optimize_split_requests reads
+// the AST unwrapped), the wrapped AST `out` only goes to the compiler. False: not wrapped.
+static bool add_top_cache_node(Engine& eng, const Json& ast, Json& out) {
+  {
+    std::lock_guard<std::mutex> g(eng.pred.mu);
+    if (!eng.pred.budget) return false;
+  }
+  Json type;
+  type.type = Json::Str;
+  type.s = "cache";
+  out = Json();
+  out.type = Json::Obj;
+  out.obj.emplace_back("type", std::move(type));
+  out.obj.emplace_back("inner", ast);
+  return true;
+}
+
 static void run_leaf_raw(Engine& eng, const pb::LeafSearchRequest& lr, LeafRun& run, bool want_merged = false, const Comm* comm = nullptr) {
   using clock = std::chrono::steady_clock;
   const pb::SearchRequest& sreq = lr.search_request;
   const auto t_compile = clock::now();
   Json ast = parse_json(sreq.query_ast, QWGPU_EINVALID_QUERY);  // once per request
+  Json cached_ast;
+  const Json* compile_ast = sreq.search_after && add_top_cache_node(eng, ast, cached_ast) ? &cached_ast : &ast;
   for (auto& ref : lr.leaf_requests) {
     if (ref.doc_mapper_ord >= lr.doc_mappers.size()) fail(QWGPU_EINVALID_ARG, "Internal error: doc_mapper_ord out of bounds");
     DocMapperInfo dm = parse_doc_mapper(lr.doc_mappers[ref.doc_mapper_ord]);
@@ -356,7 +379,7 @@ static void run_leaf_raw(Engine& eng, const pb::LeafSearchRequest& lr, LeafRun& 
       j.dev = eng.find(so.split_id);
       try {
         if (!j.dev) fail(QWGPU_ENOTFOUND, "split `%s` is not resident on this GPU", so.split_id.c_str());
-        j.plan = compile_plan(j.dev->view, so.split_id, *req, dm, &so, &ast);
+        j.plan = compile_plan(j.dev->view, so.split_id, *req, dm, &so, compile_ast);
       } catch (const Error& e) {
         // malformed queries / aggregations fail the whole request like the reference (service.rs:182-184); so does
         // a query or aggregation shape this library does not compile: every split would fail the same way

@@ -129,7 +129,7 @@ static int64_t truncate_ns(int64_t ns, int64_t prec) {  // DateTime::truncate
 
 // ---- TantivyQueryAst mirror ------------------------------------------------------------------------
 struct TQ {
-  enum Kind { Bool, Term, Range, Exists, All, None, Phrase, PhrasePrefix, TermSet } kind = None;
+  enum Kind { Bool, Term, Range, Exists, All, None, Phrase, PhrasePrefix, TermSet, Cache } kind = None;  // Cache: must[0]
   std::vector<uint32_t> phrase_terms;  // Phrase / PhrasePrefix: (exact) term ords in phrase order (offset k = position k)
   std::vector<uint32_t> prefix_terms;  // PhrasePrefix: the expansions of the last slot (offset = phrase_terms.size());
                                        // TermSet: the term ords of one field, ascending
@@ -720,8 +720,16 @@ static TQ build(const Ctx& cx, const Json& q, int depth) {
     return inner;
   }
   if (type == "cache") {
-    if (const Json* inner = q.get("inner")) return build(cx, *inner, depth + 1);
-    fail(QWGPU_EINVALID_QUERY, "invalid query: cache node without inner query");
+    // CacheNode (cache_node.rs): a QW_NODE_CACHE over the inner query, opaque to simplify like a boost. A request ranked
+    // by _score reads scores the cache does not keep: the inner query is compiled in its place.
+    const Json* inner = q.get("inner");
+    if (!inner) fail(QWGPU_EINVALID_QUERY, "invalid query: cache node without inner query");
+    if (cx.scoring) return build(cx, *inner, depth + 1);
+    TQ c;
+    c.kind = TQ::Cache;
+    c.opaque = true;
+    c.must.push_back(simplify(build(cx, *inner, depth + 1)));
+    return c;
   }
   if (type == "user_input")
     fail(QWGPU_EINVALID_QUERY, "invalid query: user_input queries must be parsed by the root before reaching a leaf");
@@ -814,6 +822,15 @@ static void emit(const TQ& t, uint32_t occur, const ImageView& img, std::vector<
         c.term_ord = t.prefix_terms[i]; c.field_id = field_id; c.column = 0xFFFFFFFFu;
         c.bm25_weight = bm25_idf(img.terms[c.term_ord].doc_freq, img.hdr->num_docs) * (1.0f + BM25_K1);
       }
+      break;
+    }
+    case TQ::Cache: {
+      n.kind = QW_NODE_CACHE;
+      const size_t first = out.size();  // (`n` dangles after the resize below)
+      out[idx].first_child = (uint32_t)first;
+      out[idx].num_children = 1;
+      out.resize(first + 1);
+      emit(t.must[0], QW_OCCUR_MUST, img, out, first);
       break;
     }
     case TQ::Bool: {

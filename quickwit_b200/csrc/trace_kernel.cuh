@@ -221,7 +221,7 @@ __global__ void __launch_bounds__(QT_TILE) k_trace_replay(const DSplitPlan* plan
   bool running = false;
   uint32_t r_ord = 0;
   uint64_t r_ts = 0;
-  const uint32_t* match = (const uint32_t*)P.tr_match;
+  const uint32_t* match = (const uint32_t*)P.match_out;
   for (uint32_t d0 = 0; d0 < P.num_docs; d0 += QT_TILE) {
     const uint32_t doc = d0 + tid;
     const bool on = doc < P.num_docs && ((match[doc >> 5] >> (doc & 31)) & 1u);

@@ -23,6 +23,7 @@ CARD_FULL, CARD_OPTIONAL, CARD_MULTI = range(3)
 NODE_TERM, NODE_RANGE, NODE_BOOL, NODE_ALL, NODE_NONE, NODE_EXISTS, NODE_PHRASE = 1, 2, 3, 4, 5, 6, 7
 NODE_PHRASE_PREFIX = 8
 NODE_TERM_SET = 9  # children: 1..MAX_SET_TERMS TERM nodes of one field, increasing term_ord; never scored
+NODE_CACHE = 10  # exactly one child, the subtree whose doc set the predicate cache keeps; never scored
 MAX_PHRASE_TERMS, MAX_PREFIX_EXPANSIONS = 8, 1024
 MAX_PHRASE_LEN = 256  # TERM children of one NODE_PHRASE; above MAX_PHRASE_TERMS they run the long-phrase pre-pass
 MAX_SET_TERMS = 65536
@@ -39,6 +40,7 @@ KERNEL_HASHED_AGGS, KERNEL_HASHED_AGGS_RETRY, KERNEL_COMPOSITE_CUT = 256, 512, 1
 KERNEL_DEEP_SELECT = 2048
 KERNEL_TERM_SET = 4096
 KERNEL_PHRASE_LONG = 8192
+KERNEL_PREDICATE_FILL = 16384
 # hashed aggregation cells (qwgpu_format.h qw_agg_hashed, qwgpu.h): dense-layout limits, the initial capacity of a
 # split's table, the largest table a split may need, the `missing` flag of an entry
 AGG_DENSE_MAX_CELLS, AGG_DENSE_MAX_TERMS = 1 << 26, 1 << 24
@@ -206,6 +208,8 @@ def lib() -> C.CDLL:
     bind("qwgpu_split_register_async", [vp, cp, vp, u64])
     bind("qwgpu_split_wait", [vp, cp])
     bind("qwgpu_residency_info", [vp, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)])
+    bind("qwgpu_set_predicate_cache_budget", [vp, u64])
+    bind("qwgpu_predicate_cache_info", [vp] + [C.POINTER(u64)] * 7)
     bind("qwgpu_split_is_resident", [vp, cp])
     bind("qwgpu_leaf_search", [vp, vp, sz, C.POINTER(vp), C.POINTER(sz)])
     bind("qwgpu_invoke_leaf_search", [vp, vp, sz, C.POINTER(vp), C.POINTER(sz)])

@@ -132,6 +132,14 @@ def bool_(children: Sequence[Node], min_should_match: Optional[int] = None, occu
     return Node(ffi.NODE_BOOL, occur, children=children, min_should_match=min_should_match)
 
 
+def cache(node: Node, occur: Optional[int] = None) -> Node:
+    """A CACHE node over `node` (the reference's CacheNode): the same docs, read from the context's predicate cache when
+    it is enabled. Never scored. `occur` defaults to the node's own; the child takes MUST."""
+    child = Node(node.kind, ffi.OCCUR_MUST, node.boost, children=node.children, min_should_match=node.msm,
+                 term_ord=node.term_ord, field_id=node.field_id, weight=node.weight, column=node.column, lo=node.lo, hi=node.hi)
+    return Node(ffi.NODE_CACHE, node.occur if occur is None else occur, children=[child])
+
+
 def _flatten(root: Node) -> List[ffi.QwPlanNode]:
     out: List[ffi.QwPlanNode] = []
     queue: List[Tuple[Node, int]] = []

@@ -109,6 +109,16 @@ class SearcherContext:
         ffi.check(self._L.qwgpu_residency_info(self._ctx, *[C.byref(x) for x in v]))
         return dict(zip(("resident_bytes", "budget_bytes", "num_splits", "evictions"), (int(x.value) for x in v)))
 
+    def set_predicate_cache_budget(self, nbytes: int):
+        """Bytes of HBM the predicate cache may hold (0, the default, disables it and frees its entries)."""
+        ffi.check(self._L.qwgpu_set_predicate_cache_budget(self._ctx, nbytes))
+
+    def predicate_cache_info(self) -> dict:
+        v = [C.c_uint64() for _ in range(7)]
+        ffi.check(self._L.qwgpu_predicate_cache_info(self._ctx, *[C.byref(x) for x in v]))
+        names = ("budget_bytes", "used_bytes", "entries", "hits", "misses", "fills", "evictions")
+        return dict(zip(names, (int(x.value) for x in v)))
+
     # -- seam C -------------------------------------------------------------------------------------
     def split_search(self, split_ids: Sequence[str], plans: Sequence[bytes]) -> List[SplitSearchResult]:
         n = len(split_ids)
