@@ -1855,46 +1855,58 @@ struct SrcGathered {
 // Pruning before the merge: with m = ceil(K / #lists), every list holds min(m, len) hits that are at least as
 // good as its own m-th hit, so if those add up to K the K-th best hit overall is at least as good as the WORST of
 // the lists' m-th hits (tau) and only hits >= tau can reach the merged top-K. cut[s] = number of such hits in
-// list s (all of the list when the short lists leave fewer than K guaranteed hits). One block, warp = list.
+// list s (all of the list when the short lists leave fewer than K guaranteed hits). One block, warp = list. The
+// bounds are reduced per warp, then across the warps, so the block prunes at any list count.
 template <class Src>
 __global__ void __launch_bounds__(1024) k_merge_prep(const Src src, uint32_t n_lists, uint32_t K, uint32_t o1, uint32_t o2, uint32_t* cut) {
-  __shared__ MKey s_key[64];
-  __shared__ MKey s_keyK[64];
-  __shared__ uint32_t s_have[64], s_full[64];
+  __shared__ MKey w_key[32];   // per warp: the worst m-th hit of its lists
+  __shared__ MKey w_keyK[32];  // per warp: the best K-th hit of its lists that hold K hits
+  __shared__ uint32_t w_have[32], w_any[32], w_full[32];
   __shared__ MKey s_tau;
   __shared__ uint32_t s_prune;
   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  if (n_lists > 64) {  // more lists than the shared tables hold: no pruning
-    for (uint32_t s = threadIdx.x; s < n_lists; s += blockDim.x) cut[s] = min(src.count(s), K);
-    return;
-  }
   uint32_t nonempty = 0;
   for (uint32_t s = lane; s < n_lists; s += 32) nonempty += src.count(s) ? 1u : 0u;  // (one round of loads per warp)
   nonempty = __reduce_add_sync(0xFFFFFFFFu, nonempty);
   const uint32_t m = nonempty ? (K + nonempty - 1) / nonempty : 0;
-  for (uint32_t s = warp; s < n_lists; s += nw) {
-    if (lane == 0) {
+  if (lane == 0) {
+    uint64_t have = 0;
+    uint32_t any = 0, full = 0;
+    MKey key{}, keyK{};
+    for (uint32_t s = warp; s < n_lists; s += nw) {
       const uint32_t nh = min(src.count(s), K), ms = min(m, nh);
-      s_have[s] = ms;
-      if (ms) { uint32_t rk; const QwHit h = src.hit(s, ms - 1, rk); s_key[s] = merge_key(h, rk, o1, o2); }
+      have += ms;
+      if (ms) {
+        uint32_t rk;
+        const MKey k = merge_key(src.hit(s, ms - 1, rk), rk, o1, o2);
+        if (!any || mkey_gt(key, k)) key = k;
+        any = 1;
+      }
       // a list that holds K hits by itself: its own K-th hit bounds the merged K-th hit as well (the bound that
       // bites when the lists are skewed — time-sorted hits of time-partitioned splits all come from one split)
-      s_full[s] = (K > 0 && nh >= K) ? 1u : 0u;
-      if (s_full[s]) { uint32_t rk; const QwHit h = src.hit(s, K - 1, rk); s_keyK[s] = merge_key(h, rk, o1, o2); }
+      if (K > 0 && nh >= K) {
+        uint32_t rk;
+        const MKey k = merge_key(src.hit(s, K - 1, rk), rk, o1, o2);
+        if (!full || mkey_gt(k, keyK)) keyK = k;
+        full = 1;
+      }
     }
+    w_have[warp] = have < 0xFFFFFFFFull ? (uint32_t)have : 0xFFFFFFFFu;
+    w_any[warp] = any; w_full[warp] = full;
+    w_key[warp] = key; w_keyK[warp] = keyK;
   }
   __syncthreads();
   if (threadIdx.x == 0) {
-    uint32_t have = 0, first = 1;
-    MKey tau;
-    tau.v1 = tau.v2 = tau.tie = 0; tau.has = 0;
-    for (uint32_t s = 0; s < n_lists; s++) {
-      have += s_have[s];
-      if (s_have[s] && (first || mkey_gt(tau, s_key[s]))) { tau = s_key[s]; first = 0; }
+    uint64_t have = 0;
+    uint32_t first = 1;
+    MKey tau{};
+    for (uint32_t w = 0; w < nw; w++) {
+      have += w_have[w];
+      if (w_any[w] && (first || mkey_gt(tau, w_key[w]))) { tau = w_key[w]; first = 0; }
     }
     uint32_t prune = have >= K ? 1u : 0u;
-    for (uint32_t s = 0; s < n_lists; s++)
-      if (s_full[s] && (!prune || mkey_gt(s_keyK[s], tau))) { tau = s_keyK[s]; prune = 1; }  // the tighter of the valid bounds
+    for (uint32_t w = 0; w < nw; w++)
+      if (w_full[w] && (!prune || mkey_gt(w_keyK[w], tau))) { tau = w_keyK[w]; prune = 1; }  // the tighter of the valid bounds
     s_tau = tau;
     s_prune = prune;
   }
@@ -1926,14 +1938,16 @@ __global__ void __launch_bounds__(1024) k_merge_prep(const Src src, uint32_t n_l
 template <class Src>
 __global__ void __launch_bounds__(256) k_merge(const Src src, const uint32_t* cut, uint32_t n_lists, uint32_t kmax, uint32_t K, uint32_t o1, uint32_t o2,
                                                DMergedHit* out, uint32_t* out_n) {
-  // one warp per surviving hit; lane = one of the other lists (the binary searches of a hit run side by side)
-  const uint32_t lane = threadIdx.x & 31, e = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  // one warp per surviving hit; lane = one of the other lists (the binary searches of a hit run side by side). The
+  // warp index is 64-bit: n_lists * kmax warps pass 2^27 (6 711 lists at K = 20 000) before the lists run out.
+  const uint32_t lane = threadIdx.x & 31;
+  const uint64_t e = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   if (e == 0 && lane == 0) {
     uint64_t total = 0;
     for (uint32_t s = 0; s < n_lists; s++) total += src.count(s);
     *out_n = (uint32_t)(total < K ? total : K);
   }
-  const uint32_t s = e / kmax, i = e % kmax;
+  const uint32_t s = (uint32_t)(e / kmax), i = (uint32_t)(e % kmax);
   if (s >= n_lists || i >= __ldg(cut + s)) return;
   uint32_t my_rk;
   const QwHit mine = src.hit(s, i, my_rk);
