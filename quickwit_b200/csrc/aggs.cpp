@@ -785,24 +785,7 @@ static std::vector<IAgg> de_top(const std::string& s) {
   return de_aggs(r);
 }
 
-// ---- build from dense cells ----------------------------------------------------------------------------
-struct BuildCtx {
-  const CompiledPlan& cp;
-  const ImageView& img;
-  const QwAggNode* nodes;
-  const QwAggCell* cells;
-  std::vector<uint32_t> bases;
-};
-
-static IAgg build_node(const BuildCtx& c, uint32_t ni, uint64_t parent_cell);
-
-static std::vector<IAgg> build_children(const BuildCtx& c, uint32_t ni, uint64_t cell) {
-  std::vector<IAgg> out;
-  const QwAggNode& n = c.nodes[ni];
-  for (uint32_t k = 0; k < n.num_children; k++) out.push_back(build_node(c, n.first_child + k, cell));
-  return out;
-}
-
+// ---- build a split's tree ------------------------------------------------------------------------------
 static IKey term_key(const ImageView& img, const AggBinding& b, uint64_t raw, bool missing) {
   IKey k;
   if (missing) {
@@ -836,18 +819,23 @@ static double metric_of(const IAgg& a, const std::string& prop) {
   return (double)a.m_count;
 }
 
-// sorts term buckets in the requested order (ties: key ascending, for determinism)
-static void sort_term_buckets(const AggReq& req, std::vector<IBucket>& bs) {
-  if (req.order_target == "_key") {
-    std::sort(bs.begin(), bs.end(), [&](const IBucket& a, const IBucket& b) { return req.order_desc ? b.key < a.key : a.key < b.key; });
-    return;
-  }
+// the requested order of term buckets (ties: key ascending, for determinism) as a permutation of their indices:
+// std::sort makes the same comparisons on indices as on the buckets themselves, so the order is the same, and no
+// (large) bucket moves
+static std::vector<uint32_t> term_order(const AggReq& req, const std::vector<IBucket>& bs) {
+  std::vector<uint32_t> perm(bs.size());
+  for (size_t i = 0; i < perm.size(); i++) perm[i] = (uint32_t)i;
+  auto sort_by = [&](auto less) {
+    std::sort(perm.begin(), perm.end(), [&](uint32_t x, uint32_t y) { return less(bs[x], bs[y]); });
+    return perm;
+  };
+  if (req.order_target == "_key")
+    return sort_by([&](const IBucket& a, const IBucket& b) { return req.order_desc ? b.key < a.key : a.key < b.key; });
   if (req.order_target == "_count") {
-    std::sort(bs.begin(), bs.end(), [&](const IBucket& a, const IBucket& b) {
+    return sort_by([&](const IBucket& a, const IBucket& b) {
       if (a.count != b.count) return req.order_desc ? a.count > b.count : a.count < b.count;
       return a.key < b.key;
     });
-    return;
   }
   std::string name = req.order_target, prop;
   size_t dot = name.find('.');
@@ -857,7 +845,7 @@ static void sort_term_buckets(const AggReq& req, std::vector<IBucket>& bs) {
   if (ci < 0) fail(QWGPU_EINVALID_AGG, "could not find aggregation with name `%s` in metric sub_aggregations", name.c_str());
   if (req.children[ci].kind == AggReq::Percentiles)
     fail(QWGPU_EUNSUPPORTED, "ordering terms by the percentiles aggregation `%s` is not implemented on the GPU path", name.c_str());
-  std::sort(bs.begin(), bs.end(), [&](const IBucket& a, const IBucket& b) {
+  return sort_by([&](const IBucket& a, const IBucket& b) {
     double x = metric_of(a.subs[ci], prop), y = metric_of(b.subs[ci], prop);
     if (x != y) return req.order_desc ? x > y : x < y;
     return a.key < b.key;
@@ -892,12 +880,16 @@ static IAgg metric_from_cell(const CompiledPlan& cp, const ImageView& img, const
 static void cut_terms(const AggReq& req, IAgg& a) {
   if (req.kind == AggReq::Terms && req.order_target.find('.') == std::string::npos &&
       (req.order_target == "_count" || req.order_target == "_key")) {
-    sort_term_buckets(req, a.buckets);
-    if (a.buckets.size() > req.segment_size) {
-      if (req.order_target == "_count" && req.order_desc) a.error_bound = a.buckets[req.segment_size].count;
-      for (size_t i = req.segment_size; i < a.buckets.size(); i++) a.sum_other += a.buckets[i].count;
-      a.buckets.resize(req.segment_size);
+    const std::vector<uint32_t> order = term_order(req, a.buckets);
+    const size_t keep = std::min<size_t>(order.size(), req.segment_size);
+    if (order.size() > keep && req.order_target == "_count" && req.order_desc) a.error_bound = a.buckets[order[keep]].count;
+    std::vector<IBucket> kept;
+    kept.reserve(keep);
+    for (size_t i = 0; i < order.size(); i++) {
+      if (i < keep) kept.push_back(std::move(a.buckets[order[i]]));
+      else a.sum_other += a.buckets[order[i]].count;
     }
+    a.buckets.swap(kept);
   }
 }
 
@@ -925,44 +917,56 @@ static void comp_sort_cut(const AggReq& req, IAgg& a) {
   if (a.buckets.size() > req.size) a.buckets.resize(req.size);
 }
 
-static IAgg build_node(const BuildCtx& c, uint32_t ni, uint64_t parent_cell) {
-  const QwAggNode& n = c.nodes[ni];
-  const AggBinding& b = c.cp.agg_bindings[ni];
-  const AggReq& req = *b.req;
-  if (req.kind == AggReq::Composite) fail(QWGPU_EINVALID_ARG, "composite aggregation results are given as entries");
-  if (req.kind == AggReq::Percentiles) fail(QWGPU_EINVALID_ARG, "percentiles aggregation results are given as entries");
-  const QwAggCell* base = c.cells + c.bases[ni];
-  if (req.is_metric()) return metric_from_cell(c.cp, c.img, c.nodes, ni, base[parent_cell]);
-  IAgg a;
-  a.kind = (uint8_t)req.kind;
-  a.is_date = req.kind == AggReq::DateHistogram;
-  for (uint32_t k = 0; k < n.num_buckets; k++) {
-    uint64_t cell = parent_cell * n.num_buckets + k;
-    uint64_t cnt = base[cell].count;
-    if (cnt == 0 && req.kind != AggReq::Range) continue;
-    IBucket bk;
-    bk.count = cnt;
-    if (req.kind == AggReq::Terms) bk.key = term_key(c.img, b, k, n.has_missing && k == n.num_buckets - 1);
-    else if (req.kind == AggReq::Range) bk.hkey = (double)k;
-    else bk.hkey = (double)(n.base_pos + (int64_t)k) * n.interval + n.offset;
-    bk.subs = build_children(c, ni, cell);
-    a.buckets.push_back(std::move(bk));
-  }
-  cut_terms(req, a);
-  return a;
+// ---- build from entries (QwAggEntry) ------------------------------------------------------------------------
+// A split's IAgg tree is built from entries whichever layout its result came in (dense cells become the entries of
+// their nonzero cells): buckets in dense order (terms by raw key with `missing` last, histograms by position, every
+// range in request order, empty ones included).
+static const QwAggNode* plan_agg_nodes(const CompiledPlan& cp) {
+  return (const QwAggNode*)(cp.bytes.data() + sizeof(QwPlanHeader) + (size_t)cp.header.num_nodes * sizeof(QwPlanNode));
 }
 
-// ---- build from hashed entries (QwAggEntry) --------------------------------------------------------------------
-// The same IAgg tree as build_node gives for the equivalent dense cells: buckets in dense order (terms by raw key
-// with `missing` last, histograms by position, every range in request order, empty ones included).
 struct EntryCtx {
   const CompiledPlan& cp;
   const ImageView& img;
   const QwAggNode* nodes;
   const QwAggEntry* entries;
-  std::map<std::pair<uint32_t, uint32_t>, std::vector<uint32_t>> kids;  // (parent entry, node) -> entries
+  // entries grouped by (parent entry, node), each group in entry order: group g is members[start[g] .. start[g + 1]).
+  // A top-level node's group is its node index; child node first_child + k of entry e's node has group first_group[e] + k.
+  std::vector<size_t> first_group, start;
+  std::vector<uint32_t> members;
 };
 static const uint32_t kNoEntry = 0xFFFFFFFEu;  // the parent of an empty range bucket: has no entries below it
+
+static size_t entry_group(const EntryCtx& c, uint32_t ni, uint32_t parent) {
+  return parent == QW_AGG_NO_PARENT ? ni : c.first_group[parent] + (ni - c.nodes[c.entries[parent].node].first_child);
+}
+struct EntryRange {
+  const uint32_t *b, *e;
+  const uint32_t* begin() const { return b; }
+  const uint32_t* end() const { return e; }
+  bool empty() const { return b == e; }
+};
+// the entries of node ni under parent entry `parent`
+static EntryRange kids(const EntryCtx& c, uint32_t ni, uint32_t parent) {
+  if (parent == kNoEntry) return {nullptr, nullptr};
+  const size_t g = entry_group(c, ni, parent);
+  return {c.members.data() + c.start[g], c.members.data() + c.start[g + 1]};
+}
+// groups the entries by a counting sort, linear in the entries; each parent must be an entry of its node's parent node
+static void index_entries(EntryCtx& c, size_t nentries) {
+  size_t groups = c.cp.header.num_aggs;
+  c.first_group.resize(nentries);
+  for (size_t e = 0; e < nentries; e++) {
+    c.first_group[e] = groups;
+    groups += c.nodes[c.entries[e].node].num_children;
+  }
+  // start[g] counts group g, then becomes its end, then (filled from the back) its begin
+  c.start.assign(groups + 1, 0);
+  for (size_t e = 0; e < nentries; e++) c.start[entry_group(c, c.entries[e].node, c.entries[e].parent)]++;
+  for (size_t g = 1; g <= groups; g++) c.start[g] += c.start[g - 1];
+  c.members.resize(nentries);
+  for (size_t e = nentries; e-- > 0;) c.members[--c.start[entry_group(c, c.entries[e].node, c.entries[e].parent)]] = (uint32_t)e;
+}
 
 static IAgg build_node_e(const EntryCtx& c, uint32_t ni, uint32_t parent);
 
@@ -993,10 +997,8 @@ static IAgg build_composite_e(const EntryCtx& c, uint32_t ni0, uint32_t parent0)
   a.kind = AggReq::Composite;
   std::vector<CompKey> path(req.sources.size());
   auto walk = [&](auto&& self, uint32_t ni, uint32_t parent, size_t level) -> void {
-    auto it = c.kids.find({parent, ni});
-    if (it == c.kids.end()) return;
     const QwAggNode& n = c.nodes[ni];
-    for (uint32_t e : it->second) {
+    for (uint32_t e : kids(c, ni, parent)) {
       const QwAggEntry& x = c.entries[e];
       if (x.cell.count == 0) continue;
       path[level] = comp_entry_key(c, ni, x);
@@ -1016,7 +1018,7 @@ static IAgg build_composite_e(const EntryCtx& c, uint32_t ni0, uint32_t parent0)
 // a percentiles node's entries under one parent bucket as a sketch in value space: table indices become bin ordinals
 // through the split's table for the column (tables differ per split, the ordinals do not); the `missing` entry counts
 // the missing value
-static IAgg build_percentiles_e(const EntryCtx& c, uint32_t ni, const std::vector<uint32_t>& es) {
+static IAgg build_percentiles_e(const EntryCtx& c, uint32_t ni, EntryRange es) {
   const AggBinding& b = c.cp.agg_bindings[ni];
   IAgg a;
   a.kind = AggReq::Percentiles;
@@ -1040,13 +1042,11 @@ static IAgg build_node_e(const EntryCtx& c, uint32_t ni, uint32_t parent) {
   const AggBinding& b = c.cp.agg_bindings[ni];
   const AggReq& req = *b.req;
   if (req.kind == AggReq::Composite) return build_composite_e(c, ni, parent);
-  static const std::vector<uint32_t> none;
-  auto it = c.kids.find({parent, ni});
-  const std::vector<uint32_t>& es = it == c.kids.end() ? none : it->second;
+  const EntryRange es = kids(c, ni, parent);
   if (req.kind == AggReq::Percentiles) return build_percentiles_e(c, ni, es);
   if (req.is_metric()) {
     QwAggCell empty = {0, 0, ~0ull, 0};
-    return metric_from_cell(c.cp, c.img, c.nodes, ni, es.empty() ? empty : c.entries[es[0]].cell);
+    return metric_from_cell(c.cp, c.img, c.nodes, ni, es.empty() ? empty : c.entries[*es.begin()].cell);
   }
   auto subs = [&](uint32_t e) {
     std::vector<IAgg> out;
@@ -1068,12 +1068,14 @@ static IAgg build_node_e(const EntryCtx& c, uint32_t ni, uint32_t parent) {
     }
     return a;
   }
-  std::vector<uint32_t> order(es);
-  std::sort(order.begin(), order.end(), [&](uint32_t x, uint32_t y) {
+  std::vector<uint32_t> order(es.begin(), es.end());
+  auto before = [&](uint32_t x, uint32_t y) {
     const QwAggEntry &p = c.entries[x], &q = c.entries[y];
     const bool pm = p.flags & QW_AGG_ENTRY_MISSING, qm = q.flags & QW_AGG_ENTRY_MISSING;
     return pm != qm ? qm : p.key < q.key;
-  });
+  };
+  if (!std::is_sorted(order.begin(), order.end(), before)) std::sort(order.begin(), order.end(), before);
+  a.buckets.reserve(order.size());
   for (uint32_t e : order) {
     const QwAggEntry& x = c.entries[e];
     if (x.cell.count == 0) continue;
@@ -1088,11 +1090,18 @@ static IAgg build_node_e(const EntryCtx& c, uint32_t ni, uint32_t parent) {
   return a;
 }
 
+static std::vector<IAgg> build_tree(const CompiledPlan& cp, const ImageView& img, const QwAggEntry* entries, size_t nentries) {
+  EntryCtx c{cp, img, plan_agg_nodes(cp), entries, {}, {}, {}};
+  index_entries(c, nentries);
+  std::vector<IAgg> top;
+  for (uint32_t i = 0; i < cp.header.num_aggs; i++) if (c.nodes[i].parent == 0xFFFFFFFFu) top.push_back(build_node_e(c, i, QW_AGG_NO_PARENT));
+  return top;
+}
+
+// entries that come from outside the program: every one must name a bucket of its node's key space, once, under its parent
 static std::vector<IAgg> build_top_entries(const CompiledPlan& cp, const ImageView& img, const QwAggEntry* entries, size_t nentries) {
   const QwPlanHeader& h = cp.header;
-  const QwAggNode* nodes = (const QwAggNode*)(cp.bytes.data() + sizeof(QwPlanHeader) + (size_t)h.num_nodes * sizeof(QwPlanNode));
-  EntryCtx c{cp, img, nodes, entries, {}};
-  // entries come from the caller: every one must name a bucket of its node's key space, once, under its parent
+  const QwAggNode* nodes = plan_agg_nodes(cp);
   std::set<std::tuple<uint32_t, uint32_t, uint64_t, uint32_t>> seen;
   for (size_t e = 0; e < nentries; e++) {
     const QwAggEntry& x = entries[e];
@@ -1121,11 +1130,56 @@ static std::vector<IAgg> build_top_entries(const CompiledPlan& cp, const ImageVi
     if (!ok) fail(QWGPU_EINVALID_ARG, "aggregation entry %zu: key %llu (flags %u) is not a bucket of node %u", e, (unsigned long long)x.key, x.flags, x.node);
     if (!seen.insert(std::make_tuple(x.parent, x.node, x.key, x.flags)).second)
       fail(QWGPU_EINVALID_ARG, "aggregation entry %zu repeats a bucket of node %u under the same parent", e, x.node);
-    c.kids[{x.parent, x.node}].push_back((uint32_t)e);
   }
-  std::vector<IAgg> top;
-  for (uint32_t i = 0; i < h.num_aggs; i++) if (nodes[i].parent == 0xFFFFFFFFu) top.push_back(build_node_e(c, i, QW_AGG_NO_PARENT));
-  return top;
+  return build_tree(cp, img, entries, nentries);
+}
+
+uint64_t agg_cell_layout(const QwAggNode* aggs, uint32_t n, std::vector<uint32_t>* bases) {
+  uint64_t total = 0;
+  if (bases) bases->resize(n);
+  for (uint32_t i = 0; i < n; i++) {
+    uint64_t cells = aggs[i].kind == QW_AGG_STATS ? 1 : aggs[i].num_buckets;
+    uint32_t p = aggs[i].parent;
+    while (p != 0xFFFFFFFFu) { cells *= aggs[p].num_buckets; p = aggs[p].parent; }
+    if (bases) (*bases)[i] = (uint32_t)total;
+    total += cells;
+    if (total > QW_AGG_DENSE_MAX_CELLS) fail(QWGPU_EINVALID_AGG, "aggregation bucket space too large (%llu cells)", (unsigned long long)total);
+  }
+  return total;
+}
+
+// The entries of a dense cell array (QwAggCell doc in qwgpu_format.h), parents before children: one per nonzero cell,
+// keyed by its bucket index within the node (a node's `missing` bucket, its last, as QW_AGG_ENTRY_MISSING with key 0;
+// a metric cell with key 0). Zero cells give none: the builder puts back every empty range bucket and metric.
+static std::vector<QwAggEntry> dense_entries(const CompiledPlan& cp, const QwAggCell* cells, size_t ncells) {
+  const QwAggNode* nodes = plan_agg_nodes(cp);
+  std::vector<uint32_t> bases;
+  const uint64_t total = agg_cell_layout(nodes, cp.header.num_aggs, &bases);
+  if (total != ncells) fail(QWGPU_EINTERNAL, "aggregation cell count mismatch (%llu vs %zu)", (unsigned long long)total, ncells);
+  std::vector<QwAggEntry> out;
+  out.reserve(std::min<size_t>(ncells, 4096));  // (larger results grow)
+  auto walk = [&](auto&& self, uint32_t ni, uint32_t parent, uint64_t parent_cell) -> void {
+    const AggReq::Kind kind = cp.agg_bindings[ni].req->kind;
+    if (kind == AggReq::Composite || kind == AggReq::Percentiles) fail(QWGPU_EINVALID_ARG, "composite and percentiles aggregation results are given as entries");
+    const QwAggNode& n = nodes[ni];
+    const uint32_t nb = n.kind == QW_AGG_STATS ? 1 : n.num_buckets;
+    const QwAggCell* base = cells + bases[ni];
+    for (uint32_t k = 0; k < nb; k++) {
+      const uint64_t cell = parent_cell * nb + k;
+      if (!base[cell].count) continue;
+      const bool missing = n.has_missing && k == nb - 1;
+      out.push_back({ni, parent, missing ? 0 : k, missing ? (uint32_t)QW_AGG_ENTRY_MISSING : 0u, 0, base[cell]});
+      const uint32_t e = (uint32_t)out.size() - 1;
+      for (uint32_t j = 0; j < n.num_children; j++) self(self, n.first_child + j, e, cell);
+    }
+  };
+  for (uint32_t i = 0; i < cp.header.num_aggs; i++) if (nodes[i].parent == 0xFFFFFFFFu) walk(walk, i, QW_AGG_NO_PARENT, 0);
+  return out;
+}
+
+static std::vector<IAgg> build_top_cells(const CompiledPlan& cp, const ImageView& img, const QwAggCell* cells, size_t ncells) {
+  const std::vector<QwAggEntry> entries = dense_entries(cp, cells, ncells);
+  return build_tree(cp, img, entries.data(), entries.size());
 }
 
 std::string build_intermediate_aggs_entries(const CompiledPlan& cp, const ImageView& img, const QwAggEntry* entries, size_t nentries) {
@@ -1207,8 +1261,7 @@ std::vector<TraceSpan> merge_span_fruits(std::vector<std::vector<TraceSpan>> fru
 
 // the split's spans from the N cells of its QW_AGG_TRACE_IDS node (QwAggNode doc), sorted
 static std::vector<TraceSpan> trace_spans_of(const CompiledPlan& cp, const ImageView& img, const QwAggCell* cells, size_t ncells) {
-  const QwAggNode* nodes = (const QwAggNode*)(cp.bytes.data() + sizeof(QwPlanHeader) + (size_t)cp.header.num_nodes * sizeof(QwPlanNode));
-  const QwAggNode& n = nodes[0];
+  const QwAggNode& n = plan_agg_nodes(cp)[0];
   if (ncells != n.num_buckets) fail(QWGPU_EINTERNAL, "aggregation cell count mismatch (%u vs %zu)", n.num_buckets, ncells);
   std::vector<TraceSpan> v;
   for (size_t j = 0; j < ncells; j++) {
@@ -1229,29 +1282,10 @@ static std::vector<TraceSpan> trace_spans_of(const CompiledPlan& cp, const Image
   return v;
 }
 
-static std::vector<IAgg> build_top(const CompiledPlan& cp, const ImageView& img, const QwAggCell* cells, size_t ncells);
 std::string build_intermediate_aggs(const CompiledPlan& cp, const ImageView& img, const QwAggCell* cells, size_t ncells) {
   // (a single split's spans go out sorted: the reference leaves them in select_nth_unstable order)
   if (is_trace_ids_request(cp.agg_request)) return encode_spans(trace_spans_of(cp, img, cells, ncells));
-  return ser_top(build_top(cp, img, cells, ncells));
-}
-static std::vector<IAgg> build_top(const CompiledPlan& cp, const ImageView& img, const QwAggCell* cells, size_t ncells) {
-  const QwPlanHeader& h = cp.header;
-  const QwAggNode* nodes = (const QwAggNode*)(cp.bytes.data() + sizeof(QwPlanHeader) + (size_t)h.num_nodes * sizeof(QwPlanNode));
-  BuildCtx c{cp, img, nodes, cells, {}};
-  uint64_t total = 0;
-  c.bases.resize(h.num_aggs);
-  for (uint32_t i = 0; i < h.num_aggs; i++) {
-    uint64_t cnt = nodes[i].kind == QW_AGG_STATS ? 1 : nodes[i].num_buckets;
-    uint32_t p = nodes[i].parent;
-    while (p != 0xFFFFFFFFu) { cnt *= nodes[p].num_buckets; p = nodes[p].parent; }
-    c.bases[i] = (uint32_t)total;
-    total += cnt;
-  }
-  if (total != ncells) fail(QWGPU_EINTERNAL, "aggregation cell count mismatch (%llu vs %zu)", (unsigned long long)total, ncells);
-  std::vector<IAgg> top;
-  for (uint32_t i = 0; i < h.num_aggs; i++) if (nodes[i].parent == 0xFFFFFFFFu) top.push_back(build_node(c, i, 0));
-  return top;
+  return ser_top(build_top_cells(cp, img, cells, ncells));
 }
 
 // ---- merge ------------------------------------------------------------------------------------------------
@@ -1309,7 +1343,7 @@ static void merge_into(const AggReq& req, IAgg& acc, IAgg&& other) {
   }
 }
 
-// Leaf-level merge of the splits of one request straight from their dense cells: what
+// Leaf-level merge of the splits of one request straight from their cells or entries: what
 // merge_intermediate_aggs(build_intermediate_aggs(split) ...) yields, without serialising every split's
 // result only to parse it again.
 std::string build_and_merge_intermediate_aggs(const std::vector<AggReq>& reqs, const std::vector<SplitAggCells>& splits) {
@@ -1320,7 +1354,7 @@ std::string build_and_merge_intermediate_aggs(const std::vector<AggReq>& reqs, c
   }
   std::vector<IAgg> acc;
   for (const SplitAggCells& sp : splits) {
-    std::vector<IAgg> top = sp.hashed ? build_top_entries(*sp.plan, *sp.img, sp.entries, sp.nentries) : build_top(*sp.plan, *sp.img, sp.cells, sp.ncells);
+    std::vector<IAgg> top = sp.hashed ? build_top_entries(*sp.plan, *sp.img, sp.entries, sp.nentries) : build_top_cells(*sp.plan, *sp.img, sp.cells, sp.ncells);
     if (acc.empty() && !top.empty()) {
       // same normalisation as a serialise / parse round trip would apply: none needed — the first
       // split's tree becomes the accumulator
@@ -1529,11 +1563,10 @@ static void fin_agg(const AggReq& req, const IAgg* a, std::string& out) {
     return;
   }
   if (req.kind == AggReq::Terms) {
-    std::vector<IBucket> bs = a->buckets;
-    sort_term_buckets(req, bs);
     uint64_t sum_other = a->sum_other;
     std::vector<const IBucket*> kept;
-    for (auto& b : bs) {
+    for (uint32_t i : term_order(req, a->buckets)) {
+      const IBucket& b = a->buckets[i];
       if (b.count < req.min_doc_count) continue;
       if (kept.size() < req.size) kept.push_back(&b);
       else sum_other += b.count;

@@ -52,6 +52,11 @@ inline float bm25_idf(uint64_t doc_freq, uint64_t doc_count) {
   return logf(1.0f + x);
 }
 
+// ---- dense aggregation layout (QwAggCell doc in qwgpu_format.h) ---------------------------------
+// Total cells of the plan's aggregation nodes and each node's first cell; fails above QW_AGG_DENSE_MAX_CELLS.
+// Defined in aggs.cpp: the engine lays out its cells and the host reads them back with the same bases.
+uint64_t agg_cell_layout(const QwAggNode* aggs, uint32_t n, std::vector<uint32_t>* bases);
+
 // ---- read-only view over a split image -------------------------------------------------------
 struct ImageView {
   const uint8_t* base = nullptr;

@@ -420,20 +420,6 @@ std::shared_ptr<SplitDev> Engine::find(const std::string& id) {
   return sp;
 }
 
-uint64_t agg_cell_layout(const QwAggNode* aggs, uint32_t n, std::vector<uint32_t>* bases) {
-  uint64_t total = 0;
-  if (bases) bases->resize(n);
-  for (uint32_t i = 0; i < n; i++) {
-    uint64_t cells = aggs[i].kind == QW_AGG_STATS ? 1 : aggs[i].num_buckets;
-    uint32_t p = aggs[i].parent;
-    while (p != 0xFFFFFFFFu) { cells *= aggs[p].num_buckets; p = aggs[p].parent; }
-    if (bases) (*bases)[i] = (uint32_t)total;
-    total += cells;
-    if (total > QW_AGG_DENSE_MAX_CELLS) fail(QWGPU_EINVALID_AGG, "aggregation bucket space too large (%llu cells)", (unsigned long long)total);
-  }
-  return total;
-}
-
 // Hashed layout: a cell exists per (node, parent cell, key) that some (doc, value path) reaches, so a node has at
 // most min(its dense cells, the (doc, value path) tuples of its bucket chain) cells. A chain of single-valued
 // columns gives at most one path per doc; a multi-valued level multiplies by that column's value count (Σ_d Π v_l(d)

@@ -167,8 +167,6 @@ struct Engine {
               const GatherSpec* gather = nullptr, std::vector<RankHeader>* rank_headers = nullptr);
 };
 
-// plan validation helper shared with the compiler: total agg cells + per-node bases
-uint64_t agg_cell_layout(const QwAggNode* aggs, uint32_t n, std::vector<uint32_t>* bases);
 // hashed layout: guaranteed upper bound on a split's distinct cells, and the device bytes of a table of `cap`
 // cells; agg_hashed_layout fails with QWGPU_EUNSUPPORTED when the table at the bound exceeds QWGPU_HASHED_MAX_BYTES
 uint64_t agg_hashed_bound(const QwAggNode* aggs, uint32_t n, const ImageView& img);

@@ -197,6 +197,7 @@ struct SplitJob {
 struct LeafRun {
   std::vector<SplitJob> jobs;
   std::vector<size_t> which;      // jobs[which[k]] <-> outs[k]
+  std::vector<uint32_t> id_rank;  // indexed like `jobs`: a searched split's rank by split id (breaks sort value ties)
   std::vector<SplitOutput> outs;
   BatchStats st;
   uint64_t wall_us = 0;
@@ -216,7 +217,30 @@ static bool same_sort_types(const std::vector<SplitJob>& jobs, const std::vector
   }
   return true;
 }
-static void sort_orders(const pb::SearchRequest& r, int* o1, int* o2);
+
+// The sort kinds of the splits `which` (same_sort_types holds) and each key's sort-field type, taken from the first
+// split that has the column (splits without it only produce None values)
+struct SortTypes {
+  uint32_t kind[2];
+  int sft[2];
+};
+static SortTypes sort_types(const std::vector<SplitJob>& jobs, const std::vector<size_t>& which) {
+  const CompiledPlan& p0 = jobs[which[0]].plan;
+  SortTypes t = {{p0.header.sort[0].kind, p0.header.sort[1].kind}, {p0.sort_field_type[0], p0.sort_field_type[1]}};
+  for (int i = 0; i < 2; i++)
+    for (size_t w : which) {
+      const CompiledPlan& p = jobs[w].plan;
+      if (p.header.sort[i].kind == QW_SORT_COLUMN && p.header.sort[i].column != 0xFFFFFFFFu) { t.sft[i] = p.sort_field_type[i]; break; }
+    }
+  return t;
+}
+// A device-format hit of split `split_id` as a wire-form PartialHit (build_split_response's conversion)
+static void append_hit(std::string& out, const std::string& split_id, const QwHit& h, const SortTypes& t) {
+  pb::SortValue sv1, sv2;
+  if (h.flags & 1) sv1 = typed_sort_value(t.kind[0], t.sft[0], h.v1);
+  if (h.flags & 2) sv2 = typed_sort_value(t.kind[1], t.sft[1], h.v2);
+  pb::append_partial_hit(out, 2, split_id, 0, h.doc_id, (h.flags & 1) != 0, sv1, (h.flags & 2) != 0, sv2);
+}
 
 // ---- pre-search pruning (SURVEY.md 8a row a16) ---------------------------------------------------------------
 // CanSplitDoBetter::{from_request, optimize_split_order, optimize} (leaf.rs:1072-1242), is_simple_all_query
@@ -400,6 +424,10 @@ static void run_leaf_raw(Engine& eng, const pb::LeafSearchRequest& lr, LeafRun& 
       lens.push_back(run.jobs[i].plan.bytes.size());
       run.which.push_back(i);
     }
+  std::vector<size_t> by_id(run.which);
+  std::sort(by_id.begin(), by_id.end(), [&](size_t a, size_t b) { return run.jobs[a].meta.split_id < run.jobs[b].meta.split_id; });
+  run.id_rank.assign(run.jobs.size(), 0);
+  for (size_t r = 0; r < by_id.size(); r++) run.id_rank[by_id[r]] = (uint32_t)r;
   auto t0 = clock::now();
   if (getenv("QWGPU_TRACE"))
     fprintf(stderr, "[qwgpu] compile: %ld us for %zu splits\n", (long)std::chrono::duration_cast<std::chrono::microseconds>(t0 - t_compile).count(), run.jobs.size());
@@ -413,11 +441,8 @@ static void run_leaf_raw(Engine& eng, const pb::LeafSearchRequest& lr, LeafRun& 
     ms.k = (uint32_t)(sreq.max_hits + sreq.start_offset);
     ms.order1 = (uint32_t)o1; ms.order2 = (uint32_t)o2;
     const size_t n = run.which.size();
-    std::vector<size_t> by_id(n);
-    for (size_t i = 0; i < n; i++) by_id[i] = i;
-    std::sort(by_id.begin(), by_id.end(), [&](size_t a, size_t b) { return run.jobs[run.which[a]].meta.split_id < run.jobs[run.which[b]].meta.split_id; });
     ms.rank.resize(n);
-    for (size_t r = 0; r < n; r++) ms.rank[by_id[r]] = (uint32_t)r;
+    for (size_t i = 0; i < n; i++) ms.rank[i] = run.id_rank[run.which[i]];
     if (gathering) {
       // tie-breaks across ranks use the split id order of the WHOLE query: ranks from the context's table
       for (size_t i = 0; i < n; i++) {
@@ -498,21 +523,7 @@ static pb::LeafSearchResponse leaf_merge_fast(const pb::SearchRequest& sreq, Lea
   int o1, o2;
   sort_orders(sreq, &o1, &o2);
   const size_t k = (size_t)(sreq.max_hits + sreq.start_offset);
-  // rank of every split id (tie-break uses the split id string order)
-  std::vector<size_t> by_id(n);
-  for (size_t i = 0; i < n; i++) by_id[i] = i;
-  std::sort(by_id.begin(), by_id.end(), [&](size_t a, size_t b) { return run.jobs[run.which[a]].meta.split_id < run.jobs[run.which[b]].meta.split_id; });
-  std::vector<uint32_t> rank(n);
-  for (size_t r = 0; r < n; r++) rank[by_id[r]] = (uint32_t)r;
-  const CompiledPlan& p0 = run.jobs[run.which[0]].plan;
-  // sort-field type of each key: taken from a split that actually has the column (splits without it
-  // only produce None values)
-  int sft[2] = {p0.sort_field_type[0], p0.sort_field_type[1]};
-  for (int i = 0; i < 2; i++)
-    for (size_t s2 = 0; s2 < n; s2++) {
-      const CompiledPlan& pp = run.jobs[run.which[s2]].plan;
-      if (pp.header.sort[i].kind == QW_SORT_COLUMN && pp.header.sort[i].column != 0xFFFFFFFFu) { sft[i] = pp.sort_field_type[i]; break; }
-    }
+  const SortTypes types = sort_types(run.jobs, run.which);
   // Heads of the per-split lists as plain integer tuples, greater = better: (has1, v1', has2, v2', tie')
   // with v' = v for a descending key and ~v for an ascending one (None — has = 0 — is last in both
   // directions, compare_opt in quickwit-proto/src/lib.rs:122-140), tie' = (split rank, doc id) in the
@@ -530,7 +541,7 @@ static pb::LeafSearchResponse leaf_merge_fast(const pb::SearchRequest& sreq, Lea
     k.has2 = (h.flags >> 1) & 1;
     k.v1 = k.has1 ? (o1 == QW_ORDER_DESC ? h.v1 : ~h.v1) : 0;
     k.v2 = k.has2 ? (o2 == QW_ORDER_DESC ? h.v2 : ~h.v2) : 0;
-    const uint64_t t = ((uint64_t)rank[sidx] << 32) | h.doc_id;
+    const uint64_t t = ((uint64_t)run.id_rank[run.which[sidx]] << 32) | h.doc_id;
     k.tie = o1 == QW_ORDER_DESC ? t : ~t;
     return k;
   };
@@ -559,11 +570,7 @@ static pb::LeafSearchResponse leaf_merge_fast(const pb::SearchRequest& sreq, Lea
     // the engine already merged on the device (k_merge): same total order, hits arrive best-first
     for (const MergedHit& mh : run.merged) {
       if (taken >= k) break;
-      const QwHit& h = mh.hit;
-      pb::SortValue sv1, sv2;
-      if (h.flags & 1) sv1 = typed_sort_value(p0.header.sort[0].kind, sft[0], h.v1);
-      if (h.flags & 2) sv2 = typed_sort_value(p0.header.sort[1].kind, sft[1], h.v2);
-      pb::append_partial_hit(m.encoded_partial_hits, 2, run.jobs[mh.split].meta.split_id, 0, h.doc_id, (h.flags & 1) != 0, sv1, (h.flags & 2) != 0, sv2);
+      append_hit(m.encoded_partial_hits, run.jobs[mh.split].meta.split_id, mh.hit, types);
       taken++;
     }
     heap.clear();
@@ -571,18 +578,13 @@ static pb::LeafSearchResponse leaf_merge_fast(const pb::SearchRequest& sreq, Lea
   while (!heap.empty() && taken < k) {
     std::pop_heap(heap.begin(), heap.end());
     size_t s = heap.back().s;
-    const SplitJob& j = run.jobs[run.which[s]];
-    const QwHit& h = run.outs[s].hits[pos[s]];
-    pb::SortValue sv1, sv2;
-    if (h.flags & 1) sv1 = typed_sort_value(p0.header.sort[0].kind, sft[0], h.v1);
-    if (h.flags & 2) sv2 = typed_sort_value(p0.header.sort[1].kind, sft[1], h.v2);
-    pb::append_partial_hit(m.encoded_partial_hits, 2, j.meta.split_id, 0, h.doc_id, (h.flags & 1) != 0, sv1, (h.flags & 2) != 0, sv2);
+    append_hit(m.encoded_partial_hits, run.jobs[run.which[s]].meta.split_id, run.outs[s].hits[pos[s]], types);
     taken++;
     if (++pos[s] < run.outs[s].hits.size()) { heap.back() = head_of(s, run.outs[s].hits[pos[s]]); std::push_heap(heap.begin(), heap.end()); }
     else heap.pop_back();
   }
   if (sreq.aggregation_request && !sreq.aggregation_request->empty())
-    m.intermediate_aggregation_result = build_and_merge_intermediate_aggs(p0.agg_request, agg_parts);
+    m.intermediate_aggregation_result = build_and_merge_intermediate_aggs(run.jobs[run.which[0]].plan.agg_request, agg_parts);
   if (any_stats) m.resource_stats = stats_acc;
   return m;
 }
@@ -612,6 +614,15 @@ static qw::Engine& engine_of(qwgpu_ctx* ctx) {
   if (!ctx) qw::fail(QWGPU_EINVALID_ARG, "null context");
   if (!ctx->engine) qw::fail(QWGPU_ENODEVICE, "host-only context: no CUDA device bound (there is no CPU search path)");
   return *ctx->engine;
+}
+
+// the split image opened into `v`, and the search request's plan on it
+static qw::CompiledPlan host_compile(qw::ImageView& v, const uint8_t* img, uint64_t img_len, const char* split_id,
+                                     const uint8_t* search_request_pb, size_t search_request_len, const char* doc_mapper_json) {
+  v.open(img, img_len);
+  qw::pb::SearchRequest req = qw::pb::decode_search_request(qw::pb::Reader(search_request_pb, search_request_len));
+  qw::DocMapperInfo dm = qw::parse_doc_mapper(doc_mapper_json ? doc_mapper_json : "");
+  return qw::compile_plan(v, split_id ? split_id : "", req, dm, nullptr);
 }
 
 namespace {
@@ -817,26 +828,13 @@ int qwgpu_leaf_search_allgather_lane(qwgpu_ctx* ctx, uint32_t lane, const uint8_
       m.num_successful_splits += h.successful;
       total_failed += h.n_failed;
     }
-    // sort-field types for the typed sort values: from a local split that has the column
-    const qw::CompiledPlan* p0 = run.which.empty() ? nullptr : &run.jobs[run.which[0]].plan;
-    if (!p0 && !run.merged.empty()) qw::fail(QWGPU_EUNSUPPORTED, "a rank without searchable splits cannot type the merged sort values");
-    int sft[2] = {0, 0};
-    if (p0) {
-      sft[0] = p0->sort_field_type[0]; sft[1] = p0->sort_field_type[1];
-      for (int i = 0; i < 2; i++)
-        for (size_t s2 = 0; s2 < run.which.size(); s2++) {
-          const qw::CompiledPlan& pp = run.jobs[run.which[s2]].plan;
-          if (pp.header.sort[i].kind == QW_SORT_COLUMN && pp.header.sort[i].column != 0xFFFFFFFFu) { sft[i] = pp.sort_field_type[i]; break; }
-        }
-    }
+    // the typed sort values come from the local splits' sort types
+    if (run.which.empty() && !run.merged.empty()) qw::fail(QWGPU_EUNSUPPORTED, "a rank without searchable splits cannot type the merged sort values");
+    const qw::SortTypes types = run.which.empty() ? qw::SortTypes{} : qw::sort_types(run.jobs, run.which);
     m.encoded_partial_hits.reserve(run.merged.size() * 72);
     for (const qw::MergedHit& mh : run.merged) {
       if (mh.split >= comm.split_ids.size()) qw::fail(QWGPU_EINTERNAL, "gathered hit carries split rank %u (table has %zu)", mh.split, comm.split_ids.size());
-      const QwHit& h = mh.hit;
-      qw::pb::SortValue sv1, sv2;
-      if (h.flags & 1) sv1 = qw::typed_sort_value(p0->header.sort[0].kind, sft[0], h.v1);
-      if (h.flags & 2) sv2 = qw::typed_sort_value(p0->header.sort[1].kind, sft[1], h.v2);
-      qw::pb::append_partial_hit(m.encoded_partial_hits, 2, comm.split_ids[mh.split], 0, h.doc_id, (h.flags & 1) != 0, sv1, (h.flags & 2) != 0, sv2);
+      qw::append_hit(m.encoded_partial_hits, comm.split_ids[mh.split], mh.hit, types);
     }
   }
   staged = total_failed != 0;
@@ -878,11 +876,7 @@ int qwgpu_compile_plan(const uint8_t* img, uint64_t img_len, const char* split_i
                        size_t search_request_len, const char* doc_mapper_json, uint8_t** plan, size_t* plan_len) {
   QW_API_BEGIN
   qw::ImageView v;
-  v.open(img, img_len);
-  qw::pb::SearchRequest req = qw::pb::decode_search_request(qw::pb::Reader(search_request_pb, search_request_len));
-  qw::DocMapperInfo dm = qw::parse_doc_mapper(doc_mapper_json ? doc_mapper_json : "");
-  qw::CompiledPlan cp = qw::compile_plan(v, split_id ? split_id : "", req, dm, nullptr);
-  give(cp.bytes, plan, plan_len);
+  give(host_compile(v, img, img_len, split_id, search_request_pb, search_request_len, doc_mapper_json).bytes, plan, plan_len);
   return 0;
   QW_API_END
 }
@@ -892,10 +886,7 @@ int qwgpu_build_leaf_response(const uint8_t* img, uint64_t img_len, const char* 
                               uint32_t num_partial_hits, const QwAggCell* cells, uint32_t num_cells, uint8_t** resp, size_t* resp_len) {
   QW_API_BEGIN
   qw::ImageView v;
-  v.open(img, img_len);
-  qw::pb::SearchRequest req = qw::pb::decode_search_request(qw::pb::Reader(search_request_pb, search_request_len));
-  qw::DocMapperInfo dm = qw::parse_doc_mapper(doc_mapper_json ? doc_mapper_json : "");
-  qw::CompiledPlan cp = qw::compile_plan(v, split_id ? split_id : "", req, dm, nullptr);
+  const qw::CompiledPlan cp = host_compile(v, img, img_len, split_id, search_request_pb, search_request_len, doc_mapper_json);
   qw::pb::LeafSearchResponse r = qw::build_split_response(cp, v, split_id ? split_id : "", num_hits, hits, num_partial_hits, cells, num_cells);
   give(qw::pb::encode_leaf_search_response(r), resp, resp_len);
   return 0;
@@ -907,10 +898,7 @@ int qwgpu_build_leaf_response_entries(const uint8_t* img, uint64_t img_len, cons
                                       uint32_t num_partial_hits, const QwAggEntry* entries, uint32_t num_entries, uint8_t** resp, size_t* resp_len) {
   QW_API_BEGIN
   qw::ImageView v;
-  v.open(img, img_len);
-  qw::pb::SearchRequest req = qw::pb::decode_search_request(qw::pb::Reader(search_request_pb, search_request_len));
-  qw::DocMapperInfo dm = qw::parse_doc_mapper(doc_mapper_json ? doc_mapper_json : "");
-  qw::CompiledPlan cp = qw::compile_plan(v, split_id ? split_id : "", req, dm, nullptr);
+  const qw::CompiledPlan cp = host_compile(v, img, img_len, split_id, search_request_pb, search_request_len, doc_mapper_json);
   qw::pb::LeafSearchResponse r = qw::build_split_response(cp, v, split_id ? split_id : "", num_hits, hits, num_partial_hits, nullptr, 0,
                                                           entries, num_entries, true);
   give(qw::pb::encode_leaf_search_response(r), resp, resp_len);
