@@ -233,6 +233,14 @@ int qwgpu_percentiles_table(const uint8_t* img, uint64_t img_len, uint32_t colum
 int qwgpu_regex_terms(const uint8_t* img, uint64_t img_len, const char* field, const char* regex, uint32_t** ords,
                       uint64_t* num_ords, uint64_t* transitions);
 
+/* `ip` field values, host only: qwgpu_parse_ip parses text[0, len) as Rust's `IpAddr::from_str` does and writes the
+ * 16 big-endian bytes of its IPv6 form (IPv4 as ::ffff:a.b.c.d) to out16, or fails with QWGPU_EINVALID_ARG; the image
+ * writer, the query compiler and aggregation `missing` all use this parser. qwgpu_format_ip writes an address the way
+ * a terms bucket key renders it (a dotted quad when IPv4-mapped, else RFC 5952) with its NUL into out[cap] and
+ * returns its length. */
+int qwgpu_parse_ip(const char* text, uint64_t len, uint8_t* out16);
+int qwgpu_format_ip(const uint8_t* addr16, char* out, uint64_t cap);
+
 /* Pre-search pruning (SURVEY.md 8a row a16), host only: what qwgpu_leaf_search does to the request of every
  * split before it searches — CanSplitDoBetter::{from_request, optimize_split_order, optimize}
  * (quickwit-search/src/leaf.rs:1072-1242), disable_search_request_hits (leaf.rs:1438-1443) and

@@ -54,7 +54,9 @@ typedef struct QwImgHeader {
 } QwImgHeader; /* 128 bytes */
 
 enum { QW_FIELD_HAS_FREQS = 1u, QW_FIELD_HAS_FIELDNORMS = 2u, QW_FIELD_HAS_POSITIONS = 4u };
-enum { QW_TOK_RAW = 0u, QW_TOK_DEFAULT = 1u };
+/* QW_TOK_IP: an indexed `type: ip` field; its terms are 16-byte big-endian IPv6 addresses (as QW_COL_IP's dictionary),
+ * recorded `basic` without fieldnorms. Query text is parsed as one address, never tokenized. */
+enum { QW_TOK_RAW = 0u, QW_TOK_DEFAULT = 1u, QW_TOK_IP = 2u };
 
 typedef struct QwImgField {
   uint32_t name_off, name_len; /* into strings blob */
@@ -137,9 +139,14 @@ enum {
   QW_COL_BOOL = 3,
   QW_COL_DATETIME = 4, /* i64 nanoseconds, truncated to fast_precision at build time */
   QW_COL_STR = 5,      /* term ordinals into a sorted dictionary */
-  QW_COL_BYTES = 6     /* `type: bytes` fast field: ordinals into a sorted dictionary of raw byte strings, stored like
+  QW_COL_BYTES = 6,    /* `type: bytes` fast field: ordinals into a sorted dictionary of raw byte strings, stored like
                           QW_COL_STR (dict_off / dict_num_terms). Only the find_trace_ids collector reads it; queries,
                           sorts and aggregations on it are refused. */
+  QW_COL_IP = 7        /* `type: ip` fast field: ordinals into a sorted dictionary of 16-byte big-endian IPv6 addresses
+                          (an IPv4 address as its IPv4-mapped form ::ffff:a.b.c.d), stored like QW_COL_STR. Byte order
+                          is numeric order, so the compiler turns every equality and range on an address into an
+                          ordinal range per split; the device only ever sees ordinals. Sorting on it is refused, and
+                          only `terms` aggregates it. */
 };
 enum { QW_CARD_FULL = 0, QW_CARD_OPTIONAL = 1, QW_CARD_MULTI = 2 };
 

@@ -20,6 +20,7 @@
 #include "compile.h"
 #include "ddsketch.h"
 #include "device_types.h"
+#include "ip_addr.h"
 
 namespace qw {
 
@@ -280,7 +281,7 @@ std::vector<AggReq> parse_agg_request(const std::string& json) {
 // ---- lowering ------------------------------------------------------------------------------------------
 static double mapped_to_f64(uint32_t type, uint64_t m) {
   switch (type) {
-    case QW_COL_U64: case QW_COL_BOOL: case QW_COL_STR: return (double)m;
+    case QW_COL_U64: case QW_COL_BOOL: case QW_COL_STR: case QW_COL_IP: return (double)m;
     case QW_COL_I64: case QW_COL_DATETIME: return (double)u64_to_i64(m);
     default: return u64_to_f64(m);
   }
@@ -440,6 +441,8 @@ static QwAggNode lower_one(const AggReq& a, const ImageView& img, AggBinding& b,
 static QwAggNode lower_comp_source(const AggReq& a, const ImageView& img, AggBinding& b, uint32_t level) {
   const AggReq& s = a.sources[level];
   QwAggNode n = lower_one(s, img, b);
+  if (b.column >= 0 && img.columns[b.column].type == QW_COL_IP)
+    fail(QWGPU_EUNSUPPORTED, "composite sources on ip field `%s` are not supported on the GPU path", s.field.c_str());
   b.req = &a;
   b.comp_level = level;
   if (s.has_missing && n.kind == QW_AGG_HISTOGRAM) n.num_buckets++;  // the missing bucket, last (as terms)
@@ -485,6 +488,8 @@ static QwAggNode lower_one(const AggReq& a, const ImageView& img, AggBinding& b,
     return n;
   }
   if (col && col->type == QW_COL_BYTES) fail(QWGPU_EUNSUPPORTED, "aggregations on bytes field `%s` are not supported on the GPU path", a.field.c_str());
+  if (col && col->type == QW_COL_IP && a.kind != AggReq::Terms)
+    fail(QWGPU_EUNSUPPORTED, "only terms aggregations on ip field `%s` are supported on the GPU path", a.field.c_str());
   switch (a.kind) {
     case AggReq::Terms: {
       n.kind = QW_AGG_TERMS;
@@ -547,7 +552,18 @@ static QwAggNode lower_one(const AggReq& a, const ImageView& img, AggBinding& b,
   return n;
 }
 
-std::vector<QwAggNode> lower_aggs(const std::vector<AggReq>& reqs, const ImageView& img, std::vector<AggBinding>& bindings) {
+// A terms node over an `ip` field keys its buckets by address (IKey::Ip), whether or not this split holds the field's
+// column: the field is `ip` when its column or its indexed field says so, or else the doc mapping.
+static bool ip_binding(const AggReq& a, const ImageView& img, const AggBinding& b, const DocMapperInfo* dm) {
+  if (b.column >= 0) return b.col_type == QW_COL_IP;
+  const int f = img.find_field(a.field);
+  if (f >= 0) return img.fields[f].tokenizer == QW_TOK_IP;
+  if (dm) for (auto& fd : dm->fields) if (fd.name == a.field) return fd.type == "ip";
+  return false;
+}
+
+std::vector<QwAggNode> lower_aggs(const std::vector<AggReq>& reqs, const ImageView& img, std::vector<AggBinding>& bindings,
+                                  const DocMapperInfo* dm) {
   std::vector<QwAggNode> out;
   bindings.clear();
   struct Pending { const AggReq* a; uint32_t idx, level; };
@@ -595,22 +611,34 @@ std::vector<QwAggNode> lower_aggs(const std::vector<AggReq>& reqs, const ImageVi
       for (size_t j = i; j < out.size(); j++)
         if (bindings[j].req == r) out[j].reserved = (out[j].reserved & ~(uint32_t)QW_AGG_COMP_HAS_AFTER) | QW_AGG_COMP_AFTER_HOST;
   }
+  for (AggBinding& b : bindings) {
+    const AggReq& a = b.req->kind == AggReq::Composite ? b.req->sources[b.comp_level] : *b.req;
+    if (b.req->kind == AggReq::TraceIds || !ip_binding(a, img, b, dm)) continue;
+    if (b.req->kind == AggReq::Composite) fail(QWGPU_EUNSUPPORTED, "composite sources on ip field `%s` are not supported on the GPU path", a.field.c_str());
+    if (a.kind != AggReq::Terms) fail(QWGPU_EUNSUPPORTED, "only terms aggregations on ip field `%s` are supported on the GPU path", a.field.c_str());
+    uint8_t addr[16];
+    if (a.has_missing && !(a.missing.type == Json::Str && parse_ip_addr(a.missing.s, addr)))
+      fail(QWGPU_EINVALID_AGG, "terms `missing` on ip field `%s` must be an IP address", a.field.c_str());
+    b.ip = true;
+  }
   return out;
 }
 
 // ---- intermediate model --------------------------------------------------------------------------------
 struct IKey {
-  enum K : uint8_t { Str = 0, F64 = 1, I64 = 2, U64 = 3 } kind = Str;
+  // Ip: the 16 big-endian bytes of an IPv6 address in `s`; keys of one kind order by address
+  enum K : uint8_t { Str = 0, F64 = 1, I64 = 2, U64 = 3, Ip = 4 } kind = Str;
   std::string s;
   double f = 0;
   int64_t i = 0;
   uint64_t u = 0;
+  bool numeric() const { return kind == F64 || kind == I64 || kind == U64; }
   bool operator<(const IKey& o) const {
     if (kind != o.kind) {
-      if (kind != Str && o.kind != Str) return num() < o.num();
+      if (numeric() && o.numeric()) return num() < o.num();
       return kind < o.kind;
     }
-    switch (kind) { case Str: return s < o.s; case F64: return f < o.f; case I64: return i < o.i; default: return u < o.u; }
+    switch (kind) { case Str: case Ip: return s < o.s; case F64: return f < o.f; case I64: return i < o.i; default: return u < o.u; }
   }
   bool operator==(const IKey& o) const { return !(*this < o) && !(o < *this); }
   double num() const { return kind == F64 ? f : (kind == I64 ? (double)i : (double)u); }
@@ -697,7 +725,7 @@ static void ser_agg(BW& w, const IAgg& a) {
   for (auto& b : a.buckets) {
     if (a.kind == AggReq::Terms) {
       w.varint(b.key.kind);
-      switch (b.key.kind) { case IKey::Str: w.str(b.key.s); break; case IKey::F64: w.f64(b.key.f); break; case IKey::I64: w.varint((uint64_t)b.key.i); break; default: w.varint(b.key.u); }
+      switch (b.key.kind) { case IKey::Str: case IKey::Ip: w.str(b.key.s); break; case IKey::F64: w.f64(b.key.f); break; case IKey::I64: w.varint((uint64_t)b.key.i); break; default: w.varint(b.key.u); }
     } else w.f64(b.hkey);
     w.varint(b.count);
     ser_aggs(w, b.subs);
@@ -757,8 +785,11 @@ static IAgg de_agg(BR& r) {
   for (uint64_t i = 0; i < n; i++) {
     IBucket b;
     if (a.kind == AggReq::Terms) {
-      b.key.kind = (IKey::K)r.varint();
-      switch (b.key.kind) { case IKey::Str: b.key.s = r.str(); break; case IKey::F64: b.key.f = r.f64(); break; case IKey::I64: b.key.i = (int64_t)r.varint(); break; default: b.key.u = r.varint(); }
+      const uint64_t kk = r.varint();
+      if (kk > IKey::Ip) fail(QWGPU_EINTERNAL, "failed to merge intermediate aggregation results: bad terms key");
+      b.key.kind = (IKey::K)kk;
+      switch (b.key.kind) { case IKey::Str: case IKey::Ip: b.key.s = r.str(); break; case IKey::F64: b.key.f = r.f64(); break; case IKey::I64: b.key.i = (int64_t)r.varint(); break; default: b.key.u = r.varint(); }
+      if (b.key.kind == IKey::Ip && b.key.s.size() != 16) fail(QWGPU_EINTERNAL, "failed to merge intermediate aggregation results: bad ip key");
     } else b.hkey = r.f64();
     b.count = r.varint();
     b.subs = de_aggs(r);
@@ -788,6 +819,13 @@ static std::vector<IAgg> de_top(const std::string& s) {
 // ---- build a split's tree ------------------------------------------------------------------------------
 static IKey term_key(const ImageView& img, const AggBinding& b, uint64_t raw, bool missing) {
   IKey k;
+  if (missing && b.ip) {  // parsed when the plan was lowered
+    uint8_t a[16];
+    parse_ip_addr(b.req->missing.s, a);
+    k.kind = IKey::Ip;
+    k.s.assign((const char*)a, 16);
+    return k;
+  }
   if (missing) {
     const Json& m = b.req->missing;
     if (m.type == Json::Str) { k.kind = IKey::Str; k.s = m.s; }
@@ -800,6 +838,7 @@ static IKey term_key(const ImageView& img, const AggBinding& b, uint64_t raw, bo
   uint64_t mapped = col.min_value + col.gcd * raw;
   switch (col.type) {
     case QW_COL_STR: { const uint8_t* p; uint32_t len; img.dict_term(col, (uint32_t)mapped, &p, &len); k.kind = IKey::Str; k.s.assign((const char*)p, len); break; }
+    case QW_COL_IP: { const uint8_t* p; uint32_t len; img.dict_term(col, (uint32_t)mapped, &p, &len); k.kind = IKey::Ip; k.s.assign((const char*)p, len); break; }
     case QW_COL_F64: k.kind = IKey::F64; k.f = u64_to_f64(mapped); break;
     case QW_COL_I64: case QW_COL_DATETIME: k.kind = IKey::I64; k.i = u64_to_i64(mapped); break;
     default: k.kind = IKey::U64; k.u = mapped; break;
@@ -1121,7 +1160,7 @@ static std::vector<IAgg> build_top_entries(const CompiledPlan& cp, const ImageVi
           ok = b.column >= 0 && img.columns[b.column].num_vals > 0 && img.columns[b.column].gcd &&
                x.key <= (img.columns[b.column].max_value - img.columns[b.column].min_value) / img.columns[b.column].gcd;
           const QwImgColumn& col = img.columns[b.column >= 0 ? b.column : 0];
-          if (ok && col.type == QW_COL_STR) ok = col.min_value + col.gcd * x.key < col.dict_num_terms;
+          if (ok && (col.type == QW_COL_STR || col.type == QW_COL_IP)) ok = col.min_value + col.gcd * x.key < col.dict_num_terms;
           break;
         }
         default: ok = false;
@@ -1411,6 +1450,7 @@ static void fin_aggs(const std::vector<AggReq>& reqs, const std::vector<IAgg>* a
 static void fin_key(const IKey& k, std::string& out) {
   switch (k.kind) {
     case IKey::Str: json_escape(k.s, out); break;
+    case IKey::Ip: json_escape(format_ip_addr((const uint8_t*)k.s.data()), out); break;
     case IKey::F64: json_f64(k.f, out); break;
     case IKey::I64: out += std::to_string(k.i); break;
     default: out += std::to_string(k.u);

@@ -89,10 +89,13 @@ struct AggBinding {
   int column = -1;
   uint32_t col_type = 0;
   uint32_t comp_level = 0;  // req is a Composite: the node is source `comp_level` of its chain
+  bool ip = false;          // a terms node over an `ip` field: buckets (and `missing`) keyed by address
 };
 // Flattens the request against one split (column lookup, dense bucket space); nodes are emitted
 // breadth-first so that the children of a node are contiguous.
-std::vector<QwAggNode> lower_aggs(const std::vector<AggReq>& reqs, const ImageView& img, std::vector<AggBinding>& bindings);
+// `dm` (optional) tells which fields absent from the split are `ip` fields.
+std::vector<QwAggNode> lower_aggs(const std::vector<AggReq>& reqs, const ImageView& img, std::vector<AggBinding>& bindings,
+                                  const DocMapperInfo* dm = nullptr);
 
 struct CompiledPlan {
   std::string bytes;  // QwPlanHeader + nodes + agg nodes

@@ -471,7 +471,7 @@ uint64_t agg_hashed_layout(const QwAggNode* aggs, uint32_t n, const ImageView& i
 // kernels.cuh mapped_to_f64 on the host (tantivy MonotonicallyMappableToU64 inverses, as f64)
 static double mapped_to_f64_host(uint32_t type, uint64_t m) {
   switch (type) {
-    case QW_COL_U64: case QW_COL_BOOL: case QW_COL_STR: return (double)m;
+    case QW_COL_U64: case QW_COL_BOOL: case QW_COL_STR: case QW_COL_IP: return (double)m;
     case QW_COL_I64: case QW_COL_DATETIME: return (double)(int64_t)(m ^ (1ull << 63));
     default: return u64_to_f64(m);
   }
@@ -951,6 +951,7 @@ static void lower_plan(Lowered& L, const SplitDev& sp, const uint8_t* plan, size
       else {
         uint32_t t = sp.view.columns[ph->sort[i].column].type;
         if (t == QW_COL_STR) fail(QWGPU_EINVALID_ARG, "Unsupported sort field type `Str`.");
+        if (t == QW_COL_IP) fail(QWGPU_EINVALID_ARG, "Unsupported sort field type `IpAddr`.");
         ks.col[i] = use_col(L, sp, ph->sort[i].column);
       }
     }
@@ -1029,6 +1030,7 @@ static void lower_plan(Lowered& L, const SplitDev& sp, const uint8_t* plan, size
       if (a.column != 0xFFFFFFFFu) {
         const uint32_t t = sp.view.columns[a.column].type;
         if (t == QW_COL_STR || t == QW_COL_BYTES) fail(QWGPU_EINVALID_AGG, "percentiles over a text or bytes column");
+        if (t == QW_COL_IP) fail(QWGPU_EUNSUPPORTED, "percentiles over an ip column are not supported on the GPU path");
         tab = percentiles_table(sp, a.column);
       }
       const uint64_t nb = tab ? tab->size() : 0;

@@ -96,6 +96,7 @@ static void add_term(qwgpu_imgb* b, uint32_t field_id, const uint8_t* term, uint
                      const uint32_t* docs, const uint32_t* tfs, uint32_t n, const uint32_t* positions = nullptr, uint64_t n_positions = 0) {
   if (field_id >= b->fields.size()) fail(QWGPU_EINVALID_ARG, "add_term: bad field id");
   if (n == 0) return;
+  if (b->fields[field_id].tokenizer == QW_TOK_IP && term_len != 16) fail(QWGPU_EINVALID_ARG, "add_term: an ip field's terms are 16-byte addresses");
   bool has_freqs = (b->fields[field_id].flags & QW_FIELD_HAS_FREQS) != 0;
   const bool has_pos = (b->fields[field_id].flags & QW_FIELD_HAS_POSITIONS) != 0;
   if (has_pos) {
@@ -253,7 +254,14 @@ static void add_column(qwgpu_imgb* b, const char* name, uint32_t type, uint32_t 
     memcpy(c.index.data(), index, 4ull * (nd + 1));
     if (((const uint32_t*)c.index.data())[nd] != num_vals) fail(QWGPU_EINVALID_ARG, "MULTI column: start[num_docs] != num_vals");
   }
-  if (type == QW_COL_STR || type == QW_COL_BYTES) {
+  if (type == QW_COL_IP) {
+    // ordinals into strictly increasing 16-byte addresses: byte order is address order
+    for (uint32_t k = 0; k < dict_n; k++)
+      if (dict_offs[k + 1] - dict_offs[k] != 16 || (k > 0 && memcmp(dict_bytes + dict_offs[k - 1], dict_bytes + dict_offs[k], 16) >= 0))
+        fail(QWGPU_EINVALID_ARG, "ip column '%s': the dictionary must hold strictly increasing 16-byte addresses", name);
+    if (num_vals && mx >= dict_n) fail(QWGPU_EINVALID_ARG, "ip column '%s': ordinal %llu outside a dictionary of %u addresses", name, (unsigned long long)mx, dict_n);
+  }
+  if (type == QW_COL_STR || type == QW_COL_BYTES || type == QW_COL_IP) {
     uint64_t blen = dict_n ? dict_offs[dict_n] : 0;
     c.dict.resize(4ull * (dict_n + 1) + blen);
     if (dict_n) memcpy(c.dict.data(), dict_offs, 4ull * (dict_n + 1));
@@ -583,6 +591,7 @@ int qwgpu_imgb_add_field(qwgpu_imgb* b, const char* name, uint32_t flags, uint32
   f.flags = flags;
   f.tokenizer = tokenizer;
   f.total_tokens = total_num_tokens;
+  if (tokenizer == QW_TOK_IP && flags != 0) qw::fail(QWGPU_EINVALID_ARG, "ip field '%s' is indexed `basic`, without fieldnorms", name);
   if (flags & QW_FIELD_HAS_FIELDNORMS) {
     if (!fieldnorm_ids) qw::fail(QWGPU_EINVALID_ARG, "field '%s' declares fieldnorms but none given", name);
     f.fieldnorms.assign(fieldnorm_ids, fieldnorm_ids + b->num_docs);

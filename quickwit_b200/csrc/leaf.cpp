@@ -956,6 +956,7 @@ int qwgpu_percentiles_table(const uint8_t* img, uint64_t img_len, uint32_t colum
   if (column >= v.hdr->num_columns) qw::fail(QWGPU_EINVALID_ARG, "column %u (split has %u)", column, v.hdr->num_columns);
   const QwImgColumn& c = v.columns[column];
   if (c.type == QW_COL_STR || c.type == QW_COL_BYTES) qw::fail(QWGPU_EINVALID_AGG, "percentiles over a text or bytes column");
+  if (c.type == QW_COL_IP) qw::fail(QWGPU_EUNSUPPORTED, "percentiles over an ip column are not supported on the GPU path");
   qw::dds::Table t;
   if (!qw::dds::column_table(c, true, &t)) qw::fail(QWGPU_EUNSUPPORTED, "percentiles over a column holding NaN or infinite values");
   *edges = nullptr;

@@ -18,6 +18,7 @@
 #include <climits>
 
 #include "compile.h"
+#include "ip_addr.h"
 #include "regex.h"
 
 namespace qw {
@@ -276,8 +277,8 @@ static bool literal_to_mapped(const QwImgColumn& c, const Json& v, const DocMapp
   }
 }
 static const char* col_type_name(uint32_t t) {
-  static const char* n[] = {"u64", "i64", "f64", "bool", "datetime", "text"};
-  return t < 6 ? n[t] : "?";
+  static const char* n[] = {"u64", "i64", "f64", "bool", "datetime", "text", "bytes", "ip"};
+  return t < 8 ? n[t] : "?";
 }
 
 struct Ctx {
@@ -426,6 +427,8 @@ static TQ regex_leaf(const Ctx& cx, const std::string& field, const std::string&
   const DocMapperInfo::Field* fd = nullptr;
   for (auto& d : cx.dm.fields) if (d.name == field) fd = &d;
   const int c = cx.img.find_column(field);
+  if ((f >= 0 && cx.img.fields[f].tokenizer == QW_TOK_IP) || (c >= 0 && cx.img.columns[c].type == QW_COL_IP))
+    fail(QWGPU_EINVALID_QUERY, "invalid query: trying to run a regex query on a non-text field");
   if (f < 0) {
     if ((c >= 0 && cx.img.columns[c].type != QW_COL_STR) || (fd && fd->type != "text" && fd->type != "json"))
       fail(QWGPU_EINVALID_QUERY, "invalid query: trying to run a regex query on a non-text field");
@@ -454,10 +457,44 @@ static TQ range_leaf(uint32_t column, uint64_t lo, uint64_t hi) {
   return t;
 }
 
+// ---- `ip` fields (json_literal.rs:135-140, query_ast/utils.rs:174-178) ----------------------------------------------
+// A fast `ip` field is a QW_COL_IP column, an indexed one a field of 16-byte terms (QW_TOK_IP); a field of neither kind
+// in this split is an `ip` field when the doc mapping declares it so.
+static bool is_ip_field(const Ctx& cx, const std::string& field) {
+  const int c = cx.img.find_column(field);
+  if (c >= 0) return cx.img.columns[c].type == QW_COL_IP;
+  const int f = cx.img.find_field(field);
+  if (f >= 0) return cx.img.fields[f].tokenizer == QW_TOK_IP;
+  for (auto& fd : cx.dm.fields) if (fd.name == field) return fd.type == "ip";
+  return false;
+}
+static std::string ip_literal(const std::string& field, const std::string& text) {
+  uint8_t a[16];
+  if (!parse_ip_addr(text, a))
+    fail(QWGPU_EINVALID_QUERY, "invalid query: expected a `ip` search value for field `%s`, got `%s`", field.c_str(), text.c_str());
+  return std::string((const char*)a, 16);
+}
+// TermQuery on an `ip` field: the whole text is one address, never tokenized. On a fast field an equality on the
+// ordinal (the dictionary is sorted, so an address present in the split has exactly one), else a posting lookup of
+// the 16-byte term. Both run unscored: a scoring clause under _score ranking is refused.
+static TQ ip_term(const Ctx& cx, const std::string& field, const std::string& text) {
+  const std::string addr = ip_literal(field, text);
+  refuse_const_score_under_ranking(cx, "ip term");
+  const int c = cx.img.find_column(field);
+  if (c >= 0) {
+    bool exact;
+    const uint32_t ord = cx.img.dict_lower_bound(cx.img.columns[c], (const uint8_t*)addr.data(), 16, &exact);
+    return exact ? range_leaf((uint32_t)c, ord, ord) : tq_none();
+  }
+  const int f = cx.img.find_field(field);
+  return f >= 0 ? term_leaf(cx, (uint32_t)f, addr) : tq_none();
+}
+
 // full_text_query / FullTextParams::make_query (full_text_query.rs:103-160, utils.rs:73-200)
 static TQ full_text(const Ctx& cx, const std::string& field, const std::string& text, const std::string& tokenizer_override,
                     const std::string& mode, bool op_and, int zero_terms_all, bool lenient, uint32_t slop = 0,
                     uint64_t max_expansions = 50) {
+  if (is_ip_field(cx, field)) return ip_term(cx, field, text);
   int f = cx.img.find_field(field);
   if (f < 0) {
     int c = cx.img.find_column(field);
@@ -547,8 +584,9 @@ static TQ range_query(const Ctx& cx, const std::string& field, const Json* lower
   bool inc;
   auto conv = [&](const Json& lit, bool is_lower, bool included) -> bool {  // false => empty range
     uint64_t m;
-    if (col.type == QW_COL_STR) {
-      std::string s = lit_str(lit);
+    if (col.type == QW_COL_STR || col.type == QW_COL_IP) {
+      // an address bound becomes an ordinal bound through the split's sorted dictionary, as a string bound does
+      std::string s = col.type == QW_COL_IP ? ip_literal(field, lit_str(lit)) : lit_str(lit);
       bool exact;
       uint32_t lb = cx.img.dict_lower_bound(col, (const uint8_t*)s.data(), (uint32_t)s.size(), &exact);
       if (is_lower) { lo = (exact && !included) ? lb + 1 : lb; return true; }
@@ -628,6 +666,7 @@ static TQ build(const Ctx& cx, const Json& q, int depth) {
     const std::string tok_name = params ? params->str_or("tokenizer", "") : "";
     const bool zero_all = params && params->str_or("zero_terms_query", "none") == "all";
     const int f = cx.img.find_field(field);
+    if (is_ip_field(cx, field)) fail(QWGPU_EINVALID_QUERY, "invalid query: trying to run a PhrasePrefix query on a non-text field");
     if (f < 0) {
       const int c = cx.img.find_column(field);
       bool known = false, text = true;
@@ -661,6 +700,7 @@ static TQ build(const Ctx& cx, const Json& q, int depth) {
     const std::string field = q.str_or("field", ""), value = q.str_or("value", "");
     const bool lenient = q.bool_or("lenient", false), ci = q.bool_or("case_insensitive", false);
     const int f = cx.img.find_field(field);
+    if (is_ip_field(cx, field)) fail(QWGPU_EINVALID_QUERY, "invalid query: trying to run a Wildcard query on a non-text field");
     if (f < 0) {
       if (cx.img.find_column(field) >= 0 && cx.img.columns[cx.img.find_column(field)].type != QW_COL_STR)
         fail(QWGPU_EINVALID_QUERY, "invalid query: trying to run a Wildcard query on a non-text field");
@@ -996,6 +1036,7 @@ CompiledPlan compile_plan(const ImageView& img, const std::string& split_id, con
       if (c >= 0) {
         uint32_t t = img.columns[c].type;
         if (t == QW_COL_STR) fail(QWGPU_EINVALID_ARG, "Unsupported sort field type `Str`.");
+        if (t == QW_COL_IP) fail(QWGPU_EINVALID_ARG, "Unsupported sort field type `IpAddr`.");
         if (t == QW_COL_BYTES) fail(QWGPU_EUNSUPPORTED, "sorting on bytes field `%s` is not supported on the GPU path", sf.field_name.c_str());
         h.sort[i].column = (uint32_t)c;
         sft[i] = t == QW_COL_U64 ? SFT_U64 : t == QW_COL_I64 ? SFT_I64 : t == QW_COL_F64 ? SFT_F64 : t == QW_COL_BOOL ? SFT_BOOL : SFT_DATETIME;
@@ -1038,7 +1079,7 @@ CompiledPlan compile_plan(const ImageView& img, const std::string& split_id, con
     // Jaeger's trace search sends the find_trace_ids collector with max_hits 0; the GPU path runs it alone
     if (is_trace_ids_request(cp.agg_request) && h.max_hits > 0)
       fail(QWGPU_EUNSUPPORTED, "find_trace_ids combined with max_hits > 0 is not implemented on the GPU path");
-    aggs = lower_aggs(cp.agg_request, img, cp.agg_bindings);
+    aggs = lower_aggs(cp.agg_request, img, cp.agg_bindings, &dm);
   }
   h.num_aggs = (uint32_t)aggs.size();
   h.count_only = (h.max_hits == 0 && aggs.empty()) ? 1 : 0;

@@ -17,8 +17,8 @@ EINTERNAL, EINVALID_QUERY, EINVALID_AGG, EINVALID_ARG, ENODEVICE, ENOTFOUND, EUN
 
 # qwgpu_format.h enums
 FIELD_HAS_FREQS, FIELD_HAS_FIELDNORMS, FIELD_HAS_POSITIONS = 1, 2, 4
-TOK_RAW, TOK_DEFAULT = 0, 1
-COL_U64, COL_I64, COL_F64, COL_BOOL, COL_DATETIME, COL_STR, COL_BYTES = range(7)
+TOK_RAW, TOK_DEFAULT, TOK_IP = 0, 1, 2  # TOK_IP: an indexed `ip` field (16-byte address terms)
+COL_U64, COL_I64, COL_F64, COL_BOOL, COL_DATETIME, COL_STR, COL_BYTES, COL_IP = range(8)
 CARD_FULL, CARD_OPTIONAL, CARD_MULTI = range(3)
 NODE_TERM, NODE_RANGE, NODE_BOOL, NODE_ALL, NODE_NONE, NODE_EXISTS, NODE_PHRASE = 1, 2, 3, 4, 5, 6, 7
 NODE_PHRASE_PREFIX = 8
@@ -276,7 +276,8 @@ def img_lib():
                 ("qwgpu_synth_split", [C.POINTER(SynthSpec), C.POINTER(vp), C.POINTER(u64)], C.c_int),
                 ("qwgpu_bm25_weight", [u64, u64, C.c_float], C.c_float),
                 ("qwgpu_bm25_phrase_weight", [vp, u32, u64, C.c_float], C.c_float),
-                ("qwgpu_fieldnorm_to_id", [u32], C.c_uint8), ("qwgpu_id_to_fieldnorm", [C.c_uint8], u32)]:
+                ("qwgpu_fieldnorm_to_id", [u32], C.c_uint8), ("qwgpu_id_to_fieldnorm", [C.c_uint8], u32),
+                ("qwgpu_parse_ip", [cp, u64, vp], C.c_int), ("qwgpu_format_ip", [vp, vp, u64], C.c_int)]:
             fn = getattr(L, name)
             fn.argtypes, fn.restype = argtypes, restype
         _img_lib = L

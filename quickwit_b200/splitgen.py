@@ -7,12 +7,14 @@ C++ writer behind `qwgpu_imgb_*`; this module only tokenizes and groups.
 
 Doc-mapping dialect: the subset of Quickwit's doc mapper JSON this path needs
 (quickwit-doc-mapper/src/doc_mapper/field_mapping_entry.rs): `field_mappings[]` entries with
-`name`, `type` (text|u64|i64|f64|bool|datetime|bytes), `tokenizer` (default|raw), `record`
+`name`, `type` (text|u64|i64|f64|bool|datetime|bytes|ip), `tokenizer` (default|raw), `record`
 (basic|freq|position; default basic, :447), `fieldnorms` (default false, :326), `fast`,
 `fast_precision` (seconds|milliseconds|microseconds|nanoseconds), `input_format` (bytes: base64|hex,
 default base64), plus `timestamp_field` and `mode: dynamic` (unknown JSON keys become fast raw-text /
-numeric columns and raw-indexed text). A fast bytes field becomes a QW_COL_BYTES column: ordinals into
-the sorted dictionary of its raw values.
+numeric columns and raw-indexed text; never `ip`). A fast bytes field becomes a QW_COL_BYTES column: ordinals into
+the sorted dictionary of its raw values. An `ip` field (`indexed` default true, `fast` default false) holds 16-byte
+IPv6 addresses (IPv4 as ::ffff:a.b.c.d): indexed, one `basic` term per distinct address of a doc; fast, a QW_COL_IP
+column of ordinals into the sorted address dictionary. A value that is not an address fails the build.
 """
 from __future__ import annotations
 
@@ -153,6 +155,25 @@ def parse_datetime_nanos(v: Any) -> int:
     epoch = _dt.datetime(1970, 1, 1, tzinfo=_dt.timezone.utc)
     delta = d - epoch
     return (delta.days * 86400 + delta.seconds) * 10**9 + delta.microseconds * 1000
+
+
+def parse_ip(v: Any) -> bytes:
+    """An `ip` value as the 16 big-endian bytes of its IPv6 form (the library's parser, Rust's `IpAddr::from_str` then
+    `into_ipv6_addr`); ValueError when it is not an address."""
+    raw = str(v).encode()
+    out = C.create_string_buffer(16)
+    L = ffi.img_lib()
+    if L.qwgpu_parse_ip(raw, len(raw), out) < 0:
+        raise ValueError(L.qwgpu_last_error().decode("utf-8", "replace"))
+    return out.raw
+
+
+def format_ip(addr: bytes) -> str:
+    """The library's rendering of a 16-byte address as a terms key: a dotted quad when IPv4-mapped, else RFC 5952."""
+    buf = C.create_string_buffer(48)
+    src = C.create_string_buffer(bytes(addr), 16)
+    ffi.img_check(ffi.img_lib().qwgpu_format_ip(src, buf, 48))
+    return buf.value.decode()
 
 
 # ---- tokenizers ----------------------------------------------------------------------------------
@@ -361,6 +382,20 @@ def build_split(docs: Sequence[Dict[str, Any]], doc_mapping: Dict[str, Any], spl
                 ords = {t: i for i, t in enumerate(dictionary)}
                 per_doc = [[ords[str(v).encode()] for v in vs] for vs in values]
                 _column_from_values(b, name, ffi.COL_STR, per_doc, dictionary)
+        elif ftype == "ip":
+            addrs = [[parse_ip(v) for v in vs] for vs in values]
+            if m.get("indexed", True):
+                postings_ip: Dict[bytes, List[int]] = {}
+                for d, vs in enumerate(addrs):
+                    for a in sorted(set(vs)):
+                        postings_ip.setdefault(a, []).append(d)
+                fid = b.add_field(name, 0, ffi.TOK_IP, None, sum(len(vs) for vs in addrs))
+                for a in sorted(postings_ip):
+                    b.add_term(fid, a, np.array(postings_ip[a], dtype=np.uint32), None)
+            if m.get("fast", False):
+                dictionary = sorted({a for vs in addrs for a in vs})
+                ords = {a: i for i, a in enumerate(dictionary)}
+                _column_from_values(b, name, ffi.COL_IP, [[ords[a] for a in vs] for vs in addrs], dictionary)
         elif ftype == "bytes":
             if m.get("fast", False):
                 raw = [[decode_bytes_value(v, m.get("input_format", "base64")) for v in vs] for vs in values]
