@@ -185,6 +185,16 @@ typedef struct qwgpu_split_result {
 #define QWGPU_KERNEL_PREDICATE_FILL 16384u /* the call filled predicate-cache entries: its QW_NODE_CACHE subtrees that
                                              missed ran first as one count-only k_window batch (with their own phrase /
                                              term-set pre-passes), counted in the call's launches and device time */
+/* Aggregation limits of one plan on the GPU path; a search whose plan exceeds one fails with QWGPU_EUNSUPPORTED (in a
+ * leaf response: a failed split, not retryable), so a caller can split such a request before it sends it:
+ *   QWGPU_MAX_AGG_NODES    QwAggNode entries (QwPlanHeader.num_aggs); a composite takes one node per source
+ *   QWGPU_MAX_AGG_LEVELS   nesting levels of the aggregation tree: a top-level node is level 1, each child one more
+ *                          (a composite's sources are one level each, its sub-aggregations below them)
+ *   QWGPU_MAX_AGG_COLUMNS  distinct columns that aggregation nodes read beyond those of the query and the sort (which
+ *                          may use 16 columns of their own) */
+#define QWGPU_MAX_AGG_NODES 32u
+#define QWGPU_MAX_AGG_LEVELS 8u
+#define QWGPU_MAX_AGG_COLUMNS 32u
 /* Initial capacity of a split's hashed cell table: min(this, the split's bound on distinct cells). */
 #define QWGPU_HASHED_INIT_CELLS 65536u
 /* Largest total of the hashed tables (cells, key records and slots, each at its split's bound) that one call may

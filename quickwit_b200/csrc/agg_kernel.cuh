@@ -37,14 +37,15 @@ namespace qwk {
 #define QA_SLOTS 2               /* per block; four blocks per SM keep eight chunks in flight */
 #define QA_MINB 4
 #define QA_MAX_CELLS 4096
+#define QA_MAX_AGGS 8            /* aggregation nodes per plan: one column staged per node, indexed by lane & 7 */
 
 struct ASmem {
   uint32_t slot0, slot_stride;
-  uint32_t col_off[QW_MAX_DAGGS];  // bytes of aggregation i's column inside a slot
+  uint32_t col_off[QA_MAX_AGGS];   // bytes of aggregation i's column inside a slot
   uint32_t hdr;                    // uint4 {split, first doc, docs, flags} inside a slot
   uint32_t bars;                   // full[QA_SLOTS], empty[QA_SLOTS]
-  uint32_t atab;                   // AggRow[QW_MAX_DAGGS]: the current split's aggregations
-  uint32_t bcache;                 // uint4[QA_CW][QW_MAX_DAGGS]: per warp, the histogram bucket it is in
+  uint32_t atab;                   // AggRow[QA_MAX_AGGS]: the current split's aggregations
+  uint32_t bcache;                 // uint4[QA_CW][QA_MAX_AGGS]: per warp, the histogram bucket it is in
   uint32_t cells;                  // uint32[n_cells]
   uint32_t total;
 };
@@ -162,13 +163,13 @@ __global__ void __launch_bounds__(QA_THREADS, QA_MINB) k_aggscan(const AParams p
         asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar_full(slot)), "r"(total) : "memory");
       }
       __syncwarp();
-      if (bytes) bulk_g2s(sbase + sl + p.sm.col_off[lane & (QW_MAX_DAGGS - 1)], src0 + ((uint64_t)d0 * bits >> 3), bytes, bar_full(slot));
+      if (bytes) bulk_g2s(sbase + sl + p.sm.col_off[lane & (QA_MAX_AGGS - 1)], src0 + ((uint64_t)d0 * bits >> 3), bytes, bar_full(slot));
     }
   } else {
     // ================================ consumers =====================================================
     uint32_t cur_split = 0xFFFFFFFFu, n_aggs = 0;
     unsigned long long my_docs = 0;  // thread 0 counts the docs of the current split
-    uint4* bcache = (uint4*)(qw_smem + p.sm.bcache) + warp * QW_MAX_DAGGS;  // {lo, hi, bucket, valid} per aggregation
+    uint4* bcache = (uint4*)(qw_smem + p.sm.bcache) + warp * QA_MAX_AGGS;  // {lo, hi, bucket, valid} per aggregation
     auto enter_split = [&](uint32_t next) {
       // all consumer warps have added their counts of the old split: named barrier over the consumers
       asm volatile("bar.sync 1, %0;" ::"n"(QA_CW * 32) : "memory");
@@ -195,7 +196,7 @@ __global__ void __launch_bounds__(QA_THREADS, QA_MINB) k_aggscan(const AParams p
           if (a.kind == QW_AGG_HISTOGRAM) { r.b0 = __ldg((const uint64_t*)a.bounds); r.bn = __ldg((const uint64_t*)a.bounds + a.num_buckets); }
           atab[tid] = r;
         }
-        if (lane < QW_MAX_DAGGS) bcache[lane] = make_uint4(1u, 0u, 0u, 0u);  // empty interval: lo > hi
+        if (lane < QA_MAX_AGGS) bcache[lane] = make_uint4(1u, 0u, 0u, 0u);  // empty interval: lo > hi
       }
       asm volatile("bar.sync 1, %0;" ::"n"(QA_CW * 32) : "memory");
     };

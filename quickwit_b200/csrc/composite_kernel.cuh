@@ -68,10 +68,10 @@ __global__ void __launch_bounds__(QC_THREADS) k_composite_cut(const DSplitPlan* 
   const uint32_t used = min(ctr & 0x7FFFFFFFu, P.h_cap);
   const DAgg* aggs = all_aggs + P.agg_base;
   const uint32_t tid = threadIdx.x;
-  __shared__ uint32_t s_comp[QW_MAX_DAGGS], s_chain[QW_MAX_DAGGS];
+  __shared__ uint32_t s_comp[QW_MAX_AGG_NODES], s_chain[QW_MAX_AGG_LEVELS];
   __shared__ uint32_t s_hist[256], s_warp[32];
   __shared__ uint32_t s_k, s_sel, s_tied, s_n_leaves, s_any;
-  if (tid < QW_MAX_DAGGS) s_comp[tid] = tid < P.n_aggs ? aggs[tid].comp : 0u;
+  if (tid < QW_MAX_AGG_NODES) s_comp[tid] = tid < P.n_aggs ? aggs[tid].comp : 0u;
   if (tid == 0) s_any = 0;
   __syncthreads();
   DHKey* keys = (DHKey*)P.h_keys;
@@ -87,7 +87,7 @@ __global__ void __launch_bounds__(QC_THREADS) k_composite_cut(const DSplitPlan* 
     uint32_t n = 0, g = top;
     bool ok = true;
     while (true) {
-      if (n >= QW_MAX_DAGGS || g >= P.n_aggs || !(s_comp[g] & QW_AGG_COMP_LEVEL) || (s_comp[g] & QW_AGG_COMP_AFTER_HOST)) { ok = false; break; }
+      if (n >= QW_MAX_AGG_LEVELS || g >= P.n_aggs || !(s_comp[g] & QW_AGG_COMP_LEVEL) || (s_comp[g] & QW_AGG_COMP_AFTER_HOST)) { ok = false; break; }
       if (tid == 0) s_chain[n] = g;
       n++;
       if (s_comp[g] & QW_AGG_COMP_LAST) break;
@@ -156,7 +156,7 @@ __global__ void __launch_bounds__(QC_THREADS) k_composite_cut(const DSplitPlan* 
   // are kept by the kept leaves below them; every other entry stays
   for (uint32_t e = tid; e < used; e += QC_THREADS) {
     uint32_t k = 1, x = e;
-    for (uint32_t hop = 0; hop <= QW_MAX_DAGGS && x != QW_AGG_NO_PARENT; hop++) {
+    for (uint32_t hop = 0; hop <= QW_MAX_AGG_LEVELS && x != QW_AGG_NO_PARENT; hop++) {
       const uint32_t c = s_comp[keys[x].node_flags & 0xFFu];
       if (c & QW_AGG_COMP_LAST) { k = st[x] == QC_DROP ? 0u : 1u; break; }
       if ((c & QW_AGG_COMP_LEVEL) && x == e) k = 0;  // above the leaves: decided by them

@@ -3,14 +3,16 @@
 #include <stddef.h>
 #include <stdint.h>
 
-#include "../../include/qwgpu_format.h"
+#include "../../include/qwgpu.h"
 
 #define QW_THREADS 512
 #define QW_MIN_BLOCKS_PER_SM 2
 #define QW_WARPS (QW_THREADS / 32)
 #define QW_MAX_INSTR 96
-#define QW_MAX_DCOLS 16
-#define QW_MAX_DAGGS 8
+#define QW_MAX_DCOLS 16                          /* columns a plan's query and sort may use */
+#define QW_MAX_AGG_NODES QWGPU_MAX_AGG_NODES    /* aggregation nodes per plan */
+#define QW_MAX_AGG_LEVELS QWGPU_MAX_AGG_LEVELS  /* nesting levels of a plan's aggregation tree (the hashed walk's stack) */
+#define QW_MAX_AGG_COLS QWGPU_MAX_AGG_COLUMNS   /* columns first used by aggregation nodes, beyond QW_MAX_DCOLS */
 #define QW_MAX_LEVELS QW_MAX_PLAN_DEPTH
 #define QW_MAX_TERMS 64      /* TERM instructions per plan */
 #define QW_BLK_TAB 160       /* staged blocks per (term, window) before falling back to direct mode */

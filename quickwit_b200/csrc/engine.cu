@@ -500,6 +500,7 @@ struct Lowered {
   uint32_t ts_blocks = 0;               // posting blocks of ts_terms
   uint32_t tr_img_col = 0;              // find_trace_ids: the trace-id column of the image
   uint64_t h_bound = 0;                 // hashed aggregation layout: upper bound on the split's distinct cells
+  uint32_t n_agg_cols = 0;              // columns of `cols` first used by an aggregation node (use_col)
   // predicate cache: `pc` is null when every QW_NODE_CACHE is lowered as its child (cache disabled, the plan's
   // stripped lowering, a fill plan)
   PredCache* pc = nullptr;
@@ -525,11 +526,17 @@ static std::shared_ptr<const std::vector<uint64_t>> percentiles_table(const Spli
   return p;
 }
 
-static uint32_t use_col(Lowered& L, const SplitDev& sp, uint32_t c) {
+// The DCol index of image column c. A column first used by an aggregation node (agg) counts against the aggregations'
+// own QW_MAX_AGG_COLS, any other against the QW_MAX_DCOLS of the query and the sort.
+static uint32_t use_col(Lowered& L, const SplitDev& sp, uint32_t c, bool agg = false) {
   if (c == 0xFFFFFFFFu) return c;
   if (c >= sp.view.hdr->num_columns) fail(QWGPU_EINVALID_ARG, "plan references column %u (split has %u)", c, sp.view.hdr->num_columns);
   if (L.col_map[c] >= 0) return (uint32_t)L.col_map[c];
-  if (L.cols.size() >= QW_MAX_DCOLS) fail(QWGPU_EUNSUPPORTED, "plan uses more than %d columns", QW_MAX_DCOLS);
+  if (agg) {
+    if (L.n_agg_cols >= QW_MAX_AGG_COLS)
+      fail(QWGPU_EUNSUPPORTED, "aggregations use more than %u columns besides those of the query and sort", QW_MAX_AGG_COLS);
+    L.n_agg_cols++;
+  } else if (L.cols.size() - L.n_agg_cols >= QW_MAX_DCOLS) fail(QWGPU_EUNSUPPORTED, "plan uses more than %d columns", QW_MAX_DCOLS);
   const QwImgColumn& ic = sp.view.columns[c];
   DCol d;
   d.values_off = ic.values_off; d.index_off = ic.index_off; d.min_value = ic.min_value; d.gcd = ic.gcd;
@@ -995,11 +1002,13 @@ static void lower_plan(Lowered& L, const SplitDev& sp, const uint8_t* plan, size
   else if (ks.kind[0] == QW_SORT_DOCID && ks.kind[1] == QW_SORT_NONE && ks.doc_bits >= 11) ks.top_mode = QW_TOP_DOC;
   else ks.top_mode = QW_TOP_FULL;
   // aggregations
-  if (ph->num_aggs > QW_MAX_DAGGS) fail(QWGPU_EUNSUPPORTED, "more than %d aggregation nodes", QW_MAX_DAGGS);
+  if (ph->num_aggs > QW_MAX_AGG_NODES) fail(QWGPU_EUNSUPPORTED, "more than %u aggregation nodes", QW_MAX_AGG_NODES);
   for (uint32_t i = 0; i < ph->num_aggs; i++) {
     uint32_t depth = 0;
     for (uint32_t p = aggs[i].parent; p != 0xFFFFFFFFu; p = aggs[p].parent)
       if (p >= ph->num_aggs || ++depth > ph->num_aggs) fail(QWGPU_EINVALID_ARG, "aggregation parent out of range");
+    // (the hashed walk keeps one stack frame per level)
+    if (depth >= QW_MAX_AGG_LEVELS) fail(QWGPU_EUNSUPPORTED, "aggregations nested more than %u levels deep", QW_MAX_AGG_LEVELS);
   }
   std::vector<uint32_t> bases(ph->num_aggs, 0);
   P.hashed = qw_agg_hashed(aggs, ph->num_aggs) ? 1u : 0u;
@@ -1010,7 +1019,7 @@ static void lower_plan(Lowered& L, const SplitDev& sp, const uint8_t* plan, size
     DAgg d;
     memset(&d, 0, sizeof d);
     d.kind = a.kind; d.parent = a.parent; d.first_child = a.first_child; d.num_children = a.num_children;
-    d.col = use_col(L, sp, a.column); d.num_buckets = a.num_buckets; d.has_bounds = a.has_bounds;
+    d.col = use_col(L, sp, a.column, true); d.num_buckets = a.num_buckets; d.has_bounds = a.has_bounds;
     d.num_ranges = a.num_ranges; d.has_missing = a.has_missing; d.cell_base = bases[i];
     d.interval = a.interval; d.offset = a.offset; d.bound_min = a.bound_min; d.bound_max = a.bound_max;
     d.base_pos = a.base_pos;
@@ -1062,7 +1071,7 @@ static void lower_plan(Lowered& L, const SplitDev& sp, const uint8_t* plan, size
     P.tr_n = a.num_buckets;
     P.tr_num_ords = std::max(sp.view.columns[a.column].dict_num_terms, 1u);
     P.tr_ord_col = L.aggs[i].col;
-    P.tr_ts_col = use_col(L, sp, a.reserved);
+    P.tr_ts_col = use_col(L, sp, a.reserved, true);
   }
   P.n_cols = (uint32_t)L.cols.size();
   // fast aggregation path: flat (no nesting) TERMS / HISTOGRAM nodes over always-present single-valued
@@ -1222,12 +1231,15 @@ static bool driver_eligible(const Lowered& L) {
   return true;
 }
 
-// match_all + flat terms / histogram aggregations, no hits: the streaming column kernel (agg_kernel.cuh). Lays out
-// its shared memory; false when a plan does not qualify or the layout does not fit.
+// match_all + 1..QA_MAX_AGGS flat terms / histogram aggregations, no hits: the streaming column kernel (agg_kernel.cuh).
+// Lays out its shared memory; false when a plan does not qualify or the layout does not fit (wider plans run on
+// k_window).
 static bool aggscan_layout(const std::vector<Lowered>& low, int max_smem_optin, qwk::ASmem* alay) {
-  uint32_t maxbits[QW_MAX_DAGGS] = {0}, a_cells = 1;
+  uint32_t maxbits[QA_MAX_AGGS] = {0}, a_cells = 1;
   for (const Lowered& L : low) {
-    if (!(L.P.n_instr == 3 && L.instrs[1].op == OP_ALL && L.P.max_hits == 0 && L.P.n_aggs > 0 && L.P.n_cells <= QA_MAX_CELLS)) return false;
+    if (!(L.P.n_instr == 3 && L.instrs[1].op == OP_ALL && L.P.max_hits == 0 && L.P.n_aggs > 0 && L.P.n_aggs <= QA_MAX_AGGS &&
+          L.P.n_cells <= QA_MAX_CELLS))
+      return false;
     for (uint32_t gi = 0; gi < L.P.n_aggs; gi++) {
       const DAgg& d = L.aggs[gi];
       const bool flat = d.parent == 0xFFFFFFFFu && d.num_children == 0 && (d.kind == QW_AGG_TERMS || d.kind == QW_AGG_HISTOGRAM) && !d.has_missing;
@@ -1238,13 +1250,13 @@ static bool aggscan_layout(const std::vector<Lowered>& low, int max_smem_optin, 
   }
   memset(alay, 0, sizeof *alay);
   Arena slot{16};
-  for (uint32_t gi = 0; gi < QW_MAX_DAGGS; gi++) alay->col_off[gi] = slot.take(maxbits[gi] ? QA_CHUNK / 8 * maxbits[gi] + 16 : 0);
+  for (uint32_t gi = 0; gi < QA_MAX_AGGS; gi++) alay->col_off[gi] = slot.take(maxbits[gi] ? QA_CHUNK / 8 * maxbits[gi] + 16 : 0);
   alay->hdr = slot.take(16);
   alay->slot_stride = slot.off;
   Arena a{16};
   alay->bars = a.take(8 * 2 * QA_SLOTS);
-  alay->atab = a.take(QW_MAX_DAGGS * sizeof(qwk::AggRow));
-  alay->bcache = a.take(QA_CW * QW_MAX_DAGGS * 16);
+  alay->atab = a.take(QA_MAX_AGGS * sizeof(qwk::AggRow));
+  alay->bcache = a.take(QA_CW * QA_MAX_AGGS * 16);
   alay->cells = a.take(a_cells * 4);
   alay->slot0 = a.take(QA_SLOTS * alay->slot_stride);
   alay->total = a.off;

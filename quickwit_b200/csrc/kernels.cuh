@@ -727,11 +727,12 @@ __device__ __forceinline__ void agg_collect_hashed(const DSplitPlan& P, const DA
   if (__shfl_sync(QW_FULL, lane == 0 && hcell_overflowed(P) ? 1u : 0u, 0)) return;
   QwAggCell* cells = (QwAggCell*)P.h_cells;
   // per level: node, value loop (k < maxv, r < nrep), next child; per lane: values [a, a + nv), parent cell, own cell
-  uint32_t node[QW_MAX_DAGGS], k[QW_MAX_DAGGS], r[QW_MAX_DAGGS], maxv[QW_MAX_DAGGS], child[QW_MAX_DAGGS];
-  uint64_t a[QW_MAX_DAGGS];
-  uint32_t nv[QW_MAX_DAGGS], parent[QW_MAX_DAGGS], cell[QW_MAX_DAGGS];
+  uint32_t node[QW_MAX_AGG_LEVELS], k[QW_MAX_AGG_LEVELS], r[QW_MAX_AGG_LEVELS], maxv[QW_MAX_AGG_LEVELS], child[QW_MAX_AGG_LEVELS];
+  uint64_t a[QW_MAX_AGG_LEVELS];
+  uint32_t nv[QW_MAX_AGG_LEVELS], parent[QW_MAX_AGG_LEVELS], cell[QW_MAX_AGG_LEVELS];
   // per lane, bit d: the lane is live at level d; bit 8 + d: level d is the `missing` bucket; bit 16 + d: the lane is
   // tight entering level d; bit 24 + d: the current key of level d keeps it tight
+  static_assert(QW_MAX_AGG_LEVELS <= 8, "flags packs four 8-bit per-level fields");
   uint32_t flags = 0;
   for (uint32_t top = 0; top < P.n_aggs; top++) {
     if (aggs[top].parent != 0xFFFFFFFFu) continue;

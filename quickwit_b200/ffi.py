@@ -45,6 +45,8 @@ KERNEL_PREDICATE_FILL = 16384
 # split's table, the largest table a split may need, the `missing` flag of an entry
 AGG_DENSE_MAX_CELLS, AGG_DENSE_MAX_TERMS = 1 << 26, 1 << 24
 HASHED_INIT_CELLS, HASHED_MAX_BYTES = 65536, 8 << 30
+# aggregation limits of one plan (qwgpu.h QWGPU_MAX_AGG_*): nodes, nesting levels, columns beside the query's and sort's
+MAX_AGG_NODES, MAX_AGG_LEVELS, MAX_AGG_COLUMNS = 32, 8, 32
 AGG_NO_PARENT, AGG_ENTRY_MISSING = 0xFFFFFFFF, 1
 # composite source nodes (qwgpu_format.h QW_AGG_COMP_*): QwAggNode.reserved flags, range_from[0] = the split's
 # `after` bound, range_to[0] = size
