@@ -54,8 +54,7 @@ struct AParams {
   const DSplitPlan* plans;
   const DCol* cols;
   const DAgg* aggs;
-  const uint32_t* first_work;  // prefix over splits of chunk counts; [n_splits + 1]
-  uint32_t n_splits, total_work;
+  DWorkList wl;  // (split, chunk of QA_CHUNK docs) list
   ASmem sm;
 };
 
@@ -109,36 +108,31 @@ __device__ __forceinline__ bool hist_bucket(const uint64_t* B, uint32_t nb, floa
 
 __global__ void __launch_bounds__(QA_THREADS, QA_MINB) k_aggscan(const AParams p) {
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  // col_off is indexed at run time, which puts the indexed struct in local memory: a copy of the layout keeps that to
+  // the layout instead of all of p
+  const ASmem sm = p.sm;
   const uint32_t sbase = smem_u32(qw_smem);
-  const uint32_t bars = sbase + p.sm.bars;
+  const uint32_t bars = sbase + sm.bars;
   auto bar_full = [&](uint32_t s) { return bars + 8u * s; };
   auto bar_empty = [&](uint32_t s) { return bars + 8u * (QA_SLOTS + s); };
-  uint32_t* cells = (uint32_t*)(qw_smem + p.sm.cells);
-  AggRow* atab = (AggRow*)(qw_smem + p.sm.atab);
+  uint32_t* cells = (uint32_t*)(qw_smem + sm.cells);
+  AggRow* atab = (AggRow*)(qw_smem + sm.atab);
   if (tid == 0) {
     for (uint32_t s = 0; s < QA_SLOTS; s++) { mbar_init(bar_full(s), 1); mbar_init(bar_empty(s), QA_CW); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
   __syncthreads();
-  const uint32_t w_begin = (uint32_t)(((uint64_t)p.total_work * blockIdx.x) / gridDim.x);
-  const uint32_t w_end = (uint32_t)(((uint64_t)p.total_work * (blockIdx.x + 1)) / gridDim.x);
-  uint32_t split = 0;
-  if (w_begin < w_end) {
-    uint32_t a = 0, b = p.n_splits;
-    while (b - a > 1) {
-      const uint32_t mid = (a + b) >> 1;
-      if (__ldg(p.first_work + mid) <= w_begin) a = mid; else b = mid;
-    }
-    split = a;
-  }
+  const uint32_t w_begin = qw_chunk_begin(p.wl.total_work, blockIdx.x, gridDim.x);
+  const uint32_t w_end = qw_chunk_begin(p.wl.total_work, blockIdx.x + 1, gridDim.x);
+  uint32_t split = work_split(p.wl, w_begin);
 
   if (warp == QA_CW) {
     // ================================ producer: lane = aggregation ====================================
     uint32_t cur = 0xFFFFFFFFu, n_aggs = 0, num_docs = 0, bits = 0;
     const uint8_t* src0 = nullptr;
     for (uint32_t work = w_begin, seq = 0; work < w_end; work++, seq++) {
-      while (__ldg(p.first_work + split + 1) <= work) split++;
+      while (__ldg(p.wl.first_work + split + 1) <= work) split++;
       if (split != cur) {
         cur = split;
         const DSplitPlan& P = p.plans[split];
@@ -149,27 +143,27 @@ __global__ void __launch_bounds__(QA_THREADS, QA_MINB) k_aggscan(const AParams p
           src0 = (const uint8_t*)P.data_base + c.values_off;
         }
       }
-      const uint32_t d0 = (work - __ldg(p.first_work + split)) * QA_CHUNK;
+      const uint32_t d0 = (work - __ldg(p.wl.first_work + split)) * QA_CHUNK;
       const uint32_t nd = min((uint32_t)QA_CHUNK, num_docs - d0);
       const uint32_t slot = seq % QA_SLOTS;
       mbar_wait(bar_empty(slot), ((seq / QA_SLOTS) & 1u) ^ 1u);
-      const uint32_t sl = p.sm.slot0 + slot * p.sm.slot_stride;
+      const uint32_t sl = sm.slot0 + slot * sm.slot_stride;
       const uint32_t bytes = (uint32_t)(((uint64_t)nd * bits + 127) >> 7) << 4;  // whole 16-byte words (the array is padded)
       uint32_t total = bytes;
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) total += __shfl_xor_sync(QW_FULL, total, o);
       if (lane == 0) {
-        *(uint4*)(qw_smem + sl + p.sm.hdr) = make_uint4(split, d0, nd, 0u);
+        *(uint4*)(qw_smem + sl + sm.hdr) = make_uint4(split, d0, nd, 0u);
         asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar_full(slot)), "r"(total) : "memory");
       }
       __syncwarp();
-      if (bytes) bulk_g2s(sbase + sl + p.sm.col_off[lane & (QA_MAX_AGGS - 1)], src0 + ((uint64_t)d0 * bits >> 3), bytes, bar_full(slot));
+      if (bytes) bulk_g2s(sbase + sl + sm.col_off[lane & (QA_MAX_AGGS - 1)], src0 + ((uint64_t)d0 * bits >> 3), bytes, bar_full(slot));
     }
   } else {
     // ================================ consumers =====================================================
     uint32_t cur_split = 0xFFFFFFFFu, n_aggs = 0;
     unsigned long long my_docs = 0;  // thread 0 counts the docs of the current split
-    uint4* bcache = (uint4*)(qw_smem + p.sm.bcache) + warp * QA_MAX_AGGS;  // {lo, hi, bucket, valid} per aggregation
+    uint4* bcache = (uint4*)(qw_smem + sm.bcache) + warp * QA_MAX_AGGS;  // {lo, hi, bucket, valid} per aggregation
     auto enter_split = [&](uint32_t next) {
       // all consumer warps have added their counts of the old split: named barrier over the consumers
       asm volatile("bar.sync 1, %0;" ::"n"(QA_CW * 32) : "memory");
@@ -180,7 +174,7 @@ __global__ void __launch_bounds__(QA_THREADS, QA_MINB) k_aggscan(const AParams p
           const uint32_t v = cells[i];
           if (v) atomicAdd((unsigned long long*)&out[i].count, (unsigned long long)v);
         }
-        if (tid == 0 && my_docs) atomicAdd((unsigned long long*)P.out_num_hits, my_docs);
+        if (tid == 0) flush_counts(P, P.sa.present, P.max_hits, my_docs, 0);
       }
       my_docs = 0;
       cur_split = next;
@@ -203,8 +197,8 @@ __global__ void __launch_bounds__(QA_THREADS, QA_MINB) k_aggscan(const AParams p
     for (uint32_t work = w_begin, seq = 0; work < w_end; work++, seq++) {
       const uint32_t slot = seq % QA_SLOTS;
       mbar_wait(bar_full(slot), (seq / QA_SLOTS) & 1u);
-      const uint32_t sl = p.sm.slot0 + slot * p.sm.slot_stride;
-      const uint4 h = *(const uint4*)(qw_smem + sl + p.sm.hdr);
+      const uint32_t sl = sm.slot0 + slot * sm.slot_stride;
+      const uint4 h = *(const uint4*)(qw_smem + sl + sm.hdr);
       if (h.x != cur_split) enter_split(h.x);
       const uint32_t nd = h.z;
       if (tid == 0) my_docs += nd;
@@ -214,7 +208,7 @@ __global__ void __launch_bounds__(QA_THREADS, QA_MINB) k_aggscan(const AParams p
       for (uint32_t gi = 0; gi < n_aggs; gi++) {
         const uint4 r0 = *(const uint4*)&atab[gi];  // kind, bits, cell_base, nb
         const uint32_t bits = r0.y;
-        const uint32_t* w = (const uint32_t*)(qw_smem + sl + p.sm.col_off[gi]) + g * bits;
+        const uint32_t* w = (const uint32_t*)(qw_smem + sl + sm.col_off[gi]) + g * bits;
         uint32_t* ctr = cells + r0.z;
         if (r0.x == QW_AGG_HISTOGRAM) {
           uint32_t mn = 0xFFFFFFFFu, mx = 0;

@@ -38,6 +38,23 @@ QW_HOST_DEVICE uint32_t qw_cand_cap(uint32_t K) { return K <= QW_MAX_TOPK ? (uin
 // chunk [qw_chunk_begin(total, b, grid), qw_chunk_begin(total, b + 1, grid)).
 QW_HOST_DEVICE uint32_t qw_chunk_begin(uint32_t total, uint32_t b, uint32_t grid) { return (uint32_t)(((uint64_t)total * b) / grid); }
 
+// A strided threshold sample takes every stride-th item of each split (window; k_driver: posting block), starting at
+// item s % stride of split s (at item 0 when stride is 1). Work item k of split s is its item qw_sample_item(k, s,
+// stride); a split of n items has qw_sample_count(n, s, stride) work items. The host sizes the work list with the
+// one and the kernels walk it with the other, so the two must agree.
+QW_HOST_DEVICE uint32_t qw_sample_item(uint32_t k, uint32_t s, uint32_t stride) { return k * stride + (stride > 1 ? s % stride : 0u); }
+QW_HOST_DEVICE uint32_t qw_sample_count(uint32_t n, uint32_t s, uint32_t stride) {
+  const uint32_t phase = stride > 1 ? s % stride : 0u;
+  return n > phase ? (n - phase + stride - 1) / stride : 0u;
+}
+
+// The flat (split, item) list a persistent launch walks
+struct DWorkList {
+  const uint32_t* first_work;  // prefix over splits of their (sampled) item counts; [n_splits + 1]
+  uint32_t n_splits, total_work;
+  uint32_t stride;             // threshold sample: every stride-th item (qw_sample_item; 1 = every item)
+};
+
 // The threshold sample of a BM25-union collect pass that samples itself (k_union<MODE_SAMPLE_COLLECT>): the first
 // window of every block's chunk of the flat window list. first_work: prefix over the n splits of their windows
 // ([n + 1]); max_hits: per split. True when the pass may run: at least 4 windows per block, and every split that
@@ -245,10 +262,7 @@ struct KParams {
   const DCol* cols;
   const DAgg* aggs;
   DThresh* thresh;
-  const uint32_t* first_work;  // prefix over splits of (sampled) window counts; [n_splits + 1]
-  uint32_t n_splits;
-  uint32_t total_work;
-  uint32_t stride;   // sampling stride over windows (1 = all)
+  DWorkList wl;      // (split, window) list; sampled passes: the sampled windows
   uint32_t W;        // window size in docs (<= 32768; a power of two, except 15360 in BM25-union batches)
   uint32_t level;    // MODE_HIST: radix level being histogrammed
   uint32_t use_prefix;  // MODE_HIST: restrict to docs whose key matches thresh prefix

@@ -25,10 +25,8 @@ struct DrvParams {
   const DInstr* instrs;
   const DCol* cols;
   const DThresh* thresh;
-  const uint32_t* first_work;  // prefix over splits of the driving term's block counts; [n_splits + 1]
-  uint32_t n_splits, total_work;
+  DWorkList wl;                // (split, posting block of the driving term) list; sampled passes: the sampled blocks
   uint32_t level, use_prefix;  // MODE_HIST
-  uint32_t stride;             // threshold sample: work item k of split s = block k * stride + s % stride (1 = every block)
 };
 
 template <int MODE>
@@ -37,26 +35,18 @@ __global__ void __launch_bounds__(QD_WARPS * 32) k_driver(const DrvParams p) {
   __shared__ unsigned long long s_cnt[2];  // hits, eligible of the current split
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   // this block's chunk of the flat (split, posting block) list
-  const uint32_t w_begin = (uint32_t)(((uint64_t)p.total_work * blockIdx.x) / gridDim.x);
-  const uint32_t w_end = (uint32_t)(((uint64_t)p.total_work * (blockIdx.x + 1)) / gridDim.x);
+  const uint32_t w_begin = qw_chunk_begin(p.wl.total_work, blockIdx.x, gridDim.x);
+  const uint32_t w_end = qw_chunk_begin(p.wl.total_work, blockIdx.x + 1, gridDim.x);
   if (w_begin >= w_end) return;
-  uint32_t split = 0;
-  {
-    uint32_t a = 0, b = p.n_splits;
-    while (b - a > 1) {
-      const uint32_t mid = (a + b) >> 1;
-      if (__ldg(p.first_work + mid) <= w_begin) a = mid; else b = mid;
-    }
-    split = a;
-  }
+  uint32_t split = work_split(p.wl, w_begin);
   if (MODE == MODE_HIST) for (uint32_t i = tid; i < QW_HIST_BINS; i += QD_WARPS * 32) s_hist[i] = 0;
   if (tid < 2) s_cnt[tid] = 0;
   __syncthreads();
 
   for (uint32_t seg = w_begin; seg < w_end;) {
-    while (__ldg(p.first_work + split + 1) <= seg) split++;
-    const uint32_t fw = __ldg(p.first_work + split);
-    const uint32_t seg_end = min(w_end, __ldg(p.first_work + split + 1));
+    while (__ldg(p.wl.first_work + split + 1) <= seg) split++;
+    const uint32_t fw = __ldg(p.wl.first_work + split);
+    const uint32_t seg_end = min(w_end, __ldg(p.wl.first_work + split + 1));
     const DSplitPlan& P = p.plans[split];
     const DKeySpec& ks = P.key;
     const DCol* cols = p.cols + P.col_base;
@@ -76,7 +66,7 @@ __global__ void __launch_bounds__(QD_WARPS * 32) k_driver(const DrvParams p) {
     uint32_t my_hits = 0, my_elig = 0;
 
     for (uint32_t w = seg + warp; w < seg_end; w += QD_WARPS) {
-      const uint32_t bb = (w - fw) * p.stride + (p.stride > 1 ? split % p.stride : 0);
+      const uint32_t bb = qw_sample_item(w - fw, split, p.wl.stride);
       const uint8_t* blk = tdata + __ldg(&skips[bb].byte_off);
       const BlkHdr h = blk_header<LdgLoad>(blk);
       uint32_t doc[4], tf[4] = {1, 1, 1, 1};
@@ -100,30 +90,9 @@ __global__ void __launch_bounds__(QD_WARPS * 32) k_driver(const DrvParams p) {
         float sc = 0.0f;
         if (scored && on) sc = __fmul_rn(term.f, tf_factor(tab, tf[j], (fnw >> (8 * j)) & 0xFFu));
         if (MODE == MODE_COLLECT) {
-          if (!on) continue;
-          if (sa_present) {
-            const DocKey dk = doc_key(P, ks, cols, base, doc[j], sc);
-            if (dk.eligible) {
-              my_elig++;
-              if (key_ge(dk.key, thr)) push_cand(P, dk.key);
-            }
-          } else if (key_top11(P, ks, cols, base, doc[j], sc) >= thr_top) {
-            const DocKey dk = doc_key(P, ks, cols, base, doc[j], sc);
-            if (key_ge(dk.key, thr)) push_cand(P, dk.key);
-          }
-        } else {
-          uint32_t digit = 0;
-          bool ranked = false;
-          if (on) {
-            if (p.level == 0 && !sa_present) { digit = key_top11(P, ks, cols, base, doc[j], sc); ranked = true; }
-            else {
-              const DocKey dk = doc_key(P, ks, cols, base, doc[j], sc);
-              ranked = dk.eligible && (!p.use_prefix || key_prefix_eq(dk.key, T.key, T.prefix_bits));
-              digit = key_digit(dk.key, p.level);
-            }
-          }
-          warp_count_uniform(s_hist, digit, ranked, lane);
-        }
+          uint32_t top;
+          if (on) my_elig += rank_collect(P, ks, cols, base, doc[j], sc, sa_present, thr, thr_top, top);
+        } else rank_hist(s_hist, P, ks, cols, base, doc[j], sc, on, sa_present, p.level, p.use_prefix, T, lane);
       }
     }
 
@@ -142,19 +111,10 @@ __global__ void __launch_bounds__(QD_WARPS * 32) k_driver(const DrvParams p) {
     __syncthreads();
     if (MODE == MODE_COLLECT) {
       if (tid == 0) {
-        const unsigned long long hits = s_cnt[0];
-        if (hits) atomicAdd((unsigned long long*)P.out_num_hits, hits);
-        const unsigned long long elig = sa_present ? s_cnt[1] : (max_hits ? hits : 0ull);  // without search_after every hit is eligible
-        if (elig) atomicAdd((unsigned long long*)P.out_num_hits + 1, elig);
+        flush_counts(P, sa_present, max_hits, s_cnt[0], s_cnt[1]);
         s_cnt[0] = s_cnt[1] = 0;
       }
-    } else {
-      uint32_t* gh = (uint32_t*)P.out_hist;
-      for (uint32_t i = tid; i < QW_HIST_BINS; i += QD_WARPS * 32) {
-        const uint32_t c = s_hist[i];
-        if (c) { atomicAdd(&gh[i], c); s_hist[i] = 0; }
-      }
-    }
+    } else flush_hist(P, s_hist, 1, true, tid, QD_WARPS * 32);
     __syncthreads();
     seg = seg_end;
   }

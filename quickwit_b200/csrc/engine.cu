@@ -1317,9 +1317,9 @@ static void plan_sample(Route& r, const std::vector<Lowered>& low, int sm_count)
     r.fw_drv.assign(n + 1, 0);
     r.fw_dsm.assign(n + 1, 0);
     for (uint32_t i = 0; i < n; i++) {
-      const uint32_t nb = low[i].empty ? 0u : low[i].instrs[1].n, phase = r.stride > 1 ? i % r.stride : 0;
+      const uint32_t nb = low[i].empty ? 0u : low[i].instrs[1].n;
       r.fw_drv[i + 1] = r.fw_drv[i] + nb;
-      r.fw_dsm[i + 1] = r.fw_dsm[i] + (nb > phase ? (nb - phase + r.stride - 1) / r.stride : 0);
+      r.fw_dsm[i + 1] = r.fw_dsm[i] + qw_sample_count(nb, i, r.stride);
     }
   }
   // the generic kernels sample an explicit window list: strided windows + the first and last window of each
@@ -1329,16 +1329,16 @@ static void plan_sample(Route& r, const std::vector<Lowered>& low, int sm_count)
   r.fw_all.assign(n + 1, 0);
   r.fw_smp.assign(n + 1, 0);
   for (uint32_t i = 0; i < n; i++) {
-    const uint32_t nw = windows(low[i], r.W_h), phase = r.stride > 1 ? i % r.stride : 0;
+    const uint32_t nw = windows(low[i], r.W_h);
     r.fw_all[i + 1] = r.fw_all[i] + windows(low[i], r.W);
-    if (r.edge_sample) {
+    if (r.edge_sample) {  // (stride > 1)
       uint32_t cnt = 0;
       for (uint32_t w = 0; w < nw; w++) {
-        const bool edge = w == 0 || w + 1 == nw, strided = w % r.stride == phase;
+        const bool edge = w == 0 || w + 1 == nw, strided = w % r.stride == i % r.stride;
         if (edge || strided) { r.sample_win.push_back(w | (edge ? 0x80000000u : 0u)); cnt++; }
       }
       r.fw_smp[i + 1] = r.fw_smp[i] + cnt;
-    } else r.fw_smp[i + 1] = r.fw_smp[i] + (nw > phase ? (nw - phase + r.stride - 1) / r.stride : 0);
+    } else r.fw_smp[i + 1] = r.fw_smp[i] + qw_sample_count(nw, i, r.stride);
   }
 }
 
@@ -1762,7 +1762,6 @@ struct Run {
     kp.cols = (const DCol*)(db + o_cols);
     kp.aggs = (const DAgg*)(db + o_aggs);
     kp.thresh = (DThresh*)(slot.d_scratch + s_thr);
-    kp.n_splits = n;
     kp.W = r.W;
     kp.stage_bytes = stage_bytes_for(r.W);
     // privatised aggregation counters (and the radix histogram, 8 KB) live in the staging area
@@ -1780,31 +1779,33 @@ struct Run {
   // one pass over the batch on the route's kernel when it serves the pass, else on k_window
   void launch(int mode, bool sampled, uint32_t level, uint32_t use_prefix, uint32_t flags) {
     const Route::Kind kind = (flags & F_SAMPLE) || r.serves(mode, level, use_prefix, flags) ? r.kind : Route::WINDOW;
-    const uint32_t stride = sampled ? r.stride : 1;
     auto launched = [&](uint32_t kernel) { stats.launches++; stats.kernel_mask |= kernel; };
-    if (kind == Route::DRIVER) {
+    // the pass's work list: k_driver walks posting blocks, every other kernel windows
+    const bool drv = kind == Route::DRIVER;
+    DWorkList wl;
+    wl.first_work = (const uint32_t*)(slot.d_blob + (drv ? (sampled ? o_fwds : o_fwd) : (sampled ? o_fws : o_fwa)));
+    wl.n_splits = n;
+    wl.total_work = drv ? (sampled ? r.fw_dsm[n] : r.fw_drv[n]) : (sampled ? r.fw_smp[n] : r.fw_all[n]);
+    wl.stride = sampled ? r.stride : 1;
+    if (wl.total_work == 0) return;
+    if (drv) {
       qwk::DrvParams d{};
       d.plans = kp.plans; d.instrs = kp.instrs; d.cols = kp.cols; d.thresh = kp.thresh;
-      d.first_work = (const uint32_t*)(slot.d_blob + (sampled ? o_fwds : o_fwd)); d.n_splits = n; d.total_work = sampled ? r.fw_dsm[n] : r.fw_drv[n];
-      d.level = level; d.use_prefix = use_prefix; d.stride = stride;
-      if (d.total_work == 0) return;
-      const uint32_t dgrid = std::min<uint32_t>((d.total_work + QD_WARPS - 1) / QD_WARPS, (uint32_t)(e.sm_count * 4));
+      d.wl = wl; d.level = level; d.use_prefix = use_prefix;
+      const uint32_t dgrid = std::min<uint32_t>((wl.total_work + QD_WARPS - 1) / QD_WARPS, (uint32_t)(e.sm_count * 4));
       if (mode == qwk::MODE_HIST) qwk::k_driver<qwk::MODE_HIST><<<dgrid, QD_WARPS * 32, 0, st>>>(d);
       else qwk::k_driver<qwk::MODE_COLLECT><<<dgrid, QD_WARPS * 32, 0, st>>>(d);
       launched(QWGPU_KERNEL_DRIVER);
       return;
     }
-    const uint32_t* first_work = (const uint32_t*)(slot.d_blob + (sampled ? o_fws : o_fwa));
-    const uint32_t total_work = sampled ? r.fw_smp[n] : r.fw_all[n];
-    if (total_work == 0) return;
     if (kind == Route::AGGSCAN) {
       qwk::AParams a{};
       a.plans = kp.plans; a.cols = kp.cols; a.aggs = kp.aggs;
-      a.first_work = first_work; a.n_splits = n; a.total_work = total_work;
+      a.wl = wl;
       a.sm = r.alay;
       int aocc = 1;
       CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&aocc, qwk::k_aggscan, QA_THREADS, r.alay.total));
-      const uint32_t agrid = std::min<uint32_t>(total_work, (uint32_t)(e.sm_count * std::max(aocc, 1)));
+      const uint32_t agrid = std::min<uint32_t>(wl.total_work, (uint32_t)(e.sm_count * std::max(aocc, 1)));
       qwk::k_aggscan<<<agrid, QA_THREADS, r.alay.total, st>>>(a);
       launched(QWGPU_KERNEL_AGGSCAN);
       return;
@@ -1812,12 +1813,12 @@ struct Run {
     if (kind == Route::UNION) {
       qwk::UParams u{};
       u.plans = kp.plans; u.instrs = kp.instrs; u.cols = kp.cols; u.thresh = kp.thresh;
-      u.first_work = first_work; u.n_splits = n; u.total_work = total_work; u.stride = stride; u.W = sampled ? r.W_h : r.W;
+      u.wl = wl; u.W = sampled ? r.W_h : r.W;
       u.sm = mode == qwk::MODE_HIST ? r.ulay_h : r.ulay_c;
       // cross-rank calls leave a few block slots free: the persistent grid would otherwise hold every SM's shared
       // memory, a concurrent call's NCCL kernel would take the place of one of its blocks, and that block — with its
       // static share of the windows — would only start when another one has finished (twice the kernel time)
-      const uint32_t ugrid = std::min<uint32_t>(total_work, (uint32_t)(e.sm_count * QU_MINB) - (do_gather ? 4u : 0u));
+      const uint32_t ugrid = std::min<uint32_t>(wl.total_work, (uint32_t)(e.sm_count * QU_MINB) - (do_gather ? 4u : 0u));
       if (flags & F_SAMPLE) {
         // one block per resident slot (occupancy x SMs, checked by qw_fused_sample_plan against the work): the grid
         // barrier after the sample needs every block resident, which only a cooperative launch guarantees
@@ -1834,16 +1835,14 @@ struct Run {
       return;
     }
     KParams q = kp;
-    q.first_work = first_work;
-    q.total_work = total_work;
-    q.stride = stride;
+    q.wl = wl;
     q.sample_win = (sampled && r.edge_sample) ? (const uint32_t*)(slot.d_blob + o_smp) : nullptr;
     q.level = level;
     q.use_prefix = use_prefix;
     q.rec_l0 = (flags & F_REC) ? 1 : 0;
     q.refine = (flags & F_REFINE) ? 1 : 0;
     q.cands_only = (flags & F_CANDS_ONLY) ? 1 : 0;
-    const uint32_t grid = std::min<uint32_t>(total_work, (uint32_t)(e.sm_count * occ));
+    const uint32_t grid = std::min<uint32_t>(wl.total_work, (uint32_t)(e.sm_count * occ));
     if (mode == qwk::MODE_HIST) qwk::k_window<qwk::MODE_HIST><<<grid, QW_THREADS, r.lay.total, st>>>(q);
     else if (any_hashed) qwk::k_window<qwk::MODE_COLLECT, true><<<grid, QW_THREADS, r.lay.total, st>>>(q);
     else qwk::k_window<qwk::MODE_COLLECT><<<grid, QW_THREADS, r.lay.total, st>>>(q);

@@ -824,6 +824,80 @@ __device__ __forceinline__ void agg_collect_hashed(const DSplitPlan& P, const DA
 // MODE_SAMPLE_COLLECT (k_union only): a collect pass that samples its own threshold from each block's first window
 enum { MODE_HIST = 0, MODE_COLLECT = 1, MODE_SAMPLE_COLLECT = 2 };
 
+// ---- steps every persistent kernel shares: work list, matched-doc ranking, per-split flushes -----------------
+// split of work item `work`: the last split whose first work item is <= work (empty splits share their entry)
+__device__ __forceinline__ uint32_t work_split(const DWorkList& wl, uint32_t work) {
+  uint32_t a = 0, b = wl.n_splits;
+  while (b - a > 1) {
+    const uint32_t mid = (a + b) >> 1;
+    if (__ldg(wl.first_work + mid) <= work) a = mid; else b = mid;
+  }
+  return a;
+}
+
+// MODE_HIST, called by all 32 lanes of a warp (`on`: the lane holds a matched doc): the digit at `level` of the doc's
+// key is counted when search_after (`sa`) lets the doc into the top-K and, with use_prefix, the key starts with the
+// threshold prefix fixed so far
+__device__ __forceinline__ void rank_hist(uint32_t* hist, const DSplitPlan& P, const DKeySpec& ks, const DCol* cols, const uint8_t* base,
+                                          uint32_t doc, float sc, bool on, bool sa, uint32_t level, uint32_t use_prefix,
+                                          const DThresh& T, uint32_t lane) {
+  uint32_t digit = 0;
+  bool ranked = false;
+  if (on) {
+    if (level == 0 && !sa) {
+      digit = key_top11(P, ks, cols, base, doc, sc);
+      ranked = true;
+    } else {
+      const DocKey dk = doc_key(P, ks, cols, base, doc, sc);
+      ranked = dk.eligible && (!use_prefix || key_prefix_eq(dk.key, T.key, T.prefix_bits));
+      digit = key_digit(dk.key, level);
+    }
+  }
+  warp_count_uniform(hist, digit, ranked, lane);
+}
+
+// MODE_COLLECT, one matched doc: a candidate when its key reaches the threshold `thr` (thr_top: its first 11 bits).
+// Without search_after (`sa`) the key's first 11 bits are a cheap pre-filter, and the composite key is only built for
+// docs that can reach the threshold. Returns whether search_after lets the doc into the top-K; then `top` holds the
+// first 11 bits of its key.
+__device__ __forceinline__ bool rank_collect(const DSplitPlan& P, const DKeySpec& ks, const DCol* cols, const uint8_t* base,
+                                             uint32_t doc, float sc, bool sa, const Key& thr, uint32_t thr_top, uint32_t& top) {
+  if (sa) {
+    const DocKey dk = doc_key(P, ks, cols, base, doc, sc);
+    if (!dk.eligible) return false;
+    top = (uint32_t)(dk.key.w0 >> 53);
+    if (key_ge(dk.key, thr)) push_cand(P, dk.key);
+    return true;
+  }
+  top = key_top11(P, ks, cols, base, doc, sc);
+  if (top >= thr_top) {
+    const DocKey dk = doc_key(P, ks, cols, base, doc, sc);
+    if (key_ge(dk.key, thr)) push_cand(P, dk.key);
+  }
+  return true;
+}
+
+// adds to a split's counters its matched docs and its docs eligible for the top-K: `counted` with search_after (`sa`),
+// without it every hit of a plan that asks for hits
+__device__ __forceinline__ void flush_counts(const DSplitPlan& P, bool sa, uint32_t max_hits, unsigned long long hits, unsigned long long counted) {
+  if (hits) atomicAdd((unsigned long long*)P.out_num_hits, hits);
+  const unsigned long long elig = sa ? counted : (max_hits ? hits : 0ull);
+  if (elig) atomicAdd((unsigned long long*)P.out_num_hits + 1, elig);
+}
+
+// adds `weight` x the shared histogram `sh` to the split's radix histogram, from threads tid, tid + nt, ...; clear:
+// zeroes the bins it adds
+__device__ __forceinline__ void flush_hist(const DSplitPlan& P, uint32_t* sh, uint32_t weight, bool clear, uint32_t tid, uint32_t nt) {
+  uint32_t* gh = (uint32_t*)P.out_hist;
+  for (uint32_t i = tid; i < QW_HIST_BINS; i += nt) {
+    const uint32_t v = sh[i];
+    if (v) {
+      atomicAdd(&gh[i], v * weight);
+      if (clear) sh[i] = 0;
+    }
+  }
+}
+
 // ---- warp-private helpers (each warp owns the doc sub-range [lo, lo + S) of the window) ------------
 __device__ __forceinline__ void wzero_u32(uint32_t* p, uint32_t first, uint32_t n, uint32_t lane) {
   for (uint32_t i = lane; i < n; i += 32) p[first + i] = 0;
@@ -960,21 +1034,12 @@ __global__ void __launch_bounds__(QW_THREADS, QW_MIN_BLOCKS_PER_SM) k_window(con
   uint8_t* s_stage = sm.u8(p.sm.stage);
   uint32_t loaded_split = 0xFFFFFFFFu;
 
-  const uint32_t per = (p.total_work + gridDim.x - 1) / gridDim.x;
-  const uint32_t w_begin = blockIdx.x * per;
-  const uint32_t w_end = min(w_begin + per, p.total_work);
-  uint32_t split = 0;
-  if (w_begin < w_end) {
-    uint32_t a = 0, b = p.n_splits;
-    while (b - a > 1) {
-      uint32_t mid = (a + b) >> 1;
-      if (__ldg(p.first_work + mid) <= w_begin) a = mid; else b = mid;
-    }
-    split = a;
-  }
+  const uint32_t w_begin = qw_chunk_begin(p.wl.total_work, blockIdx.x, gridDim.x);
+  const uint32_t w_end = qw_chunk_begin(p.wl.total_work, blockIdx.x + 1, gridDim.x);
+  uint32_t split = work_split(p.wl, w_begin);
 
   for (uint32_t work = w_begin; work < w_end; work++) {
-    while (__ldg(p.first_work + split + 1) <= work) split++;
+    while (__ldg(p.wl.first_work + split + 1) <= work) split++;
     // sampled passes with an explicit window list: the strided sample plus the first and last window of every
     // split (keys that follow doc order — doc id, timestamps of time-ordered logs — have their best K there);
     // a strided window stands for `stride` windows in the histogram, an edge window for itself
@@ -982,8 +1047,8 @@ __global__ void __launch_bounds__(QW_THREADS, QW_MIN_BLOCKS_PER_SM) k_window(con
     if (p.sample_win) {
       const uint32_t e = __ldg(p.sample_win + work);
       window = e & 0x7FFFFFFFu;
-      hist_weight = (e >> 31) ? 1u : p.stride;
-    } else window = (work - __ldg(p.first_work + split)) * p.stride + (p.stride > 1 ? split % p.stride : 0);
+      hist_weight = (e >> 31) ? 1u : p.wl.stride;
+    } else window = qw_sample_item(work - __ldg(p.wl.first_work + split), split, p.wl.stride);
     if (p.refine) {
       // second-chance passes: verified splits are final, and a window whose best level-0 digit is
       // below the threshold digit cannot hold a candidate (block-uniform tests)
@@ -1332,11 +1397,8 @@ __global__ void __launch_bounds__(QW_THREADS, QW_MIN_BLOCKS_PER_SM) k_window(con
       // hit count: one popc per bitmap word
       if (!p.cands_only) for (uint32_t wd = tid; wd < NW; wd += QW_THREADS) my_hits += __popc(res[wd]);
       auto slow_path = [&](uint32_t i, float sc) {
-        DocKey dk = doc_key(P, ks, s_cols, base, ws + i, sc);
-        if (dk.eligible) {
-          my_elig++;
-          if (key_ge(dk.key, thr)) push_cand(P, dk.key);
-        }
+        uint32_t top;
+        rank_collect(P, ks, s_cols, base, ws + i, sc, false, thr, thr_top, top);
       };
       if (max_hits && ks.kind[0] == QW_SORT_SCORE && ks.order[0] == QW_ORDER_DESC && !sa_present && rscore && !n_aggs && !rec) {
         // fast path (BM25 top-K): a float lower bound of the threshold bucket filters 4 docs per lane
@@ -1364,24 +1426,8 @@ __global__ void __launch_bounds__(QW_THREADS, QW_MIN_BLOCKS_PER_SM) k_window(con
             uint32_t top = 0;
             bool ranked = false;  // eligible for the top-K (search_after may exclude matches)
             if (on) {
-              if (sa_present) {
-                const DocKey dk = doc_key(P, ks, s_cols, base, doc, sc);
-                if (dk.eligible) {
-                  ranked = true;
-                  my_elig++;
-                  top = (uint32_t)(dk.key.w0 >> 53);
-                  if (key_ge(dk.key, thr)) push_cand(P, dk.key);
-                }
-              } else {
-                // cheap pre-filter on the key's first 11 bits; the composite key is only built for docs
-                // that can reach the threshold
-                ranked = true;
-                top = key_top11(P, ks, s_cols, base, doc, sc);
-                if (top >= thr_top) {
-                  const DocKey dk = doc_key(P, ks, s_cols, base, doc, sc);
-                  if (key_ge(dk.key, thr)) push_cand(P, dk.key);
-                }
-              }
+              ranked = rank_collect(P, ks, s_cols, base, doc, sc, sa_present, thr, thr_top, top);
+              my_elig += ranked;
             }
             if (rec) {
               warp_count_uniform(s_l0, top, ranked, lane);
@@ -1394,7 +1440,6 @@ __global__ void __launch_bounds__(QW_THREADS, QW_MIN_BLOCKS_PER_SM) k_window(con
             else agg_collect_doc(p, sm, P, s_aggs, s_cols, base, cells, doc, on, lane);
           }
         });
-        if (!sa_present) my_elig = 0;
       }
       // block-reduce the counters, one global atomic per window
 #pragma unroll
@@ -1416,11 +1461,7 @@ __global__ void __launch_bounds__(QW_THREADS, QW_MIN_BLOCKS_PER_SM) k_window(con
         for (uint32_t wd = tid; wd < NW && (ws >> 5) + wd < nwd; wd += QW_THREADS) ((uint32_t*)P.match_out)[(ws >> 5) + wd] = res[wd];
       }
       if (tid == 0 && !p.cands_only) {
-        const uint32_t hits = s_misc[2];
-        if (hits) atomicAdd((unsigned long long*)P.out_num_hits, (unsigned long long)hits);
-        // without search_after every hit is eligible
-        const uint32_t elig = sa_present ? s_misc[3] : (max_hits ? hits : 0);
-        if (elig) atomicAdd((unsigned long long*)P.out_num_hits + 1, (unsigned long long)elig);
+        flush_counts(P, sa_present, max_hits, s_misc[2], s_misc[3]);
         if (rec) p.wmax[work] = (uint16_t)s_misc[4];
       }
       if (fast_aggs && n_aggs && P.n_stat_cells) {
@@ -1453,39 +1494,16 @@ __global__ void __launch_bounds__(QW_THREADS, QW_MIN_BLOCKS_PER_SM) k_window(con
           if (v) { atomicAdd((unsigned long long*)&cells[i].count, (unsigned long long)v); s_hist[i] = 0; }
         }
       }
-      if (rec) {
-        uint32_t* gh = (uint32_t*)P.out_hist;
-        for (uint32_t i = tid; i < QW_HIST_BINS; i += QW_THREADS) {
-          const uint32_t v = s_l0[i];
-          if (v) atomicAdd(&gh[i], v);
-        }
-      }
+      if (rec) flush_hist(P, s_l0, 1, false, tid, QW_THREADS);
     } else {
       if (max_hits) {
         warp_for_hits(res, NW, warp, lane, s_hitq, [&](uint32_t i, bool on) {
-          const uint32_t doc = ws + i;
           const float sc = (on && rscore) ? rscore[i] : 0.0f;
-          uint32_t digit = 0;
-          bool ranked = false;
-          if (on) {
-            if (p.level == 0 && !sa_present) {
-              digit = key_top11(P, ks, s_cols, base, doc, sc);
-              ranked = true;
-            } else {
-              const DocKey dk = doc_key(P, ks, s_cols, base, doc, sc);
-              ranked = dk.eligible && (!p.use_prefix || key_prefix_eq(dk.key, T.key, T.prefix_bits));
-              digit = key_digit(dk.key, p.level);
-            }
-          }
-          warp_count_uniform(s_hist, digit, ranked, lane);
+          rank_hist(s_hist, P, ks, s_cols, base, ws + i, sc, on, sa_present, p.level, p.use_prefix, T, lane);
         });
       }
       __syncthreads();
-      uint32_t* gh = (uint32_t*)P.out_hist;
-      for (uint32_t i = tid; i < QW_HIST_BINS; i += QW_THREADS) {
-        uint32_t v = s_hist[i];
-        if (v) { atomicAdd(&gh[i], v * hist_weight); s_hist[i] = 0; }
-      }
+      flush_hist(P, s_hist, hist_weight, true, tid, QW_THREADS);
     }
   }
 }

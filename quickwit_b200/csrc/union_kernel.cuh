@@ -73,11 +73,11 @@ struct UParams {
   const DInstr* instrs;
   const DCol* cols;
   DThresh* thresh;             // COLLECT: read; SAMPLE_COLLECT: written for the host by each split's first block
-  const uint32_t* first_work;  // prefix over splits of (sampled) window counts; [n_splits + 1]
+  DWorkList wl;                   // (split, window) list; sampled passes: the sampled windows
   const uint32_t* sample_stride;  // SAMPLE_COLLECT: per split, the weight of its sample (qw_fused_sample_plan)
   uint32_t* sync;                 // SAMPLE_COLLECT: grid barrier counter, zero at launch
   uint32_t* err;                  // SAMPLE_COLLECT: set to 1 when the grid barrier timed out
-  uint32_t n_splits, total_work, stride, W;
+  uint32_t W;
   USmem sm;
 };
 
@@ -207,8 +207,8 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
   // this block's chunk of the flat (split, window) list (handing windows out one at a time from a global counter was
   // slower: consecutive windows of a block then belong to different splits, and the plan switch sits on the
   // producer's critical path)
-  const uint32_t w_begin = qw_chunk_begin(p.total_work, blockIdx.x, gridDim.x);
-  const uint32_t w_end = qw_chunk_begin(p.total_work, blockIdx.x + 1, gridDim.x);
+  const uint32_t w_begin = qw_chunk_begin(p.wl.total_work, blockIdx.x, gridDim.x);
+  const uint32_t w_end = qw_chunk_begin(p.wl.total_work, blockIdx.x + 1, gridDim.x);
 
   if (warp == QU_NCW) {
     // ================================ producer ======================================================
@@ -279,14 +279,14 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
       }
     };
     auto window_of = [&](uint32_t work, uint32_t split) {
-      return (work - __ldg(p.first_work + split)) * p.stride + (p.stride > 1 ? split % p.stride : 0);
+      return qw_sample_item(work - __ldg(p.wl.first_work + split), split, p.wl.stride);
     };
     // split of a work item: number of prefix entries <= work, minus one (lane-parallel; empty splits share their entry)
     auto split_of = [&](uint32_t work) {
       uint32_t cnt = 0;
-      for (uint32_t b0 = 0; b0 < p.n_splits; b0 += 32) {
+      for (uint32_t b0 = 0; b0 < p.wl.n_splits; b0 += 32) {
         const uint32_t i = b0 + lane;
-        cnt += __popc(__ballot_sync(QW_FULL, i < p.n_splits && __ldg(p.first_work + i) <= work));
+        cnt += __popc(__ballot_sync(QW_FULL, i < p.wl.n_splits && __ldg(p.wl.first_work + i) <= work));
       }
       return cnt - 1;
     };
@@ -338,7 +338,7 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
       uint32_t nx_split = split;
       const bool have_next = next_work < w_end;
       if (have_next) {
-        while (__ldg(p.first_work + nx_split + 1) <= next_work) nx_split++;
+        while (__ldg(p.wl.first_work + nx_split + 1) <= next_work) nx_split++;
         if (nx_split == split) load_widx(window_of(next_work, split));
       }
       for (uint32_t q0 = 0; q0 < G; q0 += 32) {
@@ -485,8 +485,7 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
       for (int o = 16; o > 0; o >>= 1) my_hits += __shfl_down_sync(QW_FULL, my_hits, o);
       if (lane == 0 && my_hits) {
         const DSplitPlan& P = p.plans[cur_split];
-        atomicAdd((unsigned long long*)P.out_num_hits, (unsigned long long)my_hits);
-        atomicAdd((unsigned long long*)P.out_num_hits + 1, (unsigned long long)my_hits);  // no search_after: every hit is eligible
+        flush_counts(P, P.sa.present, P.max_hits, my_hits, 0);
       }
       my_hits = 0;
     };
@@ -729,18 +728,14 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
             for (int j = 0; j < 4; j++) if (vv[j] > 0.0f) atomicAdd(&shist[score_digit(vv[j], scale)], 1u);
           }
           consumers_sync();
-          uint32_t* gh = (uint32_t*)P.out_hist;
-          for (uint32_t i = tid; i < QW_HIST_BINS; i += QU_NCT) {
-            const uint32_t v = shist[i];
-            if (v) atomicAdd(&gh[i], v);
-          }
+          flush_hist(P, shist, 1, false, tid, QU_NCT);
           consumers_sync();
           if (tid == 0 && !grid_barrier(p.sync, gridDim.x)) *p.err = 1;
           consumers_sync();
           // every block reads the same complete histograms: the same thresholds everywhere. The chunk touches the
           // split of its first window and at most one more (qw_fused_sample_plan: every split holds a first window).
           uint32_t split_b = split;
-          while (__ldg(p.first_work + split_b + 1) < w_end) split_b++;
+          while (__ldg(p.wl.first_work + split_b + 1) < w_end) split_b++;
           for (uint32_t k = 0; k < (split_b != split ? 2u : 1u); k++) {
             const uint32_t s = k ? split_b : split;
             const DSplitPlan& Ps = p.plans[s];
@@ -754,7 +749,7 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
             s_thr_split[tid] = s;
             s_thr_lo[tid] = thresh_s_lo(s_thr[tid], p.plans[s].key.score_scale);
             // for the host and later passes: written by the lowest block whose chunk touches the split
-            if (tid ? split_b != split : w_begin == __ldg(p.first_work + split)) p.thresh[s] = s_thr[tid];
+            if (tid ? split_b != split : w_begin == __ldg(p.wl.first_work + split)) p.thresh[s] = s_thr[tid];
           }
           consumers_sync();
           if (lane == 0) mbar_arrive(bar_empty(slot));  // the held slot goes back to the producer
@@ -774,11 +769,7 @@ __global__ void __launch_bounds__(QU_THREADS, QU_MINB) k_union(const UParams p) 
         if (lane == 0) mbar_arrive(bar_chain(end_stage));
         my_stage = end_stage + 1;
         wait_below(end_stage + 1);  // every warp has swept: the window's histogram is complete
-        uint32_t* gh = (uint32_t*)p.plans[split].out_hist;
-        for (uint32_t i = tid; i < QW_HIST_BINS; i += QU_NCT) {
-          const uint32_t v = hist[i];
-          if (v) { atomicAdd(&gh[i], v); hist[i] = 0; }
-        }
+        flush_hist(p.plans[split], hist, 1, true, tid, QU_NCT);
         __syncwarp();
         if (lane == 0) mbar_arrive(bar_chain(end_stage + 1));
         my_stage = end_stage + 2;
