@@ -111,7 +111,7 @@ struct DPhrase {
   uint32_t n_exp;       // phrase prefix: number of expansions of the last slot (0 = a plain phrase)
   uint64_t exp;         // phrase prefix: DPhraseTerm[n_exp]; phrase of more than QW_MAX_PHRASE_TERMS terms
                         // (k_phrase_long): DPhraseTerm[n_terms], the driver first, then by ascending doc_freq
-                        // (device address; while lowering, index into Lowered::phrase_ext)
+                        // (device address; an index into the plan's, then the batch's records until Run::stage)
   DPhraseTerm t[QW_MAX_PHRASE_TERMS];  // up to QW_MAX_PHRASE_TERMS terms (phrase prefix: the n_terms exact terms)
 };
 
@@ -119,11 +119,12 @@ struct DPhrase {
 struct DTermSetNode {
   uint64_t bitmap;  // device address
 };
+// Lowering numbers `node` within the plan; Run::lay_out renumbers it within the batch and sets `first_block`.
 struct DTermSetTerm {
   uint64_t data, skip;  // the term's posting blocks and skip list (device addresses)
   uint32_t nblk;        // its posting blocks
   uint32_t first_block; // prefix of nblk over the batch's term-set terms (the pre-pass's flat block list)
-  uint32_t node;        // DTermSetNode of the batch (while lowering: of the plan)
+  uint32_t node;        // DTermSetNode of the batch
   uint32_t pad;
 };
 
@@ -241,6 +242,32 @@ struct DHKey {
 #define QW_HSLOT_FULL 0xFFFFFFFDu
 
 static_assert(offsetof(DSplitPlan, key) % 16 == 0 && sizeof(DSplitPlan) % 16 == 0, "DKeySpec is read as uint4");
+
+// The head of a split's region in the call's output buffer; the split's hit list and aggregation cells follow it
+struct DSplitOut {
+  uint64_t num_hits;       // matching docs (out_num_hits)
+  uint64_t eligible;       // docs eligible for the top-K (out_num_hits + 1)
+  uint32_t n_hits;         // hits written by k_select (out_nhits)
+  uint32_t cand_count;     // candidates of the collect pass (out_cand_count)
+  uint32_t trace_replayed; // 1: k_trace_replay ran (tr_tie)
+  uint32_t hashed_cells;   // hashed cells claimed | overflow << 31 (h_ctr)
+};
+static_assert(sizeof(DSplitOut) == 32 && offsetof(DSplitOut, eligible) == 8 && offsetof(DSplitOut, n_hits) == 16 && offsetof(DSplitOut, cand_count) == 20 &&
+              offsetof(DSplitOut, trace_replayed) == 24 && offsetof(DSplitOut, hashed_cells) == 28, "split output header");
+
+// One hit of a device merge (k_merge): split = the list it came from, or the global split rank of a cross-rank merge
+struct MergedHit {
+  QwHit hit;
+  uint32_t split, pad;
+};
+// A device-merged list is [RankHeader][MergedHit x k]: the batch's merge (a rank's gather record) and the cross-rank
+// merge alike. k_merge writes n_hits; k_rank_header fills in a gather record the sums the root merge adds up
+// (collector.rs:914-974): num_hits over the batch's splits, split accounting from the host.
+struct RankHeader {
+  uint32_t n_hits, pad;
+  uint64_t num_hits, attempted, successful, n_failed, reserved[3];
+};
+static_assert(sizeof(MergedHit) == sizeof(QwHit) + 8 && sizeof(RankHeader) == 64, "merge records");
 
 struct SmemLevel {
   uint32_t req, shd, nt, cnt, msum, ssum;  // byte offsets; 0xFFFFFFFF = not allocated

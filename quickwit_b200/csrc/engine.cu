@@ -108,6 +108,22 @@ void PredCache::free_released(void* stream) {
   for (void* p : v) cudaFreeAsync(p, (cudaStream_t)stream);
 }
 
+// A run's pre-pass records (Run::lay_out): phrases of up to QW_MAX_PHRASE_TERMS terms (k_phrase) and longer ones
+// (k_phrase_long), each kernel numbering its driver blocks from 0, the phrases' records outside DPhrase, the term-set
+// nodes and their terms. Until Run::stage their addresses are offsets: DPhrase::out into the VBlk region, DPhrase::exp
+// into pext, DTermSetNode::bitmap into the bitmap region. A call slot keeps them, so that a call reuses the capacity of
+// the calls before it.
+struct PrePass {
+  std::vector<DPhrase> phr, phl;
+  std::vector<DPhraseTerm> pext;
+  std::vector<DTermSetNode> tsn;
+  std::vector<DTermSetTerm> tst;
+  // the batch's instructions whose operand `a` Run::stage sets: an offset into the VBlk or bitmap region, or the device
+  // address of a cache entry's bitmap
+  struct Operand { uint32_t instr; enum { VBLK, BITMAP, ADDR } kind; uint64_t off; };
+  std::vector<Operand> operands;
+};
+
 struct CallSlot {
   cudaStream_t stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr, ev3 = nullptr;
@@ -118,6 +134,7 @@ struct CallSlot {
   size_t scratch_cap = 0;
   uint8_t *d_out = nullptr, *h_out = nullptr;
   size_t out_cap = 0;
+  PrePass pre;
   void ensure(size_t blob, size_t scratch, size_t out) {
     if (blob > blob_cap) {
       if (d_blob) cudaFree(d_blob);
@@ -491,13 +508,15 @@ struct Lowered {
   uint64_t postings = 0, alg_bytes = 0, min_required_df = ~0ull;
   std::vector<std::pair<uint32_t, uint64_t>> range_cols;  // (col, driver df) for roofline accounting
   bool empty = false;                   // a required clause of the root cannot match in this split: no work at all
-  std::vector<DPhrase> phrases;         // phrase pre-pass descriptors (out / first_work filled per batch)
-  std::vector<uint32_t> phrase_instr;   // instruction that consumes phrases[i]
+  // Instructions whose operand `a` is a device address known only once the batch is laid out (Run::lay_out), each
+  // with what feeds it: a cache entry's bitmap (entry set), else the VBlk list of phrases[rec] (OP_PHRASE) or the
+  // bitmap of the plan's next term-set node (OP_TERM_SET)
+  struct Operand { uint32_t instr, rec; std::shared_ptr<PredEntry> entry; };
+  std::vector<Operand> operands;
+  std::vector<DPhrase> phrases;         // phrase pre-pass records (out / first_work / exp: Run::lay_out)
   std::vector<DPhraseTerm> phrase_ext;  // term records outside DPhrase: the expansions of phrase prefixes and the terms
-                                        // of long phrases (phrases[i].exp indexes it until staging)
-  std::vector<uint32_t> ts_instr;       // term-set nodes (pre-pass bitmaps): the instruction that reads each
-  std::vector<DTermSetTerm> ts_terms;   // their terms (first_block / node relative to this plan until staging)
-  uint32_t ts_blocks = 0;               // posting blocks of ts_terms
+                                        // of long phrases (phrases[i].exp indexes it)
+  std::vector<DTermSetTerm> ts_terms;   // the terms of the term-set nodes, node by node
   uint32_t tr_img_col = 0;              // find_trace_ids: the trace-id column of the image
   uint64_t h_bound = 0;                 // hashed aggregation layout: upper bound on the split's distinct cells
   uint32_t n_agg_cols = 0;              // columns of `cols` first used by an aggregation node (use_col)
@@ -506,7 +525,6 @@ struct Lowered {
   PredCache* pc = nullptr;
   bool has_cache = false;                                   // the plan holds a QW_NODE_CACHE
   std::map<uint32_t, std::shared_ptr<PredEntry>> cache_at;  // plan node -> the entry it reads (lower_node's input)
-  std::vector<std::pair<uint32_t, std::shared_ptr<PredEntry>>> cache_instr;  // instruction -> the entry it reads
   std::vector<std::shared_ptr<PredEntry>> misses;           // entries this plan fills (published after the call)
   std::shared_ptr<PredEntry> fill;                          // a fill plan: the entry its matches go to
   std::shared_ptr<Lowered> stripped;  // a plan that reads entries: its lowering without the cache (the fallback)
@@ -589,6 +607,25 @@ static uint32_t resolve_cache(Lowered& L, const SplitDev& sp, const QwPlanNode* 
     idx = c;
   }
   return idx;
+}
+
+// The children of a PHRASE, PHRASE_PREFIX or TERM_SET node `n` (`what` in errors) as terms of this split, all of one
+// field. A phrase's field keeps positions and each offset (lo) fits 32 bits; a term set's ords strictly increase.
+static std::vector<const QwImgTerm*> term_children(const SplitDev& sp, const QwPlanNode* nodes, const QwPlanNode& n, bool phrase,
+                                                   const char* what) {
+  std::vector<const QwImgTerm*> terms;
+  terms.reserve(n.num_children);
+  for (uint32_t i = 0; i < n.num_children; i++) {
+    const QwPlanNode& c = nodes[n.first_child + i];
+    if (c.kind != QW_NODE_TERM || c.term_ord >= sp.view.hdr->num_terms) fail(QWGPU_EINVALID_ARG, "%s child %u is not a term of this split", what, i);
+    const QwImgTerm& t = sp.view.terms[c.term_ord];
+    if (i && t.field_id != terms[0]->field_id) fail(QWGPU_EINVALID_ARG, "%s terms of different fields", what);
+    if (phrase && !t.pidx_off) fail(QWGPU_EINVALID_ARG, "%s over a field without positions", what);
+    if (phrase && c.lo > 0xFFFFFFFFull) fail(QWGPU_EINVALID_ARG, "%s offset out of range", what);
+    if (!phrase && i && c.term_ord <= nodes[n.first_child + i - 1].term_ord) fail(QWGPU_EINVALID_ARG, "%s children not in increasing term order", what);
+    terms.push_back(&t);
+  }
+  return terms;
 }
 
 static void lower_node(Lowered& L, const SplitDev& sp, const QwPlanNode* nodes, uint32_t nn, uint32_t idx,
@@ -718,112 +755,75 @@ static void lower_node(Lowered& L, const SplitDev& sp, const QwPlanNode* nodes, 
       L.instrs.push_back(en);
       break;
     }
-    case QW_NODE_PHRASE: {
-      // evaluated by a pre-pass (phrase_kernel.cuh) into one uncompressed posting block per block of its rarest
-      // term; the window program consumes those blocks (OP_PHRASE). Up to QW_MAX_PHRASE_TERMS terms: k_phrase, the
-      // terms inline in DPhrase::t. Longer: k_phrase_long, the terms in phrase_ext, the driver first and then by
-      // ascending doc_freq so that candidates die as early as possible (the phrase count is an intersection of
-      // position sets: the order cannot change it)
-      if (n.num_children < 2 || n.num_children > QW_MAX_PHRASE_LEN || n.first_child + n.num_children > nn)
+    case QW_NODE_PHRASE: case QW_NODE_PHRASE_PREFIX: {
+      // evaluated by a pre-pass (phrase_kernel.cuh) into one uncompressed posting block per block of its driver, the
+      // first rarest exact term; the window program consumes those blocks (OP_PHRASE). Up to QW_MAX_PHRASE_TERMS exact
+      // terms: k_phrase, the terms inline in DPhrase::t. Longer: k_phrase_long, the terms in phrase_ext, the driver
+      // first and then by ascending doc_freq so that candidates die as early as possible (the phrase count is an
+      // intersection of position sets: the order cannot change it). A phrase prefix is a phrase of its k exact terms
+      // whose last slot is a set of expansions (phrase_ext, k_phrase's suffix stage 2b), never scored.
+      const bool prefix = n.kind == QW_NODE_PHRASE_PREFIX;
+      if (!prefix && (n.num_children < 2 || n.num_children > QW_MAX_PHRASE_LEN || n.first_child + n.num_children > nn))
         fail(QWGPU_EINVALID_ARG, "phrase node with %u terms", n.num_children);
-      DPhrase ph;
-      memset(&ph, 0, sizeof ph);
-      ph.data_base = (uint64_t)sp.d_data;
-      ph.n_terms = n.num_children;
-      ph.weight = n.bm25_weight;
-      ph.scored = scored ? 1 : 0;
-      uint64_t best_df = ~0ull;
-      const QwImgField* fld = nullptr;
-      uint32_t field_id = 0;
-      std::vector<std::pair<uint64_t, DPhraseTerm>> terms;  // (doc_freq, record) in phrase order
-      for (uint32_t k = 0; k < n.num_children; k++) {
-        const QwPlanNode& c = nodes[n.first_child + k];
-        if (c.kind != QW_NODE_TERM || c.term_ord >= sp.view.hdr->num_terms) fail(QWGPU_EINVALID_ARG, "phrase term %u is not a term of this split", k);
-        const QwImgTerm& t = sp.view.terms[c.term_ord];
-        if (!t.pidx_off) fail(QWGPU_EINVALID_ARG, "phrase over a field without positions");
-        if (k && t.field_id != field_id) fail(QWGPU_EINVALID_ARG, "phrase terms of different fields");
-        field_id = t.field_id;
-        fld = &sp.view.fields[t.field_id];
-        DPhraseTerm pt;
-        memset(&pt, 0, sizeof pt);
-        pt.data_off = t.data_off; pt.skip_off = t.skip_off; pt.pos_off = t.pos_off; pt.pidx_off = t.pidx_off;
-        pt.nblk = t.num_blocks; pt.offset = (uint32_t)c.lo;
-        terms.push_back({t.doc_freq, pt});
-        if (t.doc_freq < best_df) { best_df = t.doc_freq; ph.driver = k; }
-        L.alg_bytes += t.data_len - t.fn_len;
+      const uint32_t k = prefix ? (uint32_t)n.lo : n.num_children;
+      if (prefix) {
+        if (n.lo < 1 || n.lo >= QW_MAX_PHRASE_TERMS || n.num_children <= k || n.first_child + n.num_children > nn)
+          fail(QWGPU_EINVALID_ARG, "phrase prefix node with %llu exact terms and %u children", (unsigned long long)n.lo, n.num_children);
+        if (n.num_children - k > QW_MAX_PREFIX_EXPANSIONS)
+          fail(QWGPU_EUNSUPPORTED, "phrase prefix with %u expansions (the GPU path takes at most %d)", n.num_children - k, QW_MAX_PREFIX_EXPANSIONS);
+        if (scored)
+          fail(QWGPU_EUNSUPPORTED, "phrase prefix in a scoring clause of a query ranked by _score is not implemented on the GPU path");
       }
-      const QwImgTerm& drv = sp.view.terms[nodes[n.first_child + ph.driver].term_ord];
-      if (n.num_children <= QW_MAX_PHRASE_TERMS) {
-        for (uint32_t k = 0; k < n.num_children; k++) ph.t[k] = terms[k].second;
-      } else {
-        // a stable sort keeps the first rarest term (the driver above) in front
-        std::stable_sort(terms.begin(), terms.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
-        ph.exp = L.phrase_ext.size();
-        ph.driver = 0;
-        for (const auto& x : terms) L.phrase_ext.push_back(x.second);
-      }
-      L.postings += drv.doc_freq;
-      L.alg_bytes += (uint64_t)drv.doc_freq * 4 * n.num_children;  // positions probed per candidate (lower bound)
-      if (occur == QW_OCCUR_MUST || occur == QW_OCCUR_FILTER) L.min_required_df = std::min<uint64_t>(L.min_required_df, drv.doc_freq);
-      ph.fn_off = (fld->flags & QW_FIELD_HAS_FIELDNORMS) ? fld->fieldnorm_off : ~0ull;
-      ph.tab = (uint64_t)(sp.d_tabs + (size_t)(256 + QW_TFF_ROWS * 256) * field_id);
-      in.op = OP_PHRASE;
-      in.c = drv.skip_off;
-      in.n = drv.num_blocks;
-      in.f = n.bm25_weight;
-      if (scored) L.score_max += n.bm25_weight > 0 ? n.bm25_weight : 0.f;
-      L.phrase_instr.push_back((uint32_t)L.instrs.size());
-      L.phrases.push_back(ph);
-      L.instrs.push_back(in);
-      break;
-    }
-    case QW_NODE_PHRASE_PREFIX: {
-      // the phrase pre-pass over the k exact terms (the rarest drives) plus its suffix stage over the E expansions
-      // (phrase_kernel.cuh 2b); consumed like a phrase (OP_PHRASE), never scored
-      const uint32_t k = (uint32_t)n.lo;
-      if (n.lo < 1 || n.lo >= QW_MAX_PHRASE_TERMS || n.num_children <= k || n.first_child + n.num_children > nn)
-        fail(QWGPU_EINVALID_ARG, "phrase prefix node with %llu exact terms and %u children", (unsigned long long)n.lo, n.num_children);
-      const uint32_t n_exp = n.num_children - k;
-      if (n_exp > QW_MAX_PREFIX_EXPANSIONS)
-        fail(QWGPU_EUNSUPPORTED, "phrase prefix with %u expansions (the GPU path takes at most %d)", n_exp, QW_MAX_PREFIX_EXPANSIONS);
-      if (scored)
-        fail(QWGPU_EUNSUPPORTED, "phrase prefix in a scoring clause of a query ranked by _score is not implemented on the GPU path");
+      const std::vector<const QwImgTerm*> terms = term_children(sp, nodes, n, true, prefix ? "phrase prefix" : "phrase");
+      for (uint32_t i = k + 1; i < n.num_children; i++)
+        if (nodes[n.first_child + i].lo != nodes[n.first_child + k].lo) fail(QWGPU_EINVALID_ARG, "phrase prefix expansions at different offsets");
+      const uint32_t field_id = terms[0]->field_id;
+      const QwImgField& fld = sp.view.fields[field_id];
+      const float weight = prefix ? 0.f : n.bm25_weight;
       DPhrase ph;
       memset(&ph, 0, sizeof ph);
       ph.data_base = (uint64_t)sp.d_data;
       ph.n_terms = k;
-      ph.n_exp = n_exp;
-      ph.exp = L.phrase_ext.size();
-      ph.fn_off = ~0ull;
+      ph.n_exp = n.num_children - k;
+      ph.weight = weight;
+      ph.scored = scored ? 1 : 0;
+      ph.fn_off = !prefix && (fld.flags & QW_FIELD_HAS_FIELDNORMS) ? fld.fieldnorm_off : ~0ull;
+      if (!prefix) ph.tab = (uint64_t)(sp.d_tabs + (size_t)(256 + QW_TFF_ROWS * 256) * field_id);
       uint64_t best_df = ~0ull;
-      uint32_t field_id = 0;
       for (uint32_t i = 0; i < n.num_children; i++) {
-        const QwPlanNode& c = nodes[n.first_child + i];
-        if (c.kind != QW_NODE_TERM || c.term_ord >= sp.view.hdr->num_terms) fail(QWGPU_EINVALID_ARG, "phrase prefix child %u is not a term of this split", i);
-        const QwImgTerm& t = sp.view.terms[c.term_ord];
-        if (!t.pidx_off) fail(QWGPU_EINVALID_ARG, "phrase prefix over a field without positions");
-        if (i && t.field_id != field_id) fail(QWGPU_EINVALID_ARG, "phrase prefix terms of different fields");
-        if (i > k && c.lo != nodes[n.first_child + k].lo) fail(QWGPU_EINVALID_ARG, "phrase prefix expansions at different offsets");
-        if (c.lo > 0xFFFFFFFFull) fail(QWGPU_EINVALID_ARG, "phrase prefix offset out of range");
-        field_id = t.field_id;
-        DPhraseTerm pt;
-        pt.data_off = t.data_off; pt.skip_off = t.skip_off; pt.pos_off = t.pos_off; pt.pidx_off = t.pidx_off;
-        pt.nblk = t.num_blocks; pt.offset = (uint32_t)c.lo;
-        if (i < k) {
-          ph.t[i] = pt;
-          if (t.doc_freq < best_df) { best_df = t.doc_freq; ph.driver = i; }
-        } else L.phrase_ext.push_back(pt);
-        L.alg_bytes += t.data_len - t.fn_len;
+        if (i < k && terms[i]->doc_freq < best_df) { best_df = terms[i]->doc_freq; ph.driver = i; }
+        L.alg_bytes += terms[i]->data_len - terms[i]->fn_len;
       }
-      const QwImgTerm& drv = sp.view.terms[nodes[n.first_child + ph.driver].term_ord];
+      const QwImgTerm& drv = *terms[ph.driver];
+      auto rec = [&](uint32_t i) {
+        const QwImgTerm& t = *terms[i];
+        DPhraseTerm pt;
+        memset(&pt, 0, sizeof pt);
+        pt.data_off = t.data_off; pt.skip_off = t.skip_off; pt.pos_off = t.pos_off; pt.pidx_off = t.pidx_off;
+        pt.nblk = t.num_blocks; pt.offset = (uint32_t)nodes[n.first_child + i].lo;
+        return pt;
+      };
+      ph.exp = L.phrase_ext.size();  // the records outside DPhrase: a long phrase's terms, a prefix's expansions
+      if (k <= QW_MAX_PHRASE_TERMS) {
+        for (uint32_t i = 0; i < k; i++) ph.t[i] = rec(i);
+      } else {
+        // a stable sort keeps the first rarest term (the driver above) in front
+        std::vector<uint32_t> order(k);
+        for (uint32_t i = 0; i < k; i++) order[i] = i;
+        std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return terms[a]->doc_freq < terms[b]->doc_freq; });
+        for (uint32_t i : order) L.phrase_ext.push_back(rec(i));
+        ph.driver = 0;
+      }
+      for (uint32_t i = k; i < n.num_children; i++) L.phrase_ext.push_back(rec(i));
       L.postings += drv.doc_freq;
       L.alg_bytes += (uint64_t)drv.doc_freq * 4 * n.num_children;  // positions probed per candidate (lower bound)
       if (occur == QW_OCCUR_MUST || occur == QW_OCCUR_FILTER) L.min_required_df = std::min<uint64_t>(L.min_required_df, drv.doc_freq);
       in.op = OP_PHRASE;
       in.c = drv.skip_off;
       in.n = drv.num_blocks;
-      in.f = 0.f;
-      L.phrase_instr.push_back((uint32_t)L.instrs.size());
+      in.f = weight;
+      if (scored) L.score_max += weight > 0 ? weight : 0.f;
+      L.operands.push_back({(uint32_t)L.instrs.size(), (uint32_t)L.phrases.size(), nullptr});
       L.phrases.push_back(ph);
       L.instrs.push_back(in);
       break;
@@ -835,31 +835,24 @@ static void lower_node(Lowered& L, const SplitDev& sp, const QwPlanNode* nodes, 
         fail(QWGPU_EINVALID_ARG, "term set node with %u terms", n.num_children);
       if (scored)
         fail(QWGPU_EUNSUPPORTED, "term set (regex) in a scoring clause of a query ranked by _score is not implemented on the GPU path");
+      // the plan's term-set nodes are numbered in order (every node holds a term)
+      const uint32_t node = L.ts_terms.empty() ? 0 : L.ts_terms.back().node + 1;
       uint64_t df = 0;
-      uint32_t field_id = 0;
-      for (uint32_t i = 0; i < n.num_children; i++) {
-        const QwPlanNode& c = nodes[n.first_child + i];
-        if (c.kind != QW_NODE_TERM || c.term_ord >= sp.view.hdr->num_terms) fail(QWGPU_EINVALID_ARG, "term set child %u is not a term of this split", i);
-        if (i && c.term_ord <= nodes[n.first_child + i - 1].term_ord) fail(QWGPU_EINVALID_ARG, "term set children not in increasing term order");
-        const QwImgTerm& t = sp.view.terms[c.term_ord];
-        if (i && t.field_id != field_id) fail(QWGPU_EINVALID_ARG, "term set terms of different fields");
-        field_id = t.field_id;
+      for (const QwImgTerm* t : term_children(sp, nodes, n, false, "term set")) {
         DTermSetTerm r;
         memset(&r, 0, sizeof r);
-        r.data = (uint64_t)(sp.d_data + t.data_off);
-        r.skip = (uint64_t)(sp.d_data + t.skip_off);
-        r.nblk = t.num_blocks;
-        r.first_block = L.ts_blocks;
-        r.node = (uint32_t)L.ts_instr.size();
-        L.ts_blocks += t.num_blocks;
+        r.data = (uint64_t)(sp.d_data + t->data_off);
+        r.skip = (uint64_t)(sp.d_data + t->skip_off);
+        r.nblk = t->num_blocks;
+        r.node = node;
         L.ts_terms.push_back(r);
-        df += t.doc_freq;
-        L.alg_bytes += t.data_len - t.fn_len;
+        df += t->doc_freq;
+        L.alg_bytes += t->data_len - t->fn_len;
       }
       L.postings += df;
       if (occur == QW_OCCUR_MUST || occur == QW_OCCUR_FILTER) L.min_required_df = std::min<uint64_t>(L.min_required_df, std::min<uint64_t>(df, sp.view.hdr->num_docs));
       in.op = OP_TERM_SET;
-      L.ts_instr.push_back((uint32_t)L.instrs.size());
+      L.operands.push_back({(uint32_t)L.instrs.size(), 0, nullptr});
       L.instrs.push_back(in);
       break;
     }
@@ -867,7 +860,7 @@ static void lower_node(Lowered& L, const SplitDev& sp, const QwPlanNode* nodes, 
       // a subtree read from its predicate-cache entry (resolve_cache acquired it): the entry's doc bitmap, consumed
       // like a term set's (OP_TERM_SET); a miss is filled by the call's fill pass first
       in.op = OP_TERM_SET;
-      L.cache_instr.push_back({(uint32_t)L.instrs.size(), L.cache_at.at(idx)});
+      L.operands.push_back({(uint32_t)L.instrs.size(), 0, L.cache_at.at(idx)});
       L.instrs.push_back(in);
       break;
     }
@@ -1482,15 +1475,10 @@ struct Run {
   std::vector<Split> at;
   bool any_topk, any_deep, any_trace, any_hashed, any_composite, any_fast_aggs;
   uint32_t kmax, deep_cap, tie_max_n;
-  uint32_t n_phrases, phrase_blocks;            // k_phrase: phrases of up to QW_MAX_PHRASE_TERMS terms, their driver blocks
-  uint32_t n_phrases_long, phrase_blocks_long;  // k_phrase_long: the longer phrases
-  size_t n_phrase_ext;                          // DPhraseTerm records outside DPhrase (Lowered::phrase_ext)
-  bool any_prefix;                              // a phrase prefix: k_phrase<true>
-  uint32_t n_ts_nodes, n_ts_terms, ts_blocks;  // term-set pre-pass: nodes, terms and posting blocks of the batch
-  size_t o_tsn, o_tst, s_tsbm, ts_bm_bytes;    // its records (blob) and bitmaps (scratch, one region)
-  std::vector<size_t> ts_bm;                    // per split: offset of its first bitmap from s_tsbm
-  size_t o_plans, o_instr, o_cols, o_aggs, o_fwa, o_fws, o_sstr, o_bounds, o_rank, o_smp, o_phr, o_phl, o_pext, o_fwd, o_fwds, blob_bytes;
-  size_t s_thr, s_hist, s_state, s_wmax, s_sync, s_cand, s_surv, s_deep_m, s_hits, s_cut, s_grecv, s_vblk, s_trace_state, s_trace_data, s_hash, scratch_bytes;
+  PrePass& pre = slot.pre;  // the batch's pre-pass records
+  size_t ts_bm_bytes;  // the bitmap region (term-set nodes)
+  size_t o_plans, o_instr, o_cols, o_aggs, o_fwa, o_fws, o_sstr, o_bounds, o_rank, o_smp, o_phr, o_phl, o_pext, o_tsn, o_tst, o_fwd, o_fwds, blob_bytes;
+  size_t s_thr, s_hist, s_state, s_wmax, s_sync, s_cand, s_surv, s_deep_m, s_hits, s_cut, s_grecv, s_vblk, s_tsbm, s_trace_state, s_trace_data, s_hash, scratch_bytes;
   size_t rec_bytes, o_merged, o_ghdr, o_final, o_err, out_bytes;
   // the collect pass samples its own threshold (qw_fused_sample_plan): its cooperative grid and per-split sample weights
   bool self_sample;
@@ -1502,6 +1490,15 @@ struct Run {
   int occ;
   float main_ms;  // device time of the run's collect passes
 
+  // the work items of k_phrase (pre.phr) or k_phrase_long (pre.phl): the driver blocks of their phrases
+  uint32_t phrase_work(const std::vector<DPhrase>& v) const {
+    if (v.empty()) return 0;
+    const DPhrase& p = v.back();
+    return p.first_work + (p.n_terms > QW_MAX_PHRASE_TERMS ? pre.pext[p.exp] : p.t[p.driver]).nblk;
+  }
+  // the work items of k_term_set: the posting blocks of its terms
+  uint32_t term_set_work() const { return pre.tst.empty() ? 0 : pre.tst.back().first_block + pre.tst.back().nblk; }
+
   // at_bound: every hashed table is sized at its bound (the re-run after an overflow), else at
   // min(bound, QWGPU_HASHED_INIT_CELLS) cells
   void lay_out(bool at_bound) {
@@ -1510,15 +1507,12 @@ struct Run {
     at.assign(n, Split{});
     any_topk = any_deep = any_trace = any_hashed = any_composite = any_fast_aggs = false;
     kmax = 1;
-    deep_cap = 0;
-    n_phrases = phrase_blocks = n_phrases_long = phrase_blocks_long = tie_max_n = 0;
-    n_phrase_ext = 0;
-    any_prefix = false;
-    n_ts_nodes = n_ts_terms = ts_blocks = 0;
+    deep_cap = tie_max_n = 0;
+    pre.phr.clear(); pre.phl.clear(); pre.pext.clear(); pre.tsn.clear(); pre.tst.clear(); pre.operands.clear();
     ts_bm_bytes = 0;
-    ts_bm.assign(n, 0);
-  h_keys.assign(n, {});
-  h_cells.assign(n, {});
+    size_t vblk_bytes = 0;
+    h_keys.assign(n, {});
+    h_cells.assign(n, {});
     uint32_t tot_instr = 0, tot_cols = 0, tot_aggs = 0, tot_bounds = 0;
     for (uint32_t i = 0; i < n; i++) {
       const Lowered& L = low[i];
@@ -1536,20 +1530,37 @@ struct Run {
         P.h_cap = (uint32_t)(at_bound ? L.h_bound : std::min<uint64_t>(L.h_bound, QWGPU_HASHED_INIT_CELLS));
         P.h_mask = agg_hashed_slots(P.h_cap) - 1;
       }
-      // phrases: one uncompressed posting block per block of each phrase's driver term (phrase_kernel.cuh)
-      for (size_t k = 0; k < L.phrases.size(); k++) {
-        const bool lng = L.phrases[k].n_terms > QW_MAX_PHRASE_TERMS;
-        (lng ? n_phrases_long : n_phrases)++;
-        (lng ? phrase_blocks_long : phrase_blocks) += L.instrs[L.phrase_instr[k]].n;
-        any_prefix |= L.phrases[k].n_exp != 0;
+      // the plan's pre-pass records in the batch's numbering
+      const uint64_t pext0 = pre.pext.size();
+      const uint32_t node0 = (uint32_t)pre.tsn.size();
+      pre.pext.insert(pre.pext.end(), L.phrase_ext.begin(), L.phrase_ext.end());
+      for (DTermSetTerm t : L.ts_terms) {
+        t.first_block = term_set_work();
+        t.node += node0;
+        pre.tst.push_back(t);
       }
-      n_phrase_ext += L.phrase_ext.size();
-      // term sets: one doc bitmap per node
-      ts_bm[i] = ts_bm_bytes;
-      ts_bm_bytes += L.ts_instr.size() * (size_t)((P.num_docs + 31) / 32) * 4;
-      n_ts_nodes += (uint32_t)L.ts_instr.size();
-      n_ts_terms += (uint32_t)L.ts_terms.size();
-      ts_blocks += L.ts_blocks;
+      for (const Lowered::Operand& f : L.operands) {
+        const uint32_t instr = P.instr_base + f.instr;
+        if (f.entry) {
+          pre.operands.push_back({instr, PrePass::Operand::ADDR, (uint64_t)f.entry->d_bits});
+        } else if (L.instrs[f.instr].op == OP_TERM_SET) {
+          // a term set: one doc bitmap
+          pre.operands.push_back({instr, PrePass::Operand::BITMAP, ts_bm_bytes});
+          pre.tsn.push_back(DTermSetNode{ts_bm_bytes});
+          ts_bm_bytes += (size_t)((P.num_docs + 31) / 32) * 4;
+        } else {
+          // a phrase: one uncompressed posting block per block of its driver term (phrase_kernel.cuh)
+          std::vector<DPhrase>& v = L.phrases[f.rec].n_terms > QW_MAX_PHRASE_TERMS ? pre.phl : pre.phr;
+          const uint32_t first_work = phrase_work(v);
+          v.push_back(L.phrases[f.rec]);
+          DPhrase& ph = v.back();
+          ph.first_work = first_work;
+          ph.out = vblk_bytes;
+          ph.exp += pext0;
+          vblk_bytes += (size_t)L.instrs[f.instr].n * sizeof(VBlk);
+          pre.operands.push_back({instr, PrePass::Operand::VBLK, ph.out});
+        }
+      }
       kmax = std::max(kmax, P.max_hits);
       any_topk |= P.max_hits > 0;
       if (P.max_hits > QW_MAX_TOPK) { any_deep = true; deep_cap = std::max(deep_cap, qw_cand_cap(P.max_hits)); }
@@ -1580,15 +1591,15 @@ struct Run {
     o_bounds = blob.take((size_t)tot_bounds * 8);
     o_rank = blob.take((size_t)n * 4);
     o_smp = blob.take(r.sample_win.size() * 4);
-    o_phr = blob.take((size_t)n_phrases * sizeof(DPhrase));
-    o_phl = blob.take((size_t)n_phrases_long * sizeof(DPhrase));
-    o_pext = blob.take(n_phrase_ext * sizeof(DPhraseTerm));
-    o_tsn = blob.take((size_t)n_ts_nodes * sizeof(DTermSetNode));
-    o_tst = blob.take((size_t)n_ts_terms * sizeof(DTermSetTerm));
+    o_phr = blob.take(pre.phr.size() * sizeof(DPhrase));
+    o_phl = blob.take(pre.phl.size() * sizeof(DPhrase));
+    o_pext = blob.take(pre.pext.size() * sizeof(DPhraseTerm));
+    o_tsn = blob.take(pre.tsn.size() * sizeof(DTermSetNode));
+    o_tst = blob.take(pre.tst.size() * sizeof(DTermSetTerm));
     o_fwd = blob.take(r.fw_drv.size() * 4);
     o_fwds = blob.take(r.fw_dsm.size() * 4);
     blob_bytes = blob.off;
-    rec_bytes = do_merge ? 64 + (size_t)merge->k * sizeof(qwk::DMergedHit) : 0;  // a rank's gather record
+    rec_bytes = do_merge ? sizeof(RankHeader) + (size_t)merge->k * sizeof(MergedHit) : 0;  // a merged list
     Arena s{256};
     s_thr = s.take(n * sizeof(DThresh));
     s_hist = s.take((size_t)n * QW_HIST_BINS * 4);
@@ -1605,7 +1616,7 @@ struct Run {
     s_hits = s.take(do_merge ? (size_t)n * kmax * sizeof(QwHit) : 0);
     s_cut = s.take((size_t)std::max<uint32_t>(n, 64) * 4 + 1024);  // split merge's cut, then the gathered merge's
     s_grecv = s.take(gather && gather->world > 1 && do_merge ? (size_t)gather->world * rec_bytes : 0);
-    s_vblk = s.take((size_t)(phrase_blocks + phrase_blocks_long) * sizeof(VBlk));
+    s_vblk = s.take(vblk_bytes);
     // term-set bitmaps: beyond s_cand, since the exact top-K path clears the prefix again after the pre-pass
     s_tsbm = s.take(ts_bm_bytes);
     // find_trace_ids: per split a DTraceState (one region, set to 0xFF bytes), then best[] + match bitmap (zeroed)
@@ -1628,12 +1639,11 @@ struct Run {
     scratch_bytes = s.off;
     Arena o{256};
     for (uint32_t i = 0; i < n; i++)
-      at[i].out = o.take(32 + out_hit_bytes(plans[i], do_merge) + (size_t)plans[i].n_cells * sizeof(QwAggCell));
-    // [RankHeader 64 B (n_hits first)][DMergedHit x k]: the batch's merged top-k = this rank's gather record
-    o_merged = o.take(rec_bytes);
+      at[i].out = o.take(sizeof(DSplitOut) + out_hit_bytes(plans[i], do_merge) + (size_t)plans[i].n_cells * sizeof(QwAggCell));
+    o_merged = o.take(rec_bytes);  // the batch's merged top-k = this rank's gather record
     if (do_gather) {
-      o_ghdr = o.take((size_t)gather->world * 64);  // (compacted copy of the gathered headers)
-      o_final = o.take(16 + (size_t)merge->k * sizeof(qwk::DMergedHit));
+      o_ghdr = o.take((size_t)gather->world * sizeof(RankHeader));  // (compacted copy of the gathered headers)
+      o_final = o.take(rec_bytes);
     }
     o_err = o.take(self_sample ? 4 : 0);  // 1: the grid barrier timed out
     out_bytes = o.off;
@@ -1661,82 +1671,46 @@ struct Run {
     const GatherSpec& g = *gather;
     uint8_t* g_recv = slot.d_scratch + s_grecv;
     if (g.allgather(g.comm, slot.d_out + o_merged, g_recv, rec_bytes, (void*)st)) fail(QWGPU_EINTERNAL, "ncclAllGather failed");
-    const qwk::SrcGathered gsrc{g_recv, (uint32_t)rec_bytes, 64u};
+    const qwk::SrcGathered gsrc{g_recv, (uint32_t)rec_bytes, (uint32_t)sizeof(RankHeader)};
     uint32_t* g_cut = (uint32_t*)(slot.d_scratch + s_cut) + std::max<uint32_t>(n, 64);
     qwk::k_merge_prep<qwk::SrcGathered><<<1, 1024, 0, st>>>(gsrc, (uint32_t)g.world, m.k, m.order1, m.order2, g_cut);
+    RankHeader* fin = (RankHeader*)(slot.d_out + o_final);
     qwk::k_merge<qwk::SrcGathered><<<(uint32_t)(((uint64_t)g.world * m.k * 32 + 255) / 256), 256, 0, st>>>(gsrc, g_cut, (uint32_t)g.world, m.k, m.k, m.order1, m.order2,
-                                                                                    (qwk::DMergedHit*)(slot.d_out + o_final + 16), (uint32_t*)(slot.d_out + o_final));
-    CUDA_CHECK(cudaMemcpy2DAsync(slot.d_out + o_ghdr, 64, g_recv, rec_bytes, 64, (size_t)g.world, cudaMemcpyDeviceToDevice, st));
+                                                                                    (MergedHit*)(fin + 1), &fin->n_hits);
+    CUDA_CHECK(cudaMemcpy2DAsync(slot.d_out + o_ghdr, sizeof(RankHeader), g_recv, rec_bytes, sizeof(RankHeader), (size_t)g.world, cudaMemcpyDeviceToDevice, st));
     CUDA_CHECK(cudaMemcpyAsync(slot.h_out + o_ghdr, slot.d_out + o_ghdr, out_bytes - o_ghdr, cudaMemcpyDeviceToHost, st));
   }
 
   // the run's plans get the slot's addresses; everything the kernels read goes to the device in one copy
   void stage() {
     uint8_t *hb = slot.h_blob, *db = slot.d_blob;
-    uint32_t phr_done = 0, phl_done = 0, phr_blocks_done = 0, phl_blocks_done = 0, vblk_done = 0;
-    uint32_t tsn_done = 0, tst_done = 0, tsb_done = 0;
-    size_t pext_done = 0;
     for (uint32_t i = 0; i < n; i++) {
       const Lowered& L = low[i];
       DSplitPlan& P = plans[i];
       any_fast_aggs |= P.fast_aggs != 0;
       if (P.tr_on) tie_max_n = std::max(tie_max_n, P.tr_n);
-      uint8_t* ob = slot.d_out + at[i].out;
-      P.out_num_hits = (uint64_t)ob;            // [0] hits, [1] eligible
-      P.out_nhits = (uint64_t)(ob + 16);
-      P.out_cand_count = (uint64_t)(ob + 20);
-      P.out_hits = do_merge ? (uint64_t)(slot.d_scratch + s_hits + (size_t)i * kmax * sizeof(QwHit)) : (uint64_t)(ob + 32);
-      P.out_cells = (uint64_t)(ob + 32 + out_hit_bytes(P, do_merge));
+      DSplitOut* ob = (DSplitOut*)(slot.d_out + at[i].out);
+      P.out_num_hits = (uint64_t)&ob->num_hits;  // (the eligible count follows)
+      P.out_nhits = (uint64_t)&ob->n_hits;
+      P.out_cand_count = (uint64_t)&ob->cand_count;
+      P.out_hits = do_merge ? (uint64_t)(slot.d_scratch + s_hits + (size_t)i * kmax * sizeof(QwHit)) : (uint64_t)(ob + 1);
+      P.out_cells = (uint64_t)((uint8_t*)(ob + 1) + out_hit_bytes(P, do_merge));
       P.out_hist = (uint64_t)(slot.d_scratch + s_hist + (size_t)i * QW_HIST_BINS * 4);
       P.out_cands = (uint64_t)(slot.d_scratch + s_cand + at[i].cand);
       if (P.tr_on) {
         P.tr_state = (uint64_t)(slot.d_scratch + s_trace_state + (size_t)i * sizeof(qwk::DTraceState));
         P.tr_best = (uint64_t)(slot.d_scratch + at[i].tr_best);
         P.match_out = (uint64_t)(slot.d_scratch + at[i].tr_match);
-        P.tr_tie = (uint64_t)(ob + 24);
+        P.tr_tie = (uint64_t)&ob->trace_replayed;
       }
       if (P.hashed) {
         P.h_table = (uint64_t)(slot.d_scratch + at[i].h_table);
         P.h_keys = (uint64_t)(slot.d_scratch + at[i].h_keys);
         P.h_cells = (uint64_t)(slot.d_scratch + at[i].h_cells);
-        P.h_ctr = (uint64_t)(ob + 28);
+        P.h_ctr = (uint64_t)&ob->hashed_cells;
       }
       if (L.fill) P.match_out = (uint64_t)L.fill->d_bits;
-      DInstr* instrs = (DInstr*)(hb + o_instr) + P.instr_base;
-      memcpy(instrs, L.instrs.data(), P.n_instr * sizeof(DInstr));
-      for (const auto& c : L.cache_instr) instrs[c.first].a = (uint64_t)c.second->d_bits;
-      // short and long phrases go to their own kernel's array, each numbering its driver blocks from 0
-      for (size_t k = 0; k < L.phrases.size(); k++) {
-        DPhrase ph = L.phrases[k];
-        const bool lng = ph.n_terms > QW_MAX_PHRASE_TERMS;
-        const uint32_t nb = instrs[L.phrase_instr[k]].n;
-        ph.first_work = lng ? phl_blocks_done : phr_blocks_done;
-        ph.out = (uint64_t)(slot.d_scratch + s_vblk + (size_t)vblk_done * sizeof(VBlk));
-        const uint32_t n_ext = ph.n_exp ? ph.n_exp : lng ? ph.n_terms : 0;
-        if (n_ext) {
-          memcpy(hb + o_pext + pext_done * sizeof(DPhraseTerm), L.phrase_ext.data() + ph.exp, (size_t)n_ext * sizeof(DPhraseTerm));
-          ph.exp = (uint64_t)(db + o_pext + pext_done * sizeof(DPhraseTerm));
-          pext_done += n_ext;
-        }
-        instrs[L.phrase_instr[k]].a = ph.out;
-        vblk_done += nb;
-        (lng ? phl_blocks_done : phr_blocks_done) += nb;
-        if (lng) memcpy(hb + o_phl + (size_t)phl_done++ * sizeof(DPhrase), &ph, sizeof ph);
-        else memcpy(hb + o_phr + (size_t)phr_done++ * sizeof(DPhrase), &ph, sizeof ph);
-      }
-      for (size_t k = 0; k < L.ts_instr.size(); k++) {
-        DTermSetNode nd;
-        nd.bitmap = (uint64_t)(slot.d_scratch + s_tsbm + ts_bm[i] + k * (size_t)((P.num_docs + 31) / 32) * 4);
-        instrs[L.ts_instr[k]].a = nd.bitmap;
-        memcpy(hb + o_tsn + (size_t)(tsn_done + k) * sizeof(DTermSetNode), &nd, sizeof nd);
-      }
-      for (DTermSetTerm t : L.ts_terms) {
-        t.first_block += tsb_done;
-        t.node += tsn_done;
-        memcpy(hb + o_tst + (size_t)tst_done++ * sizeof(DTermSetTerm), &t, sizeof t);
-      }
-      tsn_done += (uint32_t)L.ts_instr.size();
-      tsb_done += L.ts_blocks;
+      memcpy(hb + o_instr + P.instr_base * sizeof(DInstr), L.instrs.data(), P.n_instr * sizeof(DInstr));
       memcpy(hb + o_plans + i * sizeof(DSplitPlan), &P, sizeof P);
       if (P.n_cols) memcpy(hb + o_cols + P.col_base * sizeof(DCol), L.cols.data(), P.n_cols * sizeof(DCol));
       DAgg* aggs = (DAgg*)(hb + o_aggs) + P.agg_base;
@@ -1747,6 +1721,21 @@ struct Run {
           aggs[a].bounds = (uint64_t)(db + o_bounds) + (bounds_base[i] + aggs[a].bounds) * 8;
       if (!L.bounds.empty()) memcpy(hb + o_bounds + (size_t)bounds_base[i] * 8, L.bounds.data(), L.bounds.size() * 8);
     }
+    // the pre-pass records and the operands that read their output, offsets turned into addresses
+    const uint64_t vblk = (uint64_t)(slot.d_scratch + s_vblk), bm = (uint64_t)(slot.d_scratch + s_tsbm);
+    for (auto [o, v] : {std::make_pair(o_phr, &pre.phr), std::make_pair(o_phl, &pre.phl)}) {
+      DPhrase* d = (DPhrase*)(hb + o);
+      for (size_t k = 0; k < v->size(); k++) {
+        d[k] = (*v)[k];
+        d[k].out += vblk;
+        d[k].exp = (uint64_t)(db + o_pext) + d[k].exp * sizeof(DPhraseTerm);
+      }
+    }
+    if (!pre.pext.empty()) memcpy(hb + o_pext, pre.pext.data(), pre.pext.size() * sizeof(DPhraseTerm));
+    for (size_t k = 0; k < pre.tsn.size(); k++) ((DTermSetNode*)(hb + o_tsn))[k].bitmap = bm + pre.tsn[k].bitmap;
+    if (!pre.tst.empty()) memcpy(hb + o_tst, pre.tst.data(), pre.tst.size() * sizeof(DTermSetTerm));
+    for (const PrePass::Operand& f : pre.operands)
+      ((DInstr*)(hb + o_instr))[f.instr].a = f.kind == PrePass::Operand::ADDR ? f.off : (f.kind == PrePass::Operand::VBLK ? vblk : bm) + f.off;
     if (do_merge) for (uint32_t i = 0; i < n; i++) ((uint32_t*)(hb + o_rank))[i] = merge->rank[idx[i]];
     if (!r.sample_win.empty()) memcpy(hb + o_smp, r.sample_win.data(), r.sample_win.size() * 4);
     if (!r.fw_drv.empty()) { memcpy(hb + o_fwd, r.fw_drv.data(), (n + 1) * 4); memcpy(hb + o_fwds, r.fw_dsm.data(), (n + 1) * 4); }
@@ -1898,11 +1887,12 @@ struct Run {
     }
     if (do_merge) {
       uint32_t* d_cut = (uint32_t*)(slot.d_scratch + s_cut);
+      RankHeader* rec = (RankHeader*)(slot.d_out + o_merged);
       const qwk::SrcSplits src{kp.plans, (const uint32_t*)(slot.d_blob + o_rank), do_gather ? 1u : 0u};
       qwk::k_merge_prep<qwk::SrcSplits><<<1, 1024, 0, st>>>(src, n, merge->k, merge->order1, merge->order2, d_cut);
       const uint64_t threads = (uint64_t)n * kmax * 32;  // one warp per hit (warps of pruned hits leave at once)
       qwk::k_merge<qwk::SrcSplits><<<(uint32_t)((threads + 255) / 256), 256, 0, st>>>(src, d_cut, n, kmax, merge->k, merge->order1, merge->order2,
-                                                          (qwk::DMergedHit*)(slot.d_out + o_merged + 64), (uint32_t*)(slot.d_out + o_merged));
+                                                          (MergedHit*)(rec + 1), &rec->n_hits);
       stats.launches += 2;
     }
     const size_t back = do_gather ? o_ghdr : out_bytes;  // (gathering: the final hits follow in the cross-rank phase)
@@ -1918,8 +1908,8 @@ struct Run {
     for (uint32_t i = 0; i < n; i++) {
       state[i] = 0;
       if (low[i].P.max_hits == 0) continue;
-      const uint8_t* ob = slot.h_out + at[i].out;
-      const uint64_t eligible = ((const uint64_t*)ob)[1], cand = *(const uint32_t*)(ob + 20);
+      const DSplitOut& ob = *(const DSplitOut*)(slot.h_out + at[i].out);
+      const uint64_t eligible = ob.eligible, cand = ob.cand_count;
       if (cand > qw_cand_cap(low[i].P.max_hits) || cand < std::min<uint64_t>(low[i].P.max_hits, eligible)) { state[i] = 1; all = false; }
     }
     return all;
@@ -1980,25 +1970,25 @@ struct Run {
     main_ms = 0;
     CUDA_CHECK(cudaEventRecord(slot.ev0, st));
     CUDA_CHECK(cudaMemsetAsync(slot.d_scratch, 0, s_cand, st));  // thresholds, histograms, refinement state
-    if (phrase_blocks) {
+    if (const uint32_t blocks = phrase_work(pre.phr)) {
       // phrase pre-pass (inside the timed device region): every phrase of the batch becomes a posting list in
       // scratch (beyond s_cand: never cleared), read by every later pass
       uint32_t max_terms = 1;  // (over k_phrase's phrases only: a long phrase does not widen its shared memory)
-      for (const Lowered& L : low)
-        for (const DPhrase& ph : L.phrases) if (ph.n_terms <= QW_MAX_PHRASE_TERMS) max_terms = std::max(max_terms, ph.n_terms);
+      bool any_prefix = false;
+      for (const DPhrase& ph : pre.phr) { max_terms = std::max(max_terms, ph.n_terms); any_prefix |= ph.n_exp != 0; }
       const size_t psm = (size_t)QP_WARPS * QP_SMEM_WORDS(max_terms) * 4;
-      const uint32_t pgrid = (phrase_blocks + QP_WARPS - 1) / QP_WARPS;
+      const uint32_t pgrid = (blocks + QP_WARPS - 1) / QP_WARPS;
       const DPhrase* d_phr = (const DPhrase*)(slot.d_blob + o_phr);
       // the suffix stage of phrase prefixes lives in its own instantiation: plain phrases keep the lean kernel
-      if (any_prefix) qwk::k_phrase<true><<<pgrid, QP_WARPS * 32, psm, slot.stream>>>(d_phr, n_phrases, phrase_blocks, max_terms);
-      else qwk::k_phrase<false><<<pgrid, QP_WARPS * 32, psm, slot.stream>>>(d_phr, n_phrases, phrase_blocks, max_terms);
+      if (any_prefix) qwk::k_phrase<true><<<pgrid, QP_WARPS * 32, psm, slot.stream>>>(d_phr, (uint32_t)pre.phr.size(), blocks, max_terms);
+      else qwk::k_phrase<false><<<pgrid, QP_WARPS * 32, psm, slot.stream>>>(d_phr, (uint32_t)pre.phr.size(), blocks, max_terms);
       stats.launches++;
       stats.kernel_mask |= QWGPU_KERNEL_PHRASE;
     }
-    if (phrase_blocks_long) {
+    if (const uint32_t blocks = phrase_work(pre.phl)) {
       // long-phrase pre-pass (phrase_kernel.cuh): the same output, shared memory independent of the phrase length
-      qwk::k_phrase_long<<<(phrase_blocks_long + QP_WARPS - 1) / QP_WARPS, QP_WARPS * 32, 0, slot.stream>>>(
-          (const DPhrase*)(slot.d_blob + o_phl), n_phrases_long, phrase_blocks_long);
+      qwk::k_phrase_long<<<(blocks + QP_WARPS - 1) / QP_WARPS, QP_WARPS * 32, 0, slot.stream>>>(
+          (const DPhrase*)(slot.d_blob + o_phl), (uint32_t)pre.phl.size(), blocks);
       stats.launches++;
       stats.kernel_mask |= QWGPU_KERNEL_PHRASE_LONG;
     }
@@ -2007,10 +1997,10 @@ struct Run {
       // scratch, read by every later pass (cleared for every node, whether or not its terms hold a block)
       CUDA_CHECK(cudaMemsetAsync(slot.d_scratch + s_tsbm, 0, ts_bm_bytes, st));
     }
-    if (ts_blocks) {
-      const uint32_t tgrid = std::min<uint32_t>((ts_blocks + QS_WARPS - 1) / QS_WARPS, (uint32_t)e.sm_count * 8);
-      qwk::k_term_set<<<tgrid, QS_WARPS * 32, 0, st>>>((const DTermSetTerm*)(slot.d_blob + o_tst), n_ts_terms,
-                                                       (const DTermSetNode*)(slot.d_blob + o_tsn), ts_blocks);
+    if (const uint32_t blocks = term_set_work()) {
+      const uint32_t tgrid = std::min<uint32_t>((blocks + QS_WARPS - 1) / QS_WARPS, (uint32_t)e.sm_count * 8);
+      qwk::k_term_set<<<tgrid, QS_WARPS * 32, 0, st>>>((const DTermSetTerm*)(slot.d_blob + o_tst), (uint32_t)pre.tst.size(),
+                                                       (const DTermSetNode*)(slot.d_blob + o_tsn), blocks);
       stats.launches++;
       stats.kernel_mask |= QWGPU_KERNEL_TERM_SET;
     }
@@ -2045,7 +2035,7 @@ struct Run {
     else if (!sampled || !ok) exact_select(!ok && r.rec_l0, state);
     // hashed cells: a split that outgrew its capacity sends the batch round again at the bound (before any
     // cross-rank collective, which must run once); otherwise only the used cells come back
-    auto used = [&](uint32_t i) { return *(const uint32_t*)(slot.h_out + at[i].out + 28); };
+    auto used = [&](uint32_t i) { return ((const DSplitOut*)(slot.h_out + at[i].out))->hashed_cells; };
     bool overflow = false;
     for (uint32_t i = 0; i < n; i++) overflow |= plans[i].hashed && (used(i) >> 31);
     if (overflow && at_bound) fail(QWGPU_EINTERNAL, "hashed aggregation cells overflowed their bound");
@@ -2064,7 +2054,7 @@ struct Run {
         wait_call(e, slot);
       }
       if (do_gather) {
-        qwk::k_rank_header<<<1, 32, 0, st>>>(kp.plans, n, (qwk::DRankHeader*)(slot.d_out + o_merged), gather->attempted, gather->successful, gather->n_failed);
+        qwk::k_rank_header<<<1, 32, 0, st>>>(kp.plans, n, (RankHeader*)(slot.d_out + o_merged), gather->attempted, gather->successful, gather->n_failed);
         exchange();
         CUDA_CHECK(cudaEventRecord(slot.ev1, st));
         wait_call(e, slot);
@@ -2180,18 +2170,19 @@ static QwHit expand_score_hit(const QwScoreHit& s) {
 // one split's result out of its region of the copied-back buffer (and its hashed entries); P: the run's copy of
 // the split's plan
 static void unpack_split(SplitOutput& o, BatchStats& stats, const Lowered& L, const DSplitPlan& P, const SplitDev& s, const uint8_t* plan,
-                         const uint8_t* ob, bool do_merge, const std::vector<DHKey>& keys, const std::vector<QwAggCell>& cells) {
-  o.num_hits = ((const uint64_t*)ob)[0];
-  uint32_t nh = *(const uint32_t*)(ob + 16);
+                         const DSplitOut* ob, bool do_merge, const std::vector<DHKey>& keys, const std::vector<QwAggCell>& cells) {
+  o.num_hits = ob->num_hits;
+  const uint32_t nh = ob->n_hits;
+  const uint8_t* hits = (const uint8_t*)(ob + 1);
   if (!do_merge && P.score_hits) {
-    const QwScoreHit* sh = (const QwScoreHit*)(ob + 32);
+    const QwScoreHit* sh = (const QwScoreHit*)hits;
     o.hits.resize(nh);
     for (uint32_t j = 0; j < nh; j++) o.hits[j] = expand_score_hit(sh[j]);
   } else if (!do_merge) {
-    o.hits.assign((const QwHit*)(ob + 32), (const QwHit*)(ob + 32) + nh);
+    o.hits.assign((const QwHit*)hits, (const QwHit*)hits + nh);
     if (P.key.kind[0] == QW_SORT_DOCID) for (auto& h : o.hits) strip_doc_key(h);
   }
-  const QwAggCell* c = (const QwAggCell*)(ob + 32 + out_hit_bytes(P, do_merge));
+  const QwAggCell* c = (const QwAggCell*)(hits + out_hit_bytes(P, do_merge));
   o.cells.assign(c, c + P.n_cells);
   for (auto& cell : o.cells) cell.min_mapped = ~cell.min_mapped;  // device keeps max(~m); see agg_stats
   if (P.hashed) {
@@ -2209,7 +2200,7 @@ static void unpack_split(SplitOutput& o, BatchStats& stats, const Lowered& L, co
     }
   }
   if (P.tr_on) {
-    if (*(const uint32_t*)(ob + 24)) stats.kernel_mask |= QWGPU_KERNEL_TRACE_REPLAY;
+    if (ob->trace_replayed) stats.kernel_mask |= QWGPU_KERNEL_TRACE_REPLAY;
     // a matched doc without a trace id reads ordinal 0: with an empty dictionary the reference's ord_to_bytes fails
     const QwImgColumn& tc = s.view.columns[L.tr_img_col];
     for (const QwAggCell& cell : o.cells)
@@ -2238,18 +2229,16 @@ static void unpack_split(SplitOutput& o, BatchStats& stats, const Lowered& L, co
   o.algorithmic_bytes = bytes;
 }
 
-// The device merge's hits (count at `cnt`, DMergedHit records at `recs`). A batch's own merge names positions in
-// `low`, which `idx` maps back to the caller's arrays; a cross-rank merge (idx null) carries GLOBAL split ranks (the
-// caller owns the rank -> split id table), and a rank with no searchable split does not know the sort.
-static void unpack_merged(const uint8_t* cnt, const uint8_t* recs, const std::vector<Lowered>& low, const std::vector<uint32_t>* idx,
+// The hits of a device-merged list. A batch's own merge names positions in `low`, which `idx` maps back to the
+// caller's arrays; a cross-rank merge (idx null) carries GLOBAL split ranks (the caller owns the rank -> split id
+// table), and a rank with no searchable split does not know the sort.
+static void unpack_merged(const RankHeader* list, const std::vector<Lowered>& low, const std::vector<uint32_t>* idx,
                           std::vector<MergedHit>& merged) {
-  const uint32_t nm = *(const uint32_t*)cnt;
-  const qwk::DMergedHit* mh = (const qwk::DMergedHit*)recs;
-  merged.resize(nm);
-  for (uint32_t j = 0; j < nm; j++) {
-    const Lowered* L = idx ? &low[mh[j].split] : low.empty() ? nullptr : &low[0];
-    MergedHit& m = merged[j];
-    m.hit = mh[j].hit; m.split = idx ? (*idx)[mh[j].split] : mh[j].split; m.pad = 0;
+  const MergedHit* mh = (const MergedHit*)(list + 1);
+  merged.assign(mh, mh + list->n_hits);
+  for (MergedHit& m : merged) {
+    const Lowered* L = idx ? &low[m.split] : low.empty() ? nullptr : &low[0];
+    if (idx) m.split = (*idx)[m.split];
     if (L && L->P.key.kind[0] == QW_SORT_DOCID) strip_doc_key(m.hit);
   }
 }
@@ -2266,16 +2255,16 @@ static void exchange_empty(Engine& e, const MergeSpec& merge, const GatherSpec& 
   run.lay_out(false);
   run.size_slot();
   CUDA_CHECK(cudaMemsetAsync(run.slot.d_out, 0, run.out_bytes, run.st));
-  qwk::DRankHeader h{};
+  RankHeader h{};
   h.attempted = gather.attempted;
   h.successful = gather.successful;
   h.n_failed = gather.n_failed;
   CUDA_CHECK(cudaMemcpyAsync(run.slot.d_out + run.o_merged, &h, sizeof h, cudaMemcpyHostToDevice, run.st));
   run.exchange();
   wait_call(e, run.slot);
-  unpack_merged(run.slot.h_out + run.o_final, run.slot.h_out + run.o_final + 16, none, nullptr, merged);
-  rank_headers.resize(gather.world);
-  memcpy(rank_headers.data(), run.slot.h_out + run.o_ghdr, (size_t)gather.world * 64);
+  unpack_merged((const RankHeader*)(run.slot.h_out + run.o_final), none, nullptr, merged);
+  const RankHeader* hdrs = (const RankHeader*)(run.slot.h_out + run.o_ghdr);
+  rank_headers.assign(hdrs, hdrs + gather.world);
 }
 
 void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std::vector<const uint8_t*>& plans,
@@ -2364,14 +2353,14 @@ void Engine::search(const std::vector<std::shared_ptr<SplitDev>>& sp, const std:
   const auto t_searched = tclock::now();
   const uint8_t* h_out = lease.slot->h_out;
   for (uint32_t i = 0; i < low.size(); i++)
-    unpack_split(outs[idx[i]], stats, low[i], run.plans[i], *sp[idx[i]], plans[idx[i]], h_out + run.at[i].out, do_merge, run.h_keys[i], run.h_cells[i]);
+    unpack_split(outs[idx[i]], stats, low[i], run.plans[i], *sp[idx[i]], plans[idx[i]], (const DSplitOut*)(h_out + run.at[i].out), do_merge, run.h_keys[i], run.h_cells[i]);
   if (run.do_gather) {
     // the cross-rank result: hits carry GLOBAL split ranks (the caller owns the rank -> split id table)
-    unpack_merged(h_out + run.o_final, h_out + run.o_final + 16, low, nullptr, *merged);
-    rank_headers->resize(gather->world);
-    memcpy(rank_headers->data(), h_out + run.o_ghdr, (size_t)gather->world * 64);
+    unpack_merged((const RankHeader*)(h_out + run.o_final), low, nullptr, *merged);
+    const RankHeader* hdrs = (const RankHeader*)(h_out + run.o_ghdr);
+    rank_headers->assign(hdrs, hdrs + gather->world);
   } else if (do_merge) {
-    unpack_merged(h_out + run.o_merged, h_out + run.o_merged + 64, low, &idx, *merged);
+    unpack_merged((const RankHeader*)(h_out + run.o_merged), low, &idx, *merged);
   }
   if (trace) {
     // (a call re-run after a hashed overflow counts the re-run's staging in launch+wait)

@@ -11,6 +11,7 @@
 #include <vector>
 
 #include "common.h"
+#include "device_types.h"
 
 namespace qw {
 
@@ -88,19 +89,10 @@ struct MergeSpec {
   uint32_t order1 = QW_ORDER_DESC, order2 = QW_ORDER_DESC;
   std::vector<uint32_t> rank;  // per input split: rank of its split id among the batch's split ids
 };
-struct MergedHit {
-  QwHit hit;
-  uint32_t split;  // index into the caller's split array
-  uint32_t pad;
-};
 // Cross-rank exchange standing in for the root merge (SURVEY.md 8e): after the batch's own device merge the
 // rank's fixed-size record {header, best k hits tagged with GLOBAL split ranks} is all-gathered over NCCL on
 // the call's stream and the gathered lists are merged on the device again; every rank ends up with the same
 // global top-k. `allgather` is ncclAllGather bound to the context's communicator (comm.cpp).
-struct RankHeader {  // 64 bytes, written on the device
-  uint32_t n_hits, pad;
-  uint64_t num_hits, attempted, successful, n_failed, reserved[3];
-};
 struct GatherSpec {
   int world = 1, rank = 0;
   // (sendbuf, recvbuf, bytes per rank, stream) -> 0 on success

@@ -1845,26 +1845,22 @@ __device__ __forceinline__ bool mkey_gt(const MKey& a, const MKey& b) {  // a be
   if (a.v2 != b.v2) return a.v2 > b.v2;
   return a.tie > b.tie;
 }
-struct DMergedHit {
-  QwHit hit;
-  uint32_t split, pad;
-};
 // The lists a merge reads: the per-split lists of one batch (k_select output, tie-break rank per list), or
-// the per-rank merged lists gathered over NCCL (DMergedHit records that carry the global split rank).
+// the per-rank merged lists gathered over NCCL (MergedHit records that carry the global split rank).
 struct SrcSplits {
   const DSplitPlan* plans;
   const uint32_t* rank;
   uint32_t tag_rank;  // 1: output hits are tagged with the list's (global) rank instead of its index
   __device__ __forceinline__ uint32_t count(uint32_t s) const { return *(const uint32_t*)plans[s].out_nhits; }
   __device__ __forceinline__ QwHit hit(uint32_t s, uint32_t i, uint32_t& rk) const { rk = __ldg(rank + s); return ((const QwHit*)plans[s].out_hits)[i]; }
-  __device__ __forceinline__ uint32_t tag(uint32_t s, uint32_t rk) const { return tag_rank ? rk : s; }  // DMergedHit.split of an output hit
+  __device__ __forceinline__ uint32_t tag(uint32_t s, uint32_t rk) const { return tag_rank ? rk : s; }  // MergedHit.split of an output hit
 };
 struct SrcGathered {
-  const uint8_t* base;   // rank r: [uint32 n_hits ... header of hdr_bytes][DMergedHit x K]
+  const uint8_t* base;   // rank r: [RankHeader of hdr_bytes][MergedHit x K]
   uint32_t rec_bytes, hdr_bytes;
   __device__ __forceinline__ uint32_t count(uint32_t s) const { return *(const uint32_t*)(base + (size_t)s * rec_bytes); }
   __device__ __forceinline__ QwHit hit(uint32_t s, uint32_t i, uint32_t& rk) const {
-    const DMergedHit* m = (const DMergedHit*)(base + (size_t)s * rec_bytes + hdr_bytes) + i;
+    const MergedHit* m = (const MergedHit*)(base + (size_t)s * rec_bytes + hdr_bytes) + i;
     rk = m->split;
     return m->hit;
   }
@@ -1956,7 +1952,7 @@ __global__ void __launch_bounds__(1024) k_merge_prep(const Src src, uint32_t n_l
 }
 template <class Src>
 __global__ void __launch_bounds__(256) k_merge(const Src src, const uint32_t* cut, uint32_t n_lists, uint32_t kmax, uint32_t K, uint32_t o1, uint32_t o2,
-                                               DMergedHit* out, uint32_t* out_n) {
+                                               MergedHit* out, uint32_t* out_n) {
   // one warp per surviving hit; lane = one of the other lists (the binary searches of a hit run side by side). The
   // warp index is 64-bit: n_lists * kmax warps pass 2^27 (6 711 lists at K = 20 000) before the lists run out.
   const uint32_t lane = threadIdx.x & 31;
@@ -1984,16 +1980,11 @@ __global__ void __launch_bounds__(256) k_merge(const Src src, const uint32_t* cu
     r += lo;
   }
   r = __reduce_add_sync(0xFFFFFFFFu, r) + i;
-  if (lane == 0 && r < K) { DMergedHit m; m.hit = mine; m.split = src.tag(s, my_rk); m.pad = 0; out[r] = m; }
+  if (lane == 0 && r < K) { MergedHit m; m.hit = mine; m.split = src.tag(s, my_rk); m.pad = 0; out[r] = m; }
 }
 
-// Header of a rank's gather record: its hit count (already written by k_merge at offset 0) plus the sums the
-// root merge adds up (collector.rs:914-974): num_hits over the batch's splits, split accounting from the host.
-struct DRankHeader {
-  uint32_t n_hits, pad;
-  uint64_t num_hits, attempted, successful, n_failed, reserved[3];
-};
-__global__ void k_rank_header(const DSplitPlan* plans, uint32_t n_splits, DRankHeader* h, uint64_t attempted, uint64_t successful, uint64_t n_failed) {
+// The header of a rank's gather record (device_types.h), all but the hit count that k_merge has written
+__global__ void k_rank_header(const DSplitPlan* plans, uint32_t n_splits, RankHeader* h, uint64_t attempted, uint64_t successful, uint64_t n_failed) {
   if (threadIdx.x == 0 && blockIdx.x == 0) {
     uint64_t nh = 0;
     for (uint32_t s = 0; s < n_splits; s++) nh += *(const uint64_t*)plans[s].out_num_hits;

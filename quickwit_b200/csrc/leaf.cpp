@@ -822,7 +822,7 @@ int qwgpu_leaf_search_allgather_lane(qwgpu_ctx* ctx, uint32_t lane, const uint8_
   if (!run.gathered) qw::fail(QWGPU_EINTERNAL, "cross-rank merge did not run");
   uint64_t total_failed = 0;
   {
-    for (const qw::RankHeader& h : run.rank_headers) {
+    for (const RankHeader& h : run.rank_headers) {
       m.num_hits += h.num_hits;
       m.num_attempted_splits += h.attempted;
       m.num_successful_splits += h.successful;
@@ -832,7 +832,7 @@ int qwgpu_leaf_search_allgather_lane(qwgpu_ctx* ctx, uint32_t lane, const uint8_
     if (run.which.empty() && !run.merged.empty()) qw::fail(QWGPU_EUNSUPPORTED, "a rank without searchable splits cannot type the merged sort values");
     const qw::SortTypes types = run.which.empty() ? qw::SortTypes{} : qw::sort_types(run.jobs, run.which);
     m.encoded_partial_hits.reserve(run.merged.size() * 72);
-    for (const qw::MergedHit& mh : run.merged) {
+    for (const MergedHit& mh : run.merged) {
       if (mh.split >= comm.split_ids.size()) qw::fail(QWGPU_EINTERNAL, "gathered hit carries split rank %u (table has %zu)", mh.split, comm.split_ids.size());
       qw::append_hit(m.encoded_partial_hits, comm.split_ids[mh.split], mh.hit, types);
     }

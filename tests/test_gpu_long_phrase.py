@@ -12,6 +12,7 @@ from oracle import oracle as O
 from helpers import DOC_ASC, DOC_DESC, SCORE_DESC, assert_same, col_sort, terms_agg
 from long_phrase_ref import phrase_ast, values_of, windows
 from phrase_prefix_ref import GH_BODY, GH_MAPPING, GH_MSG, gharchive_docs, rewrite_as_phrases
+from regex_ref import rewrite_term_sets
 from pipeline import search_request
 
 pytestmark = pytest.mark.gpu
@@ -61,13 +62,13 @@ def edge(gpu_ctx):
 
 
 def parity(ctx, imgs, plans, label, batch=48):
-    """GPU against the oracle, `batch` plans per call; the results."""
+    """GPU against the oracle (phrase prefixes and term sets rewritten for it), `batch` plans per call; the results."""
     out = []
     for i in range(0, len(plans), batch):
         ims, ps = imgs[i:i + batch], plans[i:i + batch]
         got = ctx.split_search([im.split_id for im in ims], ps)
         for k, (g, im, p) in enumerate(zip(got, ims, ps)):
-            assert_same(g, O.split_search(im, rewrite_as_phrases(p)), ctx=f"{label} #{i + k}")
+            assert_same(g, O.split_search(im, rewrite_as_phrases(rewrite_term_sets(p))), ctx=f"{label} #{i + k}")
         out += got
     return out
 
@@ -160,6 +161,16 @@ def test_long_phrase_as_a_clause(gpu_ctx, edge):
     assert any(g.kernel_mask & ffi.KERNEL_DEEP_SELECT for g in got)
 
 
+def oracle_hits(im, clauses, k, sort):
+    """The oracle's num_hits of bool(clauses)."""
+    return O.split_search(im, rewrite_as_phrases(rewrite_term_sets(P.make_plan(P.bool_(clauses), k, sort)))).num_hits
+
+
+def oracle_hits_without_each(im, clauses, k, sort):
+    """The oracle's num_hits of bool(clauses) with each clause left out in turn."""
+    return [oracle_hits(im, clauses[:j] + clauses[j + 1:], k, sort) for j in range(len(clauses))]
+
+
 def test_mixed_batch_over_several_splits(gpu_ctx):
     imgs = [S.build_split(edge_docs(40 + i, n_filler=3000 + 500 * i, n_template=2000), MAPPING, f"long-mix-{i}")
             for i in range(3)]
@@ -171,22 +182,41 @@ def test_mixed_batch_over_several_splits(gpu_ctx):
         tmpl = lambda im: P.make_plan(P.phrase(im, "body", TEMPLATE_TOKENS, occur=ffi.OCCUR_FILTER), 100, DOC_ASC)
         prefix = lambda im: P.make_plan(P.phrase_prefix(im, "body", ["receiving", "block", "b"], 50), 100, DOC_ASC)
         ab = lambda im: P.make_plan(P.phrase(im, "body", ["a", "b", "a", "b"]), 100, SCORE_DESC)
+        ords = lambda im, words: sorted(im.term_ord("body", w) for w in words)
+        # two term-set nodes beside a phrase, numbered within the plan, then within the call. Each clause cuts the
+        # matches, and the nodes' roles differ (filter, must_not), so a bitmap left empty or read by the other node
+        # changes the result.
+        tset_clauses = lambda im: [P.phrase(im, "body", ["f1", "f2"]), P.term_set(im, "body", ords(im, ["f3", "f4", "f5", "f6"])),
+                                   P.term_set(im, "body", ords(im, ["f7"]), occur=ffi.OCCUR_MUST_NOT)]
+        tset = lambda im: P.make_plan(P.bool_(tset_clauses(im)), 100, SCORE_DESC)
         for g in parity(gpu_ctx, imgs * 2, [short(im) for im in imgs] + [ab(im) for im in imgs], "short only"):
             assert g.kernel_mask & ffi.KERNEL_PHRASE and not g.kernel_mask & ffi.KERNEL_PHRASE_LONG
         for g in parity(gpu_ctx, imgs * 2, [long_(im) for im in imgs] + [tmpl(im) for im in imgs], "long only"):
             assert g.kernel_mask & ffi.KERNEL_PHRASE_LONG and not g.kernel_mask & ffi.KERNEL_PHRASE
-        mixed_imgs = [imgs[0], imgs[1], imgs[2], imgs[0], imgs[2], imgs[1]]
-        mixed = [short(imgs[0]), long_(imgs[1]), prefix(imgs[2]), tmpl(imgs[0]), ab(imgs[2]), prefix(imgs[1])]
-        for g in parity(gpu_ctx, mixed_imgs, mixed, "mixed"):
-            assert g.kernel_mask & ffi.KERNEL_PHRASE and g.kernel_mask & ffi.KERNEL_PHRASE_LONG
-        # one plan holding a short phrase, a long phrase and a phrase prefix
+        mixed_imgs = [imgs[0], imgs[1], imgs[2], imgs[1], imgs[0], imgs[2], imgs[1], imgs[2]]
+        mixed = [short(imgs[0]), long_(imgs[1]), prefix(imgs[2]), tset(imgs[1]), tmpl(imgs[0]), ab(imgs[2]), prefix(imgs[1]),
+                 tset(imgs[2])]
+        pre_passes = ffi.KERNEL_PHRASE | ffi.KERNEL_PHRASE_LONG | ffi.KERNEL_TERM_SET
+        got = parity(gpu_ctx, mixed_imgs, mixed, "mixed")
+        for g in got:
+            assert g.kernel_mask & pre_passes == pre_passes
+        for j in (3, 7):  # the term-set plans
+            im, g = mixed_imgs[j], got[j]
+            assert g.num_hits > 0 and g.num_hits not in oracle_hits_without_each(im, tset_clauses(im), 100, SCORE_DESC)
+            swapped = tset_clauses(im)
+            swapped[1].occur, swapped[2].occur = ffi.OCCUR_MUST_NOT, ffi.OCCUR_FILTER
+            assert g.num_hits != oracle_hits(im, swapped, 100, SCORE_DESC)
+        # one plan holding a short phrase, a long phrase, a phrase prefix and a term set, each matching docs that no
+        # other clause matches
         for im in imgs:
-            root = P.bool_([P.phrase(im, "body", ["quick", "brown"], occur=ffi.OCCUR_SHOULD),
-                            P.phrase(im, "body", SENTENCE, occur=ffi.OCCUR_SHOULD),
-                            P.phrase_prefix(im, "body", ["receiving", "block", "b"], 50, occur=ffi.OCCUR_SHOULD)])
-            (g,) = parity(gpu_ctx, [im], [P.make_plan(root, 200, DOC_DESC)], "one plan")
-            assert g.kernel_mask & ffi.KERNEL_PHRASE and g.kernel_mask & ffi.KERNEL_PHRASE_LONG
+            clauses = [P.phrase(im, "body", ["a", "b"], occur=ffi.OCCUR_SHOULD),
+                       P.phrase(im, "body", SENTENCE, occur=ffi.OCCUR_SHOULD),
+                       P.phrase_prefix(im, "body", ["receiving", "block", "b"], 50, occur=ffi.OCCUR_SHOULD),
+                       P.term_set(im, "body", ords(im, ["q", "z"]), occur=ffi.OCCUR_SHOULD)]
+            (g,) = parity(gpu_ctx, [im], [P.make_plan(P.bool_(clauses), 200, DOC_DESC)], "one plan")
+            assert g.kernel_mask & pre_passes == pre_passes
             assert g.num_hits > 2000
+            assert all(h < g.num_hits for h in oracle_hits_without_each(im, clauses, 200, DOC_DESC))
     finally:
         for im in imgs:
             gpu_ctx.unregister_split(im.split_id)

@@ -159,6 +159,10 @@ def test_engine_refusals(gpu_ctx, pp_split):
     assert code(bad([kids[0], tag], 1)) == ffi.EINVALID_ARG             # terms of different fields
     shifted = P.Node(ffi.NODE_TERM, term_ord=kids[-1].term_ord, lo=2)
     assert code(bad(kids + [shifted], 1)) == ffi.EINVALID_ARG           # expansions at different offsets
+    # a term offset beyond 32 bits, in a phrase prefix and in a plain phrase
+    assert code(bad([kids[0], P.Node(ffi.NODE_TERM, term_ord=kids[-1].term_ord, lo=1 << 32)], 1)) == ffi.EINVALID_ARG
+    far = P.Node(ffi.NODE_TERM, term_ord=kids[0].term_ord, lo=1 << 32)
+    assert code(P.make_plan(P.Node(ffi.NODE_PHRASE, children=[kids[0], far]), 10, DOC_ASC)) == ffi.EINVALID_ARG
 
 
 # ---- full request paths ------------------------------------------------------------------------------------
