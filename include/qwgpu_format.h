@@ -192,9 +192,10 @@ enum {
   QW_NODE_EXISTS = 6, /* ExistsQuery on a column; const score 1 */
   QW_NODE_PHRASE = 7, /* tantivy PhraseQuery, slop 0: children = its TERM nodes in phrase order, all of one field
                          with positions, 2 <= children <= QW_MAX_PHRASE_LEN; child k's `lo` = position offset of
-                         the term inside the phrase. A doc
-                         matches when some base position b has term k at b + lo_k for every k; phrase_count =
-                         number of such b. Score = bm25_weight * tf-factor(phrase_count, fieldnorm) with
+                         the term inside the phrase, any values (tantivy PhraseQuery::new_with_offset: gapped,
+                         starting above 0, not ascending) whose spread max - min is below 2^31. A doc matches when
+                         its positions align: some integer c, which may be negative, has term k at c + lo_k for
+                         every k; phrase_count = number of such c. Score = bm25_weight * tf-factor(phrase_count, fieldnorm) with
                          bm25_weight = (sum of the terms' idf, duplicates included) * (1 + K1) * boost
                          (Bm25Weight::for_terms). */
   QW_NODE_PHRASE_PREFIX = 8, /* tantivy PhrasePrefixQuery with at least one exact term: children = the k exact TERM
@@ -202,8 +203,9 @@ enum {
                                first max_expansions terms, in byte order, that start with the prefix); the node's
                                `lo` = k; each child's `lo` = its position offset, so every expansion carries the last
                                offset. All of one field with positions; 1 <= k < QW_MAX_PHRASE_TERMS,
-                               1 <= E <= QW_MAX_PREFIX_EXPANSIONS. A doc matches when some base position b has exact
-                               term i at b + lo_i for every i and some expansion at b + lo_last. Never scored: the
+                               1 <= E <= QW_MAX_PREFIX_EXPANSIONS; offsets as in QW_NODE_PHRASE. A doc matches when
+                               its positions align: some integer c, which may be negative, has exact term i at
+                               c + lo_i for every i and some expansion at c + lo_last. Never scored: the
                                node is only valid where its score is not read (filter / must_not, or any sort
                                other than _score). */
   QW_NODE_TERM_SET = 9, /* a set of terms (tantivy AutomatonWeight of a regex query): children = E TERM nodes of one

@@ -777,6 +777,16 @@ static void lower_node(Lowered& L, const SplitDev& sp, const QwPlanNode* nodes, 
       const std::vector<const QwImgTerm*> terms = term_children(sp, nodes, n, true, prefix ? "phrase prefix" : "phrase");
       for (uint32_t i = k + 1; i < n.num_children; i++)
         if (nodes[n.first_child + i].lo != nodes[n.first_child + k].lo) fail(QWGPU_EINVALID_ARG, "phrase prefix expansions at different offsets");
+      // A doc matches when its positions align: term i at c + lo_i for one constant c, which may be negative (tantivy
+      // PhraseQuery::new_with_offset after a stop-word filter gives "a@1 b@2"). The kernels take c >= 0, so the offsets
+      // are rebased onto the smallest; then c = p - offset for every position p of a term. Refusing a spread of 2^31
+      // or more keeps the rebased offsets in 31 bits; positions within one spread of 2^32 compare modulo 2^32.
+      uint64_t lo_min = ~0ull, lo_max = 0;
+      for (uint32_t i = 0; i < n.num_children; i++) {
+        lo_min = std::min<uint64_t>(lo_min, nodes[n.first_child + i].lo);
+        lo_max = std::max<uint64_t>(lo_max, nodes[n.first_child + i].lo);
+      }
+      if (lo_max - lo_min >= (1ull << 31)) fail(QWGPU_EINVALID_ARG, "%s offsets spread over 2^31 positions or more", prefix ? "phrase prefix" : "phrase");
       const uint32_t field_id = terms[0]->field_id;
       const QwImgField& fld = sp.view.fields[field_id];
       const float weight = prefix ? 0.f : n.bm25_weight;
@@ -800,7 +810,7 @@ static void lower_node(Lowered& L, const SplitDev& sp, const QwPlanNode* nodes, 
         DPhraseTerm pt;
         memset(&pt, 0, sizeof pt);
         pt.data_off = t.data_off; pt.skip_off = t.skip_off; pt.pos_off = t.pos_off; pt.pidx_off = t.pidx_off;
-        pt.nblk = t.num_blocks; pt.offset = (uint32_t)nodes[n.first_child + i].lo;
+        pt.nblk = t.num_blocks; pt.offset = (uint32_t)(nodes[n.first_child + i].lo - lo_min);
         return pt;
       };
       ph.exp = L.phrase_ext.size();  // the records outside DPhrase: a long phrase's terms, a prefix's expansions
