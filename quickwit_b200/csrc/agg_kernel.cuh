@@ -95,17 +95,6 @@ __device__ __forceinline__ void unpack32_dyn(uint32_t bits, const uint32_t* w, F
   }
 }
 
-// bucket of a raw value through the boundary table: B[k] = smallest raw in bucket >= k, k = 0..nb
-// (same search as agg_collect_fast in kernels.cuh); false when the value lies outside [B[0], B[nb])
-__device__ __forceinline__ bool hist_bucket(const uint64_t* B, uint32_t nb, float inv_step, uint64_t b0, uint64_t bn, uint64_t raw, uint32_t& bk) {
-  if (!(raw >= b0 && raw < bn)) return false;
-  const float f = __fmul_rn((float)(raw - b0), inv_step);
-  bk = f >= (float)(nb - 1) ? nb - 1 : (uint32_t)f;
-  while (raw < __ldg(B + bk)) bk--;
-  while (raw >= __ldg(B + bk + 1)) bk++;
-  return true;
-}
-
 __global__ void __launch_bounds__(QA_THREADS, QA_MINB) k_aggscan(const AParams p) {
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   // col_off is indexed at run time, which puts the indexed struct in local memory: a copy of the layout keeps that to

@@ -279,13 +279,6 @@ std::vector<AggReq> parse_agg_request(const std::string& json) {
 }
 
 // ---- lowering ------------------------------------------------------------------------------------------
-static double mapped_to_f64(uint32_t type, uint64_t m) {
-  switch (type) {
-    case QW_COL_U64: case QW_COL_BOOL: case QW_COL_STR: case QW_COL_IP: return (double)m;
-    case QW_COL_I64: case QW_COL_DATETIME: return (double)u64_to_i64(m);
-    default: return u64_to_f64(m);
-  }
-}
 static uint64_t f64_bound_to_mapped(uint32_t type, double v) {  // smallest mapped value whose f64 is >= v
   switch (type) {
     case QW_COL_F64: return f64_to_u64(v);
@@ -347,7 +340,7 @@ static bool comp_after_bound(const QwAggNode& n, const QwImgColumn* col, const I
   if (n.kind == QW_AGG_HISTOGRAM) {
     const double unit = col->type == QW_COL_DATETIME ? 1e6 : 1.0;
     auto key = [&](int64_t p) { return comp_hist_key(n, col->type, s.kind == AggReq::DateHistogram, p); };
-    const double pos = std::floor(((k.t == CompKey::F64 ? k.f : k.t == CompKey::I64 ? (double)k.i : (double)k.u) * unit - n.offset) / n.interval);
+    const double pos = qw_hist_pos((k.t == CompKey::F64 ? k.f : k.t == CompKey::I64 ? (double)k.i : (double)k.u) * unit, n.offset, n.interval);
     if (!std::isfinite(pos) || std::fabs(pos) > 9e15) return false;
     // the position from the formula, corrected by a few steps for the rounding of key(); keys that stay equal over
     // more positions than that (an offset far larger than the interval) leave the filter to the host
@@ -512,10 +505,10 @@ static QwAggNode lower_one(const AggReq& a, const ImageView& img, AggBinding& b,
       n.offset = a.offset * scale;
       if (a.has_hard_bounds) { n.has_bounds = 1; n.bound_min = a.hard_min * scale; n.bound_max = a.hard_max * scale; }
       if (col && col->num_vals) {
-        double lo = mapped_to_f64(col->type, col->min_value), hi = mapped_to_f64(col->type, col->max_value);
+        double lo = qw_mapped_to_f64(col->type, col->min_value), hi = qw_mapped_to_f64(col->type, col->max_value);
         if (n.has_bounds) { lo = std::max(lo, n.bound_min); hi = std::min(hi, n.bound_max); }
         if (lo <= hi) {
-          double p0 = std::floor((lo - n.offset) / n.interval), p1 = std::floor((hi - n.offset) / n.interval);
+          double p0 = qw_hist_pos(lo, n.offset, n.interval), p1 = qw_hist_pos(hi, n.offset, n.interval);
           if (p1 - p0 + 1 > 65000.0 * 16) fail(QWGPU_EINVALID_AGG, "histogram would create too many buckets (%g)", p1 - p0 + 1);
           n.base_pos = (int64_t)p0;
           n.num_buckets = (uint32_t)(p1 - p0 + 1);
@@ -908,8 +901,8 @@ static IAgg metric_from_cell(const CompiledPlan& cp, const ImageView& img, const
       if (!(t == QW_COL_U64 || t == QW_COL_BOOL)) sum -= ((__int128)1 << 63) * (__int128)cell.count;
       a.m_sum = (double)sum;
     }
-    a.m_min = mapped_to_f64(t, cell.min_mapped);
-    a.m_max = mapped_to_f64(t, cell.max_mapped);
+    a.m_min = qw_mapped_to_f64(t, cell.min_mapped);
+    a.m_max = qw_mapped_to_f64(t, cell.max_mapped);
   }
   return a;
 }
@@ -1070,7 +1063,7 @@ static IAgg build_percentiles_e(const EntryCtx& c, uint32_t ni, EntryRange es) {
       const double m = b.req->missing.as_f64();
       a.sk.add(dds::bin_ord(m), x.cell.count, m, m);
     } else if (x.cell.count) {
-      a.sk.add(t.ord_lo + (int64_t)x.key, x.cell.count, dds::column_f64(col->type, x.cell.min_mapped), dds::column_f64(col->type, x.cell.max_mapped));
+      a.sk.add(t.ord_lo + (int64_t)x.key, x.cell.count, qw_mapped_to_f64(col->type, x.cell.min_mapped), qw_mapped_to_f64(col->type, x.cell.max_mapped));
     }
   }
   return a;
@@ -1185,6 +1178,53 @@ uint64_t agg_cell_layout(const QwAggNode* aggs, uint32_t n, std::vector<uint32_t
     if (total > QW_AGG_DENSE_MAX_CELLS) fail(QWGPU_EINVALID_AGG, "aggregation bucket space too large (%llu cells)", (unsigned long long)total);
   }
   return total;
+}
+
+// Hashed layout: a cell exists per (node, parent cell, key) that some (doc, value path) reaches, so a node has at
+// most min(its dense cells, the (doc, value path) tuples of its bucket chain) cells. A chain of single-valued
+// columns gives at most one path per doc; a multi-valued level multiplies by that column's value count (Σ_d Π v_l(d)
+// <= Π Σ_d v_l(d)), a `missing` bucket adds one value per doc, a range node every range.
+static uint64_t sat_mul(uint64_t a, uint64_t b) {
+  const uint64_t lim = 1ull << 62;
+  return (b && a > lim / b) ? lim : std::min(a * b, lim);
+}
+uint64_t agg_hashed_bound(const QwAggNode* aggs, uint32_t n, const ImageView& img) {
+  const uint64_t num_docs = img.hdr->num_docs;
+  uint64_t total = 0;
+  for (uint32_t i = 0; i < n; i++) {
+    uint64_t dense = 1, reps = 1, multi = 1;
+    bool any_multi = false;
+    uint32_t depth = 0;
+    for (uint32_t b = aggs[i].kind == QW_AGG_STATS ? aggs[i].parent : i; b != 0xFFFFFFFFu && depth <= n; b = aggs[b].parent, depth++) {
+      const QwAggNode& g = aggs[b];
+      dense = sat_mul(dense, g.num_buckets);
+      if (g.kind == QW_AGG_RANGE) reps = sat_mul(reps, g.num_ranges);
+      if (g.column < img.hdr->num_columns && img.columns[g.column].cardinality == QW_CARD_MULTI) {
+        any_multi = true;
+        multi = sat_mul(multi, img.columns[g.column].num_vals +
+                                   ((g.kind == QW_AGG_TERMS || g.kind == QW_AGG_HISTOGRAM || g.kind == QW_AGG_PERCENTILES) && g.has_missing ? num_docs : 0));
+      }
+    }
+    total = std::min<uint64_t>(total + std::min(dense, sat_mul(any_multi ? multi : num_docs, reps)), 1ull << 62);
+  }
+  return total;
+}
+uint32_t agg_hashed_slots(uint64_t cap) {
+  uint64_t slots = 2;
+  while (slots < 2 * cap) slots <<= 1;  // load factor <= 1/2: short probe sequences
+  return (uint32_t)std::min<uint64_t>(slots, 1ull << 31);
+}
+uint64_t agg_hashed_table_bytes(uint64_t cap) {
+  const uint64_t slots = agg_hashed_slots(cap);
+  return slots * 4 + cap * (sizeof(DHKey) + sizeof(QwAggCell));
+}
+uint64_t agg_hashed_layout(const QwAggNode* aggs, uint32_t n, const ImageView& img, const char* split_id) {
+  const uint64_t bound = std::max<uint64_t>(agg_hashed_bound(aggs, n, img), 1);
+  const uint64_t bytes = bound >= (1ull << 30) ? ~0ull : agg_hashed_table_bytes(bound);
+  if (bytes > QWGPU_HASHED_MAX_BYTES)
+    fail(QWGPU_EUNSUPPORTED, "split `%s`: the aggregation may create up to %llu buckets, whose hashed table exceeds the GPU limit of %llu bytes per call",
+         split_id, (unsigned long long)bound, (unsigned long long)QWGPU_HASHED_MAX_BYTES);
+  return bound;
 }
 
 // The entries of a dense cell array (QwAggCell doc in qwgpu_format.h), parents before children: one per nonzero cell,
@@ -1658,7 +1698,7 @@ static void fin_agg(const AggReq& req, const IAgg* a, std::string& out) {
     bool any = !by_pos.empty();
     int64_t lo = any ? by_pos.begin()->first : 0, hi = any ? by_pos.rbegin()->first : -1;
     if (req.has_extended_bounds) {
-      int64_t elo = (int64_t)std::floor((req.ext_min * unit - offset) / interval), ehi = (int64_t)std::floor((req.ext_max * unit - offset) / interval);
+      int64_t elo = (int64_t)qw_hist_pos(req.ext_min * unit, offset, interval), ehi = (int64_t)qw_hist_pos(req.ext_max * unit, offset, interval);
       if (elo <= ehi) {
         if (!any) { lo = elo; hi = ehi; any = true; }
         else { lo = std::min(lo, elo); hi = std::max(hi, ehi); }

@@ -11,6 +11,7 @@
 #include <vector>
 
 #include "../../include/qwgpu.h"
+#include "device_types.h"
 
 namespace qw {
 
@@ -29,19 +30,45 @@ struct Error : std::runtime_error {
 }
 void set_last_error(const std::string& msg);
 
-// ---- tantivy MonotonicallyMappableToU64 (tantivy-columnar; SURVEY.md Appendix A.5) -------------
-inline uint64_t i64_to_u64(int64_t v) { return (uint64_t)v ^ (1ull << 63); }
-inline int64_t u64_to_i64(uint64_t v) { return (int64_t)(v ^ (1ull << 63)); }
-inline uint64_t f64_to_u64(double d) {
-  uint64_t bits;
-  memcpy(&bits, &d, 8);
-  return (bits & (1ull << 63)) ? ~bits : (bits ^ (1ull << 63));
+// ---- raw-space boundary tables ---------------------------------------------------------------
+// The smallest raw value in [lo, hi] for which `at_least` holds, a predicate monotone in the raw value (false, then
+// true); hi itself is taken to hold and is never evaluated
+template <class F>
+inline uint64_t first_raw(uint64_t lo, uint64_t hi, F&& at_least) {
+  while (lo < hi) {
+    const uint64_t mid = lo + (hi - lo) / 2;
+    if (at_least(mid)) hi = mid; else lo = mid + 1;
+  }
+  return lo;
 }
-inline double u64_to_f64(uint64_t v) {
-  uint64_t bits = (v & (1ull << 63)) ? (v ^ (1ull << 63)) : ~v;
-  double d;
-  memcpy(&d, &bits, 8);
-  return d;
+// The boundary table of histogram node d over column c (DAgg::bounds, the fast aggregation paths): appends bounds[k]
+// for k = 0..nb, the smallest raw value in [0, max_raw + 1] whose bucket, clamped to [-1, nb], is >= k. The bucket
+// comes from qw_hist_pos as in agg_bucket, and is monotone in the raw value, so the device finds a raw value's bucket
+// in the table without f64 arithmetic and lands where agg_bucket would. max_raw = the largest raw value present:
+// searching beyond would leave the value domain (f64 columns: bit patterns past the maximum are NaNs and break the
+// order).
+inline void hist_bounds(const DCol& c, uint64_t max_raw, const DAgg& d, std::vector<uint64_t>& out) {
+  const int64_t nb = d.num_buckets;
+  auto bucket = [&](uint64_t raw) -> int64_t {
+    const unsigned __int128 wide = (unsigned __int128)c.gcd * raw + c.min_value;  // saturate beyond the column's range
+    const double val = qw_mapped_to_f64(c.type, wide > (unsigned __int128)~0ull ? ~0ull : (uint64_t)wide);
+    if (d.has_bounds) {
+      if (!(val >= d.bound_min)) return -1;
+      if (!(val <= d.bound_max)) return nb;
+    }
+    const double pos = qw_hist_pos(val, d.offset, d.interval);
+    if (!(pos >= -9.0e18)) return -1;
+    if (!(pos <= 9.0e18)) return nb;
+    const int64_t idx = (int64_t)pos - d.base_pos;
+    return idx < 0 ? -1 : (idx >= nb ? nb : idx);
+  };
+  const uint64_t raw_end = max_raw == ~0ull ? max_raw : max_raw + 1;
+  uint64_t lo = 0;
+  for (int64_t k = 0; k <= nb; k++) {
+    // (2^64 is not representable: an edge that no raw value reaches saturates at ~0)
+    lo = max_raw == ~0ull && bucket(~0ull) < k ? ~0ull : first_raw(lo, raw_end, [&](uint64_t raw) { return bucket(raw) >= k; });
+    out.push_back(lo);
+  }
 }
 
 // ---- BM25 constants (tantivy Bm25Weight; SURVEY.md Appendix A.3) -------------------------------
@@ -51,11 +78,6 @@ inline float bm25_idf(uint64_t doc_freq, uint64_t doc_count) {
   float x = ((float)(doc_count - doc_freq) + 0.5f) / ((float)doc_freq + 0.5f);
   return logf(1.0f + x);
 }
-
-// ---- dense aggregation layout (QwAggCell doc in qwgpu_format.h) ---------------------------------
-// Total cells of the plan's aggregation nodes and each node's first cell; fails above QW_AGG_DENSE_MAX_CELLS.
-// Defined in aggs.cpp: the engine lays out its cells and the host reads them back with the same bases.
-uint64_t agg_cell_layout(const QwAggNode* aggs, uint32_t n, std::vector<uint32_t>* bases);
 
 // ---- read-only view over a split image -------------------------------------------------------
 struct ImageView {
@@ -173,5 +195,18 @@ struct ImageView {
     return lo;
   }
 };
+
+// ---- aggregation cell layouts (aggs.cpp) ------------------------------------------------------
+// The engine lays out a plan's cells and the host reads them back by the same rules.
+// Dense (QwAggCell doc in qwgpu_format.h): total cells of the plan's aggregation nodes and each node's first cell;
+// fails above QW_AGG_DENSE_MAX_CELLS.
+uint64_t agg_cell_layout(const QwAggNode* aggs, uint32_t n, std::vector<uint32_t>* bases);
+// Hashed (qw_agg_hashed): guaranteed upper bound on a split's distinct cells, the table slots and device bytes of a
+// table of `cap` cells; agg_hashed_layout returns the bound and fails with QWGPU_EUNSUPPORTED when the table at the
+// bound exceeds QWGPU_HASHED_MAX_BYTES
+uint64_t agg_hashed_bound(const QwAggNode* aggs, uint32_t n, const ImageView& img);
+uint32_t agg_hashed_slots(uint64_t cap);
+uint64_t agg_hashed_table_bytes(uint64_t cap);
+uint64_t agg_hashed_layout(const QwAggNode* aggs, uint32_t n, const ImageView& img, const char* split_id);
 
 }  // namespace qw

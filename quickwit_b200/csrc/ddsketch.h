@@ -54,21 +54,11 @@ inline int64_t bin_ord(double v) {
 inline int ord_store(int64_t o) { return o < 0 ? -1 : (o > 0 ? 1 : 0); }
 inline int32_t ord_key(int64_t o) { return (int32_t)((o < 0 ? -o : o) + first_key() - 1); }
 
-// the f64 of a column value, as the stats aggregation converts it: the bit-packed raw -> mapped = min + gcd * raw
-// -> the column type's value
-inline double column_f64(uint32_t type, uint64_t mapped) {
-  switch (type) {
-    case QW_COL_I64: case QW_COL_DATETIME: return (double)u64_to_i64(mapped);
-    case QW_COL_F64: return u64_to_f64(mapped);
-    default: return (double)mapped;
-  }
-}
-
 // Boundary table of a column in raw space: the bins ord_lo .. ord_lo + edges.size() - 1 between the bins of the
 // column's minimum and maximum, empty ones included; edges[i] = the smallest raw value whose bin is >= ord_lo + i
-// (edges[0] = 0). bin_ord(column_f64(min + gcd * raw)) is monotone in raw, so each edge is a binary search, with the
-// same `log` the reference's f64::ln calls. The device finds a raw value's bin as the last edge <= raw, and never
-// evaluates a logarithm.
+// (edges[0] = 0). bin_ord(qw_mapped_to_f64(min + gcd * raw)) is monotone in raw, so each edge is a binary search
+// (first_raw), with the same `log` the reference's f64::ln calls. The device finds a raw value's bin as the last edge
+// <= raw, and never evaluates a logarithm.
 struct Table {
   int64_t ord_lo = 0;
   uint64_t num_bins = 0;
@@ -80,8 +70,8 @@ inline bool column_table(const QwImgColumn& c, bool with_edges, Table* t) {
   *t = Table();
   if (!c.num_vals) return true;
   const uint64_t gcd = c.gcd ? c.gcd : 1, max_raw = (c.max_value - c.min_value) / gcd;
-  auto ord = [&](uint64_t raw) { return bin_ord(column_f64(c.type, c.min_value + gcd * raw)); };
-  if (std::isnan(column_f64(c.type, c.min_value)) || std::isnan(column_f64(c.type, c.max_value))) return false;
+  auto ord = [&](uint64_t raw) { return bin_ord(qw_mapped_to_f64(c.type, c.min_value + gcd * raw)); };
+  if (std::isnan(qw_mapped_to_f64(c.type, c.min_value)) || std::isnan(qw_mapped_to_f64(c.type, c.max_value))) return false;
   const int64_t lo = ord(0), hi = ord(max_raw);
   if (hi - lo + 1 > kMaxTableBins) return false;
   t->ord_lo = lo;
@@ -89,14 +79,8 @@ inline bool column_table(const QwImgColumn& c, bool with_edges, Table* t) {
   if (!with_edges) return true;
   t->edges.resize(t->num_bins);
   t->edges[0] = 0;
-  for (uint64_t i = 1; i < t->num_bins; i++) {
-    uint64_t a = t->edges[i - 1], b = max_raw;  // ord(max_raw) = hi >= lo + i
-    while (a < b) {
-      const uint64_t mid = a + (b - a) / 2;
-      if (ord(mid) >= lo + (int64_t)i) b = mid; else a = mid + 1;
-    }
-    t->edges[i] = a;
-  }
+  for (int64_t i = 1; i < (int64_t)t->num_bins; i++)  // (ord(max_raw) = hi >= lo + i)
+    t->edges[i] = first_raw(t->edges[i - 1], max_raw, [&](uint64_t raw) { return ord(raw) >= lo + i; });
   return true;
 }
 

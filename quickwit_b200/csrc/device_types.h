@@ -1,7 +1,9 @@
-// device_types.h — structures shared by the host engine (engine.cu host half) and the kernels.
+// device_types.h — structures and value rules shared by the host (engine, aggregations) and the kernels.
 #pragma once
+#include <math.h>
 #include <stddef.h>
 #include <stdint.h>
+#include <string.h>
 
 #include "../../include/qwgpu.h"
 
@@ -30,6 +32,42 @@
 #else
 #define QW_HOST_DEVICE static inline
 #endif
+
+// ---- tantivy MonotonicallyMappableToU64 (tantivy-columnar; SURVEY.md Appendix A.5) -------------
+QW_HOST_DEVICE uint64_t i64_to_u64(int64_t v) { return (uint64_t)v ^ (1ull << 63); }
+QW_HOST_DEVICE int64_t u64_to_i64(uint64_t v) { return (int64_t)(v ^ (1ull << 63)); }
+// (the device takes the bit casts as intrinsics: a memcpy there compiles the aggregation walks differently)
+QW_HOST_DEVICE uint64_t f64_to_u64(double d) {
+#ifdef __CUDA_ARCH__
+  const uint64_t bits = (uint64_t)__double_as_longlong(d);
+#else
+  uint64_t bits;
+  memcpy(&bits, &d, 8);
+#endif
+  return (bits & (1ull << 63)) ? ~bits : (bits ^ (1ull << 63));
+}
+QW_HOST_DEVICE double u64_to_f64(uint64_t v) {
+  const uint64_t bits = (v & (1ull << 63)) ? (v ^ (1ull << 63)) : ~v;
+#ifdef __CUDA_ARCH__
+  return __longlong_as_double((long long)bits);
+#else
+  double d;
+  memcpy(&d, &bits, 8);
+  return d;
+#endif
+}
+// The f64 of a column's mapped value, as the stats, histogram and percentiles aggregations read it (ordinals of str
+// and ip columns as numbers)
+QW_HOST_DEVICE double qw_mapped_to_f64(uint32_t type, uint64_t m) {
+  switch (type) {
+    case QW_COL_U64: case QW_COL_BOOL: case QW_COL_STR: case QW_COL_IP: return (double)m;
+    case QW_COL_I64: case QW_COL_DATETIME: return (double)u64_to_i64(m);
+    default: return u64_to_f64(m);
+  }
+}
+// Histogram position of a value: floor((val - offset) / interval), tantivy's bucket position before base_pos. The
+// device fast paths find buckets through boundary tables the host builds with this formula, so both must share it.
+QW_HOST_DEVICE double qw_hist_pos(double val, double offset, double interval) { return floor((val - offset) / interval); }
 // Candidate capacity of a split whose plan asks for K hits: QW_CAND_CAP up to QW_MAX_TOPK (k_select's shared
 // memory), above that 2K rounded up to a multiple of 1024 (the deep selection path, deep_select_kernel.cuh).
 QW_HOST_DEVICE uint32_t qw_cand_cap(uint32_t K) { return K <= QW_MAX_TOPK ? (uint32_t)QW_CAND_CAP : (2u * K + 1023u) & ~1023u; }
@@ -141,10 +179,10 @@ struct DAgg {
   uint32_t comp;    // TERMS / HISTOGRAM: QW_AGG_COMP_* flags (QwAggNode.reserved), read by the hashed walk only
   double interval, offset, bound_min, bound_max;
   int64_t base_pos;
-  // fast path (flat bucket aggregations over single-valued columns, see lower_plan): histogram
+  // fast path (flat bucket aggregations over single-valued columns, see lower_aggs): histogram
   // buckets are found in RAW space — bounds[k] = smallest bit-packed raw value that falls into
-  // bucket >= k (k = 0..num_buckets), computed on the host with the reference f64 formula, so the
-  // device needs no f64 arithmetic and stays bit-exact
+  // bucket >= k (k = 0..num_buckets), computed on the host with the reference f64 formula
+  // (common.h hist_bounds), so the device needs no f64 arithmetic and stays bit-exact
   uint64_t bounds;       // device address of uint64[num_buckets + 1] (HISTOGRAM only)
   float inv_step;        // ~ num_buckets / (bounds[nb] - bounds[0]): first guess of the bucket
   uint32_t stat_base;    // STATS on the fast path: first of this node's {sum, ~min, max} triples in shared memory

@@ -437,63 +437,7 @@ std::shared_ptr<SplitDev> Engine::find(const std::string& id) {
   return sp;
 }
 
-// Hashed layout: a cell exists per (node, parent cell, key) that some (doc, value path) reaches, so a node has at
-// most min(its dense cells, the (doc, value path) tuples of its bucket chain) cells. A chain of single-valued
-// columns gives at most one path per doc; a multi-valued level multiplies by that column's value count (Σ_d Π v_l(d)
-// <= Π Σ_d v_l(d)), a `missing` bucket adds one value per doc, a range node every range.
-static uint64_t sat_mul(uint64_t a, uint64_t b) {
-  const uint64_t lim = 1ull << 62;
-  return (b && a > lim / b) ? lim : std::min(a * b, lim);
-}
-uint64_t agg_hashed_bound(const QwAggNode* aggs, uint32_t n, const ImageView& img) {
-  const uint64_t num_docs = img.hdr->num_docs;
-  uint64_t total = 0;
-  for (uint32_t i = 0; i < n; i++) {
-    uint64_t dense = 1, reps = 1, multi = 1;
-    bool any_multi = false;
-    uint32_t depth = 0;
-    for (uint32_t b = aggs[i].kind == QW_AGG_STATS ? aggs[i].parent : i; b != 0xFFFFFFFFu && depth <= n; b = aggs[b].parent, depth++) {
-      const QwAggNode& g = aggs[b];
-      dense = sat_mul(dense, g.num_buckets);
-      if (g.kind == QW_AGG_RANGE) reps = sat_mul(reps, g.num_ranges);
-      if (g.column < img.hdr->num_columns && img.columns[g.column].cardinality == QW_CARD_MULTI) {
-        any_multi = true;
-        multi = sat_mul(multi, img.columns[g.column].num_vals +
-                                   ((g.kind == QW_AGG_TERMS || g.kind == QW_AGG_HISTOGRAM || g.kind == QW_AGG_PERCENTILES) && g.has_missing ? num_docs : 0));
-      }
-    }
-    total = std::min<uint64_t>(total + std::min(dense, sat_mul(any_multi ? multi : num_docs, reps)), 1ull << 62);
-  }
-  return total;
-}
-uint32_t agg_hashed_slots(uint64_t cap) {
-  uint64_t slots = 2;
-  while (slots < 2 * cap) slots <<= 1;  // load factor <= 1/2: short probe sequences
-  return (uint32_t)std::min<uint64_t>(slots, 1ull << 31);
-}
-uint64_t agg_hashed_table_bytes(uint64_t cap) {
-  const uint64_t slots = agg_hashed_slots(cap);
-  return slots * 4 + cap * (sizeof(DHKey) + sizeof(QwAggCell));
-}
-uint64_t agg_hashed_layout(const QwAggNode* aggs, uint32_t n, const ImageView& img, const char* split_id) {
-  const uint64_t bound = std::max<uint64_t>(agg_hashed_bound(aggs, n, img), 1);
-  const uint64_t bytes = bound >= (1ull << 30) ? ~0ull : agg_hashed_table_bytes(bound);
-  if (bytes > QWGPU_HASHED_MAX_BYTES)
-    fail(QWGPU_EUNSUPPORTED, "split `%s`: the aggregation may create up to %llu buckets, whose hashed table exceeds the GPU limit of %llu bytes per call",
-         split_id, (unsigned long long)bound, (unsigned long long)QWGPU_HASHED_MAX_BYTES);
-  return bound;
-}
-
 // ---- lowering: QwPlan tree -> window-engine program ----------------------------------------------
-// kernels.cuh mapped_to_f64 on the host (tantivy MonotonicallyMappableToU64 inverses, as f64)
-static double mapped_to_f64_host(uint32_t type, uint64_t m) {
-  switch (type) {
-    case QW_COL_U64: case QW_COL_BOOL: case QW_COL_STR: case QW_COL_IP: return (double)m;
-    case QW_COL_I64: case QW_COL_DATETIME: return (double)(int64_t)(m ^ (1ull << 63));
-    default: return u64_to_f64(m);
-  }
-}
-
 struct Lowered {
   DSplitPlan P;
   std::vector<DInstr> instrs;
@@ -880,6 +824,111 @@ static void lower_node(Lowered& L, const SplitDev& sp, const QwPlanNode* nodes, 
 
 static inline uint32_t bits_needed64(uint64_t v) { return v == 0 ? 0 : 64 - __builtin_clzll(v); }
 
+// The aggregation half of lower_plan: the tree's depth and cell layout, one DAgg per node, the find_trace_ids checks,
+// then whether the plan takes the fast aggregation path, with its histogram boundary tables
+static void lower_aggs(Lowered& L, const SplitDev& sp, const QwPlanHeader* ph, const QwAggNode* aggs) {
+  DSplitPlan& P = L.P;
+  if (ph->num_aggs > QW_MAX_AGG_NODES) fail(QWGPU_EUNSUPPORTED, "more than %u aggregation nodes", QW_MAX_AGG_NODES);
+  for (uint32_t i = 0; i < ph->num_aggs; i++) {
+    uint32_t depth = 0;
+    for (uint32_t p = aggs[i].parent; p != 0xFFFFFFFFu; p = aggs[p].parent)
+      if (p >= ph->num_aggs || ++depth > ph->num_aggs) fail(QWGPU_EINVALID_ARG, "aggregation parent out of range");
+    // (the hashed walk keeps one stack frame per level)
+    if (depth >= QW_MAX_AGG_LEVELS) fail(QWGPU_EUNSUPPORTED, "aggregations nested more than %u levels deep", QW_MAX_AGG_LEVELS);
+  }
+  std::vector<uint32_t> bases(ph->num_aggs, 0);
+  P.hashed = qw_agg_hashed(aggs, ph->num_aggs) ? 1u : 0u;
+  if (P.hashed) L.h_bound = agg_hashed_layout(aggs, ph->num_aggs, sp.view, sp.id.c_str());
+  else P.n_cells = (uint32_t)agg_cell_layout(aggs, ph->num_aggs, &bases);
+  for (uint32_t i = 0; i < ph->num_aggs; i++) {
+    const QwAggNode& a = aggs[i];
+    DAgg d;
+    memset(&d, 0, sizeof d);
+    d.kind = a.kind; d.parent = a.parent; d.first_child = a.first_child; d.num_children = a.num_children;
+    d.col = use_col(L, sp, a.column, true); d.num_buckets = a.num_buckets; d.has_bounds = a.has_bounds;
+    d.num_ranges = a.num_ranges; d.has_missing = a.has_missing; d.cell_base = bases[i];
+    d.interval = a.interval; d.offset = a.offset; d.bound_min = a.bound_min; d.bound_max = a.bound_max;
+    d.base_pos = a.base_pos;
+    memcpy(d.range_from, a.range_from, sizeof d.range_from);
+    memcpy(d.range_to, a.range_to, sizeof d.range_to);
+    if ((a.kind == QW_AGG_TERMS || a.kind == QW_AGG_HISTOGRAM) && (a.reserved & QW_AGG_COMP_LEVEL)) {
+      d.comp = a.reserved;
+      d.comp_after = a.range_from[0];
+    }
+    if (a.parent != 0xFFFFFFFFu && (aggs[a.parent].kind == QW_AGG_STATS || aggs[a.parent].kind == QW_AGG_PERCENTILES))
+      fail(QWGPU_EINVALID_AGG, "metric aggregations cannot have sub-aggregations");
+    if (a.kind == QW_AGG_RANGE && a.num_ranges > QW_MAX_AGG_RANGES) fail(QWGPU_EUNSUPPORTED, "more than %d ranges", QW_MAX_AGG_RANGES);
+    if (a.kind == QW_AGG_PERCENTILES) {
+      // the walk finds a value's bin in the column's boundary table (d.bounds: an index into L.bounds until the blob
+      // is laid out); the plan's bin count must be the table's
+      std::shared_ptr<const std::vector<uint64_t>> tab;
+      if (a.column != 0xFFFFFFFFu) {
+        const uint32_t t = sp.view.columns[a.column].type;
+        if (t == QW_COL_STR || t == QW_COL_BYTES) fail(QWGPU_EINVALID_AGG, "percentiles over a text or bytes column");
+        if (t == QW_COL_IP) fail(QWGPU_EUNSUPPORTED, "percentiles over an ip column are not supported on the GPU path");
+        tab = percentiles_table(sp, a.column);
+      }
+      const uint64_t nb = tab ? tab->size() : 0;
+      if (a.num_buckets != nb + (a.has_missing ? 1u : 0u))
+        fail(QWGPU_EINVALID_ARG, "percentiles node %u: %u buckets, the split's column has %llu bins", i, a.num_buckets, (unsigned long long)nb);
+      d.bounds = L.bounds.size();
+      if (tab) L.bounds.insert(L.bounds.end(), tab->begin(), tab->end());
+    }
+    L.aggs.push_back(d);
+  }
+  P.n_aggs = ph->num_aggs;
+  // (once every node's column and parent are checked: the rule reads the ancestors' columns)
+  for (uint32_t i = 0; i < ph->num_aggs; i++)
+    if (aggs[i].kind == QW_AGG_STATS) L.aggs[i].is_f64 = qw_stats_sum_exact(sp.view.columns, aggs, i) ? 0u : 1u;
+  for (uint32_t i = 0; i < ph->num_aggs; i++) {
+    const QwAggNode& a = aggs[i];
+    if (a.kind != QW_AGG_TRACE_IDS) continue;
+    // FindTraceIdsCollector::for_segment: a missing trace-id bytes column or a timestamp field that is not a date
+    // column is an error of the split; an absent timestamp column reads 0 ns for every doc
+    if (ph->num_aggs != 1 || ph->max_hits) fail(QWGPU_EINVALID_ARG, "a find_trace_ids node must be the only aggregation of a plan without hits");
+    if (a.num_buckets > QW_MAX_TOPK) fail(QWGPU_EUNSUPPORTED, "find_trace_ids with num_traces = %u exceeds the GPU limit %d", a.num_buckets, QW_MAX_TOPK);
+    if (a.column >= sp.view.hdr->num_columns || sp.view.columns[a.column].type != QW_COL_BYTES)
+      fail(QWGPU_EINTERNAL, "failed to find column for trace_id field");
+    if (!sp.ids16[a.column]) fail(QWGPU_EINTERNAL, "the term dictionary of the trace_id field holds a value that is not a 16-byte trace id");
+    if (a.reserved != 0xFFFFFFFFu && (a.reserved >= sp.view.hdr->num_columns || sp.view.columns[a.reserved].type != QW_COL_DATETIME))
+      fail(QWGPU_EINTERNAL, "the span timestamp field is not a date fast field");
+    P.tr_on = 1;
+    L.tr_img_col = a.column;
+    P.tr_n = a.num_buckets;
+    P.tr_num_ords = std::max(sp.view.columns[a.column].dict_num_terms, 1u);
+    P.tr_ord_col = L.aggs[i].col;
+    P.tr_ts_col = use_col(L, sp, a.reserved, true);
+  }
+  // fast aggregation path: flat (no nesting) TERMS / HISTOGRAM nodes over always-present single-valued
+  // columns; histogram buckets are located through raw-space boundary tables (hist_bounds)
+  bool fast = ph->num_aggs > 0 && !P.hashed;
+  P.n_stat_cells = 0;
+  for (DAgg& d : L.aggs) {
+    const bool full_col = d.col != 0xFFFFFFFFu && L.cols[d.col].card == QW_CARD_FULL;
+    if (d.kind == QW_AGG_STATS) {
+      // stats: top-level, or directly under a top-level bucket node; one {sum, min, max} triple per cell
+      if (!full_col || d.num_children || (d.parent != 0xFFFFFFFFu && L.aggs[d.parent].parent != 0xFFFFFFFFu)) fast = false;
+      d.stat_base = P.n_stat_cells;
+      P.n_stat_cells += d.parent == 0xFFFFFFFFu ? 1u : L.aggs[d.parent].num_buckets;
+    } else {
+      if (d.parent != 0xFFFFFFFFu || (d.kind != QW_AGG_TERMS && d.kind != QW_AGG_HISTOGRAM) || !full_col ||
+          d.num_buckets > QW_SMEM_AGG_CELLS || d.num_buckets == 0)
+        fast = false;
+    }
+  }
+  if (!fast) P.n_stat_cells = 0;
+  if (fast) {
+    for (DAgg& d : L.aggs) {
+      if (d.kind != QW_AGG_HISTOGRAM) continue;
+      d.bounds = L.bounds.size();  // index for now; turned into a device address when the blob is laid out
+      hist_bounds(L.cols[d.col], L.col_max_raw[d.col], d, L.bounds);
+      const uint64_t b0 = L.bounds[d.bounds], bn = L.bounds.back();
+      d.inv_step = bn > b0 ? (float)((double)d.num_buckets / (double)(bn - b0)) : 0.0f;
+    }
+  }
+  P.fast_aggs = fast ? 1 : 0;
+}
+
 static void lower_plan(Lowered& L, const SplitDev& sp, const uint8_t* plan, size_t plan_len, uint32_t max_hits) {
   if (plan_len < sizeof(QwPlanHeader)) fail(QWGPU_EINVALID_ARG, "plan too short");
   const QwPlanHeader* ph = (const QwPlanHeader*)plan;
@@ -1004,140 +1053,8 @@ static void lower_plan(Lowered& L, const SplitDev& sp, const uint8_t* plan, size
   } else if (ks.kind[0] == QW_SORT_COLUMN && ks.rbits[0] >= 10) ks.top_mode = QW_TOP_COLUMN;
   else if (ks.kind[0] == QW_SORT_DOCID && ks.kind[1] == QW_SORT_NONE && ks.doc_bits >= 11) ks.top_mode = QW_TOP_DOC;
   else ks.top_mode = QW_TOP_FULL;
-  // aggregations
-  if (ph->num_aggs > QW_MAX_AGG_NODES) fail(QWGPU_EUNSUPPORTED, "more than %u aggregation nodes", QW_MAX_AGG_NODES);
-  for (uint32_t i = 0; i < ph->num_aggs; i++) {
-    uint32_t depth = 0;
-    for (uint32_t p = aggs[i].parent; p != 0xFFFFFFFFu; p = aggs[p].parent)
-      if (p >= ph->num_aggs || ++depth > ph->num_aggs) fail(QWGPU_EINVALID_ARG, "aggregation parent out of range");
-    // (the hashed walk keeps one stack frame per level)
-    if (depth >= QW_MAX_AGG_LEVELS) fail(QWGPU_EUNSUPPORTED, "aggregations nested more than %u levels deep", QW_MAX_AGG_LEVELS);
-  }
-  std::vector<uint32_t> bases(ph->num_aggs, 0);
-  P.hashed = qw_agg_hashed(aggs, ph->num_aggs) ? 1u : 0u;
-  if (P.hashed) L.h_bound = agg_hashed_layout(aggs, ph->num_aggs, sp.view, sp.id.c_str());
-  else P.n_cells = (uint32_t)agg_cell_layout(aggs, ph->num_aggs, &bases);
-  for (uint32_t i = 0; i < ph->num_aggs; i++) {
-    const QwAggNode& a = aggs[i];
-    DAgg d;
-    memset(&d, 0, sizeof d);
-    d.kind = a.kind; d.parent = a.parent; d.first_child = a.first_child; d.num_children = a.num_children;
-    d.col = use_col(L, sp, a.column, true); d.num_buckets = a.num_buckets; d.has_bounds = a.has_bounds;
-    d.num_ranges = a.num_ranges; d.has_missing = a.has_missing; d.cell_base = bases[i];
-    d.interval = a.interval; d.offset = a.offset; d.bound_min = a.bound_min; d.bound_max = a.bound_max;
-    d.base_pos = a.base_pos;
-    memcpy(d.range_from, a.range_from, sizeof d.range_from);
-    memcpy(d.range_to, a.range_to, sizeof d.range_to);
-    if ((a.kind == QW_AGG_TERMS || a.kind == QW_AGG_HISTOGRAM) && (a.reserved & QW_AGG_COMP_LEVEL)) {
-      d.comp = a.reserved;
-      d.comp_after = a.range_from[0];
-    }
-    if (a.parent != 0xFFFFFFFFu && (aggs[a.parent].kind == QW_AGG_STATS || aggs[a.parent].kind == QW_AGG_PERCENTILES))
-      fail(QWGPU_EINVALID_AGG, "metric aggregations cannot have sub-aggregations");
-    if (a.kind == QW_AGG_RANGE && a.num_ranges > QW_MAX_AGG_RANGES) fail(QWGPU_EUNSUPPORTED, "more than %d ranges", QW_MAX_AGG_RANGES);
-    if (a.kind == QW_AGG_PERCENTILES) {
-      // the walk finds a value's bin in the column's boundary table (d.bounds: an index into L.bounds until the blob
-      // is laid out); the plan's bin count must be the table's
-      std::shared_ptr<const std::vector<uint64_t>> tab;
-      if (a.column != 0xFFFFFFFFu) {
-        const uint32_t t = sp.view.columns[a.column].type;
-        if (t == QW_COL_STR || t == QW_COL_BYTES) fail(QWGPU_EINVALID_AGG, "percentiles over a text or bytes column");
-        if (t == QW_COL_IP) fail(QWGPU_EUNSUPPORTED, "percentiles over an ip column are not supported on the GPU path");
-        tab = percentiles_table(sp, a.column);
-      }
-      const uint64_t nb = tab ? tab->size() : 0;
-      if (a.num_buckets != nb + (a.has_missing ? 1u : 0u))
-        fail(QWGPU_EINVALID_ARG, "percentiles node %u: %u buckets, the split's column has %llu bins", i, a.num_buckets, (unsigned long long)nb);
-      d.bounds = L.bounds.size();
-      if (tab) L.bounds.insert(L.bounds.end(), tab->begin(), tab->end());
-    }
-    L.aggs.push_back(d);
-  }
-  P.n_aggs = ph->num_aggs;
-  // (once every node's column and parent are checked: the rule reads the ancestors' columns)
-  for (uint32_t i = 0; i < ph->num_aggs; i++)
-    if (aggs[i].kind == QW_AGG_STATS) L.aggs[i].is_f64 = qw_stats_sum_exact(sp.view.columns, aggs, i) ? 0u : 1u;
-  for (uint32_t i = 0; i < ph->num_aggs; i++) {
-    const QwAggNode& a = aggs[i];
-    if (a.kind != QW_AGG_TRACE_IDS) continue;
-    // FindTraceIdsCollector::for_segment: a missing trace-id bytes column or a timestamp field that is not a date
-    // column is an error of the split; an absent timestamp column reads 0 ns for every doc
-    if (ph->num_aggs != 1 || ph->max_hits) fail(QWGPU_EINVALID_ARG, "a find_trace_ids node must be the only aggregation of a plan without hits");
-    if (a.num_buckets > QW_MAX_TOPK) fail(QWGPU_EUNSUPPORTED, "find_trace_ids with num_traces = %u exceeds the GPU limit %d", a.num_buckets, QW_MAX_TOPK);
-    if (a.column >= sp.view.hdr->num_columns || sp.view.columns[a.column].type != QW_COL_BYTES)
-      fail(QWGPU_EINTERNAL, "failed to find column for trace_id field");
-    if (!sp.ids16[a.column]) fail(QWGPU_EINTERNAL, "the term dictionary of the trace_id field holds a value that is not a 16-byte trace id");
-    if (a.reserved != 0xFFFFFFFFu && (a.reserved >= sp.view.hdr->num_columns || sp.view.columns[a.reserved].type != QW_COL_DATETIME))
-      fail(QWGPU_EINTERNAL, "the span timestamp field is not a date fast field");
-    P.tr_on = 1;
-    L.tr_img_col = a.column;
-    P.tr_n = a.num_buckets;
-    P.tr_num_ords = std::max(sp.view.columns[a.column].dict_num_terms, 1u);
-    P.tr_ord_col = L.aggs[i].col;
-    P.tr_ts_col = use_col(L, sp, a.reserved, true);
-  }
+  lower_aggs(L, sp, ph, aggs);
   P.n_cols = (uint32_t)L.cols.size();
-  // fast aggregation path: flat (no nesting) TERMS / HISTOGRAM nodes over always-present single-valued
-  // columns. Histogram buckets are located through a raw-space boundary table built here with the
-  // reference formula (agg_bucket in kernels.cuh == tantivy's ((val - offset) / interval).floor()),
-  // which is monotone in the raw value.
-  bool fast = ph->num_aggs > 0 && !P.hashed;
-  P.n_stat_cells = 0;
-  for (DAgg& d : L.aggs) {
-    const bool full_col = d.col != 0xFFFFFFFFu && L.cols[d.col].card == QW_CARD_FULL;
-    if (d.kind == QW_AGG_STATS) {
-      // stats: top-level, or directly under a top-level bucket node; one {sum, min, max} triple per cell
-      if (!full_col || d.num_children || (d.parent != 0xFFFFFFFFu && L.aggs[d.parent].parent != 0xFFFFFFFFu)) fast = false;
-      d.stat_base = P.n_stat_cells;
-      P.n_stat_cells += d.parent == 0xFFFFFFFFu ? 1u : L.aggs[d.parent].num_buckets;
-    } else {
-      if (d.parent != 0xFFFFFFFFu || (d.kind != QW_AGG_TERMS && d.kind != QW_AGG_HISTOGRAM) || !full_col ||
-          d.num_buckets > QW_SMEM_AGG_CELLS || d.num_buckets == 0)
-        fast = false;
-    }
-  }
-  if (!fast) P.n_stat_cells = 0;
-  if (fast) {
-    for (DAgg& d : L.aggs) {
-      if (d.kind != QW_AGG_HISTOGRAM) continue;
-      const DCol& c = L.cols[d.col];
-      // raws present in the column are <= max_raw; searching beyond would leave the value domain
-      // (f64 columns: bit patterns past the maximum are NaNs and break monotonicity)
-      const uint64_t max_raw = L.col_max_raw[d.col];
-      const uint64_t raw_end = max_raw == ~0ull ? max_raw : max_raw + 1;
-      const uint32_t nb = d.num_buckets;
-      // g(raw): bucket index clamped to [-1, nb]; monotone non-decreasing in raw
-      auto g = [&](uint64_t raw) -> int64_t {
-        const unsigned __int128 wide = (unsigned __int128)c.gcd * raw + c.min_value;  // saturate beyond the column's range
-        const double val = mapped_to_f64_host(c.type, wide > (unsigned __int128)~0ull ? ~0ull : (uint64_t)wide);
-        if (d.has_bounds) {
-          if (!(val >= d.bound_min)) return -1;
-          if (!(val <= d.bound_max)) return (int64_t)nb;
-        }
-        const double pos = std::floor((val - d.offset) / d.interval);
-        if (!(pos >= -9.0e18)) return -1;
-        if (!(pos <= 9.0e18)) return (int64_t)nb;
-        const int64_t idx = (int64_t)pos - d.base_pos;
-        return idx < 0 ? -1 : (idx >= (int64_t)nb ? (int64_t)nb : idx);
-      };
-      d.bounds = L.bounds.size();  // index for now; turned into a device address when the blob is laid out
-      uint64_t lo = 0;
-      for (uint32_t k = 0; k <= nb; k++) {
-        // smallest raw in [lo, raw_end] with g(raw) >= k (raw_end when there is none)
-        uint64_t a = lo, b = raw_end;
-        if (max_raw == ~0ull && g(~0ull) < (int64_t)k) a = b = ~0ull;  // (2^64 is not representable: saturate)
-        while (a < b) {
-          const uint64_t mid = a + (b - a) / 2;
-          if (g(mid) >= (int64_t)k) b = mid; else a = mid + 1;
-        }
-        L.bounds.push_back(a);
-        lo = a;
-      }
-      const uint64_t b0 = L.bounds[d.bounds], bn = L.bounds[d.bounds + nb];
-      d.inv_step = bn > b0 ? (float)((double)nb / (double)(bn - b0)) : 0.0f;
-    }
-  }
-  P.fast_aggs = fast ? 1 : 0;
 }
 
 // Consecutive regions of one buffer or shared-memory block: each starts where the one before ends, rounded up to

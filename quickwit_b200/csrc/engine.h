@@ -159,12 +159,6 @@ struct Engine {
               const GatherSpec* gather = nullptr, std::vector<RankHeader>* rank_headers = nullptr);
 };
 
-// hashed layout: guaranteed upper bound on a split's distinct cells, and the device bytes of a table of `cap`
-// cells; agg_hashed_layout fails with QWGPU_EUNSUPPORTED when the table at the bound exceeds QWGPU_HASHED_MAX_BYTES
-uint64_t agg_hashed_bound(const QwAggNode* aggs, uint32_t n, const ImageView& img);
-uint64_t agg_hashed_table_bytes(uint64_t cap);
-uint64_t agg_hashed_layout(const QwAggNode* aggs, uint32_t n, const ImageView& img, const char* split_id);
-
 }  // namespace qw
 
 namespace qw { struct Comm; }

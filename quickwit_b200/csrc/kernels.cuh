@@ -94,20 +94,6 @@ __device__ __forceinline__ uint32_t f32_ordered(float f) {
   uint32_t b = __float_as_uint(f);
   return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
 }
-__device__ __forceinline__ uint64_t f64_to_u64_dev(double d) {
-  uint64_t b = (uint64_t)__double_as_longlong(d);
-  return (b & (1ull << 63)) ? ~b : (b ^ (1ull << 63));
-}
-__device__ __forceinline__ double mapped_to_f64(uint32_t type, uint64_t m) {
-  switch (type) {
-    case QW_COL_U64: case QW_COL_BOOL: case QW_COL_STR: return (double)m;
-    case QW_COL_I64: case QW_COL_DATETIME: return (double)(long long)(m ^ (1ull << 63));
-    default: {
-      uint64_t bits = (m & (1ull << 63)) ? (m ^ (1ull << 63)) : ~m;
-      return __longlong_as_double((long long)bits);
-    }
-  }
-}
 
 // ---- columnar reads (tantivy-bitpacker BitUnpacker::get semantics, aligned 64-bit loads) ---------
 __device__ __forceinline__ uint64_t col_raw(const uint8_t* base, const DCol& c, uint64_t idx) {
@@ -300,7 +286,7 @@ __device__ __forceinline__ DocKey doc_key(const DSplitPlan& P, const DKeySpec& k
     const bool desc = ks.order[i] == QW_ORDER_DESC;
     if (ks.kind[i] == QW_SORT_SCORE) {
       has[i] = 1;
-      v[i] = f64_to_u64_dev((double)score);
+      v[i] = f64_to_u64((double)score);
       const uint32_t o = f32_ordered(score);
       r[i] = desc ? o : ~o;
       if (i == 0) r[i] |= (uint64_t)score_lin(ks, score, desc) << 32;
@@ -416,6 +402,17 @@ __device__ __forceinline__ uint64_t col_raw_doc(const uint8_t* base, const DCol&
   }
   return col_raw(base, c, doc);
 }
+// Butterfly over the warp of the lanes' stats contributions {sum of raw offsets, f64 sum (is_f64 only), ~min, max}:
+// every lane ends with the warp's totals. A statement macro: as an inlined function call it changes the register
+// allocation of the walks that use it (k_window's hashed COLLECT instantiation spills differently).
+#define QW_WARP_STATS_REDUCE(is_f64, isum, dsum, nmin, vmax)                                                     \
+  _Pragma("unroll") for (int o_ = 16; o_ > 0; o_ >>= 1) {                                                        \
+    isum += __shfl_xor_sync(QW_FULL, isum, o_);                                                                  \
+    if (is_f64) dsum += __shfl_xor_sync(QW_FULL, dsum, o_);                                                      \
+    const unsigned long long x_ = __shfl_xor_sync(QW_FULL, nmin, o_), y_ = __shfl_xor_sync(QW_FULL, vmax, o_);    \
+    nmin = x_ > nmin ? x_ : nmin;                                                                                \
+    vmax = y_ > vmax ? y_ : vmax;                                                                                \
+  }
 // Privatised stats cell of the fast path: {sum (u64 wrapping, or f64 bits), max(~mapped) = min, max(mapped)}.
 // When the whole warp feeds one cell the three values are butterfly-reduced first.
 __device__ __forceinline__ void stat_update(unsigned long long* st, const DAgg& g, const DCol& c, const uint8_t* base, uint32_t cell, uint32_t doc, uint32_t num_docs, bool ok, uint32_t lane) {
@@ -427,27 +424,29 @@ __device__ __forceinline__ void stat_update(unsigned long long* st, const DAgg& 
   // nanosecond timestamps cannot overflow), or doubles where that sum could wrap (DAgg::is_f64)
   const bool is_f64 = g.is_f64;
   unsigned long long isum = ok ? raw : 0ull;
-  double dsum = (ok && is_f64) ? mapped_to_f64(c.type, m) : 0.0;
+  double dsum = (ok && is_f64) ? qw_mapped_to_f64(c.type, m) : 0.0;
   unsigned long long nmin = ok ? ~m : 0ull, vmax = ok ? m : 0ull;
   const uint32_t lead = __ffs(okmask) - 1;
   const uint32_t lead_cell = __shfl_sync(QW_FULL, cell, lead);
   const bool one = __ballot_sync(QW_FULL, ok && cell != lead_cell) == 0;
-  if (one) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      isum += __shfl_xor_sync(QW_FULL, isum, o);
-      if (is_f64) dsum += __shfl_xor_sync(QW_FULL, dsum, o);
-      const unsigned long long x = __shfl_xor_sync(QW_FULL, nmin, o), y = __shfl_xor_sync(QW_FULL, vmax, o);
-      nmin = x > nmin ? x : nmin;
-      vmax = y > vmax ? y : vmax;
-    }
-  }
+  if (one) { QW_WARP_STATS_REDUCE(is_f64, isum, dsum, nmin, vmax) }
   if (one ? lane == lead : ok) {
     unsigned long long* t = st + 3ull * cell;
     if (is_f64) atomicAdd((double*)t, dsum); else atomicAdd(t, isum);
     atomicMax(t + 1, nmin);
     atomicMax(t + 2, vmax);
   }
+}
+// Bucket of a raw value through a histogram's boundary table (DAgg::bounds): B[k] = the smallest raw value in bucket
+// >= k, k = 0..nb, b0 = B[0], bn = B[nb]; false when the value lies outside [b0, bn). The first guess comes from
+// inv_step, then the table corrects it.
+__device__ __forceinline__ bool hist_bucket(const uint64_t* B, uint32_t nb, float inv_step, uint64_t b0, uint64_t bn, uint64_t raw, uint32_t& bk) {
+  if (!(raw >= b0 && raw < bn)) return false;
+  const float f = __fmul_rn((float)(raw - b0), inv_step);
+  bk = f >= (float)(nb - 1) ? nb - 1 : (uint32_t)f;
+  while (raw < __ldg(B + bk)) bk--;
+  while (raw >= __ldg(B + bk + 1)) bk++;
+  return true;
 }
 __device__ __forceinline__ void agg_collect_fast(const Sm& sm, const DSplitPlan& P, const DAgg* aggs, const DCol* cols,
                                                  const uint8_t* base, uint32_t doc, bool on, uint32_t lane) {
@@ -469,12 +468,7 @@ __device__ __forceinline__ void agg_collect_fast(const Sm& sm, const DSplitPlan&
       const uint64_t b0 = __ldg(B), bn = __ldg(B + nb);
       ok = on && raw >= b0 && raw < bn;
       bk = 0;
-      if (ok) {
-        const float f = __fmul_rn((float)(raw - b0), g.inv_step);
-        bk = f >= (float)(nb - 1) ? nb - 1 : (uint32_t)f;
-        while (raw < __ldg(B + bk)) bk--;
-        while (raw >= __ldg(B + bk + 1)) bk++;
-      }
+      if (ok) hist_bucket(B, nb, g.inv_step, b0, bn, raw, bk);  // (in range: its result is true)
     }
     // histogram buckets of (time-)ordered data are usually warp-uniform; terms buckets of a
     // low-cardinality column take a few leader rounds
@@ -509,16 +503,9 @@ __device__ __forceinline__ void agg_stats(const DAgg& g, const DCol& c, const ui
     if (__all_sync(QW_FULL, !ok || peers == okmask)) {
       // the whole warp feeds one cell: butterfly-reduce, one lane issues the four atomics
       unsigned long long isum = ok ? raw : 0ull;
-      double dsum = (ok && is_f64) ? mapped_to_f64(c.type, m) : 0.0;
+      double dsum = (ok && is_f64) ? qw_mapped_to_f64(c.type, m) : 0.0;
       unsigned long long nmin = ok ? ~m : 0ull, vmax = ok ? m : 0ull;
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        isum += __shfl_xor_sync(QW_FULL, isum, o);
-        if (is_f64) dsum += __shfl_xor_sync(QW_FULL, dsum, o);
-        const unsigned long long x = __shfl_xor_sync(QW_FULL, nmin, o), y = __shfl_xor_sync(QW_FULL, vmax, o);
-        nmin = x > nmin ? x : nmin;
-        vmax = y > vmax ? y : vmax;
-      }
+      QW_WARP_STATS_REDUCE(is_f64, isum, dsum, nmin, vmax)
       if (ok && (uint32_t)(__ffs(okmask) - 1) == lane) {
         atomicAdd((unsigned long long*)&out->count, (unsigned long long)__popc(okmask));
         if (is_f64) atomicAdd((double*)&out->sum_bits, dsum);
@@ -528,7 +515,7 @@ __device__ __forceinline__ void agg_stats(const DAgg& g, const DCol& c, const ui
       }
     } else if (ok) {
       atomicAdd((unsigned long long*)&out->count, 1ull);
-      if (is_f64) atomicAdd((double*)&out->sum_bits, mapped_to_f64(c.type, m));
+      if (is_f64) atomicAdd((double*)&out->sum_bits, qw_mapped_to_f64(c.type, m));
       else atomicAdd((unsigned long long*)&out->sum_bits, (unsigned long long)raw);
       atomicMax((unsigned long long*)&out->min_mapped, (unsigned long long)~m);
       atomicMax((unsigned long long*)&out->max_mapped, (unsigned long long)m);
@@ -542,10 +529,9 @@ __device__ __forceinline__ bool agg_bucket(const DAgg& g, const DCol& c, const u
   uint64_t m = c.min_value + c.gcd * raw;
   if (g.kind == QW_AGG_HISTOGRAM) {
     if (r != 0) return false;
-    double val = mapped_to_f64(c.type, m);
+    double val = qw_mapped_to_f64(c.type, m);
     if (g.has_bounds && !(val >= g.bound_min && val <= g.bound_max)) return false;
-    double pos = floor(__ddiv_rn(__dsub_rn(val, g.offset), g.interval));
-    long long idx = (long long)pos - g.base_pos;
+    long long idx = (long long)qw_hist_pos(val, g.offset, g.interval) - g.base_pos;
     if (idx < 0 || idx >= (long long)g.num_buckets) return false;
     bucket = (uint32_t)idx;
     return true;
@@ -1633,7 +1619,7 @@ __device__ __forceinline__ void write_hit(const DSplitPlan& P, const DCol* cols,
       if (!desc) o = ~o;
       const uint32_t bits = (o & 0x80000000u) ? (o & 0x7FFFFFFFu) : ~o;
       hh.score = __uint_as_float(bits);
-      v[f] = f64_to_u64_dev((double)hh.score);
+      v[f] = f64_to_u64((double)hh.score);
     } else {
       const DCol& c = cols[ks.col[f]];
       v[f] = c.min_value + c.gcd * (desc ? r[f] : ks.raw_max[f] - r[f]);
