@@ -264,7 +264,12 @@ enum {
   QW_AGG_TERMS = 1,
   QW_AGG_HISTOGRAM = 2,      /* also date_histogram (interval/offset pre-scaled to column units) */
   QW_AGG_RANGE = 3,
-  QW_AGG_STATS = 4,          /* stats / avg / sum / min / max / value_count share one collector */
+  QW_AGG_STATS = 4,          /* stats / avg / sum / min / max / value_count share one collector. With `has_missing`
+                                (`missing_value` = the f64 bits of the `missing` value, which the device never reads)
+                                the node also counts, under every parent bucket, the matched docs without a value in
+                                its column (every matched doc when the split lacks the column): the entry with
+                                QW_AGG_ENTRY_MISSING (key 0) next to the node's cell, or in the dense layout a second
+                                bank of cells after the first. The host folds count * missing into the metric. */
   QW_AGG_TRACE_IDS = 5,      /* FindTraceIdsCollector (quickwit-search/src/find_trace_ids_collector.rs): the only node
                                 of its plan. `column` = the trace-id QW_COL_BYTES column, `reserved` = the span timestamp
                                 column (0xFFFFFFFF when absent from the split: every timestamp reads 0),
@@ -336,7 +341,7 @@ typedef struct QwAggNode {
   /* TERMS on numeric columns: dense index = raw value; on STR: ordinal */
   uint32_t has_missing;  /* `missing` parameter present (composite: `missing_bucket`) */
   uint32_t reserved;     /* TRACE_IDS: the timestamp column; TERMS / HISTOGRAM: QW_AGG_COMP_* flags */
-  uint64_t missing_value; /* mapped-u64 (numeric) or ordinal==dict_num_terms for "new key" */
+  uint64_t missing_value; /* mapped-u64 (numeric) or ordinal==dict_num_terms for "new key"; STATS / PERCENTILES: f64 bits */
 } QwAggNode;
 
 typedef struct QwPlanHeader {
@@ -386,7 +391,8 @@ typedef struct QwHit {
 } QwHit;
 
 /* Dense aggregation result (plans for which qw_agg_hashed() is 0). Every QwAggNode owns `cells(node)` = Π num_buckets over its ancestor
- * chain (itself included; metric nodes count 1) cells, laid out row-major (outermost ancestor
+ * chain (itself included; metric nodes count 1, a QW_AGG_STATS node with has_missing 2: its second bank, after the
+ * first, holds in `count` the docs without a value per parent cell) cells, laid out row-major (outermost ancestor
  * slowest). Bucket nodes use only `count` (doc_count). Metric nodes (QW_AGG_STATS) use all four:
  * `sum_bits`: where qw_stats_sum_exact() holds, the exact integer sum of the RAW offsets (value =
  * min_value + gcd * raw in the mapped space) — the host rebuilds count * min + gcd * sum in 128-bit
@@ -407,7 +413,8 @@ typedef struct QwAggCell {
  * layout when its tree is deeper than bucket -> bucket -> metric, its dense cells add up to more than
  * QW_AGG_DENSE_MAX_CELLS, or a TERMS node's dense space exceeds QW_AGG_DENSE_MAX_TERMS (qw_agg_hashed).
  *   key: TERMS = the bit-packed raw value (0 with QW_AGG_ENTRY_MISSING: the `missing` bucket); HISTOGRAM = the
- *        bucket index relative to base_pos (agg_bucket's f64 formula); RANGE = the range index; STATS = 0;
+ *        bucket index relative to base_pos (agg_bucket's f64 formula); RANGE = the range index; STATS = 0 (with
+ *        QW_AGG_ENTRY_MISSING: the count of docs without a value);
  *        PERCENTILES = the index of the value's bin in the split's boundary table (QW_AGG_PERCENTILES).
  *   cell: as in the dense layout (bucket entries use `count` only). */
 #define QW_AGG_DENSE_MAX_CELLS (1ull << 26)
@@ -435,7 +442,7 @@ static inline int qw_agg_hashed(const QwAggNode* nodes, uint32_t n) {
     if (g->kind == QW_AGG_PERCENTILES) return 1;
     if (g->kind == QW_AGG_TERMS && (uint64_t)g->num_buckets - (g->has_missing ? 1u : 0u) > QW_AGG_DENSE_MAX_TERMS) return 1;
     uint32_t depth = 0;
-    uint64_t cells = g->kind == QW_AGG_STATS ? 1 : g->num_buckets;
+    uint64_t cells = g->kind == QW_AGG_STATS ? (g->has_missing ? 2 : 1) : g->num_buckets;
     for (uint32_t p = g->parent; p != 0xFFFFFFFFu; p = nodes[p].parent) {
       depth++;
       if (depth > n) return 1; /* (a parent cycle: lowering refuses it) */

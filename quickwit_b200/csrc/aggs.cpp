@@ -151,6 +151,15 @@ static void parse_composite(const Json& spec, AggReq& a, int depth) {
   }
 }
 
+// `missing` of a metric aggregation (percentiles and the stats family): a JSON number, taken as an f64
+static void parse_metric_missing(const Json& spec, AggReq& a, const char* type) {
+  if (const Json* m = spec.get("missing")) {
+    if (!m->is_num()) fail(QWGPU_EINVALID_AGG, "%s `missing` must be a number", type);
+    a.has_missing = true;
+    a.missing = *m;
+  }
+}
+
 // percentiles: {"field", "percents": [..] (default 1, 5, 25, 50, 75, 95, 99), "keyed" (default true), "missing": number}
 static void parse_percentiles(const Json& spec, AggReq& a) {
   a.kind = AggReq::Percentiles;
@@ -167,11 +176,7 @@ static void parse_percentiles(const Json& spec, AggReq& a) {
     }
   }
   a.keyed = spec.bool_or("keyed", true);
-  if (const Json* m = spec.get("missing")) {
-    if (!m->is_num()) fail(QWGPU_EINVALID_AGG, "percentiles `missing` must be a number");
-    a.has_missing = true;
-    a.missing = *m;
-  }
+  parse_metric_missing(spec, a, "percentiles");
 }
 
 static void parse_agg_map(const Json& j, std::vector<AggReq>& out, int depth) {
@@ -236,13 +241,11 @@ static void parse_agg_map(const Json& j, std::vector<AggReq>& out, int depth) {
           a.ranges.push_back(x);
         }
         a.keyed = spec.bool_or("keyed", false);
-      } else if (t == "stats") a.kind = AggReq::Stats;
-      else if (t == "avg") a.kind = AggReq::Avg;
-      else if (t == "sum") a.kind = AggReq::Sum;
-      else if (t == "min") a.kind = AggReq::Min;
-      else if (t == "max") a.kind = AggReq::Max;
-      else if (t == "value_count" || t == "count") a.kind = AggReq::Count;
-      else if (t == "percentiles") parse_percentiles(spec, a);
+      } else if (t == "stats" || t == "avg" || t == "sum" || t == "min" || t == "max" || t == "value_count" || t == "count") {
+        a.kind = t == "stats" ? AggReq::Stats : t == "avg" ? AggReq::Avg : t == "sum" ? AggReq::Sum
+               : t == "min" ? AggReq::Min : t == "max" ? AggReq::Max : AggReq::Count;
+        parse_metric_missing(spec, a, t.c_str());
+      } else if (t == "percentiles") parse_percentiles(spec, a);
       else if (t == "cardinality" || t == "extended_stats" || t == "top_hits" || t == "filter")
         fail(QWGPU_EUNSUPPORTED, "`%s` aggregations are not implemented on the GPU path yet", t.c_str());
       else fail(QWGPU_EINVALID_AGG, "unknown aggregation type `%s`", t.c_str());
@@ -536,11 +539,14 @@ static QwAggNode lower_one(const AggReq& a, const ImageView& img, AggBinding& b,
       if (col && !dds::column_table(*col, false, &t))
         fail(QWGPU_EUNSUPPORTED, "percentiles over field `%s`, which holds NaN or infinite values, are not implemented on the GPU path", a.field.c_str());
       n.num_buckets = (uint32_t)t.num_bins + (a.has_missing ? 1u : 0u);
-      n.has_missing = a.has_missing;
-      if (a.has_missing) { const double m = a.missing.as_f64(); memcpy(&n.missing_value, &m, 8); }
       break;
     }
     default: n.kind = QW_AGG_STATS; n.num_buckets = 1; break;
+  }
+  if (n.kind == QW_AGG_STATS || n.kind == QW_AGG_PERCENTILES) {
+    // the device only counts the docs without a value; the host folds the value in (metric_from_cell, build_percentiles_e)
+    n.has_missing = a.has_missing;
+    if (a.has_missing) { const double m = a.missing.as_f64(); memcpy(&n.missing_value, &m, 8); }
   }
   return n;
 }
@@ -884,12 +890,19 @@ static std::vector<uint32_t> term_order(const AggReq& req, const std::vector<IBu
   });
 }
 
-// metric node ni from its cell (a cell with count 0 where no value reached it)
-static IAgg metric_from_cell(const CompiledPlan& cp, const ImageView& img, const QwAggNode* nodes, uint32_t ni, const QwAggCell& cell) {
+// metric node ni from its cell (a cell with count 0 where no value reached it) and, with `missing`, the count of matched
+// docs without a value under the same parent: each of those counts once as the `missing` value, an f64 in the space
+// qw_mapped_to_f64 gives the column's values. On the exact route an integer `missing` that an i64 holds joins the
+// 128-bit sum, rounded once; otherwise n * missing is added in f64 after the column's sum.
+static IAgg metric_from_cell(const CompiledPlan& cp, const ImageView& img, const QwAggNode* nodes, uint32_t ni, const QwAggCell& cell,
+                             uint64_t n_missing) {
   const AggBinding& b = cp.agg_bindings[ni];
   IAgg a;
   a.kind = (uint8_t)b.req->kind;
-  a.m_count = cell.count;
+  a.m_count = cell.count + n_missing;
+  const double m = n_missing ? b.req->missing.as_f64() : 0.0;
+  const bool m_int = n_missing && m == std::trunc(m) && m >= -0x1p63 && m < 0x1p63;
+  bool folded = false;
   if (cell.count && b.column >= 0) {
     uint32_t t = b.col_type;
     const QwImgColumn& col = img.columns[b.column];
@@ -899,10 +912,17 @@ static IAgg metric_from_cell(const CompiledPlan& cp, const ImageView& img, const
       // i64 / datetime is value + 2^63
       __int128 sum = (__int128)(unsigned __int128)col.min_value * (__int128)cell.count + (__int128)((unsigned __int128)col.gcd * cell.sum_bits);
       if (!(t == QW_COL_U64 || t == QW_COL_BOOL)) sum -= ((__int128)1 << 63) * (__int128)cell.count;
+      // (|missing| <= 2^63 and n < 2^64 keep n * missing inside 128 bits)
+      if (m_int) { sum += (__int128)(int64_t)m * (__int128)n_missing; folded = true; }
       a.m_sum = (double)sum;
     }
     a.m_min = qw_mapped_to_f64(t, cell.min_mapped);
     a.m_max = qw_mapped_to_f64(t, cell.max_mapped);
+  }
+  if (n_missing) {
+    if (!folded) a.m_sum += (double)n_missing * m;
+    if (m < a.m_min || !cell.count) a.m_min = m;
+    if (m > a.m_max || !cell.count) a.m_max = m;
   }
   return a;
 }
@@ -1077,8 +1097,14 @@ static IAgg build_node_e(const EntryCtx& c, uint32_t ni, uint32_t parent) {
   const EntryRange es = kids(c, ni, parent);
   if (req.kind == AggReq::Percentiles) return build_percentiles_e(c, ni, es);
   if (req.is_metric()) {
-    QwAggCell empty = {0, 0, ~0ull, 0};
-    return metric_from_cell(c.cp, c.img, c.nodes, ni, es.empty() ? empty : c.entries[*es.begin()].cell);
+    // the node's cell and, with `missing`, its QW_AGG_ENTRY_MISSING entry: either may be absent
+    QwAggCell cell = {0, 0, ~0ull, 0};
+    uint64_t n_missing = 0;
+    for (uint32_t e : es) {
+      if (c.entries[e].flags & QW_AGG_ENTRY_MISSING) n_missing = c.entries[e].cell.count;
+      else cell = c.entries[e].cell;
+    }
+    return metric_from_cell(c.cp, c.img, c.nodes, ni, cell, n_missing);
   }
   auto subs = [&](uint32_t e) {
     std::vector<IAgg> out;
@@ -1142,7 +1168,8 @@ static std::vector<IAgg> build_top_entries(const CompiledPlan& cp, const ImageVi
       fail(QWGPU_EINVALID_ARG, "aggregation entry %zu does not match the plan's tree", e);
     const QwAggNode& n = nodes[x.node];
     const AggBinding& b = cp.agg_bindings[x.node];
-    bool ok = x.flags == 0 || ((n.kind == QW_AGG_TERMS || n.kind == QW_AGG_HISTOGRAM || n.kind == QW_AGG_PERCENTILES) && x.flags == QW_AGG_ENTRY_MISSING);
+    bool ok = x.flags == 0 || ((n.kind == QW_AGG_TERMS || n.kind == QW_AGG_HISTOGRAM || n.kind == QW_AGG_PERCENTILES || n.kind == QW_AGG_STATS) &&
+                               x.flags == QW_AGG_ENTRY_MISSING);
     if (ok && (x.flags & QW_AGG_ENTRY_MISSING)) ok = n.has_missing && x.key == 0;
     else if (ok) {
       switch (n.kind) {
@@ -1170,7 +1197,8 @@ uint64_t agg_cell_layout(const QwAggNode* aggs, uint32_t n, std::vector<uint32_t
   uint64_t total = 0;
   if (bases) bases->resize(n);
   for (uint32_t i = 0; i < n; i++) {
-    uint64_t cells = aggs[i].kind == QW_AGG_STATS ? 1 : aggs[i].num_buckets;
+    // a STATS node with `missing` has a second bank: the count of docs without a value per parent cell
+    uint64_t cells = aggs[i].kind == QW_AGG_STATS ? (aggs[i].has_missing ? 2 : 1) : aggs[i].num_buckets;
     uint32_t p = aggs[i].parent;
     while (p != 0xFFFFFFFFu) { cells *= aggs[p].num_buckets; p = aggs[p].parent; }
     if (bases) (*bases)[i] = (uint32_t)total;
@@ -1183,7 +1211,8 @@ uint64_t agg_cell_layout(const QwAggNode* aggs, uint32_t n, std::vector<uint32_t
 // Hashed layout: a cell exists per (node, parent cell, key) that some (doc, value path) reaches, so a node has at
 // most min(its dense cells, the (doc, value path) tuples of its bucket chain) cells. A chain of single-valued
 // columns gives at most one path per doc; a multi-valued level multiplies by that column's value count (Σ_d Π v_l(d)
-// <= Π Σ_d v_l(d)), a `missing` bucket adds one value per doc, a range node every range.
+// <= Π Σ_d v_l(d)), a `missing` bucket adds one value per doc, a range node every range. A STATS node with `missing`
+// has its `missing` entry next to its cell under every parent.
 static uint64_t sat_mul(uint64_t a, uint64_t b) {
   const uint64_t lim = 1ull << 62;
   return (b && a > lim / b) ? lim : std::min(a * b, lim);
@@ -1205,7 +1234,8 @@ uint64_t agg_hashed_bound(const QwAggNode* aggs, uint32_t n, const ImageView& im
                                    ((g.kind == QW_AGG_TERMS || g.kind == QW_AGG_HISTOGRAM || g.kind == QW_AGG_PERCENTILES) && g.has_missing ? num_docs : 0));
       }
     }
-    total = std::min<uint64_t>(total + std::min(dense, sat_mul(any_multi ? multi : num_docs, reps)), 1ull << 62);
+    const uint64_t cells = std::min(dense, sat_mul(any_multi ? multi : num_docs, reps));
+    total = std::min<uint64_t>(total + sat_mul(cells, aggs[i].kind == QW_AGG_STATS && aggs[i].has_missing ? 2 : 1), 1ull << 62);
   }
   return total;
 }
@@ -1229,7 +1259,8 @@ uint64_t agg_hashed_layout(const QwAggNode* aggs, uint32_t n, const ImageView& i
 
 // The entries of a dense cell array (QwAggCell doc in qwgpu_format.h), parents before children: one per nonzero cell,
 // keyed by its bucket index within the node (a node's `missing` bucket, its last, as QW_AGG_ENTRY_MISSING with key 0;
-// a metric cell with key 0). Zero cells give none: the builder puts back every empty range bucket and metric.
+// a metric cell with key 0, and the count of its second bank as QW_AGG_ENTRY_MISSING with key 0). Zero cells give none:
+// the builder puts back every empty range bucket and metric.
 static std::vector<QwAggEntry> dense_entries(const CompiledPlan& cp, const QwAggCell* cells, size_t ncells) {
   const QwAggNode* nodes = plan_agg_nodes(cp);
   std::vector<uint32_t> bases;
@@ -1241,8 +1272,18 @@ static std::vector<QwAggEntry> dense_entries(const CompiledPlan& cp, const QwAgg
     const AggReq::Kind kind = cp.agg_bindings[ni].req->kind;
     if (kind == AggReq::Composite || kind == AggReq::Percentiles) fail(QWGPU_EINVALID_ARG, "composite and percentiles aggregation results are given as entries");
     const QwAggNode& n = nodes[ni];
-    const uint32_t nb = n.kind == QW_AGG_STATS ? 1 : n.num_buckets;
     const QwAggCell* base = cells + bases[ni];
+    if (n.kind == QW_AGG_STATS) {
+      if (base[parent_cell].count) out.push_back({ni, parent, 0, 0u, 0, base[parent_cell]});
+      if (n.has_missing) {
+        uint64_t parent_cells = 1;  // the first bank's size
+        for (uint32_t p = n.parent; p != 0xFFFFFFFFu; p = nodes[p].parent) parent_cells *= nodes[p].num_buckets;
+        const QwAggCell& m = base[parent_cells + parent_cell];
+        if (m.count) out.push_back({ni, parent, 0, (uint32_t)QW_AGG_ENTRY_MISSING, 0, m});
+      }
+      return;
+    }
+    const uint32_t nb = n.num_buckets;
     for (uint32_t k = 0; k < nb; k++) {
       const uint64_t cell = parent_cell * nb + k;
       if (!base[cell].count) continue;

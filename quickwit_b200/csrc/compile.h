@@ -43,6 +43,7 @@ struct AggReq {
   // `order_desc` and `has_missing` = missing_bucket), `size` the page size, `after` one key per source when
   // `has_after`; `children` hang below the last source
   // Percentiles: `percents` (0..100), `keyed`, and `missing` (a number) when `has_missing`
+  // Stats / Avg / Sum / Min / Max / Count: `missing` (a number) when `has_missing`
   enum Kind { Terms, Histogram, DateHistogram, Range, Stats, Avg, Sum, Min, Max, Count, TraceIds, Composite, Percentiles } kind = Terms;
   std::vector<double> percents;
   std::vector<AggReq> sources;

@@ -522,6 +522,14 @@ __device__ __forceinline__ void agg_stats(const DAgg& g, const DCol& c, const ui
     }
   }
 }
+// STATS node g with `missing`: count the lanes that are `on` and hold no value of g's column (every lane that is on
+// when the split lacks the column) in dense cell `cell` of the node's second bank
+__device__ __forceinline__ void agg_stats_missing(const KParams& p, const Sm& sm, const DAgg& g, const DCol* cols, const uint8_t* base,
+                                                  QwAggCell* cells, uint32_t cell, uint32_t doc, bool on, uint32_t lane) {
+  uint64_t a = 0, b = 0;
+  if (on && g.col != 0xFFFFFFFFu) col_range(base, cols[g.col], doc, a, b);
+  agg_count(p, sm, cells, cell, on && a == b, lane);
+}
 // bucket index of value index i for bucket aggregation g; returns false when the value falls in no bucket
 __device__ __forceinline__ bool agg_bucket(const DAgg& g, const DCol& c, const uint8_t* base, uint64_t i, uint32_t r, uint32_t& bucket) {
   uint64_t raw = col_raw(base, c, i);
@@ -560,6 +568,7 @@ __device__ void agg_collect_doc(const KParams& p, const Sm& sm, const DSplitPlan
     }
     if (g.kind == QW_AGG_STATS) {
       if (g.col != 0xFFFFFFFFu) agg_stats(g, cols[g.col], base, cells, 0, doc, on, lane);
+      if (g.has_missing) agg_stats_missing(p, sm, g, cols, base, cells, g.cell_base + 1, doc, on, lane);
       continue;
     }
     uint64_t a;
@@ -580,6 +589,7 @@ __device__ void agg_collect_doc(const KParams& p, const Sm& sm, const DSplitPlan
           const DAgg& ch = aggs[g.first_child + ci];
           if (ch.kind == QW_AGG_STATS) {
             if (ch.col != 0xFFFFFFFFu) agg_stats(ch, cols[ch.col], base, cells, bk, doc, ok, lane);
+            if (ch.has_missing) agg_stats_missing(p, sm, ch, cols, base, cells, ch.cell_base + g.num_buckets + bk, doc, ok, lane);
             continue;
           }
           uint64_t a2;
@@ -600,6 +610,8 @@ __device__ void agg_collect_doc(const KParams& p, const Sm& sm, const DSplitPlan
               for (uint32_t gc = 0; gc < ch.num_children; gc++) {
                 const DAgg& g3 = aggs[ch.first_child + gc];
                 if (g3.kind == QW_AGG_STATS && g3.col != 0xFFFFFFFFu) agg_stats(g3, cols[g3.col], base, cells, cell2, doc, ok2, lane);
+                if (g3.kind == QW_AGG_STATS && g3.has_missing)
+                  agg_stats_missing(p, sm, g3, cols, base, cells, g3.cell_base + g.num_buckets * ch.num_buckets + cell2, doc, ok2, lane);
               }
             }
           }
@@ -733,12 +745,14 @@ __device__ __forceinline__ void agg_collect_hashed(const DSplitPlan& P, const DA
       if (fresh) {
         fresh = false;
         if (g.kind == QW_AGG_STATS) {
+          uint64_t va = 0, vb = 0;
           if (g.col != 0xFFFFFFFFu) {
-            uint64_t va = 0, vb = 0;
             if (live) col_range(base, cols[g.col], doc, va, vb);
             const uint32_t id = hcell_count(P, node[d], parent[d], 0ull, live && vb > va, false, lane);
             agg_stats(g, cols[g.col], base, cells, id, doc, id != QW_HSLOT_EMPTY, lane);
           }
+          // `missing`: a live lane without a value counts in the node's missing entry
+          if (g.has_missing) hcell_count(P, node[d] | QW_AGG_ENTRY_MISSING << 8, parent[d], 0ull, live && vb == va, true, lane);
           d--;
           continue;
         }

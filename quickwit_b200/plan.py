@@ -195,11 +195,20 @@ def composite(sources: Sequence[Agg], size: int, children: Sequence[Agg] = (), d
     return sources[0]
 
 
+def _f64_bits(missing: Optional[float]) -> Optional[int]:
+    return None if missing is None else struct.unpack("<Q", struct.pack("<d", float(missing)))[0]
+
+
 def percentiles(column: int, num_bins: int, missing: Optional[float] = None) -> Agg:
     """A percentiles node over `column`: `num_bins` = the bins of the split's boundary table for that column (the
     engine builds the table and refuses another count), `missing` = the value of docs without one (kept as f64 bits)."""
-    bits = None if missing is None else struct.unpack("<Q", struct.pack("<d", float(missing)))[0]
-    return Agg(ffi.AGG_PERCENTILES, column=column, num_buckets=num_bins + (missing is not None), missing=bits)
+    return Agg(ffi.AGG_PERCENTILES, column=column, num_buckets=num_bins + (missing is not None), missing=_f64_bits(missing))
+
+
+def stats(column: int, missing: Optional[float] = None) -> Agg:
+    """A stats node (stats / avg / sum / min / max / value_count) over `column`, ffi.ABSENT when the split lacks it;
+    `missing` = the value of docs without one (kept as f64 bits: the device only counts those docs)."""
+    return Agg(ffi.AGG_STATS, column=column, missing=_f64_bits(missing))
 
 
 def _flatten_aggs(tops: Sequence[Agg]) -> List[ffi.QwAggNode]:
