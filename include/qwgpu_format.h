@@ -181,7 +181,7 @@ typedef struct QwImgColumn {
                                  long-phrase pre-pass */
 #define QW_MAX_PHRASE_LEN 256 /* TERM children of one PHRASE node */
 #define QW_MAX_PREFIX_EXPANSIONS 1024 /* expansion children of one PHRASE_PREFIX node */
-#define QW_MAX_SET_TERMS 65536 /* children of one TERM_SET node */
+#define QW_MAX_SET_TERMS 65536 /* children of one TERM_SET or COL_SET node */
 
 enum {
   QW_NODE_TERM = 1,   /* tantivy TermQuery */
@@ -213,11 +213,15 @@ enum {
                           any child. Positions are not needed, and the children do not count toward the plan's TERM
                           clauses. Never scored: the node is only valid where its score is not read (filter / must_not,
                           or any sort other than _score). */
-  QW_NODE_CACHE = 10 /* the reference's CacheNode (quickwit-query/src/query_ast/cache_node.rs): exactly one child, the
+  QW_NODE_CACHE = 10, /* the reference's CacheNode (quickwit-query/src/query_ast/cache_node.rs): exactly one child, the
                         inner subtree, matching the same docs. A context with a predicate cache
                         (qwgpu_set_predicate_cache_budget) keeps the child's doc set per split and reads it instead of
                         evaluating the child again. Never scored: in a scoring clause of a query ranked by _score, with
                         the cache disabled, or around ALL / NONE, the engine lowers it as its child. */
+  QW_NODE_COL_SET = 11 /* a set of values of one fast column (tantivy TermSetQuery / a bool of term queries on a
+                          fast-only field): the node's `column` = the column; children = E RANGE nodes on that column,
+                          each with lo == hi in mapped-u64 space, strictly increasing, 1 <= E <= QW_MAX_SET_TERMS. A doc
+                          matches when any of its values equals a child's. Never scored, like QW_NODE_TERM_SET. */
 };
 enum { QW_OCCUR_MUST = 0, QW_OCCUR_SHOULD = 1, QW_OCCUR_MUST_NOT = 2, QW_OCCUR_FILTER = 3 };
 

@@ -112,7 +112,12 @@ static inline bool qw_fused_sample_plan(const uint32_t* first_work, const uint32
   return true;
 }
 
-enum { OP_TERM = 1, OP_RANGE = 2, OP_EXISTS = 3, OP_ALL = 4, OP_BOOL_BEGIN = 5, OP_BOOL_END = 6, OP_PHRASE = 7, OP_TERM_SET = 8 };
+enum { OP_TERM = 1, OP_RANGE = 2, OP_EXISTS = 3, OP_ALL = 4, OP_BOOL_BEGIN = 5, OP_BOOL_END = 6, OP_PHRASE = 7, OP_TERM_SET = 8,
+       OP_COL_SET = 9 };
+
+// The window program's plan limits: a plan whose lowering takes more TERM instructions or more instructions than this
+// is refused. The query compiler asks the same question before it trades set groups for set nodes.
+static inline bool qw_program_fits(uint64_t n_terms, uint64_t n_instr) { return n_terms <= QW_MAX_TERMS && n_instr <= QW_MAX_INSTR; }
 enum { IF_SCORED = 1u, IF_HAS_TF = 2u, IF_HAS_FN = 4u, IF_BITS_FROM_SCORE = 8u };
 #define QW_TFF_ROWS 16 /* tf-factor table: tff[tf][fieldnorm_id] = tf / (tf + norm[id]) for tf < 16 */
 
@@ -120,9 +125,10 @@ struct DInstr {  // 64 bytes
   uint32_t op, level, occur, flags;
   uint64_t a, b, c;  // TERM: data_off, widx_off, skip_off | RANGE: lo, hi | PHRASE: a = VBlk[] (device address), c = driver skip_off
                      // | TERM_SET: a = the node's doc bitmap (device address)
-  uint32_t n;        // TERM: num_blocks   | BOOL_END: n_req
+                     // | COL_SET: a = the split's sorted table of raw values (device address)
+  uint32_t n;        // TERM: num_blocks   | BOOL_END: n_req | COL_SET: the table's length
   uint32_t m;        // TERM: win_shift    | BOOL_END: n_should
-  uint32_t r;        // TERM: fn slot      | RANGE/EXISTS: column | BOOL_END: required_should
+  uint32_t r;        // TERM: fn slot      | RANGE/EXISTS/COL_SET: column | BOOL_END: required_should
   float f;           // TERM: bm25 weight  | const-score leaves: boost
   uint32_t t;        // TERM: term slot (index among the plan's TERM instructions)
   uint32_t pad;

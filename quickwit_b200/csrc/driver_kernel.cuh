@@ -82,7 +82,7 @@ __global__ void __launch_bounds__(QD_WARPS * 32) k_driver(const DrvParams p) {
         for (uint32_t f = 0; f < n_filters && on; f++) {
           const DInstr& fi = prog[2 + f];
           if (fi.r == 0xFFFFFFFFu) { on = false; break; }  // column absent from the split: nothing matches
-          on = col_match(base, cols[fi.r], doc[j], fi.op, fi.a, fi.b);
+          on = col_match(base, cols[fi.r], doc[j], fi.op, fi.a, fi.op == OP_COL_SET ? fi.n : fi.b);
         }
         my_hits += on ? 1u : 0u;
         if (!max_hits) continue;

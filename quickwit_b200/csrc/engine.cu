@@ -442,7 +442,8 @@ struct Lowered {
   DSplitPlan P;
   std::vector<DInstr> instrs;
   std::vector<DCol> cols;
-  std::vector<uint64_t> bounds;  // raw-space histogram boundary tables of the fast aggregation path
+  std::vector<uint64_t> bounds;  // raw-space histogram boundary tables of the fast aggregation path, percentiles
+                                 // boundary tables and the sorted raw tables of column sets
   std::vector<uint64_t> col_max_raw;  // parallel to cols: largest bit-packed raw value present in the column
   std::vector<DAgg> aggs;
   std::vector<int> col_map;  // image column -> DCol index
@@ -519,7 +520,7 @@ static std::string pred_key(const QwPlanNode* nodes, uint32_t nn, uint32_t root)
     n.boost = 0.f;
     n.bm25_weight = 0.f;
     const bool parent = n.kind == QW_NODE_BOOL || n.kind == QW_NODE_PHRASE || n.kind == QW_NODE_PHRASE_PREFIX ||
-                        n.kind == QW_NODE_TERM_SET || n.kind == QW_NODE_CACHE;
+                        n.kind == QW_NODE_TERM_SET || n.kind == QW_NODE_COL_SET || n.kind == QW_NODE_CACHE;
     if (!parent || !n.num_children) { n.first_child = n.num_children = 0; continue; }
     if ((uint64_t)n.first_child + n.num_children > nn || out.size() + n.num_children > nn) fail(QWGPU_EINVALID_ARG, "plan children out of range");
     const uint32_t first = n.first_child, cnt = n.num_children;
@@ -587,7 +588,7 @@ static void lower_node(Lowered& L, const SplitDev& sp, const QwPlanNode* nodes, 
       in.op = OP_TERM;
       if (n.term_ord == 0xFFFFFFFFu && level == 0 && (occur == QW_OCCUR_MUST || occur == QW_OCCUR_FILTER)) L.empty = true;
       in.t = L.P.n_terms++;
-      if (L.P.n_terms > QW_MAX_TERMS) fail(QWGPU_EUNSUPPORTED, "more than %d term clauses", QW_MAX_TERMS);
+      if (!qw_program_fits(L.P.n_terms, 0)) fail(QWGPU_EUNSUPPORTED, "more than %d term clauses", QW_MAX_TERMS);
       in.r = 0;
       if (n.term_ord != 0xFFFFFFFFu) {
         if (n.term_ord >= sp.view.hdr->num_terms) fail(QWGPU_EINVALID_ARG, "plan term ord out of range");
@@ -657,7 +658,10 @@ static void lower_node(Lowered& L, const SplitDev& sp, const QwPlanNode* nodes, 
       for (uint32_t c = 0; c < n.num_children; c++)
         eff[c] = resolve_cache(L, sp, nodes, nn, n.first_child + c, scored && (child(c).occur == QW_OCCUR_MUST || child(c).occur == QW_OCCUR_SHOULD));
       auto is_req = [&](uint32_t c) { return child(c).occur == QW_OCCUR_MUST || child(c).occur == QW_OCCUR_FILTER; };
-      auto is_colpred = [&](uint32_t c) { const uint32_t k = nodes[eff[c]].kind; return k == QW_NODE_RANGE || k == QW_NODE_EXISTS || k == QW_NODE_ALL; };
+      auto is_colpred = [&](uint32_t c) {
+        const uint32_t k = nodes[eff[c]].kind;
+        return k == QW_NODE_RANGE || k == QW_NODE_EXISTS || k == QW_NODE_ALL || k == QW_NODE_COL_SET;
+      };
       const bool child_scored_ctx = scored_ctx;
       for (uint32_t c = 0; c < n.num_children; c++) if (is_req(c) && child_scored_ctx && child(c).occur == QW_OCCUR_MUST) order.push_back(c);
       for (int pass = 0; pass < 2; pass++)
@@ -807,6 +811,38 @@ static void lower_node(Lowered& L, const SplitDev& sp, const QwPlanNode* nodes, 
       if (occur == QW_OCCUR_MUST || occur == QW_OCCUR_FILTER) L.min_required_df = std::min<uint64_t>(L.min_required_df, std::min<uint64_t>(df, sp.view.hdr->num_docs));
       in.op = OP_TERM_SET;
       L.operands.push_back({(uint32_t)L.instrs.size(), 0, nullptr});
+      L.instrs.push_back(in);
+      break;
+    }
+    case QW_NODE_COL_SET: {
+      // a membership test of the column's values (col_match), never scored: the children's values in raw space
+      // ((mapped - min) / gcd), sorted, in the call's blob next to the aggregation tables (in.a: an index into L.bounds
+      // until the blob is laid out). A value outside the split's [min, max] or off the gcd grid cannot match.
+      if (n.num_children < 1 || n.num_children > QW_MAX_SET_TERMS || (uint64_t)n.first_child + n.num_children > nn)
+        fail(QWGPU_EINVALID_ARG, "column set node with %u values", n.num_children);
+      if (scored)
+        fail(QWGPU_EUNSUPPORTED, "column set (term set) in a scoring clause of a query ranked by _score is not implemented on the GPU path");
+      for (uint32_t i = 0; i < n.num_children; i++) {
+        const QwPlanNode& c = nodes[n.first_child + i];
+        if (c.kind != QW_NODE_RANGE || c.column != n.column || c.lo != c.hi)
+          fail(QWGPU_EINVALID_ARG, "column set child %u is not a single value of the node's column", i);
+        if (i && c.lo <= nodes[n.first_child + i - 1].lo) fail(QWGPU_EINVALID_ARG, "column set children not in increasing value order");
+      }
+      in.op = OP_COL_SET;
+      in.r = use_col(L, sp, n.column);
+      in.a = L.bounds.size();
+      if (n.column != 0xFFFFFFFFu) {
+        L.range_cols.push_back({n.column, 0});
+        const QwImgColumn& ic = sp.view.columns[n.column];
+        const uint64_t g = ic.gcd ? ic.gcd : 1;
+        for (uint32_t i = 0; i < n.num_children && ic.num_vals; i++) {
+          const uint64_t v = nodes[n.first_child + i].lo;
+          if (v >= ic.min_value && v <= ic.max_value && (v - ic.min_value) % g == 0) L.bounds.push_back((v - ic.min_value) / g);
+        }
+      }
+      in.n = (uint32_t)(L.bounds.size() - in.a);
+      if (in.n == 0) in.r = 0xFFFFFFFFu;  // no value can match: like a range that misses the column
+      if (in.r == 0xFFFFFFFFu && level == 0 && (occur == QW_OCCUR_MUST || occur == QW_OCCUR_FILTER)) L.empty = true;
       L.instrs.push_back(in);
       break;
     }
@@ -983,7 +1019,7 @@ static void lower_plan(Lowered& L, const SplitDev& sp, const uint8_t* plan, size
     }
     L.P.fused_score_root = pure ? 1 : 0;
   }
-  if (L.instrs.size() > QW_MAX_INSTR) fail(QWGPU_EUNSUPPORTED, "query too large for the GPU program (%zu > %d instructions)", L.instrs.size(), QW_MAX_INSTR);
+  if (!qw_program_fits(L.P.n_terms, L.instrs.size())) fail(QWGPU_EUNSUPPORTED, "query too large for the GPU program (%zu > %d instructions)", L.instrs.size(), QW_MAX_INSTR);
   P.n_instr = (uint32_t)L.instrs.size();
   uint32_t nl = 0;
   while (L.levels >> nl) nl++;
@@ -1135,7 +1171,7 @@ static bool union_eligible(const Lowered& L) {
 }
 
 // one driving posting list + required column filters, no aggregations: the posting-driven kernel
-// (driver_kernel.cuh). [BOOL_BEGIN, TERM, (RANGE | EXISTS) x 0..4, BOOL_END] at level 0.
+// (driver_kernel.cuh). [BOOL_BEGIN, TERM, (RANGE | EXISTS | COL_SET) x 0..4, BOOL_END] at level 0.
 static bool driver_eligible(const Lowered& L) {
   const std::vector<DInstr>& I = L.instrs;
   if (!(L.P.n_aggs == 0 && I.size() >= 3 && I.size() <= 3 + QD_MAX_FILTERS && I[0].op == OP_BOOL_BEGIN && I[1].op == OP_TERM &&
@@ -1144,7 +1180,7 @@ static bool driver_eligible(const Lowered& L) {
   const bool req = I[1].occur == QW_OCCUR_MUST || I[1].occur == QW_OCCUR_FILTER;
   if (!req && !(I[1].occur == QW_OCCUR_SHOULD && I.size() == 3 && I.back().r == 1 && I.back().n == 0)) return false;
   for (size_t k = 2; k + 1 < I.size(); k++) {
-    const bool colpred = I[k].op == OP_RANGE || I[k].op == OP_EXISTS;
+    const bool colpred = I[k].op == OP_RANGE || I[k].op == OP_EXISTS || I[k].op == OP_COL_SET;
     const bool unscored_req = I[k].occur == QW_OCCUR_FILTER || (I[k].occur == QW_OCCUR_MUST && !(I[k].flags & IF_SCORED));
     if (!colpred || !unscored_req || I[k].level != 0) return false;
   }
@@ -1275,7 +1311,7 @@ static Route choose_route(const std::vector<Lowered>& low, int max_smem_optin, i
     all_driver = all_driver && driver_eligible(L);
     if (L.P.max_hits && L.P.key.kind[0] == QW_SORT_SCORE) rec_l0 = false;
     for (const DInstr& in : L.instrs)
-      if ((in.op == OP_RANGE || in.op == OP_EXISTS) && (in.occur == QW_OCCUR_MUST || in.occur == QW_OCCUR_FILTER)) rangeq = true;
+      if ((in.op == OP_RANGE || in.op == OP_EXISTS || in.op == OP_COL_SET) && (in.occur == QW_OCCUR_MUST || in.occur == QW_OCCUR_FILTER)) rangeq = true;
     n_levels = std::max(n_levels, L.P.n_levels);
     need_cnt |= L.need_cnt; need_ssum |= L.need_ssum; need_msum |= L.need_msum;
     max_instr = std::max(max_instr, L.P.n_instr); max_cols = std::max(max_cols, L.P.n_cols); max_aggs = std::max(max_aggs, L.P.n_aggs);
@@ -1638,6 +1674,10 @@ struct Run {
       }
       if (L.fill) P.match_out = (uint64_t)L.fill->d_bits;
       memcpy(hb + o_instr + P.instr_base * sizeof(DInstr), L.instrs.data(), P.n_instr * sizeof(DInstr));
+      // (lowering left each column set's table as an index into the split's tables, like the histograms' below)
+      DInstr* instrs = (DInstr*)(hb + o_instr) + P.instr_base;
+      for (uint32_t k = 0; k < P.n_instr; k++)
+        if (instrs[k].op == OP_COL_SET) instrs[k].a = (uint64_t)(db + o_bounds) + (bounds_base[i] + instrs[k].a) * 8;
       memcpy(hb + o_plans + i * sizeof(DSplitPlan), &P, sizeof P);
       if (P.n_cols) memcpy(hb + o_cols + P.col_base * sizeof(DCol), L.cols.data(), P.n_cols * sizeof(DCol));
       DAgg* aggs = (DAgg*)(hb + o_aggs) + P.agg_base;

@@ -121,15 +121,27 @@ __device__ __forceinline__ void col_range(const uint8_t* base, const DCol& c, ui
   a = __ldg(start + d);
   b = __ldg(start + d + 1);
 }
-// OP_EXISTS: doc d has a value in column c; OP_RANGE: some value of doc d lies in [lo, hi]
+// OP_EXISTS: doc d has a value in column c; OP_RANGE: some value of doc d lies in [lo, hi]; OP_COL_SET: some raw
+// value of doc d is in the sorted table at address lo of hi entries (at most QW_MAX_SET_TERMS: 17 halvings)
 __device__ __forceinline__ bool col_match(const uint8_t* base, const DCol& c, uint32_t d, uint32_t op, uint64_t lo, uint64_t hi) {
   uint64_t a, b;
   col_range(base, c, d, a, b);
   if (op == OP_EXISTS) return a != b;
   bool hit = false;
   for (uint64_t k = a; k < b && !hit; k++) {
-    const uint64_t mv = c.min_value + c.gcd * col_raw(base, c, k);
-    hit = mv >= lo && mv <= hi;
+    if (op == OP_COL_SET) {
+      const uint64_t raw = col_raw(base, c, k), *tab = (const uint64_t*)lo;
+      uint32_t first = 0, len = (uint32_t)hi;
+      while (len) {
+        const uint32_t half = len >> 1;
+        if (__ldg(tab + first + half) < raw) { first += half + 1; len -= half + 1; }
+        else len = half;
+      }
+      hit = first < hi && __ldg(tab + first) == raw;
+    } else {
+      const uint64_t mv = c.min_value + c.gcd * col_raw(base, c, k);
+      hit = mv >= lo && mv <= hi;
+    }
   }
   return hit;
 }
@@ -1255,14 +1267,14 @@ __global__ void __launch_bounds__(QW_THREADS, QW_MIN_BLOCKS_PER_SM) k_window(con
         if (required) req_init |= 1u << level;
         __syncthreads();
         ip++;
-      } else if (op == OP_RANGE || op == OP_EXISTS || op == OP_ALL) {
+      } else if (op == OP_RANGE || op == OP_EXISTS || op == OP_ALL || op == OP_COL_SET) {
         const bool required = occur == QW_OCCUR_MUST || occur == QW_OCCUR_FILTER;
         const bool init = (req_init >> level) & 1;
         const bool gather = required && init;
         uint32_t* req = sm.u32(LV.req);
         const uint32_t col = in.r;
         const bool has_col = op == OP_ALL || col != 0xFFFFFFFFu;
-        const uint64_t lo = in.a, hi = in.b;
+        const uint64_t lo = in.a, hi = op == OP_COL_SET ? in.n : in.b;
         const float boost = in.f;
         if (gather && op != OP_ALL && p.sm.rangeq != 0xFFFFFFFFu) {
           // required clause over an already narrowed candidate set: probe only the surviving docs,

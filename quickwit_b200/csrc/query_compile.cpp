@@ -16,6 +16,7 @@
 #include <algorithm>
 #include <cctype>
 #include <climits>
+#include <map>
 
 #include "compile.h"
 #include "ip_addr.h"
@@ -130,10 +131,12 @@ static int64_t truncate_ns(int64_t ns, int64_t prec) {  // DateTime::truncate
 
 // ---- TantivyQueryAst mirror ------------------------------------------------------------------------
 struct TQ {
-  enum Kind { Bool, Term, Range, Exists, All, None, Phrase, PhrasePrefix, TermSet, Cache } kind = None;  // Cache: must[0]
+  enum Kind { Bool, Term, Range, Exists, All, None, Phrase, PhrasePrefix, TermSet, ColSet, Cache } kind = None;  // Cache: must[0]
   std::vector<uint32_t> phrase_terms;  // Phrase / PhrasePrefix: (exact) term ords in phrase order (offset k = position k)
   std::vector<uint32_t> prefix_terms;  // PhrasePrefix: the expansions of the last slot (offset = phrase_terms.size());
                                        // TermSet: the term ords of one field, ascending
+  std::vector<uint64_t> set_values;    // ColSet: the values of `column` (mapped-u64 space), ascending
+  int group = -1;  // a leaf of a set group (set_groups_to_nodes): the group's number, in query order
   bool opaque = false;  // wrapped in a BoostQuery leaf: not subject to bool flattening / const folding
   std::vector<TQ> must, must_not, should, filter;
   bool has_msm = false;
@@ -286,6 +289,7 @@ struct Ctx {
   const DocMapperInfo& dm;
   bool scoring = false;             // the request ranks by _score
   mutable int unscored_depth = 0;   // > 0 while building a must_not / filter subtree (its scores are never read)
+  mutable int groups = 0;           // set groups numbered so far
 };
 
 // Constant-score set queries (TermSetQuery, wildcard -> AutomatonWeight): tantivy gives every matching document the
@@ -406,10 +410,12 @@ static TQ phrase_prefix_leaf(const Ctx& cx, uint32_t f, const std::vector<std::s
   if (tokens.size() > 1) return ph;
   TQ b;
   b.kind = TQ::Bool;
+  const int group = cx.groups++;
   for (uint32_t t : ph.prefix_terms) {
     TQ leaf;
     leaf.kind = TQ::Term;
     leaf.term_ord = t;
+    leaf.group = group;
     b.should.push_back(std::move(leaf));
   }
   TQ outer;
@@ -719,6 +725,7 @@ static TQ build(const Ctx& cx, const Json& q, int depth) {
     TQ b;
     b.kind = TQ::Bool;
     const QwImgField& F = cx.img.fields[f];
+    const int group = cx.groups++;
     std::string folded;
     for (uint32_t t = F.first_term; t < F.first_term + F.num_terms; t++) {
       const QwImgTerm& T = cx.img.terms[t];
@@ -728,6 +735,7 @@ static TQ build(const Ctx& cx, const Json& q, int depth) {
       TQ leaf;
       leaf.kind = TQ::Term;
       leaf.term_ord = t;
+      leaf.group = group;
       b.should.push_back(std::move(leaf));
     }
     if (b.should.empty()) return tq_none();
@@ -741,8 +749,13 @@ static TQ build(const Ctx& cx, const Json& q, int depth) {
     TQ b;
     b.kind = TQ::Bool;
     if (const Json* tpf = q.get("terms_per_field"))
-      for (auto& kv : tpf->obj)
-        for (auto& v : kv.second.arr) b.should.push_back(full_text(cx, kv.first, lit_str(v), "raw", "bool", false, 0, true));
+      for (auto& kv : tpf->obj) {
+        const int group = cx.groups++;  // one set group per field
+        for (auto& v : kv.second.arr) {
+          b.should.push_back(full_text(cx, kv.first, lit_str(v), "raw", "bool", false, 0, true));
+          b.should.back().group = group;
+        }
+      }
     if (b.should.empty()) return tq_none();
     // TermSetQuery is a constant-score set membership test: wrap as filter so it never scores
     TQ outer;
@@ -864,6 +877,22 @@ static void emit(const TQ& t, uint32_t occur, const ImageView& img, std::vector<
       }
       break;
     }
+    case TQ::ColSet: {
+      // never scored (refused in scoring clauses under _score ranking): children = one RANGE lo == hi per value, ascending
+      n.kind = QW_NODE_COL_SET;
+      n.column = t.column;
+      const size_t first = out.size(), e = t.set_values.size();  // (`n` dangles after the resize below)
+      out[idx].first_child = (uint32_t)first;
+      out[idx].num_children = (uint32_t)e;
+      out.resize(first + e);
+      for (size_t i = 0; i < e; i++) {
+        QwPlanNode& c = out[first + i];
+        memset(&c, 0, sizeof c);
+        c.kind = QW_NODE_RANGE; c.occur = QW_OCCUR_SHOULD; c.boost = 1.0f; c.min_should_match = 0xFFFFFFFFu;
+        c.term_ord = 0xFFFFFFFFu; c.column = t.column; c.lo = c.hi = t.set_values[i];
+      }
+      break;
+    }
     case TQ::Cache: {
       n.kind = QW_NODE_CACHE;
       const size_t first = out.size();  // (`n` dangles after the resize below)
@@ -891,6 +920,93 @@ static void emit(const TQ& t, uint32_t occur, const ImageView& img, std::vector<
       break;
     }
   }
+}
+
+// ---- set groups -> set nodes (DESIGN §4.8) -------------------------------------------------------------
+// A set group is the leaves of one wildcard, of one one-token prefix, or of one term_set on one field: TERM leaves of
+// one text / indexed `ip` field, or RANGE lo == hi leaves of one fast column. Each compiles to one plan leaf per value,
+// as a should clause, unless the plan would then not fit the window program: then groups become set nodes, the largest
+// first (ties in query order), until it fits.
+
+// The instructions and TERM instructions the plan at nodes[i] lowers to (lower_node, engine.cu), with every CACHE node
+// lowered as its child: the lowering every plan with cache nodes also goes through
+static void program_size(const std::vector<QwPlanNode>& nodes, uint32_t i, uint64_t& terms, uint64_t& instrs) {
+  const QwPlanNode& n = nodes[i];
+  if (n.kind == QW_NODE_CACHE) return program_size(nodes, n.first_child, terms, instrs);
+  if (n.kind == QW_NODE_TERM) terms++;
+  instrs += n.kind == QW_NODE_BOOL ? 2 : 1;  // a bool: its BOOL_BEGIN / BOOL_END around the children
+  if (n.kind == QW_NODE_BOOL)
+    for (uint32_t c = 0; c < n.num_children; c++) program_size(nodes, n.first_child + c, terms, instrs);
+}
+// lower_plan's root rule: a root that is not a bool gets a bool around it
+static bool plan_fits(const std::vector<QwPlanNode>& nodes, bool scoring) {
+  uint32_t root = 0;
+  while (nodes[root].kind == QW_NODE_CACHE) root = nodes[root].first_child;
+  uint64_t terms = 0, instrs = nodes[root].kind == QW_NODE_BOOL ? 0 : 2;
+  program_size(nodes, root, terms, instrs);
+  return qw_program_fits(terms, instrs);
+}
+
+static void group_sizes(const TQ& t, std::map<int, size_t>& sizes) {
+  if (t.group >= 0) sizes[t.group]++;
+  for (auto* vec : {&t.must, &t.should, &t.must_not, &t.filter})
+    for (const TQ& c : *vec) group_sizes(c, sizes);
+}
+
+// The set node of a group's leaves: their present values, sorted and deduplicated; none present: match-nothing
+static TQ set_node(const std::vector<TQ>& leaves) {
+  TQ s;
+  for (const TQ& l : leaves) {
+    if (l.kind == TQ::Term && l.term_ord != 0xFFFFFFFFu) { s.kind = TQ::TermSet; s.prefix_terms.push_back(l.term_ord); }
+    if (l.kind == TQ::Range) { s.kind = TQ::ColSet; s.column = l.column; s.set_values.push_back(l.lo); }
+  }
+  std::sort(s.prefix_terms.begin(), s.prefix_terms.end());
+  s.prefix_terms.erase(std::unique(s.prefix_terms.begin(), s.prefix_terms.end()), s.prefix_terms.end());
+  std::sort(s.set_values.begin(), s.set_values.end());
+  s.set_values.erase(std::unique(s.set_values.begin(), s.set_values.end()), s.set_values.end());
+  const size_t e = s.prefix_terms.size() + s.set_values.size();
+  if (e > QW_MAX_SET_TERMS)
+    fail(QWGPU_EUNSUPPORTED, "term set with %zu values in split (the GPU path takes at most %d)", e, QW_MAX_SET_TERMS);
+  return e ? s : tq_none();
+}
+
+// Replaces the leaves of group g, wherever a clause list holds them, by their set node
+static void group_to_set_node(TQ& t, int g) {
+  for (auto* vec : {&t.must, &t.should, &t.must_not, &t.filter}) {
+    std::vector<TQ> leaves, kept;
+    size_t at = 0;
+    for (TQ& c : *vec) {
+      if (c.group != g) { kept.push_back(std::move(c)); continue; }
+      if (leaves.empty()) at = kept.size();
+      leaves.push_back(std::move(c));
+    }
+    if (!leaves.empty()) kept.insert(kept.begin() + at, set_node(leaves));
+    *vec = std::move(kept);
+    for (TQ& c : *vec) group_to_set_node(c, g);
+  }
+}
+
+// The plan nodes of `root`, with as many set groups turned into set nodes as the window program needs
+static std::vector<QwPlanNode> emit_fitted(TQ root, const Ctx& cx) {
+  std::vector<QwPlanNode> nodes(1);
+  emit(root, QW_OCCUR_MUST, cx.img, nodes, 0);
+  if (plan_fits(nodes, cx.scoring)) return nodes;
+  std::map<int, size_t> sizes;
+  group_sizes(root, sizes);
+  std::vector<std::pair<int, size_t>> order(sizes.begin(), sizes.end());  // (query order)
+  std::stable_sort(order.begin(), order.end(), [](const auto& a, const auto& b) { return a.second > b.second; });
+  for (const auto& g : order) {
+    // (the whole root may be the group's one leaf)
+    TQ holder;
+    holder.kind = TQ::Bool;
+    holder.must.push_back(std::move(root));
+    group_to_set_node(holder, g.first);
+    root = simplify(std::move(holder.must[0]));
+    nodes.assign(1, QwPlanNode{});
+    emit(root, QW_OCCUR_MUST, cx.img, nodes, 0);
+    if (plan_fits(nodes, cx.scoring)) break;
+  }
+  return nodes;  // (a plan that still does not fit is refused by lowering)
 }
 
 // ---- search_after conversion (collector.rs:214-372) ---------------------------------------------------
@@ -1007,8 +1123,7 @@ CompiledPlan compile_plan(const ImageView& img, const std::string& split_id, con
   root = simplify(std::move(root));
 
   CompiledPlan cp;
-  std::vector<QwPlanNode> nodes(1);
-  emit(root, QW_OCCUR_MUST, img, nodes, 0);
+  const std::vector<QwPlanNode> nodes = emit_fitted(std::move(root), cx);
 
   QwPlanHeader h;
   memset(&h, 0, sizeof h);

@@ -24,6 +24,7 @@ NODE_TERM, NODE_RANGE, NODE_BOOL, NODE_ALL, NODE_NONE, NODE_EXISTS, NODE_PHRASE 
 NODE_PHRASE_PREFIX = 8
 NODE_TERM_SET = 9  # children: 1..MAX_SET_TERMS TERM nodes of one field, increasing term_ord; never scored
 NODE_CACHE = 10  # exactly one child, the subtree whose doc set the predicate cache keeps; never scored
+NODE_COL_SET = 11  # children: 1..MAX_SET_TERMS RANGE nodes lo == hi on the node's column, increasing; never scored
 MAX_PHRASE_TERMS, MAX_PREFIX_EXPANSIONS = 8, 1024
 MAX_PHRASE_LEN = 256  # TERM children of one NODE_PHRASE; above MAX_PHRASE_TERMS they run the long-phrase pre-pass
 MAX_SET_TERMS = 65536

@@ -114,6 +114,18 @@ def term_set(img: SplitImage, field: str, ords: Sequence[int], occur=ffi.OCCUR_F
     return Node(ffi.NODE_TERM_SET, occur, children=kids, field_id=fid)
 
 
+def col_set(img: SplitImage, column: str, values: Sequence[int], occur=ffi.OCCUR_FILTER) -> Node:
+    """A COL_SET node: a doc matches when one of its values in `column` equals one of `values` (mapped-u64 space;
+    sorted and deduplicated here). Never scored. No values: matches nothing."""
+    vals = sorted(set(values))
+    if not vals:
+        return Node(ffi.NODE_NONE, occur)
+    c = img.column_ord(column)
+    c = c if c >= 0 else ffi.ABSENT
+    kids = [Node(ffi.NODE_RANGE, ffi.OCCUR_SHOULD, column=c, lo=v, hi=v) for v in vals]
+    return Node(ffi.NODE_COL_SET, occur, children=kids, column=c)
+
+
 def range_(img: SplitImage, column: str, lo: int, hi: int, occur=ffi.OCCUR_FILTER, boost=1.0) -> Node:
     c = img.column_ord(column)
     return Node(ffi.NODE_RANGE, occur, boost, column=c if c >= 0 else ffi.ABSENT, lo=lo, hi=hi)
