@@ -113,6 +113,23 @@ int qwgpu_set_predicate_cache_budget(qwgpu_ctx* ctx, uint64_t bytes);
 int qwgpu_predicate_cache_info(qwgpu_ctx* ctx, uint64_t* budget_bytes, uint64_t* used_bytes, uint64_t* entries, uint64_t* hits,
                                uint64_t* misses, uint64_t* fills, uint64_t* evictions);
 
+/* Partial-result cache (the reference's LeafSearchCache, quickwit-search/src/leaf_cache.rs:27-185; DESIGN.md §7.1): the
+ * LeafSearchResponse of each successful split search of qwgpu_leaf_search / qwgpu_invoke_leaf_search, in host memory,
+ * keyed by the split id, the doc mapper and the split's request after its rewrite, with the time range replaced by its
+ * intersection with the split's [timestamp_start, timestamp_end]. A split found there is answered without the device
+ * and does not have to be resident; its response reports partial_result_cache_num_splits = 1 and
+ * partial_result_cache_num_docs = the split's num_docs instead of the search's statistics. A dashboard that refreshes
+ * a sliding window searches only the splits at the window's edges again. Registering a split id again or unregistering
+ * it drops its entries; residency eviction does not. qwgpu_leaf_search_allgather does not use the cache.
+ *   qwgpu_set_leaf_cache_budget  bytes of encoded responses the entries may hold, least recently used evicted first
+ *                                (Quickwit's searcher.partial_request_cache_capacity, 64 MB by default there). 0 (the
+ *                                default) disables the cache, drops every entry, and leaves every call as without it.
+ *   qwgpu_leaf_cache_info        budget, bytes held, entries, hits, misses, fills and evictions so far (NULL = not
+ *                                wanted). */
+int qwgpu_set_leaf_cache_budget(qwgpu_ctx* ctx, uint64_t bytes);
+int qwgpu_leaf_cache_info(qwgpu_ctx* ctx, uint64_t* budget_bytes, uint64_t* used_bytes, uint64_t* entries, uint64_t* hits,
+                          uint64_t* misses, uint64_t* fills, uint64_t* evictions);
+
 /* ---- seam A / B: protobuf in, protobuf out ---------------------------------------------------- */
 
 /* req = quickwit.search.LeafSearchRequest, resp = quickwit.search.LeafSearchResponse
@@ -260,6 +277,11 @@ int qwgpu_format_ip(const uint8_t* addr16, char* out, uint64_t cap);
  * `json_out` (qwgpu_buf_free) = [{"split_id", "max_hits", "hits_disabled", "metadata_count", "skipped"}, ...] in the
  * reference's processing order, one entry per split of the request. */
 int qwgpu_optimize_leaf_request(const uint8_t* leaf_search_request_pb, size_t req_len, uint8_t** json_out, size_t* json_len);
+/* Host only: the partial-result cache key of every split of a LeafSearchRequest, as qwgpu_leaf_search would look it
+ * up. `json_out` (qwgpu_buf_free) = [{"split_id", "looked_up", "key", "range"}, ...] in the reference's processing
+ * order: looked_up = false for a skipped or metadata-count split (never looked up), key = the key's bytes in hex, and
+ * range = [start, end] of the merged time range (end null = unbounded; an empty range is [0, 0]). */
+int qwgpu_leaf_cache_keys(const uint8_t* leaf_search_request_pb, size_t req_len, uint8_t** json_out, size_t* json_len);
 
 /* ---- merge / finalize -------------------------------------------------------------------------- */
 

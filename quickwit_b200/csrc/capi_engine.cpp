@@ -102,6 +102,29 @@ int qwgpu_predicate_cache_info(qwgpu_ctx* ctx, uint64_t* budget_bytes, uint64_t*
   QW_API_END
 }
 
+int qwgpu_set_leaf_cache_budget(qwgpu_ctx* ctx, uint64_t bytes) {
+  QW_API_BEGIN
+  engine_of(ctx).leaf.set_budget(bytes);
+  return 0;
+  QW_API_END
+}
+
+int qwgpu_leaf_cache_info(qwgpu_ctx* ctx, uint64_t* budget_bytes, uint64_t* used_bytes, uint64_t* entries, uint64_t* hits,
+                          uint64_t* misses, uint64_t* fills, uint64_t* evictions) {
+  QW_API_BEGIN
+  qw::LeafCache& c = engine_of(ctx).leaf;
+  std::lock_guard<std::mutex> g(c.mu);
+  if (budget_bytes) *budget_bytes = c.budget;
+  if (used_bytes) *used_bytes = c.used;
+  if (entries) *entries = c.lru.size();
+  if (hits) *hits = c.hits;
+  if (misses) *misses = c.misses;
+  if (fills) *fills = c.fills;
+  if (evictions) *evictions = c.evictions;
+  return 0;
+  QW_API_END
+}
+
 int qwgpu_residency_info(qwgpu_ctx* ctx, uint64_t* resident_bytes, uint64_t* budget_bytes, uint64_t* num_splits, uint64_t* evictions) {
   QW_API_BEGIN
   qw::Engine& e = engine_of(ctx);

@@ -339,6 +339,7 @@ void Engine::register_split(const char* id, const uint8_t* img, uint64_t len) {
   CUDA_CHECK(cudaMemcpy(sp->d_tabs, tabs.data(), tabs.size() * sizeof(float), cudaMemcpyHostToDevice));
   std::lock_guard<std::mutex> g(mu);
   publish(*this, sp);
+  leaf.drop_split(sp->id);  // (after the publish: a search that reads the cache from here on finds the new image)
 }
 
 // Background upload: the split is visible (loading) at once; a loader thread stages the data region through two
@@ -360,6 +361,7 @@ void Engine::register_split_async(const char* id, const uint8_t* img, uint64_t l
   CUDA_CHECK(cudaMalloc(&sp->d_tabs, tabs.size() * sizeof(float)));
   std::lock_guard<std::mutex> g(mu);
   publish(*this, sp);
+  leaf.drop_split(sp->id);
   // loaders that have finished (state set, lock released) are reaped here
   for (size_t i = 0; i < loaders.size();) {
     if (loaders[i].sp->state != 0) { loaders[i].t.join(); loaders[i] = std::move(loaders.back()); loaders.pop_back(); }
@@ -423,6 +425,7 @@ void Engine::unregister_split(const char* id) {
   if (it != splits.end() && it->second == sp) { resident -= sp->data_len; splits.erase(it); }
   sp.reset();  // (the last reference, unless a call still uses the split: its cache entries go with it)
   pred.free_released(nullptr);
+  leaf.drop_split(id);
 }
 
 // A search takes the split in use: recency for the LRU; a split that is still loading is waited for.

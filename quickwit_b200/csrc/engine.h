@@ -2,6 +2,7 @@
 #pragma once
 #include <condition_variable>
 #include <atomic>
+#include <list>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -47,6 +48,33 @@ struct PredCache {
   bool evict_to(uint64_t limit);
   void drop_split(const SplitDev* sp);
   void free_released(void* stream);  // cudaFreeAsync of the released bitmaps on `stream`
+};
+
+// The context's partial-result cache (LeafSearchCache, quickwit-search/src/leaf_cache.rs:27-117; DESIGN.md §7.1): the
+// encoded LeafSearchResponse of a successful split search, keyed by the split and the normalised per-split request
+// (leaf_cache_key, leaf.cpp). LRU within a budget of encoded response bytes, like MemorySizedCache (keys are not
+// counted). Host memory only: an entry outlives the split's residency, and registering a split id again or
+// unregistering it drops its entries.
+struct LeafCache {
+  struct Entry {
+    std::string key, split_id, value;
+  };
+  std::mutex mu;  // guards everything below; taken under Engine::mu (never the other way round), and held only for
+                  // map updates and copies, never during a search or a merge
+  uint64_t budget = 0, used = 0;
+  uint64_t hits = 0, misses = 0, fills = 0, evictions = 0;
+  std::list<Entry> lru;  // most recently used first
+  std::unordered_map<std::string, std::list<Entry>::iterator> index;
+  bool on() {
+    std::lock_guard<std::mutex> g(mu);
+    return budget != 0;
+  }
+  bool get(const std::string& key, std::string* value);  // true and the entry's bytes on a hit
+  // stores unless the value alone exceeds the budget; the caller holds Engine::mu and has checked that the split
+  // the value was computed on is still the registered one
+  void put(const std::string& split_id, const std::string& key, std::string value);
+  void set_budget(uint64_t bytes);
+  void drop_split(const std::string& split_id);
 };
 
 struct SplitDev {
@@ -118,6 +146,7 @@ struct Engine {
   int device = -1;
   std::mutex mu;
   PredCache pred;  // (declared before `splits`: a split's destructor drops its entries here)
+  LeafCache leaf;  // off until qwgpu_set_leaf_cache_budget
   std::map<std::string, std::shared_ptr<SplitDev>> splits;
   std::vector<CallSlot*> free_slots;
   std::atomic<int> in_flight{0};  // searches between slot acquisition and release

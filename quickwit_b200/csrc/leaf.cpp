@@ -9,6 +9,8 @@
 //   * qwgpu_invoke_leaf_search LambdaLeafSearchInvoker::invoke_leaf_search (invoker.rs:27-38;
 //                             handler template quickwit-lambda-server/src/handler.rs:55-200)
 //   * partial exchange for the multi-GPU root merge stand-in (SURVEY.md §8e)
+//   * LeafCache               LeafSearchCache (quickwit-search/src/leaf_cache.rs:27-185), read and written like
+//                             leaf.rs:510-517,695-705,1872-1896
 #include <algorithm>
 #include <chrono>
 #include <tuple>
@@ -192,6 +194,8 @@ struct SplitJob {
   std::string error;
   int error_code = 0;
   bool metadata_count = false;  // answered from the split's num_docs alone (no plan, no device work)
+  std::string cache_key;        // the split's partial-result cache key (empty: the cache is off)
+  std::optional<std::string> cached;  // a cache hit: the split's encoded response (no plan, no device work)
 };
 
 struct LeafRun {
@@ -205,6 +209,7 @@ struct LeafRun {
   std::vector<MergedHit> merged;   // best-first; .split = index into `jobs` (gathered: global split rank)
   bool gathered = false;           // `merged` is the cross-rank result; rank_headers[r] = rank r's counters
   std::vector<RankHeader> rank_headers;
+  bool use_cache = false;          // the partial-result cache was on for this call (no device merge: see §7.1)
 };
 
 static bool same_sort_types(const std::vector<SplitJob>& jobs, const std::vector<size_t>& which) {
@@ -345,6 +350,144 @@ static std::vector<SplitRequest> optimize_split_requests(const pb::SearchRequest
 // fails the same way on every node, and retrying would only run it twice.
 static inline bool retryable(int code) { return code != QWGPU_EUNSUPPORTED; }
 
+// ---- partial-result cache (LeafSearchCache, leaf_cache.rs:27-185) ---------------------------------------------
+// HalfOpenRange (leaf_cache.rs:120-185): [start, end), no end = unbounded above; every empty range normalises to 0..0
+struct HalfOpenRange {
+  int64_t start = 0;
+  std::optional<int64_t> end;
+  enum Bound { Unbounded, Included, Excluded };
+  bool is_empty() const { return end && start >= *end; }  // !contains(start)
+  HalfOpenRange normalize() const { return is_empty() ? HalfOpenRange{0, int64_t(0)} : *this; }
+  static HalfOpenRange from_bounds(Bound sk, int64_t s, Bound ek, int64_t e) {
+    HalfOpenRange r;
+    if (sk == Included) r.start = s;
+    else if (sk == Excluded) {
+      if (s == INT64_MAX) return HalfOpenRange{0, int64_t(0)};  // excluding i64::MAX from below: empty
+      r.start = s + 1;
+    } else r.start = INT64_MIN;
+    if (ek == Included) { if (e != INT64_MAX) r.end = e + 1; }  // including i64::MAX above: unbounded
+    else if (ek == Excluded) r.end = e;
+    return r.normalize();
+  }
+  HalfOpenRange intersect(const HalfOpenRange& o) const {
+    HalfOpenRange r;
+    r.start = std::max(start, o.start);
+    r.end = end && o.end ? std::optional<int64_t>(std::min(*end, *o.end)) : (end ? end : o.end);
+    return r.normalize();
+  }
+};
+
+// CacheKey::from_split_meta_and_request (leaf_cache.rs:98-117): the split, the request without its time range and with
+// count_hits = CountAll (at the scale of one split every hit is counted), and the merged time range: the request's
+// [start_timestamp, end_timestamp) intersected with the split's [timestamp_start, timestamp_end]
+// (SearchRequest::time_range / SplitIdAndFooterOffsets::time_range, quickwit-proto/src/search/mod.rs:33-51). So a
+// window that covers the whole split keys like any other window that does. Requests compare by their encoded bytes.
+// The reference keys on the split id alone; here every request carries its own doc mapper, and the doc mapper decides
+// how the split is read (fields, tokenizers, the timestamp field), so the doc mapper string is part of the key: a
+// split searched through a changed mapper must not hit the entry of the old one. It costs nothing while a split's
+// mapper stays the same.
+static std::string leaf_cache_key(const pb::SplitIdAndFooterOffsets& split, pb::SearchRequest req, const std::string& doc_mapper,
+                                  HalfOpenRange* range_out = nullptr) {
+  using R = HalfOpenRange;
+  const R split_range = R::from_bounds(split.timestamp_start ? R::Included : R::Unbounded, split.timestamp_start.value_or(0),
+                                       split.timestamp_end ? R::Included : R::Unbounded, split.timestamp_end.value_or(0));
+  const R req_range = R::from_bounds(req.start_timestamp ? R::Included : R::Unbounded, req.start_timestamp.value_or(0),
+                                     req.end_timestamp ? R::Excluded : R::Unbounded, req.end_timestamp.value_or(0));
+  const R merged = req_range.intersect(split_range);
+  if (range_out) *range_out = merged;
+  req.start_timestamp.reset();
+  req.end_timestamp.reset();
+  req.count_hits = 0;  // CountHits::CountAll
+  std::string key;
+  auto field = [&](const std::string& b) {
+    const uint64_t n = b.size();
+    key.append((const char*)&n, 8);
+    key += b;
+  };
+  field(split.split_id);
+  field(doc_mapper);
+  field(pb::encode_search_request(req));
+  const int64_t r[3] = {merged.start, merged.end ? 1 : 0, merged.end.value_or(0)};
+  key.append((const char*)r, sizeof r);
+  return key;
+}
+
+bool LeafCache::get(const std::string& key, std::string* value) {
+  std::lock_guard<std::mutex> g(mu);
+  auto it = index.find(key);
+  if (it == index.end()) { misses++; return false; }
+  hits++;
+  lru.splice(lru.begin(), lru, it->second);
+  *value = it->second->value;
+  return true;
+}
+
+void LeafCache::put(const std::string& split_id, const std::string& key, std::string value) {
+  std::lock_guard<std::mutex> g(mu);
+  if (value.size() > budget) return;  // (also when the cache is off) MemorySizedCache drops what exceeds its capacity
+  auto it = index.find(key);
+  if (it != index.end()) {  // (a concurrent call filled the same key first: the newer value replaces it)
+    used -= it->second->value.size();
+    lru.erase(it->second);
+    index.erase(it);
+  }
+  while (used + value.size() > budget) {
+    used -= lru.back().value.size();
+    index.erase(lru.back().key);
+    lru.pop_back();
+    evictions++;
+  }
+  used += value.size();
+  lru.push_front(Entry{key, split_id, std::move(value)});
+  index[key] = lru.begin();
+  fills++;
+}
+
+void LeafCache::set_budget(uint64_t bytes) {
+  std::lock_guard<std::mutex> g(mu);
+  budget = bytes;
+  while (used > budget) {
+    used -= lru.back().value.size();
+    index.erase(lru.back().key);
+    lru.pop_back();
+    evictions++;
+  }
+}
+
+void LeafCache::drop_split(const std::string& split_id) {
+  std::lock_guard<std::mutex> g(mu);
+  for (auto it = lru.begin(); it != lru.end();) {
+    if (it->split_id != split_id) { ++it; continue; }
+    used -= it->value.size();
+    index.erase(it->key);
+    it = lru.erase(it);
+  }
+}
+
+// LeafSearchCache::put (leaf_cache.rs:66-80): the split's response with its resource stats replaced by the cache-hit
+// counters, so that a hit reports itself
+static std::string cache_value(const SplitJob& j, pb::LeafSearchResponse r) {
+  pb::LeafResourceStats s;
+  s.partial_result_cache_num_splits = 1;
+  s.partial_result_cache_num_docs = j.meta.num_docs;
+  r.resource_stats = s;
+  return pb::encode_leaf_search_response(r);
+}
+
+// Stores the (job index, cache_value) pairs of one call. Only successful searches come here (leaf.rs:695-705 stores
+// the response of leaf_search_single_split when a search ran; a failed, pruned or metadata-count split stores
+// nothing). A value is kept only while its split id still names the image it was computed on: under Engine::mu,
+// against the registration that drops the split's entries (Engine::register_split / unregister_split).
+static void store_responses(Engine& eng, const LeafRun& run, std::vector<std::pair<size_t, std::string>> values) {
+  if (values.empty()) return;
+  std::lock_guard<std::mutex> g(eng.mu);
+  for (auto& v : values) {
+    const SplitJob& j = run.jobs[v.first];
+    auto it = eng.splits.find(j.meta.split_id);
+    if (it != eng.splits.end() && it->second == j.dev) eng.leaf.put(j.meta.split_id, j.cache_key, std::move(v.second));
+  }
+}
+
 // add_top_cache_node (rewrite_request, leaf.rs:724-737): a request with search_after is a page of a paged search, and
 // the pages after it evaluate the same query again. With the context's predicate cache enabled, the query AST is
 // wrapped in a `cache` node, so that each split's doc set is computed once and read by every later page. A request
@@ -373,6 +516,12 @@ static void run_leaf_raw(Engine& eng, const pb::LeafSearchRequest& lr, LeafRun& 
   Json ast = parse_json(sreq.query_ast, QWGPU_EINVALID_QUERY);  // once per request
   Json cached_ast;
   const Json* compile_ast = sreq.search_after && add_top_cache_node(eng, ast, cached_ast) ? &cached_ast : &ast;
+  // the partial-result cache (process_partial_result_cache, leaf.rs:1872-1896): a split is looked up after its request
+  // rewrite and before warmup, so a hit needs neither the split's residency nor a plan. The NCCL road builds its
+  // exchanged record on the device and bypasses the cache. With the cache on, each searched split's own response is
+  // stored, so the per-split lists come back instead of the device merge's list (DESIGN.md §7.1).
+  run.use_cache = !comm && eng.leaf.on();
+  if (run.use_cache) want_merged = false;
   for (auto& ref : lr.leaf_requests) {
     if (ref.doc_mapper_ord >= lr.doc_mappers.size()) fail(QWGPU_EINVALID_ARG, "Internal error: doc_mapper_ord out of bounds");
     DocMapperInfo dm = parse_doc_mapper(lr.doc_mappers[ref.doc_mapper_ord]);
@@ -400,6 +549,15 @@ static void run_leaf_raw(Engine& eng, const pb::LeafSearchRequest& lr, LeafRun& 
         if (!have_count_req) { count_req = sreq; disable_search_request_hits(count_req); have_count_req = true; }
         req = &count_req;
       }
+      if (run.use_cache) {
+        j.cache_key = leaf_cache_key(so, *req, lr.doc_mappers[ref.doc_mapper_ord]);
+        std::string v;
+        if (eng.leaf.get(j.cache_key, &v)) {
+          j.cached = std::move(v);
+          run.jobs.push_back(std::move(j));
+          continue;
+        }
+      }
       j.dev = eng.find(so.split_id);
       try {
         if (!j.dev) fail(QWGPU_ENOTFOUND, "split `%s` is not resident on this GPU", so.split_id.c_str());
@@ -418,7 +576,7 @@ static void run_leaf_raw(Engine& eng, const pb::LeafSearchRequest& lr, LeafRun& 
   std::vector<const uint8_t*> plans;
   std::vector<size_t> lens;
   for (size_t i = 0; i < run.jobs.size(); i++)
-    if (!run.jobs[i].error_code && !run.jobs[i].metadata_count) {
+    if (!run.jobs[i].error_code && !run.jobs[i].metadata_count && !run.jobs[i].cached) {
       devs.push_back(run.jobs[i].dev);
       plans.push_back((const uint8_t*)run.jobs[i].plan.bytes.data());
       lens.push_back(run.jobs[i].plan.bytes.size());
@@ -499,6 +657,9 @@ static std::vector<pb::LambdaSingleSplitResult> run_leaf(Engine& eng, const pb::
       results[i].response = std::move(r);
     }
   }
+  for (size_t i = 0; i < run.jobs.size(); i++)
+    if (run.jobs[i].cached) results[i].response = pb::decode_leaf_search_response((const uint8_t*)run.jobs[i].cached->data(), run.jobs[i].cached->size());
+  std::vector<std::pair<size_t, std::string>> fills;
   for (size_t k = 0; k < run.which.size(); k++) {
     size_t i = run.which[k];
     SplitOutput& o = run.outs[k];
@@ -506,9 +667,11 @@ static std::vector<pb::LambdaSingleSplitResult> run_leaf(Engine& eng, const pb::
     pb::LeafSearchResponse r = build_split_response(run.jobs[i].plan, run.jobs[i].dev->view, run.jobs[i].meta.split_id, o.num_hits,
                                                     o.hits.data(), o.hits.size(), o.cells.data(), o.cells.size(),
                                                     o.entries.data(), o.entries.size(), o.hashed);
+    if (run.use_cache) fills.emplace_back(i, cache_value(run.jobs[i], r));
     r.resource_stats = split_stats(run, k);
     results[i].response = std::move(r);
   }
+  store_responses(eng, run, std::move(fills));
   return results;
 }
 
@@ -586,6 +749,39 @@ static pb::LeafSearchResponse leaf_merge_fast(const pb::SearchRequest& sreq, Lea
   if (sreq.aggregation_request && !sreq.aggregation_request->empty())
     m.intermediate_aggregation_result = build_and_merge_intermediate_aggs(run.jobs[run.which[0]].plan.agg_request, agg_parts);
   if (any_stats) m.resource_stats = stats_acc;
+  return m;
+}
+
+// The leaf merge with the partial-result cache on: each searched split's own response is built and stored, and merged
+// with the cached responses through merge_responses (the IncrementalCollector takes cached and searched responses
+// alike, leaf.rs:1872-1896). The parts keep the request's split order, the order in which leaf_merge_fast folds the
+// same splits' aggregations, so an aggregation merges the same f64 values in the same order with and without the
+// cache. `run` holds the successful searches only.
+static pb::LeafSearchResponse leaf_merge_cached(Engine& eng, const pb::SearchRequest& mreq, LeafRun& run) {
+  std::vector<int> slot(run.jobs.size(), -1);
+  for (size_t k = 0; k < run.which.size(); k++) slot[run.which[k]] = (int)k;
+  std::vector<pb::LeafSearchResponse> parts;
+  std::vector<std::pair<size_t, std::string>> fills;
+  for (size_t i = 0; i < run.jobs.size(); i++) {
+    const SplitJob& j = run.jobs[i];
+    if (j.cached) {
+      parts.push_back(pb::decode_leaf_search_response((const uint8_t*)j.cached->data(), j.cached->size()));
+      continue;
+    }
+    if (slot[i] < 0) continue;  // failed, or answered from the split's metadata
+    const size_t k = (size_t)slot[i];
+    const SplitOutput& o = run.outs[k];
+    pb::LeafSearchResponse r = build_split_response(j.plan, j.dev->view, j.meta.split_id, o.num_hits, o.hits.data(), o.hits.size(),
+                                                    o.cells.data(), o.cells.size(), o.entries.data(), o.entries.size(), o.hashed);
+    fills.emplace_back(i, cache_value(j, r));
+    r.resource_stats = split_stats(run, k);
+    parts.push_back(std::move(r));
+  }
+  store_responses(eng, run, std::move(fills));
+  pb::LeafSearchResponse m;
+  if (!parts.empty()) m = merge_responses(mreq, std::move(parts));
+  else if (mreq.aggregation_request && !mreq.aggregation_request->empty())
+    m.intermediate_aggregation_result = merge_intermediate_aggs(parse_agg_request(*mreq.aggregation_request), {});
   return m;
 }
 
@@ -680,7 +876,9 @@ int qwgpu_leaf_search(qwgpu_ctx* ctx, const uint8_t* req, size_t req_len, uint8_
   }
   const bool same_types = run.merged_valid || qw::same_sort_types(run.jobs, run.which);
   qw::pb::LeafSearchResponse merged;
-  if (run.which.empty()) {
+  if (run.use_cache) {
+    merged = qw::leaf_merge_cached(eng, mreq, run);
+  } else if (run.which.empty()) {
     if (mreq.aggregation_request && !mreq.aggregation_request->empty())
       merged.intermediate_aggregation_result = qw::merge_intermediate_aggs(qw::parse_agg_request(*mreq.aggregation_request), {});
   } else if (same_types) {
@@ -708,8 +906,10 @@ int qwgpu_leaf_search(qwgpu_ctx* ctx, const uint8_t* req, size_t req_len, uint8_
   give(qw::pb::encode_leaf_search_response(merged), resp, resp_len);
   if (trace) {
     auto us = [](tclock::time_point a, tclock::time_point b) { return (long)std::chrono::duration_cast<std::chrono::microseconds>(b - a).count(); };
-    fprintf(stderr, "[qwgpu] leaf_search: decode %ld us, compile+search %ld us (engine wall %lu us, device %.0f us, %u launches), merge %ld us, encode %ld us\n",
-            us(t_start, t_dec), us(t_dec, t_run), (unsigned long)run.wall_us, run.st.gpu_time_us, run.st.launches, us(t_run, t_merge), us(t_merge, tclock::now()));
+    size_t cached = 0;
+    for (auto& j : run.jobs) cached += j.cached ? 1 : 0;
+    fprintf(stderr, "[qwgpu] leaf_search: decode %ld us, compile+search %ld us (engine wall %lu us, device %.0f us, %u launches, %zu splits from the cache), merge %ld us, encode %ld us\n",
+            us(t_start, t_dec), us(t_dec, t_run), (unsigned long)run.wall_us, run.st.gpu_time_us, run.st.launches, cached, us(t_run, t_merge), us(t_merge, tclock::now()));
   }
   return 0;
   QW_API_END
@@ -733,6 +933,38 @@ int qwgpu_optimize_leaf_request(const uint8_t* req, size_t req_len, uint8_t** ou
       js += "{\"split_id\":\"" + id + "\",\"max_hits\":" + std::to_string(q.hits_disabled ? 0 : lr.search_request.max_hits) +
             ",\"hits_disabled\":" + (q.hits_disabled ? "true" : "false") + ",\"metadata_count\":" + (q.metadata_count ? "true" : "false") +
             ",\"skipped\":" + (q.skipped ? "true" : "false") + "}";
+    }
+  }
+  js += "]";
+  give(js, out, out_len);
+  return 0;
+  QW_API_END
+}
+
+// Host only: the partial-result cache key of every split of a LeafSearchRequest as JSON, in the reference's processing
+// order: [{"split_id", "looked_up", "key" (hex), "range": [start, end or null]} ...] per LeafRequestRef (concatenated).
+// looked_up: false for a split that is pruned or answered from its metadata, which the cache never sees.
+int qwgpu_leaf_cache_keys(const uint8_t* req, size_t req_len, uint8_t** out, size_t* out_len) {
+  QW_API_BEGIN
+  if (!req || !out || !out_len) qw::fail(QWGPU_EINVALID_ARG, "null argument");
+  qw::pb::LeafSearchRequest lr = qw::pb::decode_leaf_search_request(req, req_len);
+  qw::Json ast = qw::parse_json(lr.search_request.query_ast, QWGPU_EINVALID_QUERY);
+  std::string js = "[";
+  for (auto& ref : lr.leaf_requests) {
+    if (ref.doc_mapper_ord >= lr.doc_mappers.size()) qw::fail(QWGPU_EINVALID_ARG, "Internal error: doc_mapper_ord out of bounds");
+    qw::DocMapperInfo dm = qw::parse_doc_mapper(lr.doc_mappers[ref.doc_mapper_ord]);
+    for (const qw::SplitRequest& q : qw::optimize_split_requests(lr.search_request, ast, dm.timestamp_field, ref.split_offsets)) {
+      const qw::pb::SplitIdAndFooterOffsets& so = ref.split_offsets[q.input_pos];
+      qw::pb::SearchRequest rr = lr.search_request;
+      if (q.hits_disabled) qw::disable_search_request_hits(rr);
+      qw::HalfOpenRange range;
+      const std::string key = qw::leaf_cache_key(so, rr, lr.doc_mappers[ref.doc_mapper_ord], &range);
+      std::string hex, id;
+      for (unsigned char c : key) { hex += "0123456789abcdef"[c >> 4]; hex += "0123456789abcdef"[c & 15]; }
+      for (char c : so.split_id) { if (c == '"' || c == '\\') id += '\\'; id += c; }
+      if (js.size() > 1) js += ",";
+      js += "{\"split_id\":\"" + id + "\",\"looked_up\":" + (q.skipped || q.metadata_count ? "false" : "true") + ",\"key\":\"" + hex +
+            "\",\"range\":[" + std::to_string(range.start) + "," + (range.end ? std::to_string(*range.end) : "null") + "]}";
     }
   }
   js += "]";

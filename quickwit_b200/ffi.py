@@ -213,6 +213,8 @@ def lib() -> C.CDLL:
     bind("qwgpu_residency_info", [vp, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)])
     bind("qwgpu_set_predicate_cache_budget", [vp, u64])
     bind("qwgpu_predicate_cache_info", [vp] + [C.POINTER(u64)] * 7)
+    bind("qwgpu_set_leaf_cache_budget", [vp, u64])
+    bind("qwgpu_leaf_cache_info", [vp] + [C.POINTER(u64)] * 7)
     bind("qwgpu_split_is_resident", [vp, cp])
     bind("qwgpu_leaf_search", [vp, vp, sz, C.POINTER(vp), C.POINTER(sz)])
     bind("qwgpu_invoke_leaf_search", [vp, vp, sz, C.POINTER(vp), C.POINTER(sz)])
@@ -228,6 +230,7 @@ def lib() -> C.CDLL:
     bind("qwgpu_merge_leaf_responses", [vp, sz, u32, C.POINTER(vp), C.POINTER(sz),
                                         C.POINTER(vp), C.POINTER(sz)])
     bind("qwgpu_optimize_leaf_request", [vp, sz, C.POINTER(vp), C.POINTER(sz)])
+    bind("qwgpu_leaf_cache_keys", [vp, sz, C.POINTER(vp), C.POINTER(sz)])
     bind("qwgpu_parse_split_footer", [vp, u64, u64, C.POINTER(vp), C.POINTER(sz)])
     bind("qwgpu_finalize_aggregation", [cp, vp, sz, C.POINTER(vp)])
     bind("qwgpu_partial_size", [vp, sz, C.POINTER(u64)])

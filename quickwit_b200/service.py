@@ -119,6 +119,17 @@ class SearcherContext:
         names = ("budget_bytes", "used_bytes", "entries", "hits", "misses", "fills", "evictions")
         return dict(zip(names, (int(x.value) for x in v)))
 
+    def set_leaf_cache_budget(self, nbytes: int):
+        """Bytes of encoded leaf responses the partial-result cache may hold (Quickwit's
+        searcher.partial_request_cache_capacity). 0, the default, disables it and drops its entries."""
+        ffi.check(self._L.qwgpu_set_leaf_cache_budget(self._ctx, nbytes))
+
+    def leaf_cache_info(self) -> dict:
+        v = [C.c_uint64() for _ in range(7)]
+        ffi.check(self._L.qwgpu_leaf_cache_info(self._ctx, *[C.byref(x) for x in v]))
+        names = ("budget_bytes", "used_bytes", "entries", "hits", "misses", "fills", "evictions")
+        return dict(zip(names, (int(x.value) for x in v)))
+
     # -- seam C -------------------------------------------------------------------------------------
     def split_search(self, split_ids: Sequence[str], plans: Sequence[bytes]) -> List[SplitSearchResult]:
         n = len(split_ids)
@@ -204,6 +215,18 @@ def optimize_leaf_request(leaf_search_request_pb: bytes) -> list:
     buf = C.create_string_buffer(leaf_search_request_pb, len(leaf_search_request_pb))
     out, n = C.c_void_p(), C.c_size_t()
     ffi.check(L.qwgpu_optimize_leaf_request(C.addressof(buf), len(leaf_search_request_pb), C.byref(out), C.byref(n)))
+    return json.loads(ffi.take_bytes(out, n.value))
+
+
+def leaf_cache_keys(leaf_search_request_pb: bytes) -> list:
+    """The partial-result cache key of every split of a LeafSearchRequest (CacheKey::from_split_meta_and_request,
+    leaf_cache.rs:98-117, plus the doc mapper): [{"split_id", "looked_up", "key", "range"}] in the reference's
+    processing order; `key` is hex, `range` = [start, end or None]. Host only."""
+    import json
+    L = ffi.lib()
+    buf = C.create_string_buffer(leaf_search_request_pb, len(leaf_search_request_pb))
+    out, n = C.c_void_p(), C.c_size_t()
+    ffi.check(L.qwgpu_leaf_cache_keys(C.addressof(buf), len(leaf_search_request_pb), C.byref(out), C.byref(n)))
     return json.loads(ffi.take_bytes(out, n.value))
 
 
