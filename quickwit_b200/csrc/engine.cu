@@ -1844,7 +1844,7 @@ struct Run {
       stats.kernel_mask |= QWGPU_KERNEL_TRACE_SELECT;
     }
     const uint32_t sel_smem = 3 * 8 * QW_CAND_CAP;  // [all first words | 3 x QW_SEL_MAX survivors] or 3 x all (degenerate ties)
-    if (any_topk) { qwk::k_select<<<n, 1024, sel_smem, st>>>(kp.plans, kp.cols); stats.launches++; }
+    if (any_topk) { qwk::k_select<<<dim3(QW_SEL_TILES, n), 1024, sel_smem, st>>>(kp.plans, kp.cols); stats.launches++; }
     if (any_deep) {
       // splits with K > QW_MAX_TOPK (k_select left them): cut, tile sort, rank (deep_select_kernel.cuh)
       uint32_t* d_m = (uint32_t*)(slot.d_scratch + s_deep_m);

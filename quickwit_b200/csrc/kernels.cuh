@@ -1660,149 +1660,87 @@ __device__ __forceinline__ void write_hit(const DSplitPlan& P, const DCol* cols,
 
 // Harvest (quickwit-search/src/top_k_collector.rs:404-410, binary_heap.rs:187-193): the best
 // min(K, n) candidates of a split, best first, decoded back to QwHit (QwScoreHit where P.score_hits).
-//   1. exact radix select (8-bit digits, MSB first) of the K-th largest first key word;
-//   2. compaction of the candidates >= that word (all ties kept) — normally ~K of the ~2-3K candidates;
-//   3. bitonic sort of the survivors with the full 192-bit comparison (the reference total order).
-#define QW_SEL_MAX 2048  /* survivors sorted in shared memory; more ties than this => sort everything */
-__global__ void __launch_bounds__(1024) k_select(const DSplitPlan* plans, const DCol* all_cols) {
-  const DSplitPlan& P = plans[blockIdx.x];
-  const uint32_t tid = threadIdx.x;
-  if (P.max_hits == 0) { if (tid == 0) *(uint32_t*)P.out_nhits = 0; return; }
-  if (P.max_hits > QW_MAX_TOPK) return;  // the deep selection path's split (deep_select_kernel.cuh)
-  uint32_t n = *(const uint32_t*)P.out_cand_count;
-  if (n > QW_CAND_CAP) n = QW_CAND_CAP;  // overflow is detected by the host (cand_count > cap)
-  const uint32_t K = P.max_hits;
-  const uint64_t* src = (const uint64_t*)P.out_cands;
-  // shared memory: all first words [QW_CAND_CAP], then the compacted survivors (3 x sort capacity)
-  uint64_t* a0 = (uint64_t*)qw_smem;
-  __shared__ uint32_t s_hist[256];
-  __shared__ uint32_t s_sel[4];  // [0] digit, [1] count above digit, [2] survivor counter, [3] count in the digit's bin
-  for (uint32_t i = tid; i < n; i += 1024) a0[i] = src[3ull * i];
-  if (tid == 0) s_sel[2] = 0;
-  __syncthreads();
-  uint64_t thr = 0;  // keep candidates with w0 >= thr
-  if (n > K) {
-    uint64_t prefix = 0;
-    uint32_t need = K;  // rank of the wanted element among those matching the prefix
-    // the sort below pads to a power of two anyway: once the candidates above the current bin plus the bin itself
-    // fit that size, the remaining digits need not be resolved (the whole bin is kept)
-    uint32_t cap = 32;
-    while (cap < K) cap <<= 1;
-    for (int shift = 56; shift >= 0; shift -= 8) {
-      if (tid < 256) s_hist[tid] = 0;
-      __syncthreads();
-      const uint64_t himask = shift == 56 ? 0ull : (~0ull << (shift + 8));
-      for (uint32_t base = 0; base < n; base += 1024) {
-        const uint32_t i = base + tid;
-        const uint64_t v = i < n ? a0[i] : 0ull;
-        const bool in = i < n && (v & himask) == prefix;
-        const uint32_t bin = (uint32_t)(v >> shift) & 255u;
-        // candidates near the threshold share their leading digits: one atomic per distinct bin of the warp
-        const uint32_t act = __ballot_sync(0xFFFFFFFFu, in);
-        if (in) {
-          const uint32_t peers = __match_any_sync(act, bin);
-          if ((tid & 31) == (uint32_t)__ffs(peers) - 1u) atomicAdd(&s_hist[bin], (uint32_t)__popc(peers));
-        }
-      }
-      __syncthreads();
-      if (tid < 32) {
-        // lane owns 8 bins, top bins first: lane 0 -> bins 255..248
-        uint32_t loc[8], sum = 0;
-#pragma unroll
-        for (int j = 0; j < 8; j++) { loc[j] = s_hist[255 - (tid * 8 + j)]; sum += loc[j]; }
-        uint32_t incl = sum;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { uint32_t t = __shfl_up_sync(0xFFFFFFFFu, incl, o); if ((int)tid >= o) incl += t; }
-        uint32_t run = incl - sum;
-#pragma unroll
-        for (int j = 0; j < 8; j++) {
-          const uint32_t before = run;
-          run += loc[j];
-          if (before < need && run >= need) { s_sel[0] = 255 - (tid * 8 + j); s_sel[1] = before; s_sel[3] = loc[j]; }
-        }
-      }
-      __syncthreads();
-      prefix |= (uint64_t)s_sel[0] << shift;
-      need -= s_sel[1];
-      const uint32_t in_bin = s_sel[3];
-      __syncthreads();
-      if ((K - need) + in_bin <= cap) break;  // (block-uniform: every operand comes from shared memory)
-    }
-    thr = prefix;  // K-th largest first word with its unresolved low digits cleared: everything >= thr is kept
-  }
-  // count survivors; too many ties on the first word => sort every candidate instead
-  uint32_t mine = 0;
-  for (uint32_t i = tid; i < n; i += 1024) mine += a0[i] >= thr;
-  for (int o = 16; o > 0; o >>= 1) mine += __shfl_down_sync(0xFFFFFFFFu, mine, o);
-  if ((tid & 31) == 0 && mine) atomicAdd(&s_sel[2], mine);
-  __syncthreads();
-  uint32_t m = s_sel[2];
-  const bool all = m > QW_SEL_MAX;
-  __syncthreads();
-  uint64_t *k0, *k1, *k2;
-  uint32_t N = 32;
-  if (all) {
-    // degenerate: keys live interleaved [w0 | w1 | w2] over the whole candidate set
-    m = n;
-    while (N < m) N <<= 1;
-    k0 = a0; k1 = k0 + N; k2 = k1 + N;
-    for (uint32_t i = tid; i < N; i += 1024) {
-      if (i < n) { k0[i] = src[3ull * i]; k1[i] = src[3ull * i + 1]; k2[i] = src[3ull * i + 2]; }
-      else { k0[i] = 0; k1[i] = 0; k2[i] = 0; }
-    }
-  } else {
-    while (N < m) N <<= 1;
-    k0 = a0 + QW_CAND_CAP; k1 = k0 + QW_SEL_MAX; k2 = k1 + QW_SEL_MAX;
-    if (tid == 0) s_sel[2] = 0;
+// QW_SEL_TILES blocks of 1024 threads per split; each block of a split runs the same two steps on its own, with no
+// communication between blocks:
+//   1. cut: exact radix select (8-bit digits, MSB first) of the K-th largest first key word (select_cut), stopped as
+//      soon as at most QW_SEL_MAX candidates can survive, then a compaction of the candidates >= that word (all ties
+//      kept) in candidate order — the same survivors in the same order in every block of the split;
+//   2. rank: the survivors are grouped into buckets by the QW_RANK_BITS key bits after the bits they all share; the
+//      block takes its tile (a fixed range of the survivors) and gives each survivor its position in the reference
+//      total order: the survivors of the buckets above its own plus those of its own bucket with a larger key. Keys
+//      hold the doc id and are distinct, so the ranks are a permutation; a survivor ranked below K is decoded
+//      straight into the split's hit list.
+// A split with more than QW_SEL_MAX survivors (ties on the first word) is sorted whole by its first block instead
+// (sort_all_block).
+#define QW_SEL_MAX 2048  /* survivors ranked in shared memory; more ties than this => sort everything */
+#define QW_SEL_TILES 4   /* blocks per split (k_select's grid is QW_SEL_TILES x splits) */
+#define QW_RANK_BITS 10  /* key bits that pick a survivor's rank bucket: one bucket per thread of a block */
+
+// The cut of step 1 over the first key words a0[0..n) in shared memory: the K-th largest word with its unresolved
+// low digits cleared; every candidate whose word is >= the result survives. 0 when n <= K (all survive).
+__device__ uint64_t select_cut(const uint64_t* a0, uint32_t n, uint32_t K, uint32_t tid, uint32_t* s_hist, uint32_t* s_sel) {
+  if (n <= K) return 0;
+  uint64_t prefix = 0;
+  uint32_t need = K;  // rank of the wanted element among those matching the prefix
+  // once the candidates above the current bin plus the bin itself fit what the rank step takes (QW_SEL_MAX; K rounded
+  // up to a power of two when larger), the remaining digits need not be resolved (the whole bin is kept)
+  uint32_t cap = QW_SEL_MAX;
+  while (cap < K) cap <<= 1;
+  for (int shift = 56; shift >= 0; shift -= 8) {
+    if (tid < 256) s_hist[tid] = 0;
     __syncthreads();
+    const uint64_t himask = shift == 56 ? 0ull : (~0ull << (shift + 8));
     for (uint32_t base = 0; base < n; base += 1024) {
       const uint32_t i = base + tid;
       const uint64_t v = i < n ? a0[i] : 0ull;
-      const bool keep = i < n && v >= thr;
-      const uint32_t km = __ballot_sync(0xFFFFFFFFu, keep);  // one atomic per warp
-      uint32_t wpos = 0;
-      if ((tid & 31) == 0 && km) wpos = atomicAdd(&s_sel[2], (uint32_t)__popc(km));
-      wpos = __shfl_sync(0xFFFFFFFFu, wpos, 0);
-      if (keep) {
-        const uint32_t pos = wpos + __popc(km & ((1u << (tid & 31)) - 1u));
-        k0[pos] = v; k1[pos] = src[3ull * i + 1]; k2[pos] = src[3ull * i + 2];
+      const bool in = i < n && (v & himask) == prefix;
+      const uint32_t bin = (uint32_t)(v >> shift) & 255u;
+      // candidates near the threshold share their leading digits: one atomic per distinct bin of the warp
+      const uint32_t act = __ballot_sync(0xFFFFFFFFu, in);
+      if (in) {
+        const uint32_t peers = __match_any_sync(act, bin);
+        if ((tid & 31) == (uint32_t)__ffs(peers) - 1u) atomicAdd(&s_hist[bin], (uint32_t)__popc(peers));
       }
     }
-    for (uint32_t i = m + tid; i < N; i += 1024) { k0[i] = 0; k1[i] = 0; k2[i] = 0; }
+    __syncthreads();
+    if (tid < 32) {
+      // lane owns 8 bins, top bins first: lane 0 -> bins 255..248
+      uint32_t loc[8], sum = 0;
+#pragma unroll
+      for (int j = 0; j < 8; j++) { loc[j] = s_hist[255 - (tid * 8 + j)]; sum += loc[j]; }
+      uint32_t incl = sum;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) { uint32_t t = __shfl_up_sync(0xFFFFFFFFu, incl, o); if ((int)tid >= o) incl += t; }
+      uint32_t run = incl - sum;
+#pragma unroll
+      for (int j = 0; j < 8; j++) {
+        const uint32_t before = run;
+        run += loc[j];
+        if (before < need && run >= need) { s_sel[0] = 255 - (tid * 8 + j); s_sel[1] = before; s_sel[2] = loc[j]; }
+      }
+    }
+    __syncthreads();
+    prefix |= (uint64_t)s_sel[0] << shift;
+    need -= s_sel[1];
+    const uint32_t in_bin = s_sel[2];
+    __syncthreads();
+    if ((K - need) + in_bin <= cap) break;  // (block-uniform: every operand comes from shared memory)
+  }
+  return prefix;
+}
+
+// A split with more than QW_SEL_MAX survivors: bitonic sort of all n candidates with the full 192-bit comparison,
+// keys interleaved [w0 | w1 | w2] over the shared-memory arena (3 x 8 x QW_CAND_CAP bytes), best min(K, n) written.
+__device__ void sort_all_block(const DSplitPlan& P, const DCol* cols, uint32_t n, uint32_t K, uint32_t tid) {
+  const uint64_t* src = (const uint64_t*)P.out_cands;
+  uint32_t N = 32;
+  while (N < n) N <<= 1;
+  uint64_t *k0 = (uint64_t*)qw_smem, *k1 = k0 + N, *k2 = k1 + N;
+  for (uint32_t i = tid; i < N; i += 1024) {
+    if (i < n) { k0[i] = src[3ull * i]; k1[i] = src[3ull * i + 1]; k2[i] = src[3ull * i + 2]; }
+    else { k0[i] = 0; k1[i] = 0; k2[i] = 0; }
   }
   __syncthreads();
-  if (N <= 1024 && !all) {
-    // One key per thread, in registers: the compare-exchange partner of thread i at distance `stride` is thread
-    // i ^ stride, reached with warp shuffles below 32 and through shared memory (two buffers in turn: one barrier
-    // per exchange) from 32 up — 15 barriers for 1024 keys instead of the 55 of the generic network below.
-    const bool act = tid < N;
-    Key mine{0, 0, 0};
-    if (act) mine = Key{k0[tid], k1[tid], k2[tid]};
-    uint32_t pb = 1;  // exchange buffer: 1 = the first-word array (dead by now), 0 = the survivor arrays
-    __syncthreads();
-    for (uint32_t size = 2; size <= N; size <<= 1) {
-      for (uint32_t stride = size >> 1; stride > 0; stride >>= 1) {
-        Key other{0, 0, 0};
-        if (stride >= 32) {
-          uint64_t *b0 = pb ? a0 : k0, *b1 = pb ? a0 + 1024 : k1, *b2 = pb ? a0 + 2048 : k2;
-          if (act) { b0[tid] = mine.w0; b1[tid] = mine.w1; b2[tid] = mine.w2; }
-          __syncthreads();
-          if (act) other = Key{b0[tid ^ stride], b1[tid ^ stride], b2[tid ^ stride]};
-          pb ^= 1;
-        } else if (act) {
-          other.w0 = __shfl_xor_sync(0xFFFFFFFFu, mine.w0, stride);
-          other.w1 = __shfl_xor_sync(0xFFFFFFFFu, mine.w1, stride);
-          other.w2 = __shfl_xor_sync(0xFFFFFFFFu, mine.w2, stride);
-        }
-        // descending runs where (i & size) == 0; the lower index of a pair keeps the larger key there
-        const bool want_larger = ((tid & stride) == 0) == ((tid & size) == 0);
-        if (act && want_larger == key_lt(mine, other)) mine = other;
-      }
-    }
-    __syncthreads();
-    if (act) { k0[tid] = mine.w0; k1[tid] = mine.w1; k2[tid] = mine.w2; }
-    __syncthreads();
-  } else
   for (uint32_t size = 2; size <= N; size <<= 1) {
     for (uint32_t stride = size >> 1; stride > 0; stride >>= 1) {
       for (uint32_t i = tid; i < (N >> 1); i += 1024) {
@@ -1820,12 +1758,121 @@ __global__ void __launch_bounds__(1024) k_select(const DSplitPlan* plans, const 
       __syncthreads();
     }
   }
-  const uint32_t out_n = m < K ? m : K;
-  const DCol* cols = all_cols + P.col_base;
+  const uint32_t out_n = n < K ? n : K;
   for (uint32_t i = tid; i < out_n; i += 1024) write_hit(P, cols, Key{k0[i], k1[i], k2[i]}, i);
   if (tid == 0) *(uint32_t*)P.out_nhits = out_n;
 }
 
+__global__ void __launch_bounds__(1024) k_select(const DSplitPlan* plans, const DCol* all_cols) {
+  const DSplitPlan& P = plans[blockIdx.y];
+  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, tile = blockIdx.x;
+  if (P.max_hits == 0) { if (tile == 0 && tid == 0) *(uint32_t*)P.out_nhits = 0; return; }
+  if (P.max_hits > QW_MAX_TOPK) return;  // the deep selection path's split (deep_select_kernel.cuh)
+  uint32_t n = *(const uint32_t*)P.out_cand_count;
+  if (n > QW_CAND_CAP) n = QW_CAND_CAP;  // overflow is detected by the host (cand_count > cap)
+  const uint32_t K = P.max_hits;
+  const uint64_t* src = (const uint64_t*)P.out_cands;
+  const DCol* cols = all_cols + P.col_base;
+  // shared memory: all first words [QW_CAND_CAP], then the survivors [w0 | w1 | w2] x QW_SEL_MAX
+  uint64_t* a0 = (uint64_t*)qw_smem;
+  uint64_t *k0 = a0 + QW_CAND_CAP, *k1 = k0 + QW_SEL_MAX, *k2 = k1 + QW_SEL_MAX;
+  __shared__ uint32_t s_hist[256];
+  __shared__ uint32_t s_sel[3];  // select_cut: [0] digit, [1] count above digit, [2] count in the digit's bin
+  __shared__ uint32_t s_wpos[33];  // survivors before each warp's range of candidates; [32] = all survivors
+  __shared__ unsigned long long s_diff[3];  // OR of every survivor's key XOR the first survivor's
+  __shared__ uint32_t s_bbeg[1u << QW_RANK_BITS], s_bend[1u << QW_RANK_BITS];  // each rank bucket's survivors
+  for (uint32_t i = tid; i < n; i += 1024) a0[i] = src[3ull * i];
+  __syncthreads();
+  const uint64_t thr = select_cut(a0, n, K, tid, s_hist, s_sel);
+  // survivors in candidate order (the same in every block): warp w compacts the candidates [w R, (w + 1) R)
+  const uint32_t R = ((n + 1023u) >> 10) << 5;
+  const uint32_t wbeg = warp * R, wend = min(n, wbeg + R);
+  uint32_t cnt = 0;
+  for (uint32_t i = wbeg + lane; i < wbeg + R; i += 32) cnt += __popc(__ballot_sync(0xFFFFFFFFu, i < wend && a0[i] >= thr));
+  if (lane == 0) s_wpos[warp] = cnt;
+  __syncthreads();
+  if (warp == 0) {
+    const uint32_t c = s_wpos[lane];
+    uint32_t incl = c;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { uint32_t t = __shfl_up_sync(0xFFFFFFFFu, incl, o); if ((int)lane >= o) incl += t; }
+    s_wpos[lane] = incl - c;
+    if (lane == 31) s_wpos[32] = incl;
+  }
+  __syncthreads();
+  const uint32_t m = s_wpos[32];
+  if (m > QW_SEL_MAX) {
+    if (tile == 0) sort_all_block(P, cols, n, K, tid);
+    return;
+  }
+  uint32_t pos = s_wpos[warp];
+  for (uint32_t i = wbeg + lane; i < wbeg + R; i += 32) {
+    const bool keep = i < wend && a0[i] >= thr;
+    const uint32_t km = __ballot_sync(0xFFFFFFFFu, keep);
+    if (keep) {
+      const uint32_t p = pos + __popc(km & ((1u << lane) - 1u));
+      k0[p] = a0[i]; k1[p] = src[3ull * i + 1]; k2[p] = src[3ull * i + 2];
+    }
+    pos += __popc(km);
+  }
+  if (tile == 0 && tid == 0) *(uint32_t*)P.out_nhits = m < K ? m : K;
+  if (tid < 3) s_diff[tid] = 0;
+  s_bend[tid] = 0;
+  __syncthreads();
+  // rank buckets: the QW_RANK_BITS key bits that follow the bits every survivor shares. A larger bucket holds only
+  // larger keys, so a survivor's rank is the count of the buckets above its own plus the larger keys of its own bucket.
+  {
+    uint64_t x0 = 0, x1 = 0, x2 = 0;
+    for (uint32_t i = tid; i < m; i += 1024) { x0 |= k0[i] ^ k0[0]; x1 |= k1[i] ^ k1[0]; x2 |= k2[i] ^ k2[0]; }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      x0 |= __shfl_xor_sync(0xFFFFFFFFu, x0, o); x1 |= __shfl_xor_sync(0xFFFFFFFFu, x1, o); x2 |= __shfl_xor_sync(0xFFFFFFFFu, x2, o);
+    }
+    if (lane == 0 && (x0 | x1 | x2)) { atomicOr(&s_diff[0], x0); atomicOr(&s_diff[1], x1); atomicOr(&s_diff[2], x2); }
+  }
+  __syncthreads();
+  const uint32_t common = s_diff[0] ? __clzll(s_diff[0]) : s_diff[1] ? 64 + __clzll(s_diff[1]) : s_diff[2] ? 128 + __clzll(s_diff[2]) : 192;
+  const uint32_t at = min(common, 192u - QW_RANK_BITS);
+  for (uint32_t i = tid; i < m; i += 1024) atomicAdd(&s_bend[key_get(Key{k0[i], k1[i], k2[i]}, at, QW_RANK_BITS)], 1u);
+  __syncthreads();
+  {
+    // thread t owns bucket 1023 - t: exclusive scan of the counts from the top bucket down
+    const uint32_t c = s_bend[1023 - tid];
+    uint32_t incl = c;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { uint32_t t = __shfl_up_sync(0xFFFFFFFFu, incl, o); if ((int)lane >= o) incl += t; }
+    if (lane == 31) s_wpos[warp] = incl;
+    __syncthreads();
+    if (warp == 0) {
+      const uint32_t w = s_wpos[lane];
+      uint32_t wi = w;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) { uint32_t t = __shfl_up_sync(0xFFFFFFFFu, wi, o); if ((int)lane >= o) wi += t; }
+      s_wpos[lane] = wi - w;
+    }
+    __syncthreads();
+    const uint32_t beg = s_wpos[warp] + incl - c;
+    s_bbeg[1023 - tid] = beg;
+    s_bend[1023 - tid] = beg;
+  }
+  __syncthreads();
+  // survivors grouped by bucket over the first-word array (dead by now); the order inside a bucket does not matter
+  uint64_t *g0 = a0, *g1 = g0 + QW_SEL_MAX, *g2 = g1 + QW_SEL_MAX;
+  for (uint32_t i = tid; i < m; i += 1024) {
+    const Key k{k0[i], k1[i], k2[i]};
+    const uint32_t p = atomicAdd(&s_bend[key_get(k, at, QW_RANK_BITS)], 1u);
+    g0[p] = k.w0; g1[p] = k.w1; g2[p] = k.w2;
+  }
+  __syncthreads();
+  // this block's tile: survivors [lo, hi) in candidate order, one thread each
+  const uint32_t S = (m + QW_SEL_TILES - 1) / QW_SEL_TILES, lo = tile * S, i = lo + tid;
+  if (i >= min(m, lo + S)) return;
+  const Key mine{k0[i], k1[i], k2[i]};
+  const uint32_t b = (uint32_t)key_get(mine, at, QW_RANK_BITS), end = s_bend[b];
+  uint32_t rank = s_bbeg[b];
+  for (uint32_t j = s_bbeg[b]; j < end; j++) rank += key_lt(mine, Key{g0[j], g1[j], g2[j]});
+  if (rank < K) write_hit(P, cols, mine, rank);
+}
 
 // Leaf-level merge on the device (IncrementalCollector / top_k_partial_hits, quickwit-search/src/
 // collector.rs:1195-1313, 980-992): the per-split lists written by k_select are sorted best-first; a hit's
